@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — novel views/sec of the ViewFormer hot path on B200 (BASELINE.json metric, config 2).
+"""bench.py — novel views/sec of the ViewFormer hot path on H100 (BASELINE.json metric, config 2).
 
 One "step" = one pass of generate() over a batch of synthetic scenes:
     uint8 images [B, 10, 128, 128, 3] + cameras [B, 10, 7]
@@ -11,10 +11,11 @@ the data path — scenes are independent).
     python bench.py --gpus 1 --steps 5 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference ...     # the reference algorithm on the host CPU cores (torch-CPU oracle)
+    python bench.py ... --dump-outputs DIR    # also write what the last timed step computed, DIR/<name>.npy
 
 Prints ONE JSON line (rank 0).  `value` = views/s with inputs resident in HBM; `e2e` = same metric through the public
 generate() call with pinned-host inputs, H2D/D2H inside the timed region; `roofline` = the dominant kernel
-(tcgen05 implicit-GEMM 3x3 conv 128->128 @128x128) timed alone with CUDA events against the measured bf16 peak;
+(wgmma implicit-GEMM 3x3 conv 128->128 @128x128) timed alone with CUDA events against the bf16 peak;
 `cpu_baseline` = the oracle timed on a bounded sample on this box's host cores.
 """
 import argparse
@@ -54,6 +55,8 @@ def parse():
     ap.add_argument("--no-parity", action="store_true", help="skip the in-run parity block")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel eagerly instead of replaying the captured CUDA graph")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps write the arrays the last timed step returned as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--workload", default="generate", choices=["generate", "kvcache", "train"],
                     help="generate = BASELINE configs[1] (default, the judged line); kvcache = configs[4]: 19-context KV-cached query decode; "
                          "train = configs[3]: codebook training step (--scenes = images per GPU)")
@@ -75,7 +78,7 @@ def synth_inputs(n_scenes, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -128,23 +131,15 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops", 1590.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured"
 
 
-def ncu_traffic(rel_path, scale, what="288 images/launch"):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the roofline kernel from the committed `ncu --set full` capture (metric dump
-    under profiles/), scaled by the launch's image count.  Read from the file, not a literal; None when the capture is absent."""
-    path = os.path.join(ROOT, rel_path)
-    if not os.path.exists(path):
-        return None, "no capture committed"
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tot = 0.0
-    for line in open(path):
-        f = [c.strip().strip('"') for c in line.rstrip("\n").split(",")]
-        if f[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and len(f) >= 3 and f[1] in unit:
-            tot += float(f[2]) * unit[f[1]]
-    return (tot * scale if tot else None), f"{rel_path} (ncu --set full of this kernel, {what}) x {scale:.3f}"
+def algorithmic_traffic(n_img, exact):
+    """DRAM bytes the roofline conv has to move at least, from its shapes: the input activation read once (bf16, or the split-fp16
+    [hi | lo] pair in exact mode), the fp32 output written once; the 9 x 128 x 128 weights are negligible."""
+    px = n_img * IMG * IMG
+    return px * 128 * (4 if exact else 2) + px * 128 * 4, "algorithmic (input read once + fp32 output written once)"
 
 
 # ------------------------------------------------------------------------------------------------- reference arm (CPU)
@@ -212,7 +207,7 @@ def run_reference(args):
     }))
 
 
-# ------------------------------------------------------------------------------------------------- B200 arm
+# ------------------------------------------------------------------------------------------------- CUDA arm
 def model_pair(precision, vcfg, tcfg, dev, seed=0):
     """(codebook, transformer) of one precision mode.  ``mixed`` pairs the exact-encoder VQGAN with the bf16 transformer."""
     from viewformer_b200 import VQGAN, MIGT
@@ -248,6 +243,29 @@ def parity_block(codebook, transformer, out_timed, images_d, cams_d, vcfg, tcfg,
     }
     del xvq, xtr
     return blk, codes_x
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each returned tensor as out_dir/<name>.npy: floating tensors as float32, integer / bool / uint8 ones as float64
+    (exact for every value they hold).  A tensor beyond the size limit is cut to a fixed, seeded sample of its leading-axis rows."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name in sorted(arrays):
+        t = arrays[name].detach().cpu()
+        a = t.float().numpy() if t.is_floating_point() else t.double().numpy()
+        if total + a.nbytes > DUMP_LIMIT_BYTES and a.ndim > 0 and a.shape[0] > 1:
+            per_row = a.nbytes // a.shape[0]
+            keep = max(1, min(a.shape[0], (DUMP_LIMIT_BYTES - total) // max(1, per_row)))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=keep, replace=False))
+            a = a[rows]
+        if total + a.nbytes > DUMP_LIMIT_BYTES:
+            continue
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        total += a.nbytes
 
 
 def run_b200(args):
@@ -305,13 +323,18 @@ def run_b200(args):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def timed(fn, steps):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
+        r = None
         for _ in range(steps):
-            fn()
+            r = fn()
         e1.record()
+        if r is not None and fn is step_resident:   # copy out (after the end event) before later steps reuse static buffers
+            last.update({k: v.clone() for k, v in r.items() if torch.is_tensor(v)})
         barrier()
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
         if world > 1:
@@ -351,6 +374,8 @@ def run_b200(args):
     ms_e2e = timed(step_e2e, args.steps)
     out_timed = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in step_resident().items()}
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
 
     views = world * B * args.steps
     value = views / (ms_total / 1e3)
@@ -419,11 +444,10 @@ def run_b200(args):
     flops = 2.0 * n_img * IMG * IMG * 128 * 9 * 128          # SURVEY §8(d): 2*M*N*K of the implicit GEMM
     passes = 3 if exact else 1
     ach = passes * flops / sec / 1e12
-    cap = "profiles/r02_exact_conv_wide_ncu_metrics.csv" if exact else "profiles/r01_conv_wide_ncu_nores_metrics.csv"
-    traffic, traffic_src = ncu_traffic(cap, n_img / 288.0)
-    roof = {"kernel": ("tc_conv3x3_wide_kernel<exact>: persistent tcgen05 implicit GEMM on split-fp16 operands (3 MMA passes, chunked accumulation), "
-                       if exact else "tc_conv3x3_wide_kernel: persistent tcgen05 implicit GEMM, ") +
-                      "128 channels x 256 pixels per tile (3x3 conv 128->128 @128x128, %d images/launch)" % n_img,
+    traffic, traffic_src = algorithmic_traffic(n_img, exact)
+    roof = {"kernel": ("tc_gemm_kernel<exact>: persistent wgmma implicit GEMM on split-fp16 operands (3 MMA passes, chunked accumulation), "
+                       if exact else "tc_gemm_kernel (halo mode): persistent wgmma implicit GEMM, ") +
+                      "128 pixels x 128 channels per tile (3x3 conv 128->128 @128x128, %d images/launch)" % n_img,
             # `achieved` / `frac`: ALGORITHMIC flops of the convolution (2*M*N*K) over the launch time, as the contract defines them.  The
             # exact mode spends three fp16 MMA passes per algorithmic flop to return fp32-faithful results: `achieved_executed_mma` /
             # `frac_executed_mma` say how busy the tensor pipe actually is (the number to compare with ncu's sm__pipe_tc_cycles_active).
@@ -442,8 +466,9 @@ def run_b200(args):
     if q.get("eh") is not None:
         sec_vq = time_launch(lambda: _lib.vq_lookup_fused(zq, q["et"], q["esq"], q["eh"], emb_dk=q["emb"], want_quant=False, want_diff=False), reps=3)
         ach_vq = Mvq * (q["et"].shape[1] * 4 + 8) / sec_vq / 1e9
-        tr_vq, tr_vq_src = ncu_traffic("profiles/r02_vq_fused_ncu_metrics.csv", 1.0, "vq_lookup_fused_kernel at M = 2^20; the exact pass adds 0.03 GB")
-        roof_vq = {"kernel": "vq_lookup_fused_kernel + vq_rescue_kernel: fp16 distance GEMM on CTA pairs, top-2 from TMEM, fp64 settlement of near-ties "
+        tr_vq = float(Mvq * (q["et"].shape[1] * 4 + 8))
+        tr_vq_src = f"algorithmic (every z row read once, one int64 index written, M = {Mvq}, D = {q['et'].shape[1]})"
+        roof_vq = {"kernel": "vq_lookup_fused_kernel + vq_rescue_kernel: fp16 wgmma distance GEMM, top-2 from the accumulator registers, fp64 settlement of near-ties "
                              "(z ~ N(0,1) [2^20, 256] fp32 -> int64 indices, K = 1024)",
                    "bound": "hbm", "achieved": ach_vq, "peak": peak_hbm, "unit": "GB/s", "frac": ach_vq / peak_hbm, "traffic": tr_vq,
                    "traffic_source": tr_vq_src, "peak_source": peak_src, "launch_ms": sec_vq * 1e3,
@@ -599,6 +624,8 @@ def run_train(args):
 
 if __name__ == "__main__":
     a = parse()
+    if a.dump_outputs and (a.workload != "generate" or a.impl != "b200"):
+        sys.exit("bench.py: --dump-outputs writes the outputs of the CUDA generate() arm only (--workload generate --impl b200)")
     if a.workload == "train" and a.impl == "b200":
         run_train(a)
     elif a.workload == "kvcache" and a.impl == "b200":

@@ -1,4 +1,4 @@
-/* vf_b200.h — C-ABI of libvf_b200.so, the sm_100a kernel library underneath
+/* vf_b200.h — C-ABI of libvf_b200.so, the sm_90a kernel library underneath
  * viewformer_b200.{VQGAN,MIGT}.
  *
  * The reference (jkulhanek/viewformer) has no FFI layer: its hot path is Python calling
@@ -32,7 +32,7 @@ int vf_version(void);
 /* struct sizes, so a foreign-language binding can verify its mirror of the parameter structs */
 int vf_sizeof_simt_gemm(void);
 int vf_sizeof_tc_gemm(void);
-/* 0 when the current device is compute capability 10.x (B200); negative otherwise. */
+/* 0 when the current device is compute capability 9.0 (H100); negative otherwise. */
 int vf_device_check(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -110,7 +110,7 @@ typedef struct {
 int vf_simt_gemm(const vf_simt_gemm_t* p, vf_stream_t s);
 
 /* ------------------------------------------------------------------------------------------
- * tcgen05 tensor-core GEMM / implicit-GEMM conv (TMA -> 128B-swizzled smem -> tcgen05.mma -> TMEM)
+ * tensor-core GEMM / implicit-GEMM conv (TMA -> 128B-swizzled smem -> wgmma -> register accumulators)
  * replaces the same call sites as vf_simt_gemm on the fast path.
  *   GEMM:  C[b1,b2][m,n] = act(alpha * sum_k A[b1,b2][m,k] * B[b1,b2][n,k] + bias) + residual
  *          A and B are K-major (k contiguous), 16-byte aligned rows, dtype bf16 (or f32 -> TF32).
@@ -143,7 +143,7 @@ typedef struct {
        an image = OH*OW consecutive rows (conv) or gn_rows_per_img rows (gemm).  Feed it to vf_groupnorm_finalize. */
     double* gn_sums; int gn_groups; int gn_rows_per_img;
     /* optional: GroupNorm(+swish) of the INPUT applied while the operand sits in shared memory (3x3 stride-1 bf16 convs on
-       maps >= 32 rows tall, Cin % 64 == 0, Cout % 128 == 0 — the shapes of the wide-tile kernel; other shapes are rejected):
+       maps >= 32 rows tall, Cin % 64 == 0, Cout % 128 == 0 — the halo-tile path of the kernel; other shapes are rejected):
        A then is the RAW activation (e.g. the bf16 output of the previous conv), norm_mean_rstd float [N, norm_groups, 2]
        from vf_groupnorm_finalize, norm_gamma / norm_beta float [Cin].  Padding stays zero AFTER normalisation, as in
        vqgan_th.py:69-78 (norm -> swish -> conv with padding=1).  Removes the separate vf_groupnorm_apply pass.
@@ -151,7 +151,7 @@ typedef struct {
        2 = packed bf16 h (1 + tanh h), h = x / 2 (one MUFU op per two elements). */
     const float* norm_mean_rstd; const float* norm_gamma; const float* norm_beta; int norm_groups; int norm_swish;
     /* ab_dtype = VF_F16X2 ("exact" mode: fp32-faithful products on the tensor cores — three fp16 MMA passes hi.hi + 2^-11 (hi.lo +
-       lo.hi), accumulation drained from TMEM in short chunks and summed with round-to-nearest FFMAs; fp32 output only):
+       lo.hi), accumulation drained from the accumulators in short chunks and summed with round-to-nearest FFMAs; fp32 output only):
          conv: A = [N,H,W, hi(Cl) | lo(Cl)] with Ctot = 2*Cl, B = [Cout][tap][hi(Cin) | lo(Cin)];
          gemm: a row of A holds hi(K) at column 0 and lo(K) at column exact_lo_a (elements), B rows likewise at exact_lo_b;
                K %% 64 == 0; lda / ldb are the full row strides. */
@@ -160,7 +160,7 @@ typedef struct {
 int vf_tc_gemm(const vf_tc_gemm_t* p, vf_stream_t s);
 
 /* ------------------------------------------------------------------------------------------
- * Fused block-causal attention on tcgen05 (single-stream forward):  out = softmax(mask(Q K^T)) V, no 1/sqrt(dh) scale
+ * Fused block-causal attention on wgmma (single-stream forward):  out = softmax(mask(Q K^T)) V, no 1/sqrt(dh) scale
  * replaces: models/branching_attention.py:41-61 via models/migt.py:211-217.
  *   qk  bf16 [B, S, 2d]  rows = tokens, columns [0,d) = q, [d,2d) = k (head h at columns h*64..h*64+63)
  *   vt  bf16 [B, d, S]   V transposed (row = channel, contiguous over tokens)
@@ -271,9 +271,9 @@ int vf_vq_lookup(const float* z, const float* Et, const float* esq, int64_t M, i
 int vf_vq_split3(const float* x, int64_t rows, int D, int codebook, void* out_bf16, vf_stream_t s);
 int vf_vq_select(const float* scores, const float* z, const float* Et, const float* esq, int64_t M, int D, int K, float tol,
                  int64_t* idx, float* quant, double* diff_sum, int* n_rescored, vf_stream_t s);
-/* Fused lookup (same result as vf_vq_lookup; viewformer_b200/csrc/vf_vq_fused.cu): one tcgen05 kernel reads every z row ONCE
- * (fp32 -> fp16 in shared memory), scores it against Eh = fp16(-2 e) [K,D] (vf_vq_prepare_codebook_f16) on CTA pairs and keeps the
- * two best codes per row straight from TMEM — no score matrix in HBM, 4*D + 8 bytes of traffic per row.  Rows whose two best scores
+/* Fused lookup (same result as vf_vq_lookup; viewformer_b200/csrc/vf_vq_fused.cu): one wgmma kernel reads every z row ONCE
+ * (fp32 -> fp16 in shared memory), scores it against Eh = fp16(-2 e) [K,D] (vf_vq_prepare_codebook_f16) with wgmma and keeps the
+ * two best codes per row straight from the accumulator registers — no score matrix in HBM, 4*D + 8 bytes of traffic per row.  Rows whose two best scores
  * lie within the fp16 rounding bound (tol_factor x worst case; 0.25 recommended) are settled exactly in fp64 by a second kernel.
  *   D % 64 == 0, D <= 256, K % 256 == 0, K <= 1024, M < 2^31.  worklist: int4[M] scratch; counter: int[2] scratch, on return
  *   counter[0] = rows settled between two candidates, counter[1] = rows settled over all codes.  quant / diff_sum nullable. */

@@ -117,7 +117,7 @@ for Mq in (18432, 1 << 20):
     ms = timeit(lambda: L.vq_lookup(zq, et, esq, want_quant=False, want_diff=False), reps=3, warm=1)
     rows.append((f"VQ lookup fp32 CUDA-core  M={Mq}", ms, 2.0 * Mq * 256 * 1024 / ms / 1e9, Mq * 1032 / ms / 1e6))
     ms = timeit(lambda: L.vq_lookup_tc(zq, et, esq, et3, want_quant=False, want_diff=False), reps=3, warm=1)
-    rows.append((f"VQ lookup tcgen05 bf16x3  M={Mq}", ms, 2.0 * Mq * 256 * 1024 / ms / 1e9, Mq * 1032 / ms / 1e6))
+    rows.append((f"VQ lookup tensor-core bf16x3  M={Mq}", ms, 2.0 * Mq * 256 * 1024 / ms / 1e9, Mq * 1032 / ms / 1e6))
 
 print(f"{'kernel':58s} {'ms':>8s} {'TFLOP/s':>9s} {'%peak':>6s} {'GB/s':>8s} {'%hbm':>6s}")
 for name, ms, tf, gbs in rows:

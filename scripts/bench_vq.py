@@ -30,7 +30,7 @@ def timeit(fn, reps=5, warm=2):
 only = sys.argv[1] if len(sys.argv) > 1 else ""
 for M in ([1 << 20] if only == "fused" else [18432, 1 << 17, 1 << 20]):
     z = torch.randn((M, 256), device=dev)
-    rows = [("fused tcgen05 (1 pass, fp16 pairs)", lambda: L.vq_lookup_fused(z, et, esq, eh, emb_dk=E, want_quant=False, want_diff=False))]
+    rows = [("fused wgmma (1 pass, fp16 pairs)", lambda: L.vq_lookup_fused(z, et, esq, eh, emb_dk=E, want_quant=False, want_diff=False))]
     if only != "fused":
         rows += [("bf16x3 GEMM + select (round 1)", lambda: L.vq_lookup_tc(z, et, esq, et3, want_quant=False, want_diff=False))]
         if M <= 1 << 17:

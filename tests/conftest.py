@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100a) device; run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) device; run with -m gpu")
 
 
 @pytest.fixture(scope="session")

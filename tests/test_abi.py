@@ -36,7 +36,7 @@ def test_version_and_error_string(lib):
 
 
 def test_no_fallback_without_device():
-    """Product path must fail loudly when there is no sm_100 device (no CPU fallback)."""
+    """Product path must fail loudly when there is no sm_90 device (no CPU fallback)."""
     import pytest
     import torch
     from viewformer_b200 import _lib

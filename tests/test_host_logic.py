@@ -85,22 +85,17 @@ def test_schedule_strings():
     assert MIGTConfig(localization_weight="warmup(1,2000)").use_localization is True
 
 
-def test_bench_reads_roofline_traffic_from_committed_captures():
-    """bench.py's `roofline.traffic` / `roofline_vq_lookup.traffic` are parsed from the ncu metric dumps under profiles/ (not literals):
-    the files it names must be present and yield the kernels' DRAM bytes."""
+def test_bench_roofline_traffic_is_algorithmic():
+    """bench.py's `roofline.traffic` is the DRAM traffic the conv needs at least, computed from its shapes (not a literal)."""
     import importlib.util, os
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     spec = importlib.util.spec_from_file_location("vf_bench", os.path.join(root, "bench.py"))
     bench = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(bench)
-    conv, src = bench.ncu_traffic("profiles/r02_exact_conv_wide_ncu_metrics.csv", 1.0)
-    assert conv is not None and 4.5e9 < conv < 5.2e9, (conv, src)               # algorithmic: 288 x 16384 x 128 x 8 B = 4.83 GB
-    vq, src = bench.ncu_traffic("profiles/r02_vq_fused_ncu_metrics.csv", 1.0, "vq")
-    assert vq is not None and 1.05e9 < vq < 1.2e9, (vq, src)                      # algorithmic: 2^20 x 1032 B = 1.08 GB
-    bf16, _ = bench.ncu_traffic("profiles/r01_conv_wide_ncu_nores_metrics.csv", 1.0)
-    assert bf16 is not None and 3.3e9 < bf16 < 3.9e9
-    none, why = bench.ncu_traffic("profiles/does_not_exist.csv", 1.0)
-    assert none is None and "no capture" in why
+    conv, src = bench.algorithmic_traffic(288, True)
+    assert 4.5e9 < conv < 5.2e9 and "algorithmic" in src                        # 288 x 16384 x 128 x 8 B = 4.83 GB
+    bf16, _ = bench.algorithmic_traffic(288, False)
+    assert 3.3e9 < bf16 < 3.9e9                                                  # 288 x 16384 x 128 x 6 B = 3.62 GB
 
 
 def test_camera_metrics_match_the_reference_evaluator_fixture(golden_dir):
@@ -123,12 +118,12 @@ def test_camera_metrics_match_the_reference_evaluator_fixture(golden_dir):
 
 
 def test_bench_json_contract_of_both_arms():
-    """The keys the driver reads: (a) the committed line of the B200 arm (profiles/, produced on a B200 by this bench.py), (b) the
-    reference arm run live here on the host cores with a tiny wall budget (`bench.py --impl reference`: the CPU oracle, bounded)."""
+    """The keys of the JSON line: (a) a committed line of the CUDA arm (tests/golden/bench_line_h100.json, produced on an H100 by this
+    bench.py), (b) the reference arm run live on the host cores with a tiny wall budget (`bench.py --impl reference`: the CPU oracle, bounded)."""
     import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    line = json.load(open(os.path.join(root, "profiles", "r02_bench_n1_mixed_v6.json")))
+    line = json.load(open(os.path.join(root, "tests", "golden", "bench_line_h100.json")))
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype", "data",
               "config", "e2e", "gpu_launches", "clocks", "roofline", "cpu_baseline", "parity"):
         assert k in line, k

@@ -139,7 +139,7 @@ def test_simt_gemm_batched_strided(L):
     report("simt_gemm", out, want, 2e-5, 1e-5)
 
 
-# ----------------------------------------------------------------------------- tcgen05 GEMM
+# ----------------------------------------------------------------------------- tensor-core (wgmma) GEMM
 def _tc_case(L, dtype, M, N, K, batch=(1, 1), bias_mode=0, act=0, residual=False, alpha=1.0, out_dtype=torch.float32, seed=0):
     B1, B2 = batch
     A = torch.randn(B1, B2, M, K, generator=g(seed))
@@ -256,7 +256,7 @@ def test_tc_gemm_causal(L):
     report("pv causal", o, p.bfloat16().double() @ vt.double().cpu().t(), 2e-2, 1e-2)
 
 
-# ----------------------------------------------------------------------------- tcgen05 conv
+# ----------------------------------------------------------------------------- tensor-core (wgmma) conv
 @pytest.mark.parametrize("dtype,cin,cout,n,hw", [(torch.bfloat16, 64, 128, 2, 16), (torch.bfloat16, 128, 128, 1, 32),
                                                   (torch.bfloat16, 256, 64, 3, 8), (torch.bfloat16, 128, 256, 2, 4),
                                                   (torch.float32, 64, 128, 2, 16), (torch.bfloat16, 128, 128, 1, 20)])
@@ -306,7 +306,7 @@ def test_tc_conv3x3_wide_tiles(L, n, H, W, cin, cout, res, out_bf16):
 
 @pytest.mark.parametrize("n,H,W,cin,cout", [(2, 64, 64, 128, 128), (1, 40, 20, 64, 256), (2, 33, 9, 128, 128), (3, 32, 8, 256, 128)])
 def test_tc_conv_normalise_on_load(L, n, H, W, cin, cout):
-    """GroupNorm + swish applied to the conv operand inside the wide kernel == vf_groupnorm_apply followed by the conv, bit for
+    """GroupNorm + swish applied to the halo tile of the conv operand inside the kernel == vf_groupnorm_apply followed by the conv, bit for
     bit (same arithmetic on the same bf16 values); padding stays zero after normalisation (ragged tiles exercise the border)."""
     xr = (torch.randn(n, H, W, cin, generator=g(H * W + cin)) * 1.3 + 0.4).cuda()
     xb = xr.bfloat16()
@@ -332,7 +332,7 @@ def test_tc_conv_normalise_on_load(L, n, H, W, cin, cout):
     mean = (sums[..., 0] / (H * W * cin // 32)).cpu()
     ref = F.conv2d((xn * torch.sigmoid(xn)), w.double().cpu().reshape(cout, 3, 3, cin).permute(0, 3, 1, 2), b.double().cpu(), padding=1)
     report("norm-on-load vs fp64", got.permute(0, 3, 1, 2), ref + res.double().cpu().permute(0, 3, 1, 2), 5e-2, 3e-2)
-    with pytest.raises(Exception):      # shapes outside the wide kernel are rejected, not silently un-normalised
+    with pytest.raises(Exception):      # shapes outside the halo-tile path are rejected, not silently un-normalised
         small = torch.randn(1, 16, 16, 64).bfloat16().cuda()
         L.tc_conv(small, (torch.randn(128, 9 * 64) / 24).bfloat16().cuda(), None,
                   norm=(torch.zeros(1, 32, 2, device="cuda"), torch.ones(64, device="cuda"), torch.zeros(64, device="cuda"), 32, True))
@@ -518,7 +518,7 @@ def test_tc_conv_fused_groupnorm_statistics(L, cin, cout, n, hw):
 
 @pytest.mark.parametrize("B,T,H,blk", [(2, 4, 3, 64), (1, 10, 2, 64), (2, 3, 2, 64), (1, 5, 1, 32)])
 def test_fused_block_causal_attention(L, B, T, H, blk):
-    """Fused tcgen05 attention == softmax(q k^T * m - 1e4 (1-m)) v of branching_attention.py:5-18,41-61 (no 1/sqrt(d))."""
+    """Fused wgmma attention == softmax(q k^T * m - 1e4 (1-m)) v of branching_attention.py:5-18,41-61 (no 1/sqrt(d))."""
     d, S = H * 64, T * blk
     qk = (torch.randn(B, S, 2 * d, generator=g(S + H)) * 0.6).bfloat16()
     v = torch.randn(B, S, d, generator=g(S + H + 1)).bfloat16()
@@ -549,7 +549,7 @@ def _attn_reference(qk, v, B, S, H, d, blk):
 
 @pytest.mark.parametrize("B,T,H,blk,first", [(2, 6, 2, 64, 0), (1, 20, 2, 64, 0), (2, 20, 3, 64, 19 * 64), (1, 7, 1, 64, 6 * 64)])
 def test_fused_attention_growing_logits_and_tail(L, B, T, H, blk, first):
-    """Single-pass softmax: key norms grow from view to view, so the running reference maximum has to move (and the TMEM accumulator be
+    """Single-pass softmax: key norms grow from view to view, so the running reference maximum has to move (and the register accumulator be
     rescaled) several times per row; `first` > 0 is the KV-cache decode call (only the last view's query rows are computed)."""
     d, S = H * 64, T * blk
     qk = (torch.randn(B, S, 2 * d, generator=g(S + H + 7)) * 0.5)
@@ -616,7 +616,7 @@ def test_fused_multiend_attention(L, B, T, H):
 
 
 def test_vq_lookup_tensor_core_bit_exact(L, golden_dir):
-    """bf16x3 tcgen05 distance GEMM + exact fp64 re-score == the reference's indices, incl. the adversarial near-ties."""
+    """bf16x3 tensor-core distance GEMM + exact fp64 re-score == the reference's indices, incl. the adversarial near-ties."""
     import os
     from oracle import synth
     gd = np.load(os.path.join(golden_dir, "vq_lookup.npz"))
@@ -725,9 +725,9 @@ def test_tc_downsample_exact_split_fp16(L, cin, cout, n, hw):
     assert float(e.max() / want.abs().mean()) < 4e-6
 
 
-# ----------------------------------------------------------------------------- fused tcgen05 codebook lookup
+# ----------------------------------------------------------------------------- fused wgmma codebook lookup
 def test_vq_lookup_fused_bit_exact(L, golden_dir):
-    """One-pass fused lookup (fp16 distance GEMM on CTA pairs, top-2 from TMEM, fp64 settlement of near-ties) == the REAL
+    """One-pass fused lookup (fp16 wgmma distance GEMM, top-2 from the accumulator registers, fp64 settlement of near-ties) == the REAL
     reference's indices on the golden rows (4096 gaussian + 512 adversarial near-ties + 64 exact codes), ragged / empty M,
     quant + commit-loss outputs, and == the exact fp32 kernel on 40 960 random rows."""
     import os
@@ -778,24 +778,6 @@ def test_vq_lookup_fused_small_codebooks(L, D, K):
     a, qa, da = L.vq_lookup_fused(z.cuda(), et, esq, eh)
     b, qb, db = L.vq_lookup(z.cuda(), et, esq)
     assert torch.equal(a, b) and torch.equal(qa, qb) and abs(float(da) - float(db)) <= 1e-9 * abs(float(db))
-
-
-def test_cta_pair_mma_path_matches_single_cta():
-    """`cta_group::2` pairs in the 128x128 tcgen05 kernel (opt-in, VF_TC_2CTA=1): same results as the single-CTA path on a GEMM and a conv
-    the wide kernels do not take (the flag is read once per process, hence the subprocesses)."""
-    import os, subprocess, sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    outs = {}
-    for flag in ("0", "1"):
-        env = dict(os.environ, VF_TC_2CTA=flag, VF_TC_WIDE2=flag)
-        r = subprocess.run([sys.executable, os.path.join(root, "scripts", "two_cta_check.py")], capture_output=True, text=True, env=env, timeout=600)
-        assert r.returncode == 0, r.stderr[-2000:]
-        outs[flag] = [l for l in r.stdout.splitlines() if l.startswith(("gemm", "conv", "wide"))]
-        print(f"[VF_TC_2CTA={flag}]", " | ".join(outs[flag]))
-        for l in outs[flag]:
-            assert float(l.split()[2]) < 2e-2, l
-    # the accumulation order inside a tile is the same (K blocks in order, fp32 TMEM accumulators): identical sums
-    assert outs["0"] == outs["1"]
 
 
 @pytest.mark.parametrize("n,h,w,cin,cout", [(2, 16, 16, 128, 128), (3, 8, 8, 256, 128), (1, 32, 24, 128, 256), (5, 8, 8, 128, 128)])

@@ -4,8 +4,8 @@ weights and inputs, and against the golden vectors produced by the real referenc
 Tolerances (stated per precision):
   fp32  (exact CUDA-core path): codes bit-exact; pixels / logits atol 2e-4 (reference's own th<->tf harness: 1e-5 on
         single layers, viewformer/utils/testing.py:98; a 60-conv network accumulates ~1e-5..1e-4).
-  tf32  (tcgen05 kind::tf32): pixels atol 2e-2, >= 97% codes identical.
-  bf16  (tcgen05 kind::f16, the benchmarked mode): pixels atol 1.5e-1 / mean err <= 2e-2, >= 85% codes identical,
+  tf32  (wgmma .tf32): pixels atol 2e-2, >= 97% codes identical.
+  bf16  (wgmma .bf16, the benchmarked mode): pixels atol 1.5e-1 / mean err <= 2e-2, >= 85% codes identical,
         logits: top-1 agreement >= 90% with |dlogit| small relative to the logit spread.
 """
 import os

@@ -1,4 +1,4 @@
-"""viewformer_b200 — B200-native (sm_100a) implementation of ViewFormer's novel-view-synthesis hot path:
+"""viewformer_b200 — H100-native (sm_90a) implementation of ViewFormer's novel-view-synthesis hot path:
 VQGAN codebook encode/decode + MIGT context-view transformer, behind the reference's model surface."""
 from .config import VQGANConfig, MIGTConfig, load_config, ModelNotFoundError  # noqa: F401
 

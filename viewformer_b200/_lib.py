@@ -2,7 +2,7 @@
 
 torch is used here only as the device-memory / stream plumbing: every helper passes raw
 ``data_ptr()`` values and the current CUDA stream handle across the C-ABI.  There is no CPU or
-PyTorch fallback: if the shared library is missing or the device is not sm_100, calls raise.
+PyTorch fallback: if the shared library is missing or the device is not sm_90, calls raise.
 """
 import ctypes as C
 import os
@@ -92,7 +92,7 @@ def load(require_device=False):
         _lib = lib
     if require_device and not _device_ok:
         if not torch.cuda.is_available():
-            raise LibraryError("viewformer_b200 needs a CUDA device (sm_100a); no CPU fallback exists")
+            raise LibraryError("viewformer_b200 needs a CUDA device (sm_90a); no CPU fallback exists")
         rc = _lib.vf_device_check()
         if rc != 0:
             raise LibraryError(_lib.vf_last_error().decode())
@@ -357,7 +357,7 @@ def simt_gemm(A, B, out, *, M, N, K, a_strides, b_strides, ldc, batch=(1, 1), a_
 def tc_gemm(A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0), b_bs=(0, 0), c_bs=(0, 0), alpha=1.0,
             bias=None, bias_mode=BIAS_NONE, act=ACT_NONE, residual=None, a_off=0, b_off=0, c_off=0, causal_block=0,
             causal_skip_n=False, out2=None, gn_rows_per_img=0, gn_groups=32, lo_a=None, lo_b=None, k_offsets=None):
-    """tcgen05 GEMM: C[m,n] = act(alpha*sum_k A[m,k] B[n,k] + bias) + residual; A,B K-major bf16 (or f32 -> TF32).
+    """Tensor-core (wgmma) GEMM: C[m,n] = act(alpha*sum_k A[m,k] B[n,k] + bias) + residual; A,B K-major bf16 (or f32 -> TF32).
     ``out2`` optionally receives a second copy in the other dtype (f32 + bf16 from one epilogue).
     float16 operands = split-fp16 pairs (exact mode): a row holds hi(K) at column 0 and lo(K) at column ``lo_a`` / ``lo_b``."""
     lib = load(True)
@@ -402,7 +402,7 @@ def tc_gemm(A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0), b_b
 
 
 def gn_fusable(channels, groups, rows, rows_per_img, ldc):
-    """Shapes for which the tcgen05 epilogue can accumulate GroupNorm statistics (see vf_tc_gemm_t.gn_sums)."""
+    """Shapes for which the tensor-core epilogue can accumulate GroupNorm statistics (see vf_tc_gemm_t.gn_sums)."""
     if channels % groups:
         return False
     cpg = channels // groups
@@ -448,10 +448,10 @@ def conv3x3_small_cout(x, w_kn, bias):
 
 
 def conv_norm_fusable(x, cout):
-    """Shapes for which vf_tc_gemm can apply GroupNorm+swish to the conv INPUT on the fly (vf_tc_gemm_t.norm_*)."""
+    """Shapes for which vf_tc_gemm can apply GroupNorm+swish to the conv INPUT on the fly (vf_tc_gemm_t.norm_*): the halo-tile
+    path of 3x3 bf16 convs on maps >= 32 rows."""
     n, h, w, c = x.shape
-    return (os.environ.get("VF_TC_WIDE", "1") != "0" and x.dtype == torch.bfloat16
-            and c % 64 == 0 and cout % 128 == 0 and h >= 32 and w >= 8 and n * h * w * cout < 2 ** 31)
+    return x.dtype == torch.bfloat16 and c % 64 == 0 and cout % 128 == 0 and h >= 32 and w >= 8 and n * h * w * cout < 2 ** 31
 
 
 def gn_mean_rstd(x, groups=32, eps=1e-6):
@@ -473,7 +473,7 @@ def gn_mean_rstd(x, groups=32, eps=1e-6):
 
 def tc_conv(x, w_nk, bias, *, taps=TAPS_3x3, coffs=None, cin=None, out_hw=None, residual=None, out=None,
             out_dtype=torch.float32, out2=None, gn_groups=0, norm=None):
-    """tcgen05 implicit-GEMM conv.  x [N,H,W,Ctot] bf16|f32 NHWC; w_nk [Cout, ntaps*Cin] (K-major, same dtype).
+    """Tensor-core (wgmma) implicit-GEMM conv.  x [N,H,W,Ctot] bf16|f32 NHWC; w_nk [Cout, ntaps*Cin] (K-major, same dtype).
     ``norm=(mean_rstd, gamma, beta, groups, swish)``: x is the RAW activation and GroupNorm(+swish) is applied to it inside the
     kernel (only for ``conv_norm_fusable`` shapes)."""
     lib = load(True)
@@ -566,7 +566,7 @@ def vq_split3(x, codebook):
 
 
 def vq_lookup_tc(z_rows, et, esq, et3, want_quant=True, want_diff=True, tol=1e-4, count_rescored=False):
-    """Tensor-core lookup: bf16x3 distance GEMM on tcgen05 + exact fp64 re-score of near-ties.  Same outputs as vq_lookup."""
+    """Tensor-core lookup: bf16x3 distance GEMM on the tensor cores + exact fp64 re-score of near-ties.  Same outputs as vq_lookup."""
     lib = load(True)
     _dev(z_rows, torch.float32)
     m, d = z_rows.shape
@@ -598,7 +598,7 @@ def vq_fused_ok(d, k):
 
 
 def vq_lookup_fused(z_rows, et, esq, eh, emb_dk=None, want_quant=True, want_diff=True, tol_factor=0.25, return_counts=False):
-    """Fused tcgen05 lookup (vf_vq_fused.cu): z read once, top-2 from TMEM, exact fp64 settlement of near-ties.  Same outputs as
+    """Fused wgmma lookup (vf_vq_fused.cu): z read once, top-2 from the accumulator registers, exact fp64 settlement of near-ties.  Same outputs as
     vq_lookup; ``return_counts`` adds the int32[2] tensor (rows settled between two candidates, rows settled over all codes)."""
     lib = load(True)
     _dev(z_rows, torch.float32)
@@ -661,7 +661,7 @@ def migt_embed(ids_i32, fixed_token, wte, wpe, pose_rows, BT, L):
 
 
 def attn_block_causal(qk, vt, B, S, H, d, block, first_query=0, out=None, skip_view=-1):
-    """Fused tcgen05 block-causal attention: qk bf16 [B,S,2d] (q|k), vt bf16 [B,d,S] -> bf16 [B*S, d].
+    """Fused wgmma block-causal attention: qk bf16 [B,S,2d] (q|k), vt bf16 [B,d,S] -> bf16 [B*S, d].
     ``first_query`` > 0 computes only the query rows from that row's 128-row tile on (KV-cache decode); ``skip_view`` >= 0 leaves the
     keys of that view out (an unused slot of the cache)."""
     lib = load(True)
@@ -814,7 +814,7 @@ def conv_wgrad_tc(x, dy, dw, *, accumulate=True):
     pitch = (w + 2 + 7) // 8 * 8
     ppad = n * (h + 2) * pitch
     tiles = (3 * cin // 128) * (cout // 128)
-    splits = max(1, min(64, (148 + 3 * tiles - 1) // (3 * tiles)))
+    splits = max(1, min(64, (132 + 3 * tiles - 1) // (3 * tiles)))
     kc = (ppad + splits - 1) // splits
     kc = (kc + 63) // 64 * 64                                  # the exact GEMM walks K in blocks of 64
     kpad = kc * splits
@@ -849,7 +849,7 @@ def dense_wgrad_tc(x_rows, dy_rows, dw_kn, *, accumulate=True):
     m, k = x_rows.shape
     n = dy_rows.shape[1]
     tiles = (k // 128) * (n // 128)
-    splits = max(1, min(32, (148 + tiles - 1) // tiles))
+    splits = max(1, min(32, (132 + tiles - 1) // tiles))
     kc = ((m + splits - 1) // splits + 63) // 64 * 64
     lm = kc * splits
     key = ("dense", x_rows.device, m, k, n)

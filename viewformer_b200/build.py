@@ -1,9 +1,9 @@
-"""Builds viewformer_b200/libvf_b200.so (sm_100a only) with nvcc, in-tree.
+"""Builds viewformer_b200/libvf_b200.so (sm_90a only) with nvcc, in-tree.
 
     python -m viewformer_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the
-repository snapshot.  No torch dependency: the library is a plain C-ABI shared object (include/vf_b200.h).
+nvcc cross-compiles without a GPU; the .so is a build product (git-ignored) and is rebuilt whenever a source or the
+public header is newer.  No torch dependency: the library is a plain C-ABI shared object (include/vf_b200.h).
 """
 import os
 import shutil
@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("VF_B200_LIB") or os.path.join(HERE, "libvf_b200.so")   # VF_B200_LIB: side-by-side profiling builds
 SOURCES = ["vf_misc.cu", "vf_norm.cu", "vf_simt_gemm.cu", "vf_conv_small.cu", "vf_vq.cu", "vf_tc_gemm.cu", "vf_attn_fused.cu", "vf_vq_fused.cu", "vf_eval.cu", "vf_backward.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 
@@ -34,10 +34,6 @@ def needs_build():
 
 
 def build(force=False, verbose=True):
-    if os.environ.get("VF_TC_STALL_COUNTERS") == "1":      # profiling build: clock64 stall counters in the tcgen05 kernel
-        force = True
-        if "-DVF_TC_STALL_COUNTERS" not in NVCC_FLAGS:
-            NVCC_FLAGS.append("-DVF_TC_STALL_COUNTERS")
     if not force and not needs_build():
         return LIB
     nvcc = _nvcc()

@@ -1,37 +1,35 @@
-// Fused block-causal attention on tcgen05 tensor cores (sm_100a):  O = softmax(mask(Q K^T)) V  per (batch, head).
+// Fused block-causal attention on Hopper tensor cores (sm_90a, wgmma):  O = softmax(mask(Q K^T)) V  per (batch, head).
 //
 // Replaces viewformer/models/branching_attention.py:41-61 (compute_causal_block_attention: a view attends to all tokens
 // of its own and of every earlier view; logits are NOT scaled by 1/sqrt(dh); masked logits are -1e4 in the reference,
 // whose exp underflows to exactly 0 in fp32, so masked keys are simply skipped here) for the single-stream forward.
 //
-// One CTA = 128 queries (two 64-token views) of one (batch, head); two CTAs share an SM (256 TMEM columns, ~72 KB of shared
-// memory each), so one CTA's prologue / epilogue hides behind the other's main loop.  Keys are walked ONCE in 64-key tiles:
-//   S_j = Q K_j^T   128x64 fp32 in TMEM (double-buffered)
-//   softmax warps (one query row per thread, no shuffles): row max of the tile, P_j = exp2(S_j log2e - m_ref) as packed bf16
-//   written straight back to TMEM (tcgen05.st), row sums in registers
-//   O  += P_j V_j   with P as the TMEM A operand of tcgen05.mma (no shared-memory round trip for P), O 128x64 fp32 in TMEM.
+// One CTA = 128 queries (two 64-token views) of one (batch, head); two CTAs share an SM (~90 KB of shared memory each), so one
+// CTA's prologue / epilogue hides behind the other's main loop.  Keys are walked ONCE in 64-key tiles; each of the two MMA
+// warpgroups owns 64 query rows:
+//   S_j = Q K_j^T   64x64 fp32 in registers (wgmma, Q and K from shared memory)
+//   row max of the tile (4 lanes per row), P_j = exp2(S_j log2e - m_ref) packed to bf16 straight into the A-operand registers
+//   O  += P_j V_j   (wgmma with A from registers, V^T from shared memory), O 64x64 fp32 in registers.
 // Online softmax with a lazy reference maximum: m_ref only moves when a tile's maximum exceeds it by more than 2^8, and only
-// then is the O accumulator rescaled in TMEM (tcgen05.ld -> scale -> tcgen05.st, after the previous P V has retired).  The
-// final O / l does not depend on which reference was used, so this is the same softmax, not an approximation.
-// Fully masked key tiles are never loaded; a 64-key tile a warp's rows cannot see costs that warp one zero store.
+// then is the O accumulator row rescaled.  The final O / l does not depend on which reference was used, so this is the same
+// softmax, not an approximation.  Fully masked key tiles are never loaded; a warpgroup whose rows cannot see a tile skips it.
 //
-// Warp roles (192 threads): warp 0 TMA producer, warp 1 MMA issuer (+TMEM alloc), warps 2..5 softmax / correction / epilogue.
-#include "vf_tcgen05.cuh"
+// Warp roles (288 threads): warps 0..7 two MMA / softmax warpgroups, warp 8 TMA producer.
+#include "vf_wgmma.cuh"
 
 namespace {
 using namespace vftc;
 
 constexpr int QT = 128;            // queries per CTA
-constexpr int KT = 64;             // keys per tile (= one 128-byte swizzle row of V^T, one TMEM S buffer of 64 columns)
+constexpr int KT = 64;             // keys per tile (= one 128-byte swizzle row of V^T)
 constexpr int DH = 64;             // head dim (one 128-byte swizzle row)
 constexpr int KSTAGES = 4;         // K tile ring
 constexpr int VSTAGES = 3;         // V^T tile ring
 constexpr int Q_BYTES = QT * 128;              // 16 KB (double-buffered: the next work item's Q streams in behind the current one)
 constexpr int K_BYTES = KT * 128;              // 8 KB
 constexpr int V_BYTES = DH * 128;              // [64 dh rows x 64 keys] = 8 KB
-constexpr int ATTN_THREADS = 192;
-constexpr int TMEM_COLS = 256;                 // S0 [0,64) S1 [64,128) P0 [128,160) P1 [160,192) O [192,256)
-constexpr int TM_S = 0, TM_P = 128, TM_O = 192;
+constexpr int MMA_THREADS = 256;
+constexpr int ATTN_THREADS = MMA_THREADS + 32;
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LAZY_LOG2 = 8.0f;              // the reference maximum moves only when a tile exceeds it by more than 2^8
 
@@ -41,42 +39,8 @@ struct AttnParams {
     int stream, stream_rows;                // multi-end mode (stream > 0): rows of stream s start at s * stream_rows in qk / V^T
     int skip_tile;                          // >= 0: this 64-key tile of stream 0 is never visited (an unused view slot of the KV cache)
     __nv_bfloat16* out;
-    unsigned idesc;                         // M = 128, N = 64 for both Q K^T and P V
 };
 
-// D[tmem] (+)= A[tmem] * B[smem]^T: A = 128 lanes x (K/2) 32-bit columns, two K-adjacent 16-bit elements per column
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-          "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-          "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-          "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// two back-to-back 32-column loads, one wait
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t (&r)[64]) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        uint32_t* q = r + 32 * h;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]),
-              "=r"(q[9]), "=r"(q[10]), "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15]), "=r"(q[16]),
-              "=r"(q[17]), "=r"(q[18]), "=r"(q[19]), "=r"(q[20]), "=r"(q[21]), "=r"(q[22]), "=r"(q[23]), "=r"(q[24]),
-              "=r"(q[25]), "=r"(q[26]), "=r"(q[27]), "=r"(q[28]), "=r"(q[29]), "=r"(q[30]), "=r"(q[31])
-            : "r"(taddr + 32 * h));
-    }
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ float ex2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -88,7 +52,6 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     return r;
 }
 
-// tile t of a CTA uses ring buffer t & 1; its k-th use completes the barrier's k-th phase (k = t >> 1)
 __device__ __forceinline__ uint32_t use_parity(int t) { return (uint32_t)(t >> 1) & 1u; }
 
 __global__ void __launch_bounds__(ATTN_THREADS, 2) attn_block_causal_kernel(const __grid_constant__ AttnParams p) {
@@ -99,40 +62,23 @@ __global__ void __launch_bounds__(ATTN_THREADS, 2) attn_block_causal_kernel(cons
     uint8_t* sV = sK + KSTAGES * K_BYTES;
     uint64_t* bars = reinterpret_cast<uint64_t*>(sV + VSTAGES * V_BYTES);
     uint64_t* q_full = bars;                 // 2
-    uint64_t* q_empty = q_full + 2;          // 2: the item's last Q K^T retired (MMA commit)
+    uint64_t* q_empty = q_full + 2;          // 2: the item's last Q K^T retired (every MMA thread arrives)
     uint64_t* k_full = q_empty + 2;          // KSTAGES
     uint64_t* k_empty = k_full + KSTAGES;    // KSTAGES
     uint64_t* v_full = k_empty + KSTAGES;    // VSTAGES
     uint64_t* v_empty = v_full + VSTAGES;    // VSTAGES
-    uint64_t* s_full = v_empty + VSTAGES;    // 2: S_t written (MMA commit)
-    uint64_t* s_empty = s_full + 2;          // 2: S_t read by all four softmax warps
-    uint64_t* p_full = s_empty + 2;          // 2: P_t written by all four softmax warps
-    uint64_t* pv_done = p_full + 2;          // 2: P_t V_t retired (MMA commit): P buffer free, O stable up to tile t
-    uint64_t* o_full = pv_done + 2;          // 1: the item's last P V retired
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_items = p.BH * p.n_qtiles;
 
-    if (threadIdx.x == 0) { prefetch_tmap(&p.tmQ); prefetch_tmap(&p.tmK); prefetch_tmap(&p.tmV); }
-    if (threadIdx.x == 32) {
-        for (int i = 0; i < 2; ++i) { mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], 1); }
-        for (int i = 0; i < KSTAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 1); }
-        for (int i = 0; i < VSTAGES; ++i) { mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&s_full[i], 1);
-            mbar_init(&s_empty[i], 4);       // one arrive per softmax warp
-            mbar_init(&p_full[i], 4);
-            mbar_init(&pv_done[i], 1);
-        }
-        mbar_init(o_full, 1);
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&p.tmQ); prefetch_tmap(&p.tmK); prefetch_tmap(&p.tmV);
+        for (int i = 0; i < 2; ++i) { mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], MMA_THREADS); }
+        for (int i = 0; i < KSTAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], MMA_THREADS); }
+        for (int i = 0; i < VSTAGES; ++i) { mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], MMA_THREADS); }
         mbar_fence_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
     // Work items = (query tile, batch*head), heaviest query tiles (most visible keys) first; a CTA walks items blockIdx.x, + gridDim.x, ...
     // Every role derives the same sequence, so nothing has to be broadcast; tile counters run on across items (ring parities stay valid).
@@ -162,7 +108,7 @@ __global__ void __launch_bounds__(ATTN_THREADS, 2) attn_block_causal_kernel(cons
         else { krow = p.stream * p.stream_rows + (t0 + 1) * KT; halves = 2u; }
     };
 
-    if (warp == 0) {
+    if (warp == MMA_THREADS / 32) {
         // ===================== TMA producer =====================
         if (elect_one()) {
             int ks = 0, vs = 0, it = 0;
@@ -188,198 +134,121 @@ __global__ void __launch_bounds__(ATTN_THREADS, 2) attn_block_causal_kernel(cons
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            int ks = 0, vs = 0;
-            uint32_t kph = 0, vph = 0;
-            // S tiles are issued one ahead of the P V they belong to — across item boundaries too, so the first Q K^T of the next item
-            // runs while the softmax warps are still in the epilogue of this one.  `sq` walks the (item, tile) sequence of S issues.
-            int s_item = blockIdx.x, s_it = 0, s_j = 0, s_nkt = 0, s_t = 0;
-            uint64_t s_qdesc = 0;
-            bool s_live = s_item < n_items;
-            auto s_open = [&]() {             // first tile of an item: its Q must have landed
-                int b, h, q0;
-                item_coords(s_item, b, h, q0, s_nkt);
-                mbar_wait(&q_full[s_it & 1], use_parity(s_it), "vf_attn issuer(Q)");
-                s_qdesc = sw128_desc(smem_u32(sQ + (s_it & 1) * Q_BYTES));
-            };
-            auto issue_s = [&]() {            // S[t & 1] = Q K_t^T for the next (item, tile)
-                if (s_j == 0) s_open();
-                mbar_wait(&k_full[ks], kph, "vf_attn issuer(K)");
-                if (s_t >= 2) mbar_wait(&s_empty[s_t & 1], use_parity(s_t - 2), "vf_attn issuer(S free)");
-                tc_fence_after();
-                const uint64_t kdesc = sw128_desc(smem_u32(sK + ks * K_BYTES));
-#pragma unroll
-                for (int k = 0; k < 4; ++k) umma_f16(tmem + TM_S + (s_t & 1) * KT, s_qdesc + 2 * k, kdesc + 2 * k, p.idesc, k > 0);
-                tc_commit(&k_empty[ks]);
-                tc_commit(&s_full[s_t & 1]);
-                if (++ks == KSTAGES) { ks = 0; kph ^= 1; }
-                ++s_t;
-                if (++s_j == s_nkt) {         // item finished on the S side: its Q buffer is free once these MMAs retire
-                    tc_commit(&q_empty[s_it & 1]);
-                    s_j = 0; ++s_it; s_item += gridDim.x;
-                    s_live = s_item < n_items;
-                }
-            };
-            if (s_live) issue_s();
-            int t = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                int b, h, q0, n_kt;
-                item_coords(item, b, h, q0, n_kt);
-                for (int j = 0; j < n_kt; ++j, ++t) {
-                    if (s_live) issue_s();                     // tile t + 1: its softmax overlaps the P V MMAs of tile t
-                    mbar_wait(&p_full[t & 1], use_parity(t), "vf_attn issuer(P)");
-                    mbar_wait(&v_full[vs], vph, "vf_attn issuer(V)");
-                    tc_fence_after();
-                    const uint32_t va = smem_u32(sV + vs * V_BYTES);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {      // 64 keys = 4 steps of 16
-                        const uint64_t bdesc = sw128_desc(va) + 2 * k;
-                        umma_ts(tmem + TM_O, tmem + TM_P + (t & 1) * (KT / 2) + 8 * k, bdesc, p.idesc, (j > 0 || k > 0) ? 1u : 0u);
-                    }
-                    tc_commit(&pv_done[t & 1]);
-                    tc_commit(&v_empty[vs]);
-                    if (++vs == VSTAGES) { vs = 0; vph ^= 1; }
-                }
-                tc_commit(o_full);
-            }
-        }
-    } else {
-        // ===================== softmax / correction / epilogue: thread = query row =====================
-        const int quarter = warp & 3;
-        const int row = quarter * 32 + lane;
-        const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-        int t = 0, it = 0;
-        for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
-            int b, h, q0, n_kt;
-            item_coords(item, b, h, q0, n_kt);
-            const int qpos = q0 + row;
-            const int vis = min(p.S, (min(qpos, p.S - 1) / p.block + 1) * p.block);     // keys [0, vis) are visible to this row
-            const int vis_lo = __reduce_min_sync(0xffffffffu, vis), vis_hi = __reduce_max_sync(0xffffffffu, vis);
-            float m2 = -INFINITY;          // reference maximum, in log2 units (S * log2 e)
-            float l = 0.f;
-            for (int j = 0; j < n_kt; ++j, ++t) {
-                int kbase;
-                uint32_t halves;
-                tile_at(q0, j, kbase, halves);
-                const int sb = t & 1;
-                uint32_t pk[32];
-                mbar_wait(&s_full[sb], use_parity(t), "vf_attn softmax(S)");
-                tc_fence_after();
-                // rows beyond the sequence (upper half of a last, half-filled query tile) are never stored: skip their arithmetic
-                bool warp_sees = kbase < vis_hi && q0 + quarter * 32 < p.S, partial = kbase + KT > vis_lo;
-                if (p.stream > 0) {                 // multi-end: whole 64-row halves see or do not see a tile, nothing is partially masked
-                    warp_sees = ((halves >> (quarter >> 1)) & 1u) != 0 && q0 + (quarter >> 1) * KT < p.S;
-                    partial = false;
-                }
-                if (warp_sees) {
-                    uint32_t r[64];
-                    tmem_ld64(tmem + lane_base + TM_S + sb * KT, r);
-                    // S has been copied to registers: the buffer can take tile t + 2
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&s_empty[sb]);
-                    if (partial) {
-#pragma unroll
-                        for (int i = 0; i < 64; ++i)
-                            if (kbase + i >= vis) r[i] = 0xff800000u;                  // -inf
-                    }
-                    // four independent chains (a single 63-deep dependent FMNMX chain costs 4 cycles per link)
-                    float mx[4];
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) mx[c] = fmaxf(__uint_as_float(r[c]), __uint_as_float(r[4 + c]));
-#pragma unroll
-                    for (int i = 8; i < 64; i += 8) {
-#pragma unroll
-                        for (int c = 0; c < 4; ++c) mx[c] = fmaxf(mx[c], fmaxf(__uint_as_float(r[i + c]), __uint_as_float(r[i + 4 + c])));
-                    }
-                    float mt = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])) * LOG2E;      // log2 e > 0: the maximum commutes with the scaling
-                    if (__all_sync(0xffffffffu, m2 == -INFINITY)) {
-                        // first tile these rows see: nothing accumulated for them yet (their accumulator rows are exact zeros or, at the
-                        // item's first tile, not yet written), so there is nothing to rescale
-                        m2 = mt;
-                    } else {
-                        const bool grow = mt > m2 + LAZY_LOG2;
-                        if (__any_sync(0xffffffffu, grow)) {
-                            // rescale this warp's 32 accumulator rows: O *= 2^(m_old - m_new); needs P_{t-1} V_{t-1} retired
-                            const float sc = grow ? ex2(m2 - mt) : 1.0f;
-                            mbar_wait(&pv_done[(t - 1) & 1], use_parity(t - 1), "vf_attn correction");
-                            tc_fence_after();
-#pragma unroll 1
-                            for (int c0 = 0; c0 < DH; c0 += 32) {
-                                uint32_t o[32];
-                                tmem_ld32(tmem + lane_base + TM_O + c0, o);
-#pragma unroll
-                                for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * sc);
-                                tmem_st32(tmem + lane_base + TM_O + c0, o);
-                            }
-                            tmem_wait_st();
-                            l *= sc;
-                            if (grow) m2 = mt;
-                        }
-                    }
-                    const float nm = -m2;
-                    float ls[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                    for (int i = 0; i < 64; i += 2) {
-                        const float e0 = ex2(fmaf(__uint_as_float(r[i]), LOG2E, nm));          // exp2(-inf) = 0 for masked keys
-                        const float e1 = ex2(fmaf(__uint_as_float(r[i + 1]), LOG2E, nm));
-                        ls[(i >> 1) & 3] += e0 + e1;
-                        pk[i >> 1] = pack_bf16(e0, e1);
-                    }
-                    l += (ls[0] + ls[1]) + (ls[2] + ls[3]);
-                } else {
-                    // no row of this warp sees the tile
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&s_empty[sb]);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) pk[i] = 0u;
-                }
-                if (t >= 2) mbar_wait(&pv_done[sb], use_parity(t - 2), "vf_attn softmax(P free)");
-                tc_fence_after();
-                tmem_st32(tmem + lane_base + TM_P + sb * (KT / 2), pk);
-                tmem_wait_st();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&p_full[sb]);
-            }
-            // ---- epilogue: O / l -> bf16.  The next item's first P V cannot start before these warps hand over its P tile, i.e. after
-            // the accumulator has been read here, so O needs no second buffer.
-            mbar_wait(o_full, (uint32_t)it & 1u, "vf_attn epilogue");
-            tc_fence_after();
-            const float inv = 1.0f / l;
-            __nv_bfloat16* orow = p.out + ((long long)b * p.S + qpos) * p.d + h * DH;
-#pragma unroll 1
-            for (int c0 = 0; c0 < DH; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld32(tmem + lane_base + TM_O + c0, r);
-                if (qpos < p.S) {
-#pragma unroll
-                    for (int i = 0; i < 32; i += 8) {
-                        uint4 u;
-                        u.x = pack_bf16(__uint_as_float(r[i]) * inv, __uint_as_float(r[i + 1]) * inv);
-                        u.y = pack_bf16(__uint_as_float(r[i + 2]) * inv, __uint_as_float(r[i + 3]) * inv);
-                        u.z = pack_bf16(__uint_as_float(r[i + 4]) * inv, __uint_as_float(r[i + 5]) * inv);
-                        u.w = pack_bf16(__uint_as_float(r[i + 6]) * inv, __uint_as_float(r[i + 7]) * inv);
-                        *reinterpret_cast<uint4*>(orow + c0 + i) = u;
-                    }
-                }
-            }
-            tc_fence_before();
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, TMEM_COLS);
+    // ===================== MMA + softmax + epilogue: warpgroup wg = query rows [64 wg, 64 wg + 64) of the tile =====================
+    // accumulator layout (vf_wgmma.cuh): this thread holds rows r_h = 16 (warp % 4) + lane / 4 + 8 h (h = 0, 1) and, for every
+    // 8-column block j, columns 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 h + {0, 1}]
+    const int wg = warp >> 2;
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int c_ln = 2 * (lane & 3);
+    int ks = 0, vs = 0, it = 0;
+    uint32_t kph = 0, vph = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++it) {
+        int b, h, q0, n_kt;
+        item_coords(item, b, h, q0, n_kt);
+        const int wq0 = q0 + 64 * wg;                       // first query of this warpgroup
+        const bool wg_live = wq0 < p.S;                     // rows beyond the sequence are never stored: skip their arithmetic
+        const int vis_lo = min(p.S, (min(wq0, p.S - 1) / p.block + 1) * p.block);
+        const int vis_hi = min(p.S, (min(wq0 + 63, p.S - 1) / p.block + 1) * p.block);
+        int vis[2];
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) vis[hh] = min(p.S, (min(q0 + r0 + 8 * hh, p.S - 1) / p.block + 1) * p.block);
+        mbar_wait(&q_full[it & 1], use_parity(it), "vf_attn mma(Q)");
+        const uint64_t qdesc = sw128_desc(smem_u32(sQ + (it & 1) * Q_BYTES + wg * 64 * 128));
+        float o[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[i] = 0.f;
+        float m2[2] = {-INFINITY, -INFINITY};               // reference maximum per row, in log2 units (S * log2 e)
+        float l[2] = {0.f, 0.f};
+        for (int j = 0; j < n_kt; ++j) {
+            int kbase;
+            uint32_t halves;
+            tile_at(q0, j, kbase, halves);
+            bool sees = wg_live && kbase < vis_hi, partial = kbase + KT > vis_lo;
+            if (p.stream > 0) {                 // multi-end: whole 64-row halves see or do not see a tile, nothing is partially masked
+                sees = wg_live && ((halves >> wg) & 1u) != 0;
+                partial = false;
+            }
+            float s[32];
+            mbar_wait(&k_full[ks], kph, "vf_attn mma(K)");
+            if (sees) {
+                const uint64_t kdesc = sw128_desc(smem_u32(sK + ks * K_BYTES));
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_ss<64, BF16>(s, qdesc + 2 * k, kdesc + 2 * k, k > 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(s);
+            }
+            mbar_arrive(&k_empty[ks]);
+            if (++ks == KSTAGES) { ks = 0; kph ^= 1; }
+            mbar_wait(&v_full[vs], vph, "vf_attn mma(V)");
+            if (sees) {
+                if (partial) {
+#pragma unroll
+                    for (int i = 0; i < 32; ++i)
+                        if (kbase + 8 * (i >> 2) + c_ln + (i & 1) >= vis[(i >> 1) & 1]) s[i] = -INFINITY;
+                }
+                uint32_t pa[4][4];
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    float mx = -INFINITY;
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * hh], s[4 * jj + 2 * hh + 1]));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                    const float mt = mx * LOG2E;      // log2 e > 0: the maximum commutes with the scaling
+                    if (m2[hh] == -INFINITY) {
+                        m2[hh] = mt;                  // first tile this row sees: nothing accumulated yet, nothing to rescale
+                    } else if (mt > m2[hh] + LAZY_LOG2) {
+                        const float sc = ex2(m2[hh] - mt);
+#pragma unroll
+                        for (int jj = 0; jj < 8; ++jj) { o[4 * jj + 2 * hh] *= sc; o[4 * jj + 2 * hh + 1] *= sc; }
+                        l[hh] *= sc;
+                        m2[hh] = mt;
+                    }
+                    const float nm = m2[hh] == -INFINITY ? 0.f : -m2[hh];
+                    float ls = 0.f;
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) {
+                        const float e0 = ex2(fmaf(s[4 * jj + 2 * hh], LOG2E, nm));          // exp2(-inf) = 0 for masked keys
+                        const float e1 = ex2(fmaf(s[4 * jj + 2 * hh + 1], LOG2E, nm));
+                        ls += e0 + e1;
+                        // A fragment of k-step jj / 2: regs {0, 1} = rows (r0, r0 + 8) of its first 8 keys, {2, 3} of its last 8
+                        pa[jj >> 1][2 * (jj & 1) + hh] = pack_bf16(e0, e1);
+                    }
+                    l[hh] += ls;
+                }
+                const uint64_t vdesc = sw128_desc(smem_u32(sV + vs * V_BYTES));
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) wgmma_rs_bf16_n64(o, pa[k], vdesc + 2 * k, 1u);     // 64 keys = 4 steps of 16
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(o);
+            }
+            mbar_arrive(&v_empty[vs]);
+            if (++vs == VSTAGES) { vs = 0; vph ^= 1; }
+        }
+        mbar_arrive(&q_empty[it & 1]);                      // every Q K^T of this item has retired
+        // ---- epilogue: O / l -> bf16 (row sums: the 4 lanes of a row hold disjoint key columns)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            float lt = l[hh];
+            lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+            lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+            const int qpos = q0 + r0 + 8 * hh;
+            if (!wg_live || qpos >= p.S) continue;
+            const float inv = 1.0f / lt;
+            __nv_bfloat16* orow = p.out + ((long long)b * p.S + qpos) * p.d + h * DH;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+                *reinterpret_cast<uint32_t*>(orow + 8 * jj + c_ln) = pack_bf16(o[4 * jj + 2 * hh] * inv, o[4 * jj + 2 * hh + 1] * inv);
+        }
     }
 }
-
-unsigned idesc_bf16(int M, int N) { return make_idesc_16bit(1, M, N); }
 
 }  // namespace
 
@@ -433,7 +302,6 @@ static int attn_launch(const void* qk, const void* vt, int B, int S, int n_strea
     prm.qt0 = first_query / QT;
     prm.n_qtiles = (S + QT - 1) / QT - prm.qt0;
     prm.out = reinterpret_cast<__nv_bfloat16*>(out);
-    prm.idesc = idesc_bf16(128, 64);
     int rc;
     const uint64_t row = (uint64_t)2 * d * 2;                  // bytes per qk row
     {   // Q / K: [B, S, 2d] viewed as (dh, S, H, B); K is the second half of every row
@@ -450,7 +318,7 @@ static int attn_launch(const void* qk, const void* vt, int B, int S, int n_strea
         const uint32_t box[4] = {(uint32_t)KT, (uint32_t)DH, 1, 1};
         if ((rc = make_tmap_16bit(&prm.tmV, vt, dims, str, box)) != VF_OK) return rc;
     }
-    constexpr int smem = 2 * Q_BYTES + KSTAGES * K_BYTES + VSTAGES * V_BYTES + 1024 + 256;
+    constexpr int smem = 2 * Q_BYTES + KSTAGES * K_BYTES + VSTAGES * V_BYTES + 1024 + 256;     // ~90 KB: two CTAs per SM
     static vf_per_device_flag configured_pd;          // function attributes are per device
     bool& configured = configured_pd.current();
     if (!configured) {
@@ -465,9 +333,9 @@ static int attn_launch(const void* qk, const void* vt, int B, int S, int n_strea
     if (num_sms == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
+        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
     }
-    // persistent: two CTAs per SM (256 TMEM columns each), every CTA walks items blockIdx.x, blockIdx.x + gridDim.x, ...
+    // persistent: two CTAs per SM, every CTA walks items blockIdx.x, blockIdx.x + gridDim.x, ...
     const unsigned grid = (unsigned)(items < 2ll * num_sms ? items : 2ll * num_sms);
     attn_block_causal_kernel<<<grid, ATTN_THREADS, smem, vf_s(s)>>>(prm);
     VF_CHECK_LAUNCH("vf_attn_block_causal");

@@ -498,7 +498,7 @@ extern "C" int vf_pad_transpose_split(const float* x, int N, int H, int W, int C
 }
 extern "C" int vf_sum_splits(const float* partial, int groups, int splits, int64_t n, int accumulate, float* out, vf_stream_t s) {
     VF_CHECK_ARG(partial && out && groups > 0 && splits > 0 && n > 0, "vf_sum_splits: bad args");
-    { long long tot_ = (long long)groups * n; unsigned g_ = (unsigned)((tot_ + 255) / 256 < 148 * 16 ? (tot_ + 255) / 256 : 148 * 16);
+    { long long tot_ = (long long)groups * n; unsigned g_ = (unsigned)((tot_ + 255) / 256 < 132 * 16 ? (tot_ + 255) / 256 : 132 * 16);
     sum_splits_kernel<<<g_, 256, 0, vf_s(s)>>>(partial, groups, splits, n, accumulate, out); }
     VF_CHECK_LAUNCH("vf_sum_splits");
     return VF_OK;
@@ -545,12 +545,12 @@ extern "C" int vf_groupnorm_bwd(const float* x, const float* dout, const float* 
     if (e != cudaSuccess) { vf_set_error("vf_groupnorm_bwd: memset: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
     const int lanes = 256 / (C / 4);
     int ppb = lanes * 128;          // few, long blocks: the per-channel sums end in global atomics
-    while (ppb > lanes * 4 && (long long)((HW + ppb - 1) / ppb) * N < 148 * 4) ppb >>= 1;
+    while (ppb > lanes * 4 && (long long)((HW + ppb - 1) / ppb) * N < 132 * 4) ppb >>= 1;
     dim3 grid((HW + ppb - 1) / ppb, N);
     gn_bwd_stats_kernel<<<grid, 256, sizeof(double) * 2 * groups + sizeof(float) * 2 * C, vf_s(s)>>>(x, dout, mean_rstd, gamma, beta, HW, C, groups, swish, ppb, gsums, dgamma, dbeta);
     VF_CHECK_LAUNCH("vf_groupnorm_bwd(stats)");
     int ppb2 = lanes * 16;          // the streaming pass keeps many short blocks in flight
-    while (ppb2 > lanes * 4 && (long long)((HW + ppb2 - 1) / ppb2) * N < 148 * 8) ppb2 >>= 1;
+    while (ppb2 > lanes * 4 && (long long)((HW + ppb2 - 1) / ppb2) * N < 132 * 8) ppb2 >>= 1;
     dim3 grid2((HW + ppb2 - 1) / ppb2, N);
     gn_bwd_apply_kernel<<<grid2, 256, 0, vf_s(s)>>>(x, dout, mean_rstd, gamma, beta, gsums, add, HW, C, groups, swish, ppb2, dx);
     VF_CHECK_LAUNCH("vf_groupnorm_bwd(apply)");
@@ -569,7 +569,7 @@ extern "C" int vf_l1_grad(const float* x, const float* y, int64_t n, float scale
     VF_CHECK_ARG(x && y && dy && loss_sum, "vf_l1_grad: null pointer");
     if (n == 0) return VF_OK;
     long long blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     l1_grad_kernel<<<(unsigned)blocks, 256, 0, vf_s(s)>>>(x, y, n, scale, dy, loss_sum);
     VF_CHECK_LAUNCH("vf_l1_grad");
     return VF_OK;
@@ -579,7 +579,7 @@ extern "C" int vf_lincomb3(float a, const float* x, float b, const float* y, flo
     VF_CHECK_ARG(x && out, "vf_lincomb3: null pointer");
     if (n == 0) return VF_OK;
     long long blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     lincomb3_kernel<<<(unsigned)blocks, 256, 0, vf_s(s)>>>(a, x, b, y, c, z, n, out);
     VF_CHECK_LAUNCH("vf_lincomb3");
     return VF_OK;
@@ -590,7 +590,7 @@ extern "C" int vf_sumpool2x2(const float* x, int N, int H, int W, int C, float* 
     const long long total = (long long)N * H * W * C;
     if (total == 0) return VF_OK;
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     sumpool2x2_kernel<<<(unsigned)blocks, 256, 0, vf_s(s)>>>(x, N, H, W, C, y);
     VF_CHECK_LAUNCH("vf_sumpool2x2");
     return VF_OK;
@@ -602,7 +602,7 @@ extern "C" int vf_adam(float* p, const float* g, float* m, float* v, int64_t n, 
     if (n == 0) return VF_OK;
     const float bc1 = 1.0f - powf(beta1, (float)step), bc2 = 1.0f - powf(beta2, (float)step);
     long long blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     adam_kernel<<<(unsigned)blocks, 256, 0, vf_s(s)>>>(p, g, m, v, n, lr, beta1, beta2, eps, bc1, sqrtf(bc2), grad_scale);
     VF_CHECK_LAUNCH("vf_adam");
     return VF_OK;
@@ -610,7 +610,7 @@ extern "C" int vf_adam(float* p, const float* g, float* m, float* v, int64_t n, 
 
 static unsigned grid_for(long long n) {
     long long b = (n + 255) / 256;
-    return (unsigned)(b > 148 * 16 ? 148 * 16 : b);
+    return (unsigned)(b > 132 * 16 ? 132 * 16 : b);
 }
 
 extern "C" int vf_layernorm_bwd(const float* x, const float* dy, const float* gamma, const float* add, int64_t rows, int D, float eps,

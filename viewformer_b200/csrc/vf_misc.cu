@@ -22,8 +22,8 @@ extern "C" int vf_device_check(void) {
         vf_set_error("vf_device_check: no CUDA device");
         return VF_ERR_CUDA;
     }
-    if (prop.major != 10) {
-        vf_set_error("vf_device_check: device %s is sm_%d%d, this library is built for sm_100a only", prop.name, prop.major,
+    if (prop.major != 9 || prop.minor != 0) {
+        vf_set_error("vf_device_check: device %s is sm_%d%d, this library is built for sm_90a only", prop.name, prop.major,
                      prop.minor);
         return VF_ERR_UNSUPPORTED;
     }

@@ -298,7 +298,7 @@ extern "C" int vf_split_f16x2(const float* x, int64_t rows, int C, void* out_f16
     if (rows == 0) return VF_OK;
     const long long quads = rows * (C / 4);
     long long blocks = (quads + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     split_rows_kernel<<<(unsigned)blocks, 256, 0, vf_s(s)>>>(x, quads, C / 4, reinterpret_cast<__half*>(out_f16));
     VF_CHECK_LAUNCH("vf_split_f16x2");
     return VF_OK;
@@ -313,7 +313,7 @@ extern "C" int vf_groupnorm_stats(const float* x, int N, int HW, int C, int grou
     if (e != cudaSuccess) { vf_set_error("vf_groupnorm_stats: memset: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
     // enough blocks to fill the machine, at least 64 pixels per block
     int chunks = (HW + 63) / 64;
-    const int target = (148 * 8 + N - 1) / N;
+    const int target = (132 * 8 + N - 1) / N;
     if (chunks > target) chunks = target;
     if (chunks < 1) chunks = 1;
     const int ppb = (HW + chunks - 1) / chunks;
@@ -341,7 +341,7 @@ static void gn_apply_launch(const void* x, const float* stats, const float* gamm
     const int lanes = 256 / (C / 4);
     // 16 pixel rounds per thread (4 x 4 loads in flight) unless that leaves the machine short of blocks
     int ppb = lanes * 16;
-    while (ppb > lanes * 4 && (int64_t)((HW + ppb - 1) / ppb) * N < 148 * 8) ppb >>= 1;
+    while (ppb > lanes * 4 && (int64_t)((HW + ppb - 1) / ppb) * N < 132 * 8) ppb >>= 1;
     dim3 grid((HW + ppb - 1) / ppb, N);
     const InT* xi = reinterpret_cast<const InT*>(x);
     OutT* yo = reinterpret_cast<OutT*>(y);

@@ -1,34 +1,32 @@
-// tcgen05 tensor-core GEMMs and implicit-GEMM convolutions for sm_100a.  Three persistent kernels behind one entry point
-// (vf_tc_gemm picks by shape):
-//   tc_conv3x3_wide_kernel  3x3 stride-1 bf16 convs on maps >= 32 rows: weights on the M side, 256 pixels of one halo tile on
-//                           the N side, register epilogue (the benchmarked conv path, 0.83 of the measured bf16 peak)
-//   tc_gemm_wide_kernel     un-batched bf16 linear layers, same 128 x 256 tile shape
-//   tc_gemm_kernel          128 x (64|128) tiles: batched / causal GEMMs, tap-table and small-map convs, TF32, 2-CTA pairs
-// Common structure:
-//   TMA (cp.async.bulk.tensor, 128B swizzle)  ->  smem ring  ->  tcgen05.mma.cta_group::1 issued by ONE ELECTED thread
-//   (elect.sync, not lane == 0: see elect_one) with fp32 accumulators double-buffered in TMEM  ->  tcgen05.ld epilogue warps:
-//   alpha, bias, GELU, residual, GroupNorm statistics, f32/bf16 stores.
+// Tensor-core GEMMs and implicit-GEMM convolutions for sm_90a (Hopper): one persistent kernel, tc_gemm_kernel, 128 x (64|128)
+// output tiles: plain / batched / causal GEMMs, tap-table and halo-tile convolutions, bf16, fp16 (split-fp16 "exact" mode) and TF32.
+// Structure:
+//   TMA (cp.async.bulk.tensor, 128B swizzle)  ->  smem ring (mbarrier full / empty pairs)  ->  two MMA warpgroups, each issuing
+//   wgmma.mma_async for 64 rows of the tile with fp32 accumulators in registers  ->  the same 8 warps as epilogue: accumulators ->
+//   shared-memory staging tile -> alpha, bias, GELU, residual, GroupNorm statistics, f32/bf16 stores.
 //
-// tc_gemm_kernel warp roles (320 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer, warps 2..9 = epilogue.
-// A CTA walks 128 x BLOCK_N output tiles.  GEMM operands are K-major; the convolution reads its A
-// operand straight from the NHWC activation tensor with a 4-D tensor map: for every filter tap the box
-// [TN images x TH rows x TW cols x 64 channels] shifted by (dy,dx) lands in shared memory as a 128-row K-major
-// tile, out-of-image pixels zero-filled by TMA — no im2col buffer exists anywhere.
+// Warp roles (384 threads): warps 0..7 = MMA + epilogue (warpgroup g owns tile rows [64g, 64g+64)), warps 8..11 = TMA producer
+// warpgroup (one elected thread issues the loads; the warpgroup hands its registers to the MMA warpgroups).
+// A CTA walks 128 x BLOCK_N output tiles; the producer runs ahead across tiles, so the next tile's operands stream in while the
+// epilogue of this one runs.  GEMM operands are K-major; the convolution reads its A operand straight from the NHWC activation
+// tensor with a 4-D tensor map: for every filter tap the box [TN images x TH rows x TW cols x 64 channels] shifted by (dy,dx)
+// lands in shared memory as a 128-row K-major tile, out-of-image pixels zero-filled by TMA — no im2col buffer exists anywhere.
 //
 // Replaces: torch.nn.Conv2d sites of viewformer/models/vqgan_th.py (3x3 stride-1 convs, 1x1 convs),
 //           tf.matmul sites of viewformer/models/migt.py:93 (Conv1D), :54 (tied LM head) and
 //           viewformer/models/branching_attention.py:7,18 (QK^T, PV) on the fast path.
-#include "vf_common.cuh"
-#include <cuda.h>
+#include "vf_wgmma.cuh"
 #include <stdlib.h>
 
 namespace {
+using namespace vftc;
 
 constexpr int BLOCK_M = 128;
 constexpr int ROW_BYTES = 128;                 // one swizzle-128B row = one K block
 constexpr int A_STAGE_BYTES = BLOCK_M * ROW_BYTES;
-constexpr int NUM_EPI_WARPS = 8;                // 2 warps per TMEM lane quarter, each owning half of the tile's columns
-constexpr int NUM_THREADS = 64 + 32 * NUM_EPI_WARPS;
+constexpr int NUM_EPI_WARPS = 8;               // the two MMA warpgroups; in the epilogue 2 warps per 32-row quarter of the tile
+constexpr int NUM_MMA_THREADS = 32 * NUM_EPI_WARPS;
+constexpr int NUM_THREADS = NUM_MMA_THREADS + 128;  // + the producer warpgroup (one elected thread issues TMA; see setmaxnreg_dec)
 
 struct TcParams {
     CUtensorMap tmA, tmB;
@@ -50,209 +48,41 @@ struct TcParams {
     float* C_f32;
     __nv_bfloat16* C_bf16;
     long long ldc, c_sb1, c_sb2;
-    unsigned idesc;
     int vec_ok;                // output/residual/bias addressing is 16-byte friendly -> vector epilogue
-    long long* dbg;            // profiling aid: per-CTA {total, wait_operands, wait_tmem_empty, tiles} MMA-issuer cycles (null in production)
     int halo;                  // conv only: 1 = load one (TH+2)x(TW+2) halo tile per 64-channel block and address the 9 taps
-                               // as row-shifted UMMA descriptors into it (9x fewer A bytes from L2); 0 = one shifted TMA box per tap
+                               // as row-shifted wgmma descriptors into it (9x fewer A bytes from L2); 0 = one shifted TMA box per tap
     double* gn_sums;           // optional fused GroupNorm statistics of the OUTPUT: [images][groups][2] (sum, sum of squares)
     int gn_groups, gn_cpg, gn_rows_per_img;
-    int dbg_flags;             // profiling builds only: 1 = no epilogue work, 2 = no B loads, 4 = no A loads (stale smem is consumed)
-    int exact;                 // conv only: split-fp16 operands (VF_F16X2), three product passes, chunked accumulation (see EXACT_LO_SCALE)
+    int exact;                 // split-fp16 operands (VF_F16X2), three product passes, chunked accumulation (see EXACT_LO_SCALE)
     int exact_kc;              // k-blocks per accumulation chunk (divides ntaps * cin_blocks)
     int exact_clog;            // logical channels of the split activation tensor (= Ctot / 2): the lo half starts there
     int exact_kpp;             // k-blocks per product pass = ntaps * cin_blocks (conv) or K / 64 (gemm)
     int exact_lo_b;            // gemm only: element offset of the lo half inside a B row (exact_clog is the A side's)
+    const float2* norm_mr;     // halo mode only, optional GroupNorm(+swish) of the INPUT applied to each halo tile in shared memory:
+    const float* norm_gamma;   //   (mean, rstd) [N][groups], gamma / beta [Cin]
+    const float* norm_beta;
+    int norm_groups, norm_cpg, norm_swish;
 };
 
-// ------------------------------------------------------------------------------------------ PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// ---- exact mode (VF_F16X2 operands): fp32-faithful GEMMs and convolutions on the tensor cores ----------------------------------
+// An fp32 value v travels as TWO fp16 numbers  hi = fp16(v),  lo = fp16((v - hi) * 2^11)  (22-23 significand bits; the scaling keeps
+// lo out of the fp16 subnormal range), activations as [.., hi(C) | lo(C)], weights as [Cout][tap][hi(Cin) | lo(Cin)].
+//   x * w  =  hi_x hi_w  +  2^-11 (hi_x lo_w + lo_x hi_w)  +  O(2^-22 |x w|)            -> three fp16 MMAs per product block
+// The tensor cores add into their fp32 accumulators without round-to-nearest, so a long K loop is not fp32-faithful.  The
+// accumulator is therefore drained every `exact_kc` k-blocks (a "chunk" of MMA steps from a ZERO accumulator) and the chunks are
+// summed in the staging tile with round-to-nearest FFMA, scaled by 2^-11 for the cross terms, small terms first.
+constexpr float EXACT_LO_SCALE = 1.0f / 2048.0f;
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-// elect.sync: exactly one lane of a converged warp gets `true`; unlike `lane == 0` the compiler KNOWS a single thread is active in
-// the guarded region, so tcgen05.mma / TMA operands move to uniform registers with a plain R2UR instead of an
-// ELECT + R2UR.BROADCAST + BRA.U.ANY waterfall loop around every instruction
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// non-blocking poll (never suspends the thread): used to look at the NEXT stage's barrier before this stage's MMAs are issued
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-// Bounded spin: a protocol bug traps (-> CUDA error) instead of hanging the GPU box.
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    for (uint32_t i = 0; i < (1u << 22); ++i)
-        if (mbar_try_wait(bar, parity)) return;
-    printf("vf_tc_gemm: mbarrier timeout (block %d,%d,%d thread %d)\n", blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x);
-    __trap();
-}
-
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tcgen05_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; kind::f16 covers bf16/f16 inputs, kind::tf32 fp32 inputs
-template <bool kTF32>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (kTF32) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-
-// ---- 2-CTA (cta_group::2) helpers: PTX forms follow cute/arch/copy_sm100_tma.hpp (SM100_TMA_2SM_LOAD_4D) and
-// cutlass/arch/barrier.h (umma_arrive_multicast_2x1SM, ClusterBarrier::arrive(cta_id))
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(cta));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {      // acquire at cluster scope: sees the peer CTA's arrivals
-    for (uint32_t i = 0; i < (1u << 24); ++i) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (ok) return;
-    }
-    printf("vf_tc_gemm: cluster mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-    __trap();
-}
-// both CTAs of the pair issue their own load; the transaction bytes are credited to the LEADER's barrier (peer bit cleared)
-__device__ __forceinline__ uint32_t leader_addr(const void* p) {      // shared::cluster address of the same location in CTA 0
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(p)), "r"(0));
-    return ra;
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* smem_dst, const CUtensorMap* tm, uint32_t leader_bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tcgen05_commit_2sm(uint64_t* bar) {      // arrives on the same barrier offset in both CTAs
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-template <bool kTF32>
-__device__ __forceinline__ void umma_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (kTF32) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
-//   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (8 rows x 128B = 1024B)
-//   [46,48) version = 1 (Blackwell) | [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// 32 lanes x 32 columns of fp32 accumulator -> 32 registers per thread (thread i <- lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 32 lanes x 16 columns (half the registers of tmem_ld_32x32: the exact-mode epilogue keeps 64 running sums per thread)
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ------------------------------------------------------------------------------------------ kernel
 struct TileInfo {
     int m0, n0, b1, b2, img0, oy0, ox0, nkb;
     bool skip;
 };
 
-// 2-CTA mode: `t` walks PAIRS of vertically adjacent M tiles (p.tiles_m = number of pairs); CTA `rank` owns tile 2*pair + rank
-__device__ __forceinline__ TileInfo decode_tile(const TcParams& p, int t, int block_n, int pair = 0, int rank = 0) {
+__device__ __forceinline__ TileInfo decode_tile(const TcParams& p, int t, int block_n) {
     TileInfo ti;
     const int n_tile = t % p.tiles_n;
     const int r = t / p.tiles_n;
-    const int m_tile = pair ? 2 * (r % p.tiles_m) + rank : r % p.tiles_m;
+    const int m_tile = r % p.tiles_m;
     const int bz = r / p.tiles_m;
     ti.b1 = bz / p.batch2;
     ti.b2 = bz % p.batch2;
@@ -280,1319 +110,407 @@ __device__ __forceinline__ TileInfo decode_tile(const TcParams& p, int t, int bl
     return ti;
 }
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-constexpr float EXACT_LO_SCALE = 1.0f / 2048.0f;      // exact (VF_F16X2) mode: weight of the cross-term passes, see WideParams below
-constexpr int KGROUP = 1;          // k-blocks per producer/consumer hand-shake (2 measured no faster: the ring gets too coarse)
 constexpr int HALO_BYTES = 23552;  // one (16+2) x (8+2) halo tile of 128-byte rows, rounded up to 1024
 constexpr int HALO_SLOTS = 6;      // weight-tile slots of the halo-mode ring
 __host__ __device__ constexpr int operand_bytes(int stages, int stage_bytes, int b_stage_bytes) {
     return stages * stage_bytes > 2 * HALO_BYTES + HALO_SLOTS * b_stage_bytes ? stages * stage_bytes
                                                                                : 2 * HALO_BYTES + HALO_SLOTS * b_stage_bytes;
 }
+constexpr int MAX_STAGES = 8;
+template <int kBlockN, int kStages>
+__host__ __device__ constexpr int tc_smem_bytes() {
+    return operand_bytes(kStages, A_STAGE_BYTES + kBlockN * ROW_BYTES, kBlockN * ROW_BYTES) +
+           NUM_EPI_WARPS * 32 * (kBlockN / 2 + 4) * 4 /*epilogue staging*/ + 1024 /*align slack*/ + 8 * (2 * MAX_STAGES + 4) /*barriers*/;
+}
+
+// Normalise-on-load: GroupNorm (+ swish) of the raw halo tile of channel block cb, in place, by the 256 MMA threads.  The tile holds
+// (TH+2) x (TW+2) rows (pixels) of 64 bf16 channels, 128B-swizzled: physical 16-byte chunk pc of row r holds logical chunk
+// pc ^ (r & 7) (the buffers are 1024-byte aligned).  Rows outside the image were zero-filled by TMA and stay zero (the reference
+// pads AFTER norm + swish, vqgan_th.py:69-78).  Same arithmetic as vf_groupnorm_apply, so the operand is bit-identical.
+__device__ __forceinline__ void normalise_halo(const TcParams& p, uint8_t* tile, int cb, int img, int oy0, int ox0, int tid) {
+    const int rows = (p.TW + 2) * (p.TH + 2);
+    for (int idx = tid; idx < rows * 8; idx += NUM_MMA_THREADS) {
+        const int r = idx >> 3, pc = idx & 7;
+        const int py = r / (p.TW + 2), px = r - py * (p.TW + 2);
+        const int iy = oy0 - 1 + py, ix = ox0 - 1 + px;
+        if (iy < 0 || iy >= p.OH || ix < 0 || ix >= p.OW) continue;
+        const int c0 = cb * 64 + ((pc ^ (r & 7)) << 3);                  // first of the chunk's 8 channels
+        uint4* ptr = reinterpret_cast<uint4*>(tile + r * ROW_BYTES + pc * 16);
+        const uint4 v = *ptr;
+        uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int c = c0 + 2 * k;
+            const float2 ma = __ldg(p.norm_mr + (img * p.norm_groups + c / p.norm_cpg));
+            const float2 mb = __ldg(p.norm_mr + (img * p.norm_groups + (c + 1) / p.norm_cpg));
+            const float sa = ma.y * __ldg(p.norm_gamma + c), sb = mb.y * __ldg(p.norm_gamma + c + 1);
+            float a = __uint_as_float(w[k] << 16), b = __uint_as_float(w[k] & 0xffff0000u);
+            a = fmaf(a, sa, __ldg(p.norm_beta + c) - ma.x * sa);
+            b = fmaf(b, sb, __ldg(p.norm_beta + c + 1) - mb.x * sb);
+            if (p.norm_swish == 1) {          // same arithmetic as vf_groupnorm_apply (bit-identical operand)
+                a = __fdividef(a, 1.0f + __expf(-a));
+                b = __fdividef(b, 1.0f + __expf(-b));
+            }
+            __nv_bfloat162 o = __floats2bfloat162_rn(a, b);
+            w[k] = *reinterpret_cast<uint32_t*>(&o);
+            if (p.norm_swish == 2) {
+                // packed bf16: swish(y) = h * (1 + tanh(h)), h = y / 2 — ONE MUFU op per two elements instead of four
+                uint32_t h, th;
+                asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(h) : "r"(w[k]), "r"(0x3f003f00u));
+                asm("tanh.approx.bf16x2 %0, %1;" : "=r"(th) : "r"(h));
+                asm("fma.rn.bf16x2 %0, %1, %2, %1;" : "=r"(w[k]) : "r"(h), "r"(th));
+            }
+        }
+        *ptr = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+}
 
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...
-//   warp 0      TMA producer   — smem ring runs continuously across tiles
-//   warp 1      MMA issuer     — accumulates tile i into TMEM stage (i & 1) while the epilogue drains stage (i-1) & 1
-//   warps 2..9  epilogue       — TMEM -> registers (alpha, bias, GELU) -> per-warp smem staging -> TMEM stage released
-//                                -> coalesced row-wise residual loads / global stores
-// k2Cta: thread-block cluster of two CTAs = one `cta_group::2` MMA of M = 256: each CTA loads its own 128 A rows and HALF of the
-// B tile (the tensor cores of both SMs read B from both shared memories), accumulators stay in each CTA's own TMEM; the
-// leader CTA issues the MMAs and its tcgen05.commit arrives on both CTAs' barriers.
-template <int kBlockN, int kStages, bool kTF32, bool k2Cta>
+template <int kBlockN, int kStages, WgKind kKind>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_constant__ TcParams p) {
-    constexpr int B_ROWS = k2Cta ? kBlockN / 2 : kBlockN;      // B rows held by this CTA
-    constexpr int B_STAGE_BYTES = B_ROWS * ROW_BYTES;
-    constexpr uint32_t CTAS = k2Cta ? 2 : 1;
-    const uint32_t rank = k2Cta ? cluster_ctarank() : 0;
-    const int sched_id = k2Cta ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-    const int sched_stride = k2Cta ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+    constexpr int B_STAGE_BYTES = kBlockN * ROW_BYTES;
     constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-    constexpr int UMMA_K_BYTES = 32;           // 16 bf16 or 8 tf32 per instruction
-    constexpr int MMAS_PER_STAGE = ROW_BYTES / UMMA_K_BYTES;
+    constexpr int K_STEPS = 4;                 // MMA steps per 128-byte K block: 16 bf16/fp16 or 8 tf32 elements (32 bytes) each
     constexpr int HALF_N = kBlockN / 2;        // columns per epilogue warp
-    constexpr int STG_LD = HALF_N + 4;         // staging row stride (floats): +4 keeps 128-bit row writes conflict-free
+    constexpr int STG_LD = HALF_N + 4;         // staging row stride (floats): +4 keeps 128-bit row reads conflict-free
     constexpr int STG_BYTES = NUM_EPI_WARPS * 32 * STG_LD * 4;
+    constexpr int NACC = kBlockN / 2;          // accumulator registers per thread (64 rows x kBlockN per warpgroup)
 
     extern __shared__ uint8_t smem_raw[];
-    // 1024B alignment required by the 128B swizzle atoms (descriptor base_offset = 0)
+    // 1024B alignment required by the 128B swizzle atoms
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     constexpr int OPER_BYTES = operand_bytes(kStages, STAGE_BYTES, B_STAGE_BYTES);
     float* staging = reinterpret_cast<float*>(smem + OPER_BYTES);
-    constexpr int MAX_STAGES = 8;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OPER_BYTES + STG_BYTES);   // [MAX_STAGES], one per k-block GROUP
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OPER_BYTES + STG_BYTES);   // [MAX_STAGES]
     uint64_t* empty_bar = full_bar + MAX_STAGES;        // [MAX_STAGES]
-    uint64_t* tmem_full_bar = empty_bar + MAX_STAGES;   // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;       // [2]
-    uint64_t* a_full_bar = tmem_empty_bar + 2;          // [2]  halo mode: A halo tiles
+    uint64_t* a_full_bar = empty_bar + MAX_STAGES;      // [2]  halo mode: A halo tiles
     uint64_t* a_empty_bar = a_full_bar + 2;             // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(a_empty_bar + 2);
-    // Hand-shake granularity: KGROUP k-blocks share one full / one empty barrier (the issuer polls the NEXT group's barrier
-    // before issuing this group's MMAs; see scripts/mma_rate_probe.cu for what a poll behind queued MMAs costs).
-    constexpr int NG = kStages / KGROUP;                // ring depth in groups (normal mode)
+    constexpr int NG = kStages;                         // ring depth (normal mode)
     // halo mode carves the same operand region differently: 2 halo buffers, then a ring of B-only slots
-    constexpr int HALO_BUF_BYTES = HALO_BYTES;          // >= 18*10 rows x 128 B, multiple of 1024
-    constexpr int NGH = HALO_SLOTS / KGROUP;            // ring depth in groups (halo mode)
-    uint8_t* halo_b_base = smem + 2 * HALO_BUF_BYTES;
+    constexpr int NGH = HALO_SLOTS;
+    uint8_t* halo_b_base = smem + 2 * HALO_BYTES;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tmA)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tmB)) : "memory");
-    }
-    if (threadIdx.x == 32) {
+        prefetch_tmap(&p.tmA);
+        prefetch_tmap(&p.tmB);
         for (int s = 0; s < MAX_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);                     // 2-CTA: only the leader arrives (expect_tx of both CTAs' bytes)
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], NUM_MMA_THREADS);     // every MMA thread arrives once its wgmma reading the slot retired
         }
         for (int a = 0; a < 2; ++a) {
             mbar_init(&a_full_bar[a], 1);
-            mbar_init(&a_empty_bar[a], 1);
+            mbar_init(&a_empty_bar[a], NUM_MMA_THREADS);
         }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&tmem_full_bar[a], 1);
-            mbar_init(&tmem_empty_bar[a], NUM_EPI_WARPS * CTAS);   // one arrive per epilogue warp (of both CTAs)
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
-    if (warp == 1) {   // whole warp allocates 2 accumulator stages = 2*kBlockN TMEM columns (power of two >= 32)
-        if constexpr (k2Cta) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(2 * kBlockN)
-                         : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(2 * kBlockN)
-                         : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    if constexpr (k2Cta) cluster_sync_all();               // both CTAs' barriers are initialised before any remote arrive / TMA
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // 1-CTA / 2-CTA variants of the four pipeline primitives
-    // 2-CTA: every load of either CTA credits its bytes to the LEADER's barrier; only the leader arms it (with both CTAs'
-    // byte count).  A peer load may land before the leader has armed the phase: the tx-count just goes negative meanwhile.
-    uint32_t lead_full = 0, lead_afull = 0;
-    if constexpr (k2Cta) { lead_full = leader_addr(full_bar); lead_afull = leader_addr(a_full_bar); }
-    auto arm_full = [&](uint64_t* bar, uint32_t bytes_this_cta) {
-        if constexpr (k2Cta) {
-            if (rank == 0) mbar_expect_tx(bar, bytes_this_cta * 2);
-        } else {
-            mbar_expect_tx(bar, bytes_this_cta);
-        }
-    };
-    auto load = [&](void* dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2, int c3) {
-        if constexpr (k2Cta) {
-            const bool is_a = bar >= a_full_bar && bar < a_full_bar + 2;
-            const uint32_t lb = is_a ? lead_afull + (uint32_t)((bar - a_full_bar) * 8) : lead_full + (uint32_t)((bar - full_bar) * 8);
-            tma_load_4d_2sm(dst, tm, lb, c0, c1, c2, c3);
-        } else {
-            tma_load_4d(dst, tm, bar, c0, c1, c2, c3);
-        }
-    };
-    auto commit = [&](uint64_t* bar) {
-        if constexpr (k2Cta) tcgen05_commit_2sm(bar);
-        else tcgen05_commit(bar);
-    };
-    auto mma = [&](uint32_t d, uint64_t a, uint64_t b, uint32_t accumulate) {
-        if constexpr (k2Cta) umma_2sm<kTF32>(d, a, b, p.idesc, accumulate);
-        else umma<kTF32>(d, a, b, p.idesc, accumulate);
-    };
-    const int n_off = (int)rank * B_ROWS;                               // this CTA's slice of the B tile (2-CTA: half)
-
-    if (warp == 0) {
+    if (warp >= NUM_EPI_WARPS) {
         // ===================== TMA producer =====================
-        if (elect_one()) {
+        setmaxnreg_dec<40>();
+        if (warp == NUM_EPI_WARPS && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
             int ab = 0;
             uint32_t aphase = 0;
-#ifdef VF_TC_STALL_COUNTERS
-            const bool pdbg = p.dbg != nullptr;
-#else
-            constexpr bool pdbg = false;
-#endif
-            long long pc_wait = 0, pc0 = 0;
-            const long long pc_start = pdbg ? clock64() : 0;
-            for (int t = sched_id; t < p.total_tiles; t += sched_stride) {
-                const TileInfo ti = decode_tile(p, t, kBlockN, k2Cta, (int)rank);
+            for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+                const TileInfo ti = decode_tile(p, t, kBlockN);
                 if (ti.skip) continue;
                 if (p.halo) {
                     const uint32_t halo_bytes = (uint32_t)((p.TW + 2) * (p.TH + 2)) * ROW_BYTES;
                     const int nkb = 9 * p.cin_blocks;
                     int tap = 0, cb = 0;
-                    for (int kb = 0; kb < nkb; kb += KGROUP) {
-                        const int n = (nkb - kb < KGROUP) ? nkb - kb : KGROUP;
-                        if (pdbg) pc0 = clock64();
-                        mbar_wait(&empty_bar[stage], phase ^ 1);
-                        if (pdbg) pc_wait += clock64() - pc0;
-                        bool b_loads = true, a_loads = true;
-#ifdef VF_TC_STALL_COUNTERS
-                        b_loads = !(p.dbg_flags & 2);
-                        a_loads = !(p.dbg_flags & 4);
-#endif
-                        if (b_loads) arm_full(&full_bar[stage], (uint32_t)n * B_STAGE_BYTES);
-                        else mbar_arrive(&full_bar[stage]);
-                        for (int g = 0; g < n; ++g) {
-                            if (tap == 0) {      // first tap of a channel block: its halo tile
-                                mbar_wait(&a_empty_bar[ab], aphase ^ 1);
-                                if (a_loads) {
-                                    arm_full(&a_full_bar[ab], halo_bytes);
-                                    load(smem + ab * HALO_BUF_BYTES, &p.tmA, &a_full_bar[ab], cb * p.bk_elems, ti.ox0 - 1, ti.oy0 - 1, ti.img0);
-                                } else {
-                                    mbar_arrive(&a_full_bar[ab]);
-                                }
-                                if (++ab == 2) { ab = 0; aphase ^= 1; }
-                            }
-                            if (b_loads)
-                                load(halo_b_base + (stage * KGROUP + g) * B_STAGE_BYTES, &p.tmB, &full_bar[stage],
-                                     (tap * p.cin_blocks + cb) * p.bk_elems, ti.n0 + n_off, 0, 0);
-                            if (++tap == 9) { tap = 0; ++cb; }
+                    for (int kb = 0; kb < nkb; ++kb) {
+                        mbar_wait(&empty_bar[stage], phase ^ 1, "vf_tc_gemm producer");
+                        mbar_expect_tx(&full_bar[stage], (uint32_t)B_STAGE_BYTES);
+                        if (tap == 0) {      // first tap of a channel block: its halo tile
+                            mbar_wait(&a_empty_bar[ab], aphase ^ 1, "vf_tc_gemm producer(halo)");
+                            mbar_expect_tx(&a_full_bar[ab], halo_bytes);
+                            tma_load_4d(smem + ab * HALO_BYTES, &p.tmA, &a_full_bar[ab], cb * p.bk_elems, ti.ox0 - 1, ti.oy0 - 1, ti.img0);
+                            if (++ab == 2) { ab = 0; aphase ^= 1; }
                         }
+                        tma_load_4d(halo_b_base + stage * B_STAGE_BYTES, &p.tmB, &full_bar[stage], (tap * p.cin_blocks + cb) * p.bk_elems,
+                                    ti.n0, 0, 0);
+                        if (++tap == 9) { tap = 0; ++cb; }
                         if (++stage == NGH) { stage = 0; phase ^= 1; }
                     }
                     continue;
                 }
-                for (int kb0 = 0; kb0 < ti.nkb; kb0 += KGROUP) {
-                    const int n = (ti.nkb - kb0 < KGROUP) ? ti.nkb - kb0 : KGROUP;
-                    if (pdbg) pc0 = clock64();
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    if (pdbg) pc_wait += clock64() - pc0;
-#ifdef VF_TC_STALL_COUNTERS
-                    if ((p.dbg_flags & 6) == 6) { mbar_arrive(&full_bar[stage]); if (++stage == NG) { stage = 0; phase ^= 1; } continue; }
-#endif
-                    arm_full(&full_bar[stage], (uint32_t)n * STAGE_BYTES);
-                    for (int g = 0; g < n; ++g) {
-                        const int kb = kb0 + g;
-                        uint8_t* sa = smem + (stage * KGROUP + g) * STAGE_BYTES;
-                        uint8_t* sb = sa + A_STAGE_BYTES;
-                        int kcoord_b = kb * p.bk_elems;
-                        if (p.conv) {
-                            int kbr = kb, a_half = 0;
-                            if (p.exact) {       // product pass j: 0 = (lo_x, hi_w), 1 = (hi_x, lo_w), 2 = (hi_x, hi_w)
-                                const int j = kb / p.exact_kpp;
-                                kbr = kb - j * p.exact_kpp;
-                                a_half = (j == 0) ? p.exact_clog : 0;
-                                const int tap_ = kbr / p.cin_blocks, cb_ = kbr - tap_ * p.cin_blocks;
-                                kcoord_b = ((tap_ * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb_) * p.bk_elems;
-                            }
-                            const int tap = kbr / p.cin_blocks;
-                            const int cb = kbr - tap * p.cin_blocks;
-                            load(sa, &p.tmA, &full_bar[stage], a_half + p.tap_coff[tap] + cb * p.bk_elems, ti.ox0 + p.tap_dx[tap],
-                                 ti.oy0 + p.tap_dy[tap], ti.img0);
-                        } else {
-                            int kcoord_a = kb * p.bk_elems;
-                            if (p.exact) {       // same three passes for a plain GEMM: A rows [hi(K) .. | lo(K) ..], B rows likewise
-                                const int j = kb / p.exact_kpp, kbr = kb - j * p.exact_kpp;
-                                kcoord_a = (j == 0 ? p.exact_clog : 0) + kbr * p.bk_elems;
-                                kcoord_b = (j == 1 ? p.exact_lo_b : 0) + kbr * p.bk_elems;
-                            }
-                            if (p.gemm_koff) kcoord_a += p.tap_coff[ti.b1];
-                            load(sa, &p.tmA, &full_bar[stage], kcoord_a, ti.m0, ti.b2 * p.a_bm2, ti.b1 * p.a_bm1);
+                for (int kb = 0; kb < ti.nkb; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1, "vf_tc_gemm producer");
+                    mbar_expect_tx(&full_bar[stage], (uint32_t)STAGE_BYTES);
+                    uint8_t* sa = smem + stage * STAGE_BYTES;
+                    uint8_t* sb = sa + A_STAGE_BYTES;
+                    int kcoord_b = kb * p.bk_elems;
+                    if (p.conv) {
+                        int kbr = kb, a_half = 0;
+                        if (p.exact) {       // product pass j: 0 = (lo_x, hi_w), 1 = (hi_x, lo_w), 2 = (hi_x, hi_w)
+                            const int j = kb / p.exact_kpp;
+                            kbr = kb - j * p.exact_kpp;
+                            a_half = (j == 0) ? p.exact_clog : 0;
+                            const int tap_ = kbr / p.cin_blocks, cb_ = kbr - tap_ * p.cin_blocks;
+                            kcoord_b = ((tap_ * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb_) * p.bk_elems;
                         }
-                        load(sb, &p.tmB, &full_bar[stage], kcoord_b, ti.n0 + n_off, ti.b2 * p.b_bm2, ti.b1 * p.b_bm1);
+                        const int tap = kbr / p.cin_blocks;
+                        const int cb = kbr - tap * p.cin_blocks;
+                        tma_load_4d(sa, &p.tmA, &full_bar[stage], a_half + p.tap_coff[tap] + cb * p.bk_elems, ti.ox0 + p.tap_dx[tap],
+                                    ti.oy0 + p.tap_dy[tap], ti.img0);
+                    } else {
+                        int kcoord_a = kb * p.bk_elems;
+                        if (p.exact) {       // same three passes for a plain GEMM: A rows [hi(K) .. | lo(K) ..], B rows likewise
+                            const int j = kb / p.exact_kpp, kbr = kb - j * p.exact_kpp;
+                            kcoord_a = (j == 0 ? p.exact_clog : 0) + kbr * p.bk_elems;
+                            kcoord_b = (j == 1 ? p.exact_lo_b : 0) + kbr * p.bk_elems;
+                        }
+                        if (p.gemm_koff) kcoord_a += p.tap_coff[ti.b1];
+                        tma_load_4d(sa, &p.tmA, &full_bar[stage], kcoord_a, ti.m0, ti.b2 * p.a_bm2, ti.b1 * p.a_bm1);
                     }
+                    tma_load_4d(sb, &p.tmB, &full_bar[stage], kcoord_b, ti.n0, ti.b2 * p.b_bm2, ti.b1 * p.b_bm1);
                     if (++stage == NG) { stage = 0; phase ^= 1; }
                 }
             }
-            if (pdbg) {
-                long long* d = p.dbg + 8 * blockIdx.x;
-                d[4] = clock64() - pc_start; d[5] = pc_wait;
+        }
+        return;
+    }
+
+    // ===================== MMA + epilogue (warps 0..7) =====================
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;                          // MMA: warpgroup wg computes tile rows [64 wg, 64 wg + 64)
+    const int quarter = warp & 3;                      // epilogue: this warp stores tile rows [32 quarter, +32) ...
+    const int col_half = warp >> 2;                    // ... of column half col_half
+    float* stg = staging + warp * (32 * STG_LD);       // the epilogue's staging tile of this warp [32][STG_LD]
+    int stage = 0, ab = 0;
+    uint32_t phase = 0, aphase = 0;
+    float acc[NACC];
+
+    // accumulator fragment -> staging: element (r, c) of the 128 x kBlockN tile goes to the staging tile of the epilogue warp that
+    // stores it.  add = 0: dst = acc * sc; add = 1: dst = fma(acc, sc, dst) (exact mode: chunks summed with round-to-nearest)
+    auto to_staging = [&](float sc, bool add) {
+        const int r_lo = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < NACC / 4; ++j) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = r_lo + 8 * h, c = 8 * j + 2 * (lane & 3);
+                float* dst = staging + ((c / HALF_N) * 4 + (r >> 5)) * (32 * STG_LD) + (r & 31) * STG_LD + (c % HALF_N);
+                float2 v;
+                if (add) {
+                    v = *reinterpret_cast<float2*>(dst);
+                    v.x = fmaf(acc[4 * j + 2 * h], sc, v.x);
+                    v.y = fmaf(acc[4 * j + 2 * h + 1], sc, v.y);
+                } else {
+                    v = make_float2(acc[4 * j + 2 * h] * sc, acc[4 * j + 2 * h + 1] * sc);
+                }
+                *reinterpret_cast<float2*>(dst) = v;
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (2-CTA: the leader CTA issues for the pair) =====================
-        if (rank == 0 && elect_one()) {
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            int ab_m = 0;
-            uint32_t aphase_m = 0;
-            // A barrier poll issued right after tcgen05.mma instructions only returns once those MMAs have drained into the tensor
-            // pipe (measured: scripts/mma_rate_probe.cu, ~220 cycles per k-block with 128-wide tiles), so the full barrier of
-            // the NEXT ring slot is polled BEFORE this slot's MMAs are issued and the blocking wait is only the fallback.
-            bool ready = false;
-            long long c_ops = 0, c_tmem = 0, c_tiles = 0, c0 = 0;       // stall counters, only maintained when p.dbg != null
-#ifdef VF_TC_STALL_COUNTERS
-            const bool dbg = p.dbg != nullptr;
-#else
-            constexpr bool dbg = false;          // build with -DVF_TC_STALL_COUNTERS for scripts/tc_stall_probe.py
-#endif
-            const long long c_start = dbg ? clock64() : 0;
-            for (int t = sched_id; t < p.total_tiles; t += sched_stride) {
-                const TileInfo ti = decode_tile(p, t, kBlockN, k2Cta, 0);
-                if (ti.skip) continue;
-                const int acc = it & 1;
-                const uint32_t acc_phase = (it >> 1) & 1;
-                if (dbg) c0 = clock64();
-                mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);       // epilogue has drained this accumulator stage
-                if (dbg) { c_tmem += clock64() - c0; ++c_tiles; }
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * kBlockN);
-                if (p.halo) {
-                    // tile = TH rows of TW=8 pixels: MMA row group g (8 rows) = image row g of the tile; inside the halo tile
-                    // (pitch TW+2 rows) tap (dy,dx) starts (dy*(TW+2)+dx) rows in, consecutive groups are (TW+2) rows apart.
-                    // The 128B swizzle is a pure function of the absolute smem address (probed: scripts/desc_shift_probe.cu),
-                    // so row-shifted descriptors with base_offset 0 read exactly what TMA wrote.
-                    const uint32_t pitch = (uint32_t)(p.TW + 2);
-                    const int nkb = 9 * p.cin_blocks;
-                    int tap = 0;
-                    uint32_t a_base = 0;
-                    for (int kb = 0; kb < nkb; kb += KGROUP) {
-                        const int n = (nkb - kb < KGROUP) ? nkb - kb : KGROUP;
-                        if (dbg) c0 = clock64();
-                        if (!ready) mbar_wait(&full_bar[stage], phase);
-                        if (dbg) c_ops += clock64() - c0;
-                        {
-                            const int ns = (stage + 1 == NGH) ? 0 : stage + 1;
-                            ready = mbar_test_wait(&full_bar[ns], ns == 0 ? (phase ^ 1) : phase);
-                        }
-                        tcgen05_fence_after();
-#pragma unroll
-                        for (int g = 0; g < KGROUP; ++g) {
-                            if (g < n) {
-                                if (tap == 0) {
-                                    if (dbg) c0 = clock64();
-                                    mbar_wait(&a_full_bar[ab_m], aphase_m);
-                                    if (dbg) c_ops += clock64() - c0;
-                                    tcgen05_fence_after();
-                                    a_base = smem_u32(smem + ab_m * HALO_BUF_BYTES);
-                                }
-                                const uint32_t a_addr = a_base + ((uint32_t)(tap / 3) * pitch + (uint32_t)(tap % 3)) * ROW_BYTES;
-                                uint64_t adesc = make_sw128_desc(a_addr);
-                                adesc = (adesc & ~((uint64_t)0x3FFF << 32)) | ((uint64_t)((pitch * ROW_BYTES) >> 4) << 32);     // SBO = pitch rows
-                                const uint64_t bdesc = make_sw128_desc(smem_u32(halo_b_base + (stage * KGROUP + g) * B_STAGE_BYTES));
-#pragma unroll
-                                for (int k = 0; k < MMAS_PER_STAGE; ++k)
-                                    mma(tmem_d, adesc + (uint64_t)(k * (UMMA_K_BYTES >> 4)), bdesc + (uint64_t)(k * (UMMA_K_BYTES >> 4)),
-                                        (kb + g > 0 || k > 0) ? 1u : 0u);
-                                if (++tap == 9) {
-                                    tap = 0;
-                                    commit(&a_empty_bar[ab_m]);      // halo buffer free once its 36 MMAs retire
-                                    if (++ab_m == 2) { ab_m = 0; aphase_m ^= 1; }
-                                }
-                            }
-                        }
-                        commit(&empty_bar[stage]);
-                        if (++stage == NGH) { stage = 0; phase ^= 1; }
-                    }
-                    commit(&tmem_full_bar[acc]);
-                    ++it;
-                    continue;
-                }
-                uint32_t tmem_dd = tmem_d;
-                int in_chunk = 0;
-                bool fresh = true;
-                for (int kb0 = 0; kb0 < ti.nkb; kb0 += KGROUP) {
-                    const int n = (ti.nkb - kb0 < KGROUP) ? ti.nkb - kb0 : KGROUP;
-                    if (p.exact && in_chunk == 0 && kb0 > 0) {        // next chunk: a fresh accumulator stage (the first one was opened above)
-                        const int a2 = it & 1;
-                        mbar_wait(&tmem_empty_bar[a2], ((it >> 1) & 1) ^ 1);
-                        tcgen05_fence_after();
-                        tmem_dd = tmem_base + (uint32_t)(a2 * kBlockN);
-                        fresh = true;
-                    }
-                    if (dbg) c0 = clock64();
-                    if (!ready) mbar_wait(&full_bar[stage], phase);
-                    if (dbg) c_ops += clock64() - c0;
-                    {
-                        const int ns = (stage + 1 == NG) ? 0 : stage + 1;
-                        ready = mbar_test_wait(&full_bar[ns], ns == 0 ? (phase ^ 1) : phase);
-                    }
-                    tcgen05_fence_after();
-#pragma unroll
-                    for (int g = 0; g < KGROUP; ++g) {
-                        if (g < n) {
-                            const uint32_t sa = smem_u32(smem + (stage * KGROUP + g) * STAGE_BYTES);
-                            const uint32_t sb = sa + A_STAGE_BYTES;
-                            const uint64_t adesc = make_sw128_desc(sa);
-                            const uint64_t bdesc = make_sw128_desc(sb);
-#pragma unroll
-                            for (int k = 0; k < MMAS_PER_STAGE; ++k) {
-                                // advance along K inside the 128B swizzle atom: +32 bytes => +2 in the (addr >> 4) field
-                                mma(tmem_dd, adesc + (uint64_t)(k * (UMMA_K_BYTES >> 4)), bdesc + (uint64_t)(k * (UMMA_K_BYTES >> 4)),
-                                    (fresh && k == 0) ? 0u : 1u);
-                            }
-                            fresh = false;
-                        }
-                    }
-                    commit(&empty_bar[stage]);               // frees the group's smem slots (in both CTAs) once these MMAs retire
-                    if (++stage == NG) { stage = 0; phase ^= 1; }
-                    if (p.exact && ++in_chunk == p.exact_kc && kb0 + KGROUP < ti.nkb) {      // chunk complete (the last one is committed below)
-                        in_chunk = 0;
-                        commit(&tmem_full_bar[it & 1]);
-                        ++it;
-                    }
-                }
-                commit(&tmem_full_bar[it & 1]);               // accumulator (or last chunk) complete
-                ++it;
-            }
-            if (dbg) {
-                long long* d = p.dbg + 8 * blockIdx.x;
-                d[0] = clock64() - c_start; d[1] = c_ops; d[2] = c_tmem; d[3] = c_tiles;
-            }
-        }
-    } else {
-        // ===================== epilogue (warps 2..9) =====================
-        const int quarter = warp & 3;                     // TMEM lanes [32q, 32q+32) are only visible to warps with id%4 == q
-        const int col_half = (warp - 2) >> 2;             // which half of the tile's columns this warp owns
-        float* stg = staging + (warp - 2) * (32 * STG_LD);   // this warp's private staging tile [32][STG_LD]
-        int it = 0;
-        for (int t = sched_id; t < p.total_tiles; t += sched_stride) {
-            const TileInfo ti = decode_tile(p, t, kBlockN, k2Cta, (int)rank);
-            if (ti.skip) continue;
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            ++it;
-
-            // row bookkeeping: lane l owns tile row 32*quarter + l
-            const int row = quarter * 32 + lane;
-            long long my_off;
-            int my_ok, gm;
-            if (p.conv) {
-                const int lx = row % p.TW;
-                const int q = row / p.TW;
-                const int ly = q % p.TH;
-                const int ln = q / p.TH;
-                const int img = ti.img0 + ln, oy = ti.oy0 + ly, ox = ti.ox0 + lx;
-                my_ok = (img < p.Nimg) && (oy < p.OH) && (ox < p.OW);
-                gm = (img * p.OH + oy) * p.OW + ox;
-                my_off = (long long)gm * p.ldc;
-            } else {
-                gm = ti.m0 + row;
-                my_ok = gm < p.M;
-                my_off = (long long)ti.b1 * p.c_sb1 + (long long)ti.b2 * p.c_sb2 + (long long)gm * p.ldc;
-            }
-#ifdef VF_TC_STALL_COUNTERS
-            if (p.dbg_flags & 1) {
-                mbar_wait(&tmem_full_bar[acc], acc_phase);
-                tcgen05_fence_after();
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-                continue;
-            }
-#endif
-            const float bias_m = (p.bias_mode == VF_BIAS_M && my_ok) ? __ldg(p.bias + gm) : 0.f;
-
-            // phase-2 geometry: VPR float4 vectors span one tile row; a warp covers RPI rows per iteration
-            constexpr int VPR = HALF_N / 4;                // 16 (BLOCK_N=128) or 8 (BLOCK_N=64) vectors per half row
-            constexpr int RPI = 32 / VPR;                  // 2 or 4 rows per iteration
-            constexpr int ITERS = 32 / RPI;
-            const int r_sub = lane / VPR;
-            const int c_ln = (lane % VPR) * 4;             // column inside this warp's half
-            const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
-            // fast path: full-width tile, 16-byte aligned rows -> vector I/O and the whole residual tile prefetched into
-            // registers BEFORE waiting for the accumulator, so its DRAM latency hides behind this tile's MMAs
-            const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
-            float4 resv[ITERS];
-            if (fast && p.residual) {
-#pragma unroll
-                for (int i = 0; i < ITERS; ++i) {
-                    const int rr = i * RPI + r_sub;
-                    const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                    const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                    // unconditional load (out-of-range rows read row 0 and are never stored): a predicated load would make
-                    // the compiler funnel all 32 loads through one temporary and serialise their DRAM latencies
-                    const long long o = ok ? off_row + n_ln : (long long)n_ln;
-                    resv[i] = __ldg(reinterpret_cast<const float4*>(p.residual + o));
-                }
-            }
-            float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (fast && p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
-
-            if (p.exact) {
-                // ---- phase 1, exact mode: one TMEM hand-off per accumulation chunk; chunks are summed into the staging tile with RN
-                // FFMAs (cross-term passes scaled by 2^-11), see EXACT_LO_SCALE.  `it` was advanced once above: count chunks instead.
-                const int nchunks = ti.nkb / p.exact_kc, nsmall = 2 * p.exact_kpp / p.exact_kc;
-                --it;
-#pragma unroll 1
-                for (int ck = 0; ck < nchunks; ++ck) {
-                    const int a = it & 1;
-                    const uint32_t aph = (it >> 1) & 1;
-                    ++it;
-                    const float sc = (ck < nsmall ? EXACT_LO_SCALE : 1.0f) * p.alpha;
-                    mbar_wait(&tmem_full_bar[a], aph);
-                    tcgen05_fence_after();
-#pragma unroll 1
-                    for (int c0 = 0; c0 < HALF_N; c0 += 32) {
-                        uint32_t r[32];
-                        tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(a * kBlockN + col_half * HALF_N + c0), r);
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            float4* dst = reinterpret_cast<float4*>(stg + lane * STG_LD + c0 + j);
-                            float4 o = ck ? *dst : make_float4(0.f, 0.f, 0.f, 0.f);
-                            o.x = fmaf(__uint_as_float(r[j]), sc, o.x);
-                            o.y = fmaf(__uint_as_float(r[j + 1]), sc, o.y);
-                            o.z = fmaf(__uint_as_float(r[j + 2]), sc, o.z);
-                            o.w = fmaf(__uint_as_float(r[j + 3]), sc, o.w);
-                            *dst = o;
-                        }
-                    }
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tmem_empty_bar[a]);
-                }
-            } else {
-            mbar_wait(&tmem_full_bar[acc], acc_phase);
-            tcgen05_fence_after();
-
-            // ---- phase 1: TMEM -> registers -> staging row `lane` (scaled by alpha)
-#pragma unroll 1
-            for (int c0 = 0; c0 < HALF_N; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * kBlockN + col_half * HALF_N + c0), r);
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4*>(stg + lane * STG_LD + c0 + j) =
-                        make_float4(__uint_as_float(r[j]) * p.alpha, __uint_as_float(r[j + 1]) * p.alpha,
-                                    __uint_as_float(r[j + 2]) * p.alpha, __uint_as_float(r[j + 3]) * p.alpha);
-            }
-            // all TMEM reads of this warp are complete (tcgen05.wait::ld inside tmem_ld) -> hand the stage back
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (k2Cta && rank != 0) mbar_arrive_remote(&tmem_empty_bar[acc], 0);    // the leader's issuer waits for both CTAs
-                else mbar_arrive(&tmem_empty_bar[acc]);
-            }
-            }
-
-            // ---- phase 2: lanes span the columns of a tile row -> fully coalesced stores; bias / activation / residual here
-            if (fast) {
-                float gs = 0.f, gq = 0.f;                 // fused GroupNorm statistics of this lane's 4 channels
-#pragma unroll
-                for (int i = 0; i < ITERS; ++i) {
-                    const int rr = i * RPI + r_sub;
-                    const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                    const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                    const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
-                    float4 v = *reinterpret_cast<const float4*>(stg + rr * STG_LD + c_ln);
-                    if (p.bias_mode == VF_BIAS_N) { v.x += bias4.x; v.y += bias4.y; v.z += bias4.z; v.w += bias4.w; }
-                    else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
-                    if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
-                    if (p.residual) { v.x += resv[i].x; v.y += resv[i].y; v.z += resv[i].z; v.w += resv[i].w; }
-                    if (ok) {
-                        gs += (v.x + v.y) + (v.z + v.w);
-                        gq += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
-                        const long long off = off_row + n_ln;
-                        if (p.C_f32) *reinterpret_cast<float4*>(p.C_f32 + off) = v;
-                        if (p.C_bf16) {
-                            __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-                            uint2 u;
-                            u.x = *reinterpret_cast<uint32_t*>(&lo);
-                            u.y = *reinterpret_cast<uint32_t*>(&hi);
-                            *reinterpret_cast<uint2*>(p.C_bf16 + off) = u;
-                        }
-                    }
-                }
-                if (p.gn_sums) {
-                    // the 32 rows of a warp lie in one image; lanes with equal column vector (different r_sub) and the
-                    // cpg/4 neighbouring lanes of a group are folded with shuffles, then one fp64 RED per (image, group)
-                    const unsigned okmask = __ballot_sync(0xffffffffu, my_ok);
-#pragma unroll
-                    for (int o = VPR; o < 32; o <<= 1) {
-                        gs += __shfl_xor_sync(0xffffffffu, gs, o);
-                        gq += __shfl_xor_sync(0xffffffffu, gq, o);
-                    }
-                    const int lpg = p.gn_cpg >> 2;
-                    for (int o = 1; o < lpg; o <<= 1) {
-                        gs += __shfl_xor_sync(0xffffffffu, gs, o);
-                        gq += __shfl_xor_sync(0xffffffffu, gq, o);
-                    }
-                    const int gm_first = __shfl_sync(0xffffffffu, gm, okmask ? (__ffs(okmask) - 1) : 0);
-                    if (okmask && r_sub == 0 && (lane % lpg) == 0) {
-                        const long long slot = ((long long)(gm_first / p.gn_rows_per_img) * p.gn_groups + n_ln / p.gn_cpg) * 2;
-                        atomicAdd(p.gn_sums + slot, (double)gs);
-                        atomicAdd(p.gn_sums + slot + 1, (double)gq);
-                    }
-                }
-            } else {
-                // generic path (N tails, unaligned leading dimensions): scalar, same arithmetic order
-#pragma unroll 1
-                for (int rr = 0; rr < 32; ++rr) {
-                    const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                    const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                    const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
-                    if (!ok) continue;
-                    for (int c = lane; c < HALF_N; c += 32) {
-                        const int n = ti.n0 + col_half * HALF_N + c;
-                        if (n >= p.Ncols) continue;
-                        float x = stg[rr * STG_LD + c];
-                        x += (p.bias_mode == VF_BIAS_N) ? __ldg(p.bias + n) : bm;
-                        if (p.act == VF_ACT_GELU_ERF) x = vf_gelu_erf(x);
-                        const long long off = off_row + n;
-                        if (p.residual) x += __ldg(p.residual + off);
-                        if (p.C_f32) p.C_f32[off] = x;
-                        if (p.C_bf16) p.C_bf16[off] = __float2bfloat16(x);
-                    }
-                }
-            }
-            __syncwarp();                                  // staging is reused by the next tile
-        }
-    }
-
-    // ---- teardown: everyone done with TMEM, then the allocating warp frees it
-    tcgen05_fence_before();
-    __syncthreads();
-    if constexpr (k2Cta) cluster_sync_all();               // no CTA leaves while its peer may still signal or read it
-    if (warp == 1) {
-        tcgen05_fence_after();
-        if constexpr (k2Cta)
-            asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * kBlockN) : "memory");
-        else
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(2 * kBlockN) : "memory");
-    }
-}
-
-
-// ==============================================================================================================
-// Wide-tile 3x3 convolution (stride 1, pad 1): operands SWAPPED with respect to tc_gemm_kernel.
-//   A (M = 128)  = a 128-channel slice of the weights  [Cout][tap*Cin + c]      (16 KB per (tap, 64-channel block))
-//   B (N = 256)  = an 8-wide x 32-tall patch of pixels, read out of ONE (8+2) x (32+2) halo tile per 64-channel block through
-//                  row-shifted SWIZZLE_128B descriptors (SBO = 10 rows), exactly like the halo mode above
-//   D            = TMEM lane = output channel, TMEM column = pixel of the patch
-// Why: a tcgen05.mma with N <= 128 keeps the issuing thread and the shared-memory read port busier than the tensor pipe
-// (scripts/mma_rate_probe.cu: every barrier poll between 4-MMA groups costs tensor time unless the MMAs are 128 cycles long);
-// N = 256 halves the operand bytes per FLOP (12 KB per 128x256x16 MMA instead of 8 KB per 128x128x16), halves the weight-tile
-// traffic per pixel, and puts 32 consecutive channels of one pixel into the 32 lanes of a warp, so the epilogue writes
-// 128-byte rows straight from registers — no shared-memory staging at all.
-// ==============================================================================================================
-struct WideParams {
-    CUtensorMap tmX;           // activations [N, H, W, Cin] bf16: box {64, 10, 34, 1}
-    CUtensorMap tmW;           // weights [Cout, 9*Cin] bf16: box {64, 128}
-    const float* bias;         // [Cout] or null
-    const float* residual;     // [N, H, W, Cout] fp32 or null
-    float* C_f32;              // [N, H, W, Cout] or null
-    __nv_bfloat16* C_bf16;     // [N, H, W, Cout] or null
-    double* gn_sums;           // [N][groups][2] or null
-    int gn_groups, gn_cpg;
-    const float2* norm_mr;     // optional GroupNorm(+swish) of the INPUT, applied to the halo tile in shared memory: (mean, rstd) [N][groups]
-    const float* norm_gamma;   // [Cin]
-    const float* norm_beta;    // [Cin]
-    int norm_groups, norm_cpg, norm_swish;
-    int N, H, W, Cout, cin_blocks;
-    int tiles_x, tiles_y, tiles_c, total_tiles;
-    unsigned idesc;
-    long long* dbg;            // profiling builds: per-CTA stall counters
-    int dbg_flags;
-    int kc;                    // exact (split-fp16) mode: filter taps per accumulation chunk (1, 3 or 9)
-};
-
-// ---- exact mode (VF_F16X2 operands): fp32-faithful convolution on the tensor cores ------------------------------------------
-// An fp32 value v travels as TWO fp16 numbers  hi = fp16(v),  lo = fp16((v - hi) * 2^11)  (22-23 significand bits; the scaling keeps
-// lo out of the fp16 subnormal range), activations as [.., hi(C) | lo(C)], weights as [Cout][tap][hi(Cin) | lo(Cin)].
-//   x * w  =  hi_x hi_w  +  2^-11 (hi_x lo_w + lo_x hi_w)  +  O(2^-22 |x w|)            -> three fp16 MMAs per product block
-// tcgen05.mma adds into its fp32 accumulator with TRUNCATION (measured: scripts/acc_rounding_probe.py, relative bias ~1.3e-8 per
-// MMA step towards zero), so a long K loop in TMEM is not fp32-faithful.  The accumulator is therefore drained every `kc` filter
-// taps (a "chunk" of kc x 4 MMA steps from a ZERO accumulator) and the chunks are summed in registers with round-to-nearest
-// FFMA, scaled by 2^-11 for the cross terms, small terms first.  Measured against fp64: rms 1.3e-7 of |y| (the fp32 FFMA chain of
-// vf_simt_gemm: 6.1e-7) — the encoder on this path reproduces the fp32 path's codebook indices (tests/test_baseline_configs_gpu.py).
-
-
-// wide kernels: 16 epilogue warps (4 per TMEM lane quarter, 64 accumulator columns each): with 2 warps per scheduler the register
-// epilogue ran at ~0.25 IPC per warp (ncu: stall_wait / short scoreboard) and held every tile for 10-20k cycles
-constexpr int WIDE_EPI_WARPS = 16;
-constexpr int WIDE_XFORM_WARPS = 8;           // conv only: GroupNorm + swish applied to the halo tile in place (normalise-on-load)
-constexpr int WIDE_THREADS = 64 + 32 * WIDE_EPI_WARPS;
-constexpr int WIDE_TW = 8, WIDE_TH = 32;
-constexpr int WIDE_HALO_ROWS = (WIDE_TW + 2) * (WIDE_TH + 2);          // 340 rows of 128 B
-constexpr int WIDE_HALO_BYTES = 44032;                                  // >= 340 * 128, multiple of 1024
-constexpr int WIDE_W_SLOTS = 8;
-constexpr int WIDE_W_BYTES = 128 * ROW_BYTES;                           // one (tap, channel block) weight tile
-constexpr int WIDE_SMEM = 2 * WIDE_HALO_BYTES + WIDE_W_SLOTS * WIDE_W_BYTES + 1024 /*align*/ + 512 /*barriers*/ + 1024 /*scale, shift*/;
-
-// <16, false>: plain conv, 16 epilogue warps x 2 chunks; <8, true>: + 4 normalise-on-load warps, 8 epilogue warps x 4 chunks
-// (the thread count bounds the registers per thread: 704 threads left the epilogue 80 registers and spills)
-template <int kEpiWarps, bool kNorm, bool kExact = false>
-__global__ void __launch_bounds__(64 + 32 * kEpiWarps + (kNorm ? 32 * WIDE_XFORM_WARPS : 0), 1)
-tc_conv3x3_wide_kernel(const __grid_constant__ WideParams p) {
-    static_assert(!(kNorm && kExact), "normalise-on-load is a bf16-path feature");
-    constexpr int CPW = 256 / ((kEpiWarps / 4) * 32);        // 32-pixel chunks per epilogue warp
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* w_base = smem + 2 * WIDE_HALO_BYTES;
-    uint64_t* w_full = reinterpret_cast<uint64_t*>(w_base + WIDE_W_SLOTS * WIDE_W_BYTES);
-    uint64_t* w_empty = w_full + WIDE_W_SLOTS;
-    uint64_t* h_full = w_empty + WIDE_W_SLOTS;          // [2]
-    uint64_t* h_empty = h_full + 2;                     // [2]
-    uint64_t* tmem_full_bar = h_empty + 2;              // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;       // [2]
-    uint64_t* h_ready = tmem_empty_bar + 2;             // [2]  halo tile normalised in place (norm mode)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(h_ready + 2);
-    float* ssf = reinterpret_cast<float*>(w_base + WIDE_W_SLOTS * WIDE_W_BYTES + 512);       // [2][64 scales | 64 shifts] per halo buffer
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    constexpr bool norm = kNorm;
-
-    if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tmX)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tmW)) : "memory");
-    }
-    if (threadIdx.x == 32) {
-        for (int s = 0; s < WIDE_W_SLOTS; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&h_full[a], 1);
-            mbar_init(&h_empty[a], 1);
-            mbar_init(&h_ready[a], WIDE_XFORM_WARPS);
-            mbar_init(&tmem_full_bar[a], 1);
-            mbar_init(&tmem_empty_bar[a], kEpiWarps);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {   // 2 accumulator stages x 256 columns = the whole TMEM
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    // tile t -> (channel tile fastest, then x, y, image): neighbouring CTAs share halo tiles and weight slices in L2
-    auto decode = [&](int t, int& c0, int& ox0, int& oy0, int& img) {
-        c0 = (t % p.tiles_c) * 128;
-        int r = t / p.tiles_c;
-        ox0 = (r % p.tiles_x) * WIDE_TW;
-        r /= p.tiles_x;
-        oy0 = (r % p.tiles_y) * WIDE_TH;
-        img = r / p.tiles_y;
     };
 
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (elect_one()) {
-            int ws = 0, hb = 0;
-            uint32_t wph = 0, hph = 0;
-            for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
-                int c0, ox0, oy0, img;
-                decode(t, c0, ox0, oy0, img);
-                // exact mode walks 3 product passes over the channel blocks: (lo_x, hi_w), (hi_x, lo_w), (hi_x, hi_w) — small terms first
-                const int nv = kExact ? 3 * p.cin_blocks : p.cin_blocks;
-                for (int v = 0; v < nv; ++v) {
-                    const int j = kExact ? v / p.cin_blocks : 0, cb = kExact ? v - j * p.cin_blocks : v;
-                    const int xblk = kExact ? ((j == 0 ? p.cin_blocks : 0) + cb) : cb;            // channel block inside [hi | lo]
-                    mbar_wait(&h_empty[hb], hph ^ 1);
-                    mbar_expect_tx(&h_full[hb], WIDE_HALO_ROWS * ROW_BYTES);
-                    tma_load_4d(smem + hb * WIDE_HALO_BYTES, &p.tmX, &h_full[hb], xblk * 64, ox0 - 1, oy0 - 1, img);
-                    if (++hb == 2) { hb = 0; hph ^= 1; }
-                    for (int tap = 0; tap < 9; ++tap) {
-                        const int wblk = kExact ? (tap * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb : tap * p.cin_blocks + cb;
-                        mbar_wait(&w_empty[ws], wph ^ 1);
-                        mbar_expect_tx(&w_full[ws], WIDE_W_BYTES);
-                        tma_load_4d(w_base + ws * WIDE_W_BYTES, &p.tmW, &w_full[ws], wblk * 64, c0, 0, 0);
-                        if (++ws == WIDE_W_SLOTS) { ws = 0; wph ^= 1; }
-                    }
-                }
+    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+        const TileInfo ti = decode_tile(p, t, kBlockN);
+        if (ti.skip) continue;
+
+        // row bookkeeping: lane l stores tile row 32*quarter + l
+        const int row = quarter * 32 + lane;
+        long long my_off;
+        int my_ok, gm;
+        if (p.conv) {
+            const int lx = row % p.TW;
+            const int q = row / p.TW;
+            const int ly = q % p.TH;
+            const int ln = q / p.TH;
+            const int img = ti.img0 + ln, oy = ti.oy0 + ly, ox = ti.ox0 + lx;
+            my_ok = (img < p.Nimg) && (oy < p.OH) && (ox < p.OW);
+            gm = (img * p.OH + oy) * p.OW + ox;
+            my_off = (long long)gm * p.ldc;
+        } else {
+            gm = ti.m0 + row;
+            my_ok = gm < p.M;
+            my_off = (long long)ti.b1 * p.c_sb1 + (long long)ti.b2 * p.c_sb2 + (long long)gm * p.ldc;
+        }
+        const float bias_m = (p.bias_mode == VF_BIAS_M && my_ok) ? __ldg(p.bias + gm) : 0.f;
+
+        // phase-2 geometry: VPR float4 vectors span one tile row; a warp covers RPI rows per iteration
+        constexpr int VPR = HALF_N / 4;                // 16 (BLOCK_N=128) or 8 (BLOCK_N=64) vectors per half row
+        constexpr int RPI = 32 / VPR;                  // 2 or 4 rows per iteration
+        constexpr int ITERS = 32 / RPI;
+        const int r_sub = lane / VPR;
+        const int c_ln = (lane % VPR) * 4;             // column inside this warp's half
+        const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
+        // fast path: full-width tile, 16-byte aligned rows -> vector I/O and the whole residual tile prefetched into
+        // registers BEFORE the main loop, so its DRAM latency hides behind this tile's MMAs
+        const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
+        float4 resv[ITERS];
+        if (fast && p.residual) {
+#pragma unroll
+            for (int i = 0; i < ITERS; ++i) {
+                const int rr = i * RPI + r_sub;
+                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
+                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
+                // unconditional load (out-of-range rows read row 0 and are never stored): a predicated load would make
+                // the compiler funnel all 32 loads through one temporary and serialise their DRAM latencies
+                const long long o = ok ? off_row + n_ln : (long long)n_ln;
+                resv[i] = __ldg(reinterpret_cast<const float4*>(p.residual + o));
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            int ws = 0, hb = 0, it = 0;
-            uint32_t wph = 0, hph = 0;
-            bool ready = false;                 // next weight slot already seen full (polled ahead of the previous MMAs)
-            constexpr uint32_t PITCH = WIDE_TW + 2;
-#ifdef VF_TC_STALL_COUNTERS
-            const bool dbg = p.dbg != nullptr;
-#else
-            constexpr bool dbg = false;
-#endif
-            long long c_ops = 0, c_tmem = 0, c_tiles = 0, c0 = 0;
-            const long long c_start = dbg ? clock64() : 0;
-            for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
-                uint32_t tmem_d = 0;
-                bool fresh = true;                // next MMA starts a zeroed accumulator (tile start, or chunk start in exact mode)
-                auto open_acc = [&]() {
-                    const int acc = it & 1;
-                    const uint32_t acc_phase = (it >> 1) & 1;
-                    if (dbg) c0 = clock64();
-                    mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-                    if (dbg) { c_tmem += clock64() - c0; ++c_tiles; }
-                    tcgen05_fence_after();
-                    tmem_d = tmem_base + (uint32_t)(acc * 256);
-                    fresh = true;
-                };
-                auto close_acc = [&]() {
-                    tcgen05_commit(&tmem_full_bar[it & 1]);
-                    ++it;
-                };
-                if (!kExact) open_acc();
-                const int nv = kExact ? 3 * p.cin_blocks : p.cin_blocks;
-                for (int cb = 0; cb < nv; ++cb) {
-                    if (dbg) c0 = clock64();
-                    mbar_wait(norm ? &h_ready[hb] : &h_full[hb], hph);
-                    if (dbg) c_ops += clock64() - c0;
-                    tcgen05_fence_after();
-                    const uint32_t h_addr = smem_u32(smem + hb * WIDE_HALO_BYTES);
-                    int in_chunk = 0;
+        float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (fast && p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
+
+        // ---- phase 1: K loop.  One wgmma group (4 MMA steps of one k-block) stays in flight: once the group of k-block kb is
+        // issued, wait for kb-1's and hand its ring slot back to the producer.
+        const int nkb = p.halo ? 9 * p.cin_blocks : ti.nkb;
+        const int nsmall = p.exact ? 2 * p.exact_kpp / p.exact_kc : 0;     // exact mode: cross-term chunks come first
+        int prev_stage = -1, prev_halo = -1, in_chunk = 0, ck = 0, tap = 0;
+        bool fresh = true;
+        uint32_t a_base = 0;
+        const uint32_t pitch = (uint32_t)(p.TW + 2);
+        auto retire_prev = [&]() {
+            if (prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
+            if (prev_halo >= 0) mbar_arrive(&a_empty_bar[prev_halo]);
+            prev_stage = prev_halo = -1;
+        };
 #pragma unroll 1
-                    for (int tap = 0; tap < 9; ++tap) {
-                        if (kExact && in_chunk == 0) open_acc();
-                        if (dbg) c0 = clock64();
-                        if (!ready) mbar_wait(&w_full[ws], wph);
-                        if (dbg) c_ops += clock64() - c0;
-                        {
-                            const int ns = (ws + 1 == WIDE_W_SLOTS) ? 0 : ws + 1;
-                            ready = mbar_test_wait(&w_full[ns], ns == 0 ? (wph ^ 1) : wph);
-                        }
-                        tcgen05_fence_after();
-                        const uint64_t adesc = make_sw128_desc(smem_u32(w_base + ws * WIDE_W_BYTES));
-                        const uint32_t b_addr = h_addr + ((uint32_t)(tap / 3) * PITCH + (uint32_t)(tap % 3)) * ROW_BYTES;
-                        uint64_t bdesc = make_sw128_desc(b_addr);
-                        bdesc = (bdesc & ~((uint64_t)0x3FFF << 32)) | ((uint64_t)((PITCH * ROW_BYTES) >> 4) << 32);     // SBO = one halo row pitch
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            umma<false>(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), p.idesc, (fresh && k == 0) ? 0u : 1u);
-                        fresh = false;
-                        tcgen05_commit(&w_empty[ws]);
-                        if (++ws == WIDE_W_SLOTS) { ws = 0; wph ^= 1; }
-                        // cross-term passes (scaled by 2^-11: their accumulation error is far below fp32) drain once per channel block,
-                        // the hi.hi pass every p.kc taps
-                        if (kExact && ++in_chunk == (cb < 2 * p.cin_blocks ? 9 : p.kc)) { in_chunk = 0; close_acc(); }
+        for (int kb = 0; kb < nkb; ++kb) {
+            uint64_t adesc, bdesc;
+            const int this_halo = (p.halo && tap == 8) ? ab : -1;
+            if (p.halo) {
+                // tile = TH rows of TW=8 pixels: MMA row group g (8 rows) = image row g of the tile; inside the halo tile
+                // (pitch TW+2 rows) tap (dy,dx) starts (dy*(TW+2)+dx) rows in, consecutive groups are (TW+2) rows apart
+                if (tap == 0) {
+                    mbar_wait(&a_full_bar[ab], aphase, "vf_tc_gemm mma(halo)");
+                    a_base = smem_u32(smem + ab * HALO_BYTES);
+                    if (p.norm_mr) {              // every thread's MMAs read the whole tile: transform, then publish it to the async proxy
+                        normalise_halo(p, smem + ab * HALO_BYTES, kb / 9, ti.img0, ti.oy0, ti.ox0, threadIdx.x);
+                        fence_async_smem();
+                        named_sync(1, NUM_MMA_THREADS);
                     }
-                    tcgen05_commit(&h_empty[hb]);
-                    if (++hb == 2) { hb = 0; hph ^= 1; }
                 }
-                if (!kExact) close_acc();
+                mbar_wait(&full_bar[stage], phase, "vf_tc_gemm mma");
+                const uint32_t a_addr = a_base + ((uint32_t)(tap / 3) * pitch + (uint32_t)(tap % 3) + (uint32_t)(8 * wg) * pitch) * ROW_BYTES;
+                adesc = sw128_desc(a_addr, pitch * ROW_BYTES);
+                bdesc = sw128_desc(smem_u32(halo_b_base + stage * B_STAGE_BYTES));
+            } else {
+                mbar_wait(&full_bar[stage], phase, "vf_tc_gemm mma");
+                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+                adesc = sw128_desc(sa + (uint32_t)(wg * 64 * ROW_BYTES));
+                bdesc = sw128_desc(sa + A_STAGE_BYTES);
             }
-            if (dbg) {
-                long long* d = p.dbg + 8 * blockIdx.x;
-                d[0] = clock64() - c_start; d[1] = c_ops; d[2] = c_tmem; d[3] = c_tiles; d[4] = 1; d[5] = 0;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < K_STEPS; ++k)      // +32 bytes along K inside the swizzle atom => +2 in the (addr >> 4) field
+                wgmma_ss<kBlockN, kKind>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (fresh && k == 0) ? 0u : 1u);
+            wgmma_commit();
+            fresh = false;
+            wgmma_wait<1>();
+            retire_prev();
+            prev_stage = stage;
+            prev_halo = this_halo;
+            if (p.halo) {
+                if (++stage == NGH) { stage = 0; phase ^= 1; }
+                if (++tap == 9) { tap = 0; if (++ab == 2) { ab = 0; aphase ^= 1; } }
+            } else {
+                if (++stage == NG) { stage = 0; phase ^= 1; }
+            }
+            if (p.exact && ++in_chunk == p.exact_kc) {
+                // chunk complete: fold it into the staging tile (the first chunk initialises it), restart from a zero accumulator
+                in_chunk = 0;
+                wgmma_wait<0>();
+                reg_fence(acc);
+                if (ck == 0) named_sync(1, NUM_MMA_THREADS);      // the previous tile's epilogue is done with the staging tile
+                to_staging((ck < nsmall ? EXACT_LO_SCALE : 1.0f) * p.alpha, ck > 0);
+                ++ck;
+                fresh = true;
             }
         }
-    } else if (warp >= 2 + kEpiWarps) {
-        // ===================== normalise-on-load (4 warps): GroupNorm + swish of the raw halo tile, in place =====================
-        // The tile holds 340 rows (pixels of the (8+2) x (32+2) halo) of 64 bf16 channels, 128B-swizzled: physical 16-byte chunk pc
-        // of row r holds logical chunk pc ^ (r & 7) (the buffers are 1024-byte aligned).  Rows outside the image were zero-filled
-        // by TMA and must stay zero (the reference pads AFTER norm + swish, vqgan_th.py:69-78), so they are skipped.
-        if (norm) {
-            const int tid = threadIdx.x - (2 + kEpiWarps) * 32;
-            int hb = 0;
-            uint32_t hph = 0;
-            for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
-                int c0, ox0, oy0, img;
-                decode(t, c0, ox0, oy0, img);
-                for (int cb = 0; cb < p.cin_blocks; ++cb) {
-                    if (tid < 64) {
-                        const int c = cb * 64 + tid;
-                        const float2 mr = __ldg(p.norm_mr + (img * p.norm_groups + c / p.norm_cpg));
-                        const float sc = mr.y * __ldg(p.norm_gamma + c);
-                        ssf[hb * 128 + tid] = sc;                                    // [hb][0..63] scale, [hb][64..127] shift
-                        ssf[hb * 128 + 64 + tid] = __ldg(p.norm_beta + c) - mr.x * sc;
-                    }
-                    asm volatile("bar.sync 1, %0;" ::"n"(32 * WIDE_XFORM_WARPS) : "memory");
-                    mbar_wait(&h_full[hb], hph);
-                    uint8_t* tile = smem + hb * WIDE_HALO_BYTES;
-                    const int pc = tid & 7;                      // this thread's physical 16-byte chunk in every row it visits
-                    // rows advance by 32, so (r & 7) and with it the LOGICAL chunk (= 8 channels) of this thread never change:
-                    // its 8 (scale, shift) pairs are read once per block, not once per row (that re-read was 4x the tile traffic
-                    // and competes with the MMA's operand reads for the same shared-memory port)
-                    const float* sc8 = ssf + hb * 128 + ((pc ^ ((tid >> 3) & 7)) << 3);
-                    const float4 s0 = *reinterpret_cast<const float4*>(sc8), s1 = *reinterpret_cast<const float4*>(sc8 + 4);
-                    const float4 h0 = *reinterpret_cast<const float4*>(sc8 + 64), h1 = *reinterpret_cast<const float4*>(sc8 + 68);
-                    const float scv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-                    const float shv[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-#pragma unroll 2
-                    for (int r = tid >> 3; r < WIDE_HALO_ROWS; r += 4 * WIDE_XFORM_WARPS) {
-                        const int py = (r * 205) >> 11, px = r - py * (WIDE_TW + 2);       // r / 10 for r < 1029
-                        const int iy = oy0 - 1 + py, ix = ox0 - 1 + px;
-                        if (iy < 0 || iy >= p.H || ix < 0 || ix >= p.W) continue;
-                        uint4* ptr = reinterpret_cast<uint4*>(tile + r * ROW_BYTES + pc * 16);
-                        const uint4 v = *ptr;
-                        uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            float a = __uint_as_float(w[k] << 16), b = __uint_as_float(w[k] & 0xffff0000u);
-                            a = fmaf(a, scv[2 * k], shv[2 * k]);
-                            b = fmaf(b, scv[2 * k + 1], shv[2 * k + 1]);
-                            if (p.norm_swish == 1) {          // same arithmetic as vf_groupnorm_apply (bit-identical operand)
-                                a = __fdividef(a, 1.0f + __expf(-a));
-                                b = __fdividef(b, 1.0f + __expf(-b));
-                            }
-                            __nv_bfloat162 o = __floats2bfloat162_rn(a, b);
-                            w[k] = *reinterpret_cast<uint32_t*>(&o);
-                            if (p.norm_swish == 2) {
-                                // packed bf16: swish(y) = h * (1 + tanh(h)), h = y / 2 — ONE MUFU op per two elements instead of four
-                                uint32_t h, th;
-                                asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(h) : "r"(w[k]), "r"(0x3f003f00u));
-                                asm("tanh.approx.bf16x2 %0, %1;" : "=r"(th) : "r"(h));
-                                asm("fma.rn.bf16x2 %0, %1, %2, %1;" : "=r"(w[k]) : "r"(h), "r"(th));
-                            }
-                        }
-                        *ptr = make_uint4(w[0], w[1], w[2], w[3]);
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> visible to the MMA
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&h_ready[hb]);
-                    if (++hb == 2) { hb = 0; hph ^= 1; }
-                }
-            }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        retire_prev();
+        if (!p.exact) {
+            named_sync(1, NUM_MMA_THREADS);                       // the previous tile's epilogue is done with the staging tile
+            to_staging(p.alpha, false);
         }
-    } else {
-        // ===================== epilogue: lane = output channel, register j = pixel =====================
-        const int quarter = warp & 3;                     // TMEM lanes [32q, 32q+32) = channels c0 + 32q + lane
-        const int grp = (warp - 2) >> 2;                  // pixels [32*CPW*grp, +32*CPW) of the patch = patch rows [4*CPW*grp, +4*CPW)
-        int it = 0;
-        for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
-            int c0, ox0, oy0, img;
-            decode(t, c0, ox0, oy0, img);
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            ++it;
-            const int ch = c0 + quarter * 32 + lane;
-            const float bias = p.bias ? __ldg(p.bias + ch) : 0.f;
-            // element index of (pixel (ty, tx) of the patch, channel ch) = base + ty * row_stride + tx * Cout; 32-bit (host-checked)
-            const int base = ((img * p.H + oy0) * p.W + ox0) * p.Cout + ch;
-            const int row_stride = p.W * p.Cout;
-            const int rows_ok = p.H - oy0, cols_ok = p.W - ox0;          // valid rows / columns of this patch
-            const bool full = rows_ok >= WIDE_TH && cols_ok >= WIDE_TW;
-            const bool has_res = p.residual != nullptr;
-            // chunk c of this warp = patch rows [4*CPW*grp + 4c, +4), register j -> (row j/8, column j%8)
-            float rv[32];
-            auto load_res = [&](int c) {
-                const int r0 = grp * (4 * CPW) + c * 4;
+        named_sync(1, NUM_MMA_THREADS);                           // staging tile complete
+
+        // ---- phase 2: lanes span the columns of a tile row -> fully coalesced stores; bias / activation / residual here
+        if (fast) {
+            float gs = 0.f, gq = 0.f;                 // fused GroupNorm statistics of this lane's 4 channels
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    int ty = r0 + (j >> 3), tx = j & 7;
-                    if (!full) {                          // clamp (never stored): the 32 loads stay unconditional and in flight together
-                        ty = ty < rows_ok ? ty : rows_ok - 1;
-                        tx = tx < cols_ok ? tx : cols_ok - 1;
-                    }
-                    rv[j] = __ldg(p.residual + (base + ty * row_stride + tx * p.Cout));
-                }
-            };
-            float gs = 0.f, gq = 0.f;
-#ifdef VF_TC_STALL_COUNTERS
-            if (p.dbg_flags & 1) {
-                mbar_wait(&tmem_full_bar[acc], acc_phase);
-                tcgen05_fence_after();
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-                continue;
-            }
-#endif
-            if constexpr (kExact) {
-                // chunked accumulation: every chunk arrives in a TMEM stage that started from zero; sum them here with RN FFMAs
-                // (cross-term chunks scaled by 2^-11).  (acc, acc_phase, it) above described the tile's FIRST chunk.
-                static_assert(!kExact || CPW == 2, "exact epilogue holds 2 x 32 accumulator columns per thread");
-                // The running sums START from the residual (64 loads in flight behind the first chunk's MMAs, no extra registers); the
-                // chunk sums are then added in increasing magnitude.  18+ RN additions at the magnitude of the output cost ~1e-7
-                // relative — the same order as the single rounding of the reference's own `conv + residual`.
-                float a0[32], a1[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    if (has_res) {
-                        int ty0 = grp * 8 + (j >> 3), ty1 = ty0 + 4, tx = j & 7;
-                        if (!full) {
-                            ty0 = ty0 < rows_ok ? ty0 : rows_ok - 1;
-                            ty1 = ty1 < rows_ok ? ty1 : rows_ok - 1;
-                            tx = tx < cols_ok ? tx : cols_ok - 1;
-                        }
-                        a0[j] = __ldg(p.residual + (base + ty0 * row_stride + tx * p.Cout));
-                        a1[j] = __ldg(p.residual + (base + ty1 * row_stride + tx * p.Cout));
-                    } else {
-                        a0[j] = 0.f;
-                        a1[j] = 0.f;
-                    }
-                }
-                // chunks: one per channel block of the two cross-term passes, 9 / kc per channel block of the hi.hi pass
-                const int nsmall = 2 * p.cin_blocks, nchunks = nsmall + p.cin_blocks * (9 / p.kc);
-                int a = acc;
-                uint32_t aph = acc_phase;
-                --it;                                                   // undo the per-tile increment: one hand-off per chunk
-#pragma unroll 1
-                for (int ck = 0; ck < nchunks; ++ck) {
-                    a = it & 1;
-                    aph = (it >> 1) & 1;
-                    ++it;
-                    const float sc = ck < nsmall ? EXACT_LO_SCALE : 1.0f;
-                    mbar_wait(&tmem_full_bar[a], aph);
-                    tcgen05_fence_after();
-                    const uint32_t ta = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(a * 256 + grp * 64);
-                    uint32_t r[16];
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        tmem_ld_32x16(ta + 16 * q, r);
-                        if (q == 3) {                                   // all TMEM reads of this chunk are done
-                            tcgen05_fence_before();
-                            __syncwarp();
-                            if (lane == 0) mbar_arrive(&tmem_empty_bar[a]);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            if (q < 2) a0[16 * q + j] = fmaf(__uint_as_float(r[j]), sc, a0[16 * q + j]);
-                            else a1[16 * (q - 2) + j] = fmaf(__uint_as_float(r[j]), sc, a1[16 * (q - 2) + j]);
-                        }
-                    }
-                }
-                // final: bias, statistics, store
-#pragma unroll
-                for (int j = 0; j < 64; ++j) {
-                    const float v = (j < 32 ? a0[j] : a1[j - 32]) + bias;
-                    const int ty = grp * 8 + (j >> 3), tx = j & 7;
-                    if (full || (ty < rows_ok && tx < cols_ok)) {       // warp-uniform
-                        gs += v;
-                        gq = fmaf(v, v, gq);
-                        p.C_f32[base + ty * row_stride + tx * p.Cout] = v;
-                    }
-                }
-                if (p.gn_sums) {
-                    for (int o = 1; o < p.gn_cpg; o <<= 1) {
-                        gs += __shfl_xor_sync(0xffffffffu, gs, o);
-                        gq += __shfl_xor_sync(0xffffffffu, gq, o);
-                    }
-                    if ((lane & (p.gn_cpg - 1)) == 0) {
-                        double* d = p.gn_sums + ((long long)img * p.gn_groups + ch / p.gn_cpg) * 2;
-                        atomicAdd(d, (double)gs);
-                        atomicAdd(d + 1, (double)gq);
-                    }
-                }
-                continue;
-            }
-            if (has_res) load_res(0);                     // flies behind this tile's MMAs
-            mbar_wait(&tmem_full_bar[acc], acc_phase);
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < CPW; ++c) {
-                uint32_t r[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 256 + grp * (32 * CPW) + c * 32), r);
-                if (c == CPW - 1) {                       // all TMEM reads of this warp are done -> hand the accumulator stage back
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tmem_empty_bar[acc]);
-                }
-                const int r0 = grp * (4 * CPW) + c * 4;
-                float v[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    v[j] = __uint_as_float(r[j]) + bias;
-                    if (has_res) v[j] += rv[j];
-                }
-                if (has_res && c + 1 < CPW) load_res(c + 1);      // the next chunk's residual rows fly while this chunk is stored
-                if (full) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) { gs += v[j]; gq = fmaf(v[j], v[j], gq); }
-                    if (p.C_f32) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)      // 32 lanes = 32 consecutive channels of one pixel = one 128-byte row
-                            p.C_f32[base + (r0 + (j >> 3)) * row_stride + (j & 7) * p.Cout] = v[j];
-                    }
+            for (int i = 0; i < ITERS; ++i) {
+                const int rr = i * RPI + r_sub;
+                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
+                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
+                const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
+                float4 v = *reinterpret_cast<const float4*>(stg + rr * STG_LD + c_ln);
+                if (p.bias_mode == VF_BIAS_N) { v.x += bias4.x; v.y += bias4.y; v.z += bias4.z; v.w += bias4.w; }
+                else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
+                if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
+                if (p.residual) { v.x += resv[i].x; v.y += resv[i].y; v.z += resv[i].z; v.w += resv[i].w; }
+                if (ok) {
+                    gs += (v.x + v.y) + (v.z + v.w);
+                    gq += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
+                    const long long off = off_row + n_ln;
+                    if (p.C_f32) *reinterpret_cast<float4*>(p.C_f32 + off) = v;
                     if (p.C_bf16) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            p.C_bf16[base + (r0 + (j >> 3)) * row_stride + (j & 7) * p.Cout] = __float2bfloat16(v[j]);
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int ty = r0 + (j >> 3), tx = j & 7;
-                        if (ty < rows_ok && tx < cols_ok) {       // warp-uniform
-                            const int idx = base + ty * row_stride + tx * p.Cout;
-                            gs += v[j];
-                            gq = fmaf(v[j], v[j], gq);
-                            if (p.C_f32) p.C_f32[idx] = v[j];
-                            if (p.C_bf16) p.C_bf16[idx] = __float2bfloat16(v[j]);
-                        }
+                        __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+                        uint2 u;
+                        u.x = *reinterpret_cast<uint32_t*>(&lo);
+                        u.y = *reinterpret_cast<uint32_t*>(&hi);
+                        *reinterpret_cast<uint2*>(p.C_bf16 + off) = u;
                     }
                 }
             }
             if (p.gn_sums) {
-                // lanes of one GroupNorm group are adjacent: fold them, one fp64 RED per (image, group) and warp
-                for (int o = 1; o < p.gn_cpg; o <<= 1) {
+                // the 32 rows of a warp lie in one image; lanes with equal column vector (different r_sub) and the
+                // cpg/4 neighbouring lanes of a group are folded with shuffles, then one fp64 RED per (image, group)
+                const unsigned okmask = __ballot_sync(0xffffffffu, my_ok);
+#pragma unroll
+                for (int o = VPR; o < 32; o <<= 1) {
                     gs += __shfl_xor_sync(0xffffffffu, gs, o);
                     gq += __shfl_xor_sync(0xffffffffu, gq, o);
                 }
-                if ((lane & (p.gn_cpg - 1)) == 0) {
-                    double* d = p.gn_sums + ((long long)img * p.gn_groups + ch / p.gn_cpg) * 2;
-                    atomicAdd(d, (double)gs);
-                    atomicAdd(d + 1, (double)gq);
+                const int lpg = p.gn_cpg >> 2;
+                for (int o = 1; o < lpg; o <<= 1) {
+                    gs += __shfl_xor_sync(0xffffffffu, gs, o);
+                    gq += __shfl_xor_sync(0xffffffffu, gq, o);
+                }
+                const int gm_first = __shfl_sync(0xffffffffu, gm, okmask ? (__ffs(okmask) - 1) : 0);
+                if (okmask && r_sub == 0 && (lane % lpg) == 0) {
+                    const long long slot = ((long long)(gm_first / p.gn_rows_per_img) * p.gn_groups + n_ln / p.gn_cpg) * 2;
+                    atomicAdd(p.gn_sums + slot, (double)gs);
+                    atomicAdd(p.gn_sums + slot + 1, (double)gq);
                 }
             }
-        }
-    }
-
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-}
-
-
-// ==============================================================================================================
-// Wide-tile GEMM for the un-batched linear layers, same operand swap as the wide convolution:
-//   A (M = 128) = 128 output features of the weight matrix W [Nf][K]; B (N = 256) = 256 rows (tokens) of X [M][K];
-//   D: TMEM lane = feature, column = token.  out[token][feature] = act(alpha * sum_k X W + bias[feature]) + residual.
-// 4 stages x (16 KB W + 32 KB X); epilogue straight from registers (32 lanes = 32 consecutive features = one 128-byte row).
-// ==============================================================================================================
-struct WideGemmParams {
-    CUtensorMap tmW;           // weights [Nf, K]: box {bk, 128}
-    CUtensorMap tmX;           // rows    [M, K]:  box {bk, 256}
-    CUtensorMap tmX2;          // pair kernel: the same rows with a 128-row box (each CTA loads half of the 256 rows)
-    const float* bias;         // [Nf] or null
-    const float* residual;     // [M, ldc] fp32 or null
-    float* C_f32;
-    __nv_bfloat16* C_bf16;
-    float alpha;
-    int act;
-    int M, Nf, ldc, num_k_blocks;
-    int tiles_f, total_tiles;
-    unsigned idesc;
-    long long* dbg;
-    int dbg_flags;
-};
-constexpr int WG_STAGES = 4;
-constexpr int WG_W_BYTES = 128 * ROW_BYTES, WG_X_BYTES = 256 * ROW_BYTES;
-constexpr int WG_STAGE_BYTES = WG_W_BYTES + WG_X_BYTES;
-constexpr int WG_SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
-
-// erf-GELU for bf16 outputs: Abramowitz-Stegun 7.1.26 (|abs err| < 1.5e-7 on erf, far below bf16 rounding) with ex2/rcp
-// approximations — the exact erff() costs more issue slots than the MMAs of a K = 768 tile leave to the epilogue
-__device__ __forceinline__ float gelu_erf_fast(float x) {
-    const float z = fabsf(x) * 0.70710678118654752440f;
-    const float t = __fdividef(1.0f, fmaf(0.3275911f, z, 1.0f));
-    float poly = fmaf(1.061405429f, t, -1.453152027f);
-    poly = fmaf(poly, t, 1.421413741f);
-    poly = fmaf(poly, t, -0.284496736f);
-    poly = fmaf(poly, t, 0.254829592f);
-    const float e = 1.0f - poly * t * __expf(-z * z);          // erf(|x| / sqrt 2)
-    return 0.5f * x * (1.0f + copysignf(e, x));
-}
-
-// kGelu / kBf16Out are compile-time so that each instantiation carries one epilogue (the fully unrolled runtime-switched version
-// was ~13k instructions and ran out of the instruction cache: 30k cycles per tile)
-// k2Cta: a thread-block cluster of two CTAs computes a 256-feature x 256-row tile with `cta_group::2` MMAs (M = 256): each CTA loads its own
-// 128 weight rows and HALF of the 256 activation rows (32 KB per k-block instead of 48 KB — the single-CTA kernel waits for operands
-// 43-55 % of the time), the leader CTA issues the MMAs for the pair, every CTA drains its own 128 TMEM lanes.
-template <bool kGelu, bool kBf16Out, bool k2Cta>
-__global__ void __launch_bounds__(WIDE_THREADS, 1) tc_gemm_wide_kernel(const __grid_constant__ WideGemmParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES);
-    uint64_t* empty_bar = full_bar + WG_STAGES;
-    uint64_t* tmem_full_bar = empty_bar + WG_STAGES;    // [2]
-    uint64_t* tmem_empty_bar = tmem_full_bar + 2;       // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const uint32_t rank = k2Cta ? cluster_ctarank() : 0;
-    // work units: single CTA = one 128 x 256 tile per step; pair = one 256 x 256 tile per step (this CTA: features f0 + 128 * rank)
-    const int unit0 = k2Cta ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, unit_stride = k2Cta ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    const int tiles_f = k2Cta ? p.tiles_f / 2 : p.tiles_f, n_units = k2Cta ? p.total_tiles / 2 : p.total_tiles;
-    constexpr int X_ROWS = k2Cta ? 128 : 256;                       // activation rows this CTA loads per stage
-    constexpr int STAGE = WG_W_BYTES + X_ROWS * ROW_BYTES;
-
-    if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tmW)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tmX)) : "memory");
-    }
-    if (threadIdx.x == 32) {
-        for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full_bar[a], 1); mbar_init(&tmem_empty_bar[a], (k2Cta ? 2 : 1) * WIDE_EPI_WARPS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        if (k2Cta) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
         } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (k2Cta) cluster_sync_all();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (elect_one()) {          // ===================== TMA producer =====================
-            int stage = 0;
-            uint32_t phase = 0;
-            const uint32_t lead_full = k2Cta ? leader_addr(full_bar) : 0;
-            for (int t = unit0; t < n_units; t += unit_stride) {
-                const int f0 = (t % tiles_f) * (k2Cta ? 256 : 128) + (int)rank * 128, m0 = (t / tiles_f) * 256 + (int)rank * (k2Cta ? 128 : 0);
-                for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t* sw = smem + stage * STAGE;
-                    if (k2Cta) {
-                        if (rank == 0) mbar_expect_tx(&full_bar[stage], 2 * STAGE);            // both CTAs' bytes land on the leader's barrier
-                        tma_load_4d_2sm(sw, &p.tmW, lead_full + (uint32_t)(stage * 8), kb * 64, f0, 0, 0);
-                        tma_load_4d_2sm(sw + WG_W_BYTES, &p.tmX2, lead_full + (uint32_t)(stage * 8), kb * 64, m0, 0, 0);
-                        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-                        continue;
-                    }
-                    mbar_expect_tx(&full_bar[stage], WG_STAGE_BYTES);
-                    tma_load_4d(sw, &p.tmW, &full_bar[stage], kb * 64, f0, 0, 0);
-                    tma_load_4d(sw + WG_W_BYTES, &p.tmX, &full_bar[stage], kb * 64, m0, 0, 0);
-                    if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0 && elect_one()) {          // ===================== MMA issuer (pair: the leader issues for both CTAs) =====================
-            int stage = 0, it = 0;
-            uint32_t phase = 0;
-            bool ready = false;
-#ifdef VF_TC_STALL_COUNTERS
-            const bool dbg = p.dbg != nullptr;
-#else
-            constexpr bool dbg = false;
-#endif
-            long long c_ops = 0, c_tmem = 0, c_tiles = 0, c0 = 0;
-            const long long c_start = dbg ? clock64() : 0;
-            for (int t = unit0; t < n_units; t += unit_stride) {
-                const int acc = it & 1;
-                const uint32_t acc_phase = (it >> 1) & 1;
-                if (dbg) c0 = clock64();
-                if (k2Cta) mbar_wait_cluster(&tmem_empty_bar[acc], acc_phase ^ 1); else
-                mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-                if (dbg) { c_tmem += clock64() - c0; ++c_tiles; }
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * 256);
+            // generic path (N tails, unaligned leading dimensions): scalar, same arithmetic order
 #pragma unroll 1
-                for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    if (dbg) c0 = clock64();
-                    if (!ready) mbar_wait(&full_bar[stage], phase);
-                    if (dbg) c_ops += clock64() - c0;
-                    {
-                        const int ns = (stage + 1 == WG_STAGES) ? 0 : stage + 1;
-                        ready = mbar_test_wait(&full_bar[ns], ns == 0 ? (phase ^ 1) : phase);
-                    }
-                    tcgen05_fence_after();
-                    const uint32_t sw = smem_u32(smem + stage * STAGE);
-                    const uint64_t adesc = make_sw128_desc(sw), bdesc = make_sw128_desc(sw + WG_W_BYTES);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        if (k2Cta) umma_2sm<false>(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), p.idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                        else umma<false>(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), p.idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                    }
-                    if (k2Cta) tcgen05_commit_2sm(&empty_bar[stage]); else tcgen05_commit(&empty_bar[stage]);
-                    if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-                }
-                if (k2Cta) tcgen05_commit_2sm(&tmem_full_bar[acc]); else tcgen05_commit(&tmem_full_bar[acc]);
-                ++it;
-            }
-            if (dbg) {
-                long long* d = p.dbg + 8 * blockIdx.x;
-                d[0] = clock64() - c_start; d[1] = c_ops; d[2] = c_tmem; d[3] = c_tiles; d[4] = 1; d[5] = 0;
-            }
-        }
-    } else {
-        // ===================== epilogue (warps 2..17): lane = feature, register j = token =====================
-        const int quarter = warp & 3;
-        const int grp = (warp - 2) >> 2;                             // tokens [64*grp, +64) of the tile
-        int it = 0;
-        for (int t = unit0; t < n_units; t += unit_stride) {
-            const int f0 = (t % tiles_f) * (k2Cta ? 256 : 128) + (int)rank * 128, m0 = (t / tiles_f) * 256;
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            ++it;
-            const int f = f0 + quarter * 32 + lane;
-            const float bias = p.bias ? __ldg(p.bias + f) : 0.f;
-            const int row0 = m0 + grp * 64;                          // first token of this warp's 64 columns
-            const int base = row0 * p.ldc + f;                       // 32-bit (host-checked)
-            const int rows_ok = p.M - row0;                          // tokens of this warp that exist (may be <= 0 or >= 64)
-            const bool has_res = p.residual != nullptr;
-            float rv[32];
-            auto load_res = [&](int c) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    int r = c * 32 + j;
-                    r = r < rows_ok ? r : (rows_ok > 0 ? rows_ok - 1 : 0);        // clamped, never stored
-                    rv[j] = rows_ok > 0 ? __ldg(p.residual + (base + r * p.ldc)) : 0.f;
-                }
-            };
-#ifdef VF_TC_STALL_COUNTERS
-            if (p.dbg_flags & 1) {
-                mbar_wait(&tmem_full_bar[acc], acc_phase);
-                tcgen05_fence_after();
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) { if (k2Cta && rank != 0) mbar_arrive_remote(&tmem_empty_bar[acc], 0); else mbar_arrive(&tmem_empty_bar[acc]); }
-                continue;
-            }
-#endif
-            if (has_res) load_res(0);
-            mbar_wait(&tmem_full_bar[acc], acc_phase);
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < 2; ++c) {
-                uint32_t r[32];
-                tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 256 + grp * 64 + c * 32), r);
-                if (c == 1) {
-                    tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) {
-                        if (k2Cta && rank != 0) mbar_arrive_remote(&tmem_empty_bar[acc], 0);       // the leader's issuer waits for both CTAs
-                        else mbar_arrive(&tmem_empty_bar[acc]);
-                    }
-                }
-                float v[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    v[j] = fmaf(__uint_as_float(r[j]), p.alpha, bias);
-                    if (kGelu) v[j] = kBf16Out ? gelu_erf_fast(v[j]) : vf_gelu_erf(v[j]);
-                    if (has_res) v[j] += rv[j];
-                }
-                if (has_res && c == 0) load_res(1);
-                const int cb = base + c * 32 * p.ldc;
-                if (rows_ok >= (c + 1) * 32) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        if (kBf16Out) p.C_bf16[cb + j * p.ldc] = __float2bfloat16(v[j]);
-                        else p.C_f32[cb + j * p.ldc] = v[j];
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        if (c * 32 + j < rows_ok) {
-                            if (kBf16Out) p.C_bf16[cb + j * p.ldc] = __float2bfloat16(v[j]);
-                            else p.C_f32[cb + j * p.ldc] = v[j];
-                        }
-                    }
+            for (int rr = 0; rr < 32; ++rr) {
+                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
+                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
+                const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
+                if (!ok) continue;
+                for (int c = lane; c < HALF_N; c += 32) {
+                    const int n = ti.n0 + col_half * HALF_N + c;
+                    if (n >= p.Ncols) continue;
+                    float x = stg[rr * STG_LD + c];
+                    x += (p.bias_mode == VF_BIAS_N) ? __ldg(p.bias + n) : bm;
+                    if (p.act == VF_ACT_GELU_ERF) x = vf_gelu_erf(x);
+                    const long long off = off_row + n;
+                    if (p.residual) x += __ldg(p.residual + off);
+                    if (p.C_f32) p.C_f32[off] = x;
+                    if (p.C_bf16) p.C_bf16[off] = __float2bfloat16(x);
                 }
             }
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (k2Cta) cluster_sync_all();          // the peer may still be reading this CTA's shared memory / signalling its barriers
-    if (warp == 1) {
-        if (k2Cta) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    }
-    return fn;
 }
 
 // 4-D tensor map, dims innermost first, 128B swizzle, zero OOB fill.  strides[i] = byte stride of dim i+1.
 int make_tmap(CUtensorMap* tm, int dtype, const void* base, const uint64_t dims[4], const uint64_t strides_bytes[3],
               const uint32_t box[4]) {
-    EncodeTiledFn fn = get_encode_fn();
+    EncodeTiledFn fn = encode_fn();
     if (!fn) { vf_set_error("vf_tc_gemm: cuTensorMapEncodeTiled unavailable"); return VF_ERR_CUDA; }
     cuuint64_t gdim[4] = {dims[0], dims[1], dims[2], dims[3]};
     cuuint64_t gstr[3] = {strides_bytes[0], strides_bytes[1], strides_bytes[2]};
@@ -1611,268 +529,31 @@ int make_tmap(CUtensorMap* tm, int dtype, const void* base, const uint64_t dims[
     return VF_OK;
 }
 
-// cute::UMMA::InstrDescriptor: [4,6) D fmt (1=f32) | [7,10) A fmt | [10,13) B fmt (0 f16, 1 bf16, 2 tf32)
-// | [15] A major (0=K) | [16] B major (0=K) | [17,23) N>>3 | [24,29) M>>4
-unsigned make_idesc(bool tf32, int M, int N, bool f16 = false) {
-    unsigned d = 0;
-    d |= 1u << 4;
-    const unsigned fmt = tf32 ? 2u : (f16 ? 0u : 1u);
-    d |= fmt << 7;
-    d |= fmt << 10;
-    d |= (unsigned)(N >> 3) << 17;
-    d |= (unsigned)(M >> 4) << 24;
-    return d;
-}
-
-template <int kBlockN, int kStages, bool kTF32, bool k2Cta>
+template <int kBlockN, int kStages, WgKind kKind>
 int launch(const TcParams& prm, dim3 grid, cudaStream_t st) {
-    constexpr int b_rows = k2Cta ? kBlockN / 2 : kBlockN;
-    constexpr int smem = operand_bytes(kStages, A_STAGE_BYTES + b_rows * ROW_BYTES, b_rows * ROW_BYTES) +
-                         NUM_EPI_WARPS * 32 * (kBlockN / 2 + 4) * 4 /*epilogue staging*/ + 1024 /*align slack*/ + 256 /*barriers*/;
-    static_assert(kStages % KGROUP == 0 && HALO_SLOTS % KGROUP == 0, "ring slots must form whole groups");
+    constexpr int smem = tc_smem_bytes<kBlockN, kStages>();
+    static_assert(kStages <= MAX_STAGES, "ring depth");
     static_assert(smem <= 232448, "shared memory budget");
-    static_assert((4 * WIDE_XFORM_WARPS) % 8 == 0, "transform rows must advance by a multiple of 8");
     static vf_per_device_flag configured_pd;          // function attributes are per device
     bool& configured = configured_pd.current();
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<kBlockN, kStages, kTF32, k2Cta>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaError_t e = cudaFuncSetAttribute(tc_gemm_kernel<kBlockN, kStages, kKind>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) { vf_set_error("vf_tc_gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
         configured = true;
     }
-    if constexpr (k2Cta) {
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = grid;
-        cfg.blockDim = dim3(NUM_THREADS);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;      // CTA pair on one TPC
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        cudaError_t e = cudaLaunchKernelEx(&cfg, tc_gemm_kernel<kBlockN, kStages, kTF32, k2Cta>, prm);
-        if (e != cudaSuccess) { vf_set_error("vf_tc_gemm: cluster launch failed: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
-    } else {
-        tc_gemm_kernel<kBlockN, kStages, kTF32, k2Cta><<<grid, NUM_THREADS, smem, st>>>(prm);
-    }
+    tc_gemm_kernel<kBlockN, kStages, kKind><<<grid, NUM_THREADS, smem, st>>>(prm);
     VF_CHECK_LAUNCH("vf_tc_gemm");
     return VF_OK;
 }
 
+template <int kBlockN, int kStages>
+int launch_kind(const TcParams& prm, WgKind kind, dim3 grid, cudaStream_t st) {
+    if (kind == TF32) return launch<kBlockN, kStages, TF32>(prm, grid, st);
+    if (kind == F16) return launch<kBlockN, kStages, F16>(prm, grid, st);
+    return launch<kBlockN, kStages, BF16>(prm, grid, st);
+}
+
 }  // namespace
-
-
-static long long* g_tc_dbg = nullptr;
-static int g_tc_dbg_flags = 0;
-// 3x3 stride-1 pad-1 bf16 convolutions on maps at least 32 rows tall go to the wide-tile kernel (VF_TC_WIDE=0 disables)
-static int launch_conv_wide(const vf_tc_gemm_t* q, cudaStream_t st) {
-    WideParams prm;
-    memset(&prm, 0, sizeof(prm));
-    const int es = 2;
-    const bool exact = q->ab_dtype == VF_F16X2;          // split fp16 operands: [hi | lo] along the channel axis (16-bit elements either way)
-    const uint64_t dimsX[4] = {(uint64_t)q->Ctot, (uint64_t)q->W, (uint64_t)q->H, (uint64_t)q->N};
-    const uint64_t strX[3] = {(uint64_t)q->Ctot * es, (uint64_t)q->W * q->Ctot * es, (uint64_t)q->H * q->W * q->Ctot * es};
-    const uint32_t boxX[4] = {64, WIDE_TW + 2, WIDE_TH + 2, 1};
-    int rc;
-    if ((rc = make_tmap(&prm.tmX, VF_BF16, q->A, dimsX, strX, boxX)) != VF_OK) return rc;
-    const uint64_t Ktot = (exact ? 18ull : 9ull) * q->Cin;
-    const uint64_t dimsW[4] = {Ktot, (uint64_t)q->Ncols, 1, 1};
-    const uint64_t strW[3] = {Ktot * es, Ktot * es * q->Ncols, Ktot * es * q->Ncols};
-    const uint32_t boxW[4] = {64, 128, 1, 1};
-    if ((rc = make_tmap(&prm.tmW, VF_BF16, q->B, dimsW, strW, boxW)) != VF_OK) return rc;
-    prm.bias = q->bias_mode == VF_BIAS_N ? q->bias : nullptr;
-    prm.residual = q->residual;
-    prm.C_f32 = q->C_f32;
-    prm.C_bf16 = reinterpret_cast<__nv_bfloat16*>(q->C_bf16);
-    if (q->norm_mean_rstd) {
-        VF_CHECK_ARG(q->norm_gamma && q->norm_beta && q->norm_groups > 0 && q->Cin % q->norm_groups == 0,
-                     "vf_tc_gemm: fused input GroupNorm needs gamma, beta and a group count dividing Cin");
-        prm.norm_mr = reinterpret_cast<const float2*>(q->norm_mean_rstd);
-        prm.norm_gamma = q->norm_gamma;
-        prm.norm_beta = q->norm_beta;
-        prm.norm_groups = q->norm_groups;
-        prm.norm_cpg = q->Cin / q->norm_groups;
-        prm.norm_swish = q->norm_swish;
-    }
-    prm.N = q->N; prm.H = q->H; prm.W = q->W; prm.Cout = q->Ncols; prm.cin_blocks = q->Cin / 64;
-    prm.tiles_x = (q->W + WIDE_TW - 1) / WIDE_TW;
-    prm.tiles_y = (q->H + WIDE_TH - 1) / WIDE_TH;
-    prm.tiles_c = q->Ncols / 128;
-    const long long total = (long long)prm.tiles_x * prm.tiles_y * prm.tiles_c * q->N;
-    VF_CHECK_ARG(total > 0 && total < (1ll << 31), "vf_tc_gemm: tile count out of range");
-    prm.total_tiles = (int)total;
-    prm.idesc = make_idesc(false, 128, 256, exact);
-    prm.dbg = g_tc_dbg;
-    prm.dbg_flags = g_tc_dbg_flags;
-    prm.kc = 3;
-    if (exact) {
-        static int kc_env = -1;
-        if (kc_env < 0) { const char* e = getenv("VF_EXACT_KC"); kc_env = e ? atoi(e) : 3; if (kc_env != 1 && kc_env != 3 && kc_env != 9) kc_env = 3; }
-        prm.kc = kc_env;
-        VF_CHECK_ARG(!q->norm_mean_rstd && !q->C_bf16 && q->C_f32, "vf_tc_gemm: the exact (split-fp16) conv writes fp32 and has no fused input norm");
-    }
-    if (q->gn_sums) {
-        const int cpg = q->Ncols / q->gn_groups;
-        prm.gn_sums = q->gn_sums;
-        prm.gn_groups = q->gn_groups;
-        prm.gn_cpg = cpg;
-        cudaError_t e = cudaMemsetAsync(q->gn_sums, 0, sizeof(double) * 2 * q->gn_groups * q->N, st);
-        if (e != cudaSuccess) { vf_set_error("vf_tc_gemm: memset gn_sums: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
-    }
-    static vf_per_device_flag configured_pd;          // function attributes are per device
-    bool& configured = configured_pd.current();
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(tc_conv3x3_wide_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_conv3x3_wide_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_conv3x3_wide_kernel<16, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM);
-        if (e != cudaSuccess) { vf_set_error("vf_tc_gemm: cudaFuncSetAttribute(wide): %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
-        configured = true;
-    }
-    static int num_sms = 0;
-    if (num_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
-    }
-    const unsigned grid = (unsigned)(total < num_sms ? total : num_sms);
-    if (exact) tc_conv3x3_wide_kernel<16, false, true><<<grid, 64 + 32 * 16, WIDE_SMEM, st>>>(prm);
-    else if (prm.norm_mr) tc_conv3x3_wide_kernel<8, true><<<grid, 64 + 32 * 8 + 32 * WIDE_XFORM_WARPS, WIDE_SMEM, st>>>(prm);
-    else tc_conv3x3_wide_kernel<16, false><<<grid, 64 + 32 * 16, WIDE_SMEM, st>>>(prm);
-    VF_CHECK_LAUNCH("vf_tc_gemm(wide conv)");
-    return VF_OK;
-}
-
-
-// un-batched bf16 linear layers (features % 128 == 0) go to the wide-tile GEMM
-static bool gemm_wide_eligible(const vf_tc_gemm_t* q, long long* M_flat) {
-    static int enabled = -1;
-    if (enabled < 0) { const char* e = getenv("VF_TC_WIDE"); enabled = (e && e[0] == '0') ? 0 : 1; }
-    if (!enabled || q->conv || q->ab_dtype != VF_BF16 || q->causal_block != 0 || q->gn_sums) return false;
-    if ((q->C_f32 != nullptr) == (q->C_bf16 != nullptr)) return false;            // exactly one output dtype per instantiation
-    if (q->bias_mode == VF_BIAS_M || q->Ncols % 128 || q->K <= 0 || (q->K * 2) % 16 || (q->lda * 2) % 16 || (q->ldb * 2) % 16) return false;
-    long long M = q->M;
-    if (q->batch2 != 1) return false;
-    if (q->batch1 > 1) {        // a batch that is really one contiguous row range with a shared B
-        if (q->b_sb1 != 0 || q->a_sb1 != (long long)q->M * q->lda || q->c_sb1 != (long long)q->M * q->ldc) return false;
-        M *= q->batch1;
-    }
-    if (M < 256 || M * (long long)q->ldc >= (1ll << 31)) return false;
-    auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-    if (!a16(q->A) || !a16(q->B)) return false;
-    *M_flat = M;
-    return true;
-}
-
-static int launch_gemm_wide(const vf_tc_gemm_t* q, long long M, cudaStream_t st) {
-    WideGemmParams prm;
-    memset(&prm, 0, sizeof(prm));
-    const int es = 2;
-    int rc;
-    const uint64_t dimsW[4] = {(uint64_t)q->K, (uint64_t)q->Ncols, 1, 1};
-    const uint64_t strW[3] = {(uint64_t)q->ldb * es, (uint64_t)q->ldb * es * q->Ncols, (uint64_t)q->ldb * es * q->Ncols};
-    const uint32_t boxW[4] = {64, 128, 1, 1};
-    if ((rc = make_tmap(&prm.tmW, VF_BF16, q->B, dimsW, strW, boxW)) != VF_OK) return rc;
-    const uint64_t dimsX[4] = {(uint64_t)q->K, (uint64_t)M, 1, 1};
-    const uint64_t strX[3] = {(uint64_t)q->lda * es, (uint64_t)q->lda * es * M, (uint64_t)q->lda * es * M};
-    const uint32_t boxX[4] = {64, 256, 1, 1};
-    if ((rc = make_tmap(&prm.tmX, VF_BF16, q->A, dimsX, strX, boxX)) != VF_OK) return rc;
-    const uint32_t boxX2[4] = {64, 128, 1, 1};
-    if ((rc = make_tmap(&prm.tmX2, VF_BF16, q->A, dimsX, strX, boxX2)) != VF_OK) return rc;
-    prm.bias = q->bias_mode == VF_BIAS_N ? q->bias : nullptr;
-    prm.residual = q->residual;
-    prm.C_f32 = q->C_f32;
-    prm.C_bf16 = reinterpret_cast<__nv_bfloat16*>(q->C_bf16);
-    prm.alpha = q->alpha;
-    prm.act = q->act;
-    prm.M = (int)M; prm.Nf = q->Ncols; prm.ldc = q->ldc;
-    prm.num_k_blocks = (q->K + 63) / 64;
-    prm.tiles_f = q->Ncols / 128;
-    const long long total = (long long)prm.tiles_f * ((M + 255) / 256);
-    prm.total_tiles = (int)total;
-    prm.dbg = g_tc_dbg;
-    prm.dbg_flags = g_tc_dbg_flags;
-    // CTA pairs (cta_group::2, 256 features x 256 rows per pair, 32 KB of operands per CTA and k-block instead of 48 KB): opt-in with
-    // VF_TC_WIDE2=1.  Measured on the MIGT linears (scripts/bench_kernels.py, round 2): on par with single CTAs (c_fc 855 vs 878, fc2 1021
-    // vs 1012, qk 1006 vs 1000, c_proj 549 vs 596 TFLOP/s) — the wide GEMM is not bound by operand ingest, so single CTAs stay the default.
-    static int pair_enabled = -1;
-    if (pair_enabled < 0) { const char* e = getenv("VF_TC_WIDE2"); pair_enabled = (e && e[0] == '1') ? 1 : 0; }
-    const bool k2 = pair_enabled && q->Ncols % 256 == 0 && prm.tiles_f % 2 == 0;
-    prm.idesc = make_idesc(false, k2 ? 256 : 128, 256);
-    static vf_per_device_flag configured_pd;          // function attributes are per device
-    bool& configured = configured_pd.current();
-    if (!configured) {
-        cudaError_t e = cudaSuccess;
-        auto cfg = [&](const void* f) { if (e == cudaSuccess) e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM); };
-        cfg((const void*)tc_gemm_wide_kernel<false, false, false>); cfg((const void*)tc_gemm_wide_kernel<false, true, false>);
-        cfg((const void*)tc_gemm_wide_kernel<true, false, false>); cfg((const void*)tc_gemm_wide_kernel<true, true, false>);
-        cfg((const void*)tc_gemm_wide_kernel<false, false, true>); cfg((const void*)tc_gemm_wide_kernel<false, true, true>);
-        cfg((const void*)tc_gemm_wide_kernel<true, false, true>); cfg((const void*)tc_gemm_wide_kernel<true, true, true>);
-        if (e != cudaSuccess) { vf_set_error("vf_tc_gemm: cudaFuncSetAttribute(wide gemm): %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
-        configured = true;
-    }
-    static int num_sms = 0;
-    if (num_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
-    }
-    const bool gelu = q->act == VF_ACT_GELU_ERF, b16 = q->C_bf16 != nullptr;
-    if (k2) {
-        const long long units = total / 2, pairs = units < num_sms / 2 ? units : num_sms / 2;
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3((unsigned)(2 * pairs));
-        cfg.blockDim = dim3(WIDE_THREADS);
-        cfg.dynamicSmemBytes = WG_SMEM;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
-        cudaError_t e;
-        if (gelu && b16) e = cudaLaunchKernelEx(&cfg, tc_gemm_wide_kernel<true, true, true>, prm);
-        else if (gelu) e = cudaLaunchKernelEx(&cfg, tc_gemm_wide_kernel<true, false, true>, prm);
-        else if (b16) e = cudaLaunchKernelEx(&cfg, tc_gemm_wide_kernel<false, true, true>, prm);
-        else e = cudaLaunchKernelEx(&cfg, tc_gemm_wide_kernel<false, false, true>, prm);
-        if (e != cudaSuccess) { vf_set_error("vf_tc_gemm(wide gemm): cluster launch failed: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
-        VF_CHECK_LAUNCH("vf_tc_gemm(wide gemm, pairs)");
-        return VF_OK;
-    }
-    const unsigned grid = (unsigned)(total < num_sms ? total : num_sms);
-    if (gelu && b16) tc_gemm_wide_kernel<true, true, false><<<grid, WIDE_THREADS, WG_SMEM, st>>>(prm);
-    else if (gelu) tc_gemm_wide_kernel<true, false, false><<<grid, WIDE_THREADS, WG_SMEM, st>>>(prm);
-    else if (b16) tc_gemm_wide_kernel<false, true, false><<<grid, WIDE_THREADS, WG_SMEM, st>>>(prm);
-    else tc_gemm_wide_kernel<false, false, false><<<grid, WIDE_THREADS, WG_SMEM, st>>>(prm);
-    VF_CHECK_LAUNCH("vf_tc_gemm(wide gemm)");
-    return VF_OK;
-}
-
-static bool conv_wide_eligible(const vf_tc_gemm_t* q) {
-    static int enabled = -1;
-    if (enabled < 0) { const char* e = getenv("VF_TC_WIDE"); enabled = (e && e[0] == '0') ? 0 : 1; }
-    if (!enabled || !q->conv || q->ntaps != 9 || q->OH != q->H || q->OW != q->W) return false;
-    if (!((q->ab_dtype == VF_BF16 && q->Ctot == q->Cin) || (q->ab_dtype == VF_F16X2 && q->Ctot == 2 * q->Cin))) return false;
-    if (q->Cin % 64 || q->Ncols % 128 || q->H < 32 || q->W < 8 || q->ldc != q->Ncols || q->alpha != 1.0f || q->act != VF_ACT_NONE) return false;
-    if (q->bias_mode == VF_BIAS_M) return false;
-    if ((long long)q->N * q->H * q->W * q->Ncols >= (1ll << 31)) return false;      // the epilogue indexes with 32 bits
-    for (int t = 0; t < 9; ++t)
-        if (q->tap_dy[t] != t / 3 - 1 || q->tap_dx[t] != t % 3 - 1 || q->tap_coff[t] != 0) return false;
-    if (q->gn_sums) {
-        if (q->gn_groups <= 0 || q->Ncols % q->gn_groups) return false;
-        const int cpg = q->Ncols / q->gn_groups;
-        if (cpg > 32 || (cpg & (cpg - 1)) || 32 % cpg) return false;
-    }
-    return true;
-}
-
-
-extern "C" void vf_tc_debug_flags(int f) { g_tc_dbg_flags = f; }
-// profiling aid (scripts/tc_stall_probe.py), not in the public header: MMA-issuer stall counters of the following launches ([grid][4] int64)
-extern "C" void vf_tc_debug_counters(long long* buf) { g_tc_dbg = buf; }
 
 extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     VF_CHECK_ARG(q && q->A && q->B, "vf_tc_gemm: null operand");
@@ -1888,13 +569,7 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
                           (long long)q->exact_lo_a, (long long)q->exact_lo_b);
     }
     VF_CHECK_ARG(q->bias_mode == VF_BIAS_NONE || q->bias, "vf_tc_gemm: bias pointer missing");
-    if (conv_wide_eligible(q)) return launch_conv_wide(q, vf_s(s));
-    VF_CHECK_ARG(!q->norm_mean_rstd, "vf_tc_gemm: fused input GroupNorm is only available for 3x3 stride-1 bf16 convs on maps >= 32 rows "
-                                      "(Cin %% 64 == 0, Cout %% 128 == 0)");
-    {
-        long long m_flat = 0;
-        if (gemm_wide_eligible(q, &m_flat)) return launch_gemm_wide(q, m_flat, vf_s(s));
-    }
+    VF_CHECK_ARG(!q->norm_mean_rstd || q->conv, "vf_tc_gemm: fused input GroupNorm is a convolution option");
     const bool tf32 = q->ab_dtype == VF_F32;
     const int tm_dtype = tf32 ? VF_F32 : VF_BF16;        // tensor-map element type (fp16 and bf16 move identically)
     const int es = tf32 ? 4 : 2;
@@ -1915,18 +590,10 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     prm.ldc = q->ldc;
     prm.causal_block = q->causal_block;
     prm.causal_skip_n = q->causal_skip_n;
-    prm.dbg = g_tc_dbg;
-    prm.dbg_flags = g_tc_dbg_flags;
 
-    // N tile: 128 when the problem is wide enough, else 64 (fewer wasted MMA columns / TMEM)
+    // N tile: 128 when the problem is wide enough, else 64 (fewer wasted MMA columns and accumulator registers)
     const int block_n = (q->Ncols > 64) ? 128 : 64;
-    // CTA pairs (cta_group::2, M = 256 per MMA, B tile split across the pair) for the plain un-batched GEMMs and the convolutions
-    static int two_cta_enabled = -1;
-    // measured in round 1 (profiles/r01_tc_kernel_analysis.md): at BLOCK_N = 128 the pair is on par with two single CTAs, so it is
-    // opt-in (VF_TC_2CTA=1) until the 256-wide tiles that make it pay are in
-    if (two_cta_enabled < 0) { const char* e = getenv("VF_TC_2CTA"); two_cta_enabled = (e && e[0] == '1') ? 1 : 0; }
-    const bool k2 = two_cta_enabled && !exact && block_n == 128 && q->causal_block == 0 && (q->conv || q->batch1 * q->batch2 == 1);
-    const int b_box_rows = k2 ? block_n / 2 : block_n;
+    const int b_box_rows = block_n;
     dim3 grid;
     int rc;
     if (q->conv) {
@@ -1939,12 +606,22 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         if (TH > q->OH) { TH = 1; while (TH * 2 <= q->OH) TH *= 2; }
         int TN = 128 / (TW * TH);
         // halo mode: plain stride-1 pad-1 3x3 conv on maps at least 16 rows tall -> 8x16-pixel tiles, one halo load per channel block
-        static int halo_enabled = -1;
-        if (halo_enabled < 0) { const char* e = getenv("VF_TC_HALO"); halo_enabled = (e && e[0] == '0') ? 0 : 1; }
-        bool halo = halo_enabled && !exact && q->ntaps == 9 && q->Ctot == q->Cin && q->OH == q->H && q->OW == q->W && q->OH >= 16 && q->OW >= 8;
+        bool halo = !exact && q->ntaps == 9 && q->Ctot == q->Cin && q->OH == q->H && q->OW == q->W && q->OH >= 16 && q->OW >= 8;
         for (int t = 0; halo && t < 9; ++t) halo = q->tap_dy[t] == t / 3 - 1 && q->tap_dx[t] == t % 3 - 1 && q->tap_coff[t] == 0;
         if (halo) { TW = 8; TH = 16; TN = 1; }
         prm.halo = halo ? 1 : 0;
+        if (q->norm_mean_rstd) {
+            VF_CHECK_ARG(halo && q->ab_dtype == VF_BF16 && q->H >= 32 && q->Ncols % 128 == 0 && q->Cin % 64 == 0,
+                         "vf_tc_gemm: fused input GroupNorm needs a 3x3 stride-1 bf16 conv on a map >= 32 rows (Cin %% 64 == 0, Cout %% 128 == 0)");
+            VF_CHECK_ARG(q->norm_gamma && q->norm_beta && q->norm_groups > 0 && q->Cin % q->norm_groups == 0,
+                         "vf_tc_gemm: fused input GroupNorm needs gamma, beta and a group count dividing Cin");
+            prm.norm_mr = reinterpret_cast<const float2*>(q->norm_mean_rstd);
+            prm.norm_gamma = q->norm_gamma;
+            prm.norm_beta = q->norm_beta;
+            prm.norm_groups = q->norm_groups;
+            prm.norm_cpg = q->Cin / q->norm_groups;
+            prm.norm_swish = q->norm_swish;
+        }
         VF_CHECK_ARG(TW * TH * TN == 128 && TN <= 256, "vf_tc_gemm: cannot tile %dx%d output", q->OH, q->OW);
         prm.TW = TW; prm.TH = TH; prm.TN = TN;
         prm.tiles_x = (q->OW + TW - 1) / TW;
@@ -2021,7 +698,7 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         grid = dim3((q->M + BLOCK_M - 1) / BLOCK_M, (q->Ncols + block_n - 1) / block_n, q->batch1 * q->batch2);
     }
     // persistent launch: `grid` so far is the tile space (m tiles, n tiles, batches); one CTA per SM walks it, n fastest
-    prm.tiles_m = k2 ? (int)((grid.x + 1) / 2) : (int)grid.x;      // 2-CTA: pairs of M tiles
+    prm.tiles_m = (int)grid.x;
     prm.tiles_n = (int)grid.y;
     const long long total = (long long)prm.tiles_m * grid.y * grid.z;
     VF_CHECK_ARG(total > 0 && total < (1ll << 31), "vf_tc_gemm: tile count out of range");
@@ -2030,11 +707,9 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     if (num_sms == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
+        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
     }
-    const long long sched_units = k2 ? num_sms / 2 : num_sms;       // persistent CTAs (or CTA pairs)
-    const dim3 pgrid((unsigned)((total < sched_units ? total : sched_units) * (k2 ? 2 : 1)), 1, 1);
-    prm.idesc = make_idesc(tf32, k2 ? 2 * BLOCK_M : BLOCK_M, block_n, exact);
+    const dim3 pgrid((unsigned)(total < num_sms ? total : num_sms), 1, 1);      // persistent CTAs
     {
         auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
         auto a8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };
@@ -2058,7 +733,7 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         if (e != cudaSuccess) { vf_set_error("vf_tc_gemm: memset gn_sums: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
     }
     cudaStream_t st = vf_s(s);
-    if (k2) return tf32 ? launch<128, 6, true, true>(prm, pgrid, st) : launch<128, 6, false, true>(prm, pgrid, st);
-    if (block_n == 128) return tf32 ? launch<128, 4, true, false>(prm, pgrid, st) : launch<128, 4, false, false>(prm, pgrid, st);
-    return tf32 ? launch<64, 6, true, false>(prm, pgrid, st) : launch<64, 6, false, false>(prm, pgrid, st);
+    const WgKind kind = tf32 ? TF32 : (exact ? F16 : BF16);
+    if (block_n == 128) return launch_kind<128, 4>(prm, kind, pgrid, st);
+    return launch_kind<64, 6>(prm, kind, pgrid, st);
 }

@@ -1,13 +1,13 @@
-// Fused codebook lookup on tcgen05 (sm_100a):  idx[m] = argmin_k |z_m - e_k|^2   — viewformer/models/utils_th.py:34-41.
+// Fused codebook lookup on Hopper tensor cores (sm_90a, wgmma):  idx[m] = argmin_k |z_m - e_k|^2   — viewformer/models/utils_th.py:34-41.
 //
 // HBM traffic is the algorithmic minimum: every z row (fp32, 4*D bytes) is read ONCE, one int64 index is written; the distance
-// matrix never exists outside TMEM.  Per CTA PAIR (thread-block cluster of 2 = one `cta_group::2` MMA of M = 256):
-//   converter warps   z fp32 [128 rows x D] --LDG.128--> fp16 --> 128B-swizzled K-major A tile in shared memory (double-buffered);
+// matrix never exists outside registers.  Per CTA and 128-row tile (persistent CTAs walk the tiles):
+//   convert (8 warps) z fp32 [128 rows x D] --LDG.128--> fp16 --> 128B-swizzled K-major A tile in shared memory;
 //                     also |z|^2 per row and a range check (|z_i| beyond fp16 -> the row goes to the exact path)
-//   TMA producer      B stages: this CTA's HALF (128 codes x 64 k) of a 256-code sub-tile of Eh = fp16(-2 e)   [K, D] K-major
-//   MMA issuer        (leader CTA) S[256 rows, 256 codes] = A . B^T into one of two TMEM stages (fp32), 4 sub-tiles per row tile
-//   epilogue warps    TMEM -> registers: s = S + |e|^2 (fp32, shared memory table), the code index is packed into the 6 low mantissa
-//                     bits and a running (min, second min) pair per (row, 64-code set) is kept with 3 FMNMX per score
+//   TMA producer      B stages (256 codes x 64 k) of Eh = fp16(-2 e)   [K, D] K-major, running ahead across sub-tiles and tiles
+//   MMA (2 warpgroups) S[64 rows, 256 codes] = A . B^T per warpgroup and sub-tile, fp32 in registers; s = S + |e|^2 (fp32, shared
+//                     memory table), the code index is packed into the 6 low mantissa bits and a running (min, second min) pair
+//                     per (row, 64-code set) is kept with integer min / max, merged over the 4 lanes that share a row
 //   merge (4 warps)   per row: best code over the 16 sets; if the runner-up lies within the fp16 rounding bound of the best the row
 //                     is queued for the exact pass (PAIR: both candidates known; FULL: a third may hide inside one set)
 // vq_rescue_kernel then settles queued rows in fp64 (direct sum of squared differences, ties to the smaller index — the same rule as
@@ -16,26 +16,25 @@
 // Rounding model (why the tolerance is safe): fp16 operands carry 11 significand bits, |d(z.e)| <= 2^-10 sum|z_i e_i| <= 2^-10 |z||e|;
 // the score -2 z.e + |e|^2 of two codes therefore moves by at most 2^-9 |z| (|e_a| + |e_b|) against each other (worst case, all
 // roundings aligned; rms is ~40x smaller).  `tol_factor` scales that bound (1.0 = worst case; default 0.25 = ~10 sigma); index
-// packing (6 mantissa bits) and the truncating TMEM accumulation add 2^-16 |s| which is always included unscaled.
-#include "vf_tcgen05.cuh"
+// packing (6 mantissa bits) and the truncating tensor-core accumulation add 2^-16 |s| which is always included unscaled.
+#include "vf_wgmma.cuh"
 #include <cuda_fp16.h>
 
 namespace {
 using namespace vftc;
 
-constexpr int TM = 128;                 // z rows per CTA tile (256 per pair)
+constexpr int TM = 128;                 // z rows per CTA tile
 constexpr int TN = 256;                 // codes per sub-tile (MMA N)
 constexpr int KB_BYTES = TM * 128;      // one A k-block: 128 rows x 128 B
 constexpr int A_BYTES = 4 * KB_BYTES;   // up to D = 256
-constexpr int B_STAGE = 128 * 128;      // this CTA's half of a (256 codes x 64 k) stage
+constexpr int B_STAGE = TN * 128;       // one (256 codes x 64 k) stage
 constexpr int B_STAGES = 4;
-constexpr int NCONV = 8, NEPI = 16;
-constexpr int THREADS = 64 + 32 * (NCONV + NEPI);      // 832
-constexpr int CONV_W0 = 2, EPI_W0 = 2 + NCONV;
+constexpr int NCONV = 8;                // converter warps (= the MMA warps)
+constexpr int MMA_THREADS = 32 * NCONV;
+constexpr int THREADS = MMA_THREADS + 128;     // + the producer warpgroup (one elected thread issues TMA; see setmaxnreg_dec)
 constexpr int MAXK = 1024;
-constexpr int RES_BYTES = 4 * TM * 16;     // per tile: 4 column groups x 128 rows x (3 best keys + pad), double-buffered
-constexpr int ZRING = 4;                // |z|^2 / range-flag ring (the merge of tile t reads them after the converters moved on)
-constexpr int SMEM = 2 * A_BYTES + B_STAGES * B_STAGE + MAXK * 4 + ZRING * TM * 4 * 2 + 2 * RES_BYTES + 512 + 1024;
+constexpr int RES_BYTES = 4 * TM * 16;  // 4 column groups x 128 rows x (3 best keys + pad)
+constexpr int SMEM = A_BYTES + B_STAGES * B_STAGE + MAXK * 4 + TM * 4 * 2 + RES_BYTES + 8 * 2 * B_STAGES + 1024;
 
 struct VqParams {
     CUtensorMap tmB;            // Eh [K, D] fp16: box {64, 128}
@@ -43,67 +42,16 @@ struct VqParams {
     const float* esq;           // [K]
     long long M;
     int D, K, kblocks, nsub;
-    long long n_pair_tiles;     // ceil(M / 256)
+    long long n_tiles;          // ceil(M / 128)
     float tol_factor;
     int key_mul;                // 256, passed as data so the key is ONE IMAD (fma pipe) instead of a shift + add on the alu pipe
     long long* idx;             // [M]
     int4* worklist;             // {row, c1, c2 (-1: all codes), 0}
     int* counter;               // [0] queued rows, [1] of which FULL
-    unsigned idesc;
 };
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_cta(const void* p, uint32_t cta) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(p)), "r"(cta));
-    return ra;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// arrival without a memory payload (TMEM stage hand-back: ordered by tcgen05.fence::before_thread_sync): no cluster-scope release
-// fence — `mbarrier.arrive.release.cluster` costs an ERRBAR per warp per sub-tile (26 % of the epilogue's stall samples in ncu)
-__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {      // acquire at cluster scope: the peer CTA's arrivals
-    for (uint32_t i = 0; i < (1u << 24); ++i) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (ok) return;
-    }
-    printf("vq_fused: cluster mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-    __trap();
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* tm, uint32_t leader_bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void commit_2sm(uint64_t* bar) {       // arrives on the same barrier offset in both CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void umma_2sm_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
 
 // explicit shared-state-space accesses: pointers derived from the aligned dynamic-smem base are "generic" to the compiler, and a
 // generic LD to shared memory is tracked on the long scoreboard like a global load
-__device__ __forceinline__ float4 lds_f4(uint32_t addr) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
 __device__ __forceinline__ uint4 lds_u4(uint32_t addr) {
     uint4 v;
     asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
@@ -121,34 +69,20 @@ __device__ __forceinline__ float lds_f(uint32_t addr) {
 __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __grid_constant__ VqParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* sA = smem;                                          // [2][A_BYTES]
-    uint8_t* sB = sA + 2 * A_BYTES;                              // [B_STAGES][B_STAGE]
+    uint8_t* sA = smem;                                          // [A_BYTES]
+    uint8_t* sB = sA + A_BYTES;                                  // [B_STAGES][B_STAGE]
     float* esq_s = reinterpret_cast<float*>(sB + B_STAGES * B_STAGE);            // [MAXK]
-    float* zz_s = esq_s + MAXK;                                  // [ZRING][TM]
-    int* bad_s = reinterpret_cast<int*>(zz_s + ZRING * TM);      // [ZRING][TM]
-    uint8_t* res_s = reinterpret_cast<uint8_t*>(bad_s + ZRING * TM);             // [2][4 groups][TM] x uint4 (3 best keys of the thread)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(res_s + 2 * RES_BYTES);
-    uint64_t* b_full = bars;                    // [B_STAGES]  (leader's copy is the one that counts)
-    uint64_t* b_empty = b_full + B_STAGES;      // [B_STAGES]
-    uint64_t* a_ready = b_empty + B_STAGES;     // [2]  leader: 2 * NCONV arrivals
-    uint64_t* a_free = a_ready + 2;             // [2]  multicast commit
-    uint64_t* t_full = a_free + 2;              // [2]  multicast commit
-    uint64_t* t_empty = t_full + 2;             // [2]  leader: 2 * NEPI arrivals
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
+    float* zz_s = esq_s + MAXK;                                  // [TM]
+    int* bad_s = reinterpret_cast<int*>(zz_s + TM);              // [TM]
+    uint8_t* res_s = reinterpret_cast<uint8_t*>(bad_s + TM);     // [4 groups][TM] x uint4 (3 best keys of the (row, group))
+    uint64_t* b_full = reinterpret_cast<uint64_t*>(res_s + RES_BYTES);          // [B_STAGES]
+    uint64_t* b_empty = b_full + B_STAGES;                       // [B_STAGES]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const long long pair0 = blockIdx.x >> 1, pair_stride = gridDim.x >> 1;
 
-    if (threadIdx.x == 0) prefetch_tmap(&p.tmB);
-    if (threadIdx.x == 32) {
-        for (int s = 0; s < B_STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(&a_ready[a], 2 * NCONV);
-            mbar_init(&a_free[a], 1);
-            mbar_init(&t_full[a], 1);
-            mbar_init(&t_empty[a], 2 * NEPI);
-        }
+    if (threadIdx.x == 0) {
+        prefetch_tmap(&p.tmB);
+        for (int s = 0; s < B_STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], MMA_THREADS); }
         mbar_fence_init();
     }
     // Fixed-point scores: with C = 1.5 * 2^k and |score| < 2^(k-1), the fp32 sum  t = acc + (|e|^2 + C)  stays inside the binade [2^k, 2^(k+1)),
@@ -176,80 +110,52 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
     const float zcap = (half_range - esqmax) / (2.02f * sqrtf(esqmax));        // 2 |z| |e| (1 + 2^-10 ...) + |e|^2 < 2^(kexp - 1)
     const float zz_cap = codebook_ok ? fminf(zcap * zcap, 3.6e9f) : -1.0f;     // |z_i| <= |z| < 60000: inside the fp16 range
     for (int i = threadIdx.x; i < p.K; i += THREADS) esq_s[i] = __ldg(p.esq + i) + c_off;
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ===================== TMA producer: this CTA's half of every B stage =====================
-        if (elect_one()) {
-            const uint32_t lead_full = mapa_cta(b_full, 0);
+    if (warp >= MMA_THREADS / 32) {
+        // ===================== TMA producer: every B stage (256 codes x 64 k) =====================
+        setmaxnreg_dec<40>();
+        if (warp == MMA_THREADS / 32 && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
-            for (long long t = pair0; t < p.n_pair_tiles; t += pair_stride) {
+            for (long long t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
                 for (int n = 0; n < p.nsub; ++n)
                     for (int kb = 0; kb < p.kblocks; ++kb) {
                         mbar_wait(&b_empty[stage], phase ^ 1, "vq_fused(b_empty)");
-                        if (rank == 0) mbar_expect_tx(&b_full[stage], 2 * B_STAGE);
-                        tma_load_4d_2sm(sB + stage * B_STAGE, &p.tmB, lead_full + (uint32_t)(stage * 8), kb * 64, n * TN + (int)rank * 128, 0, 0);
+                        mbar_expect_tx(&b_full[stage], B_STAGE);
+                        tma_load_4d(sB + stage * B_STAGE, &p.tmB, &b_full[stage], kb * 64, n * TN, 0, 0);
                         if (++stage == B_STAGES) { stage = 0; phase ^= 1; }
                     }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader CTA issues for the pair) =====================
-        if (rank == 0 && elect_one()) {
-            int stage = 0, it = 0, tl = 0;
-            uint32_t phase = 0;
-            for (long long t = pair0; t < p.n_pair_tiles; t += pair_stride, ++tl) {
-                const int ab = tl & 1;
-                mbar_wait_cluster(&a_ready[ab], (tl >> 1) & 1);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(sA + ab * A_BYTES);
-                for (int n = 0; n < p.nsub; ++n) {
-                    const int acc = it & 1;
-                    mbar_wait_cluster(&t_empty[acc], ((it >> 1) & 1) ^ 1);
-                    tc_fence_after();
-                    const uint32_t tmem_d = tmem_base + (uint32_t)(acc * TN);
-                    for (int kb = 0; kb < p.kblocks; ++kb) {
-                        mbar_wait(&b_full[stage], phase, "vq_fused(b_full)");
-                        tc_fence_after();
-                        const uint64_t adesc = sw128_desc(a_addr + kb * KB_BYTES), bdesc = sw128_desc(smem_u32(sB + stage * B_STAGE));
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) umma_2sm_f16(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), p.idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                        commit_2sm(&b_empty[stage]);
-                        if (++stage == B_STAGES) { stage = 0; phase ^= 1; }
-                    }
-                    commit_2sm(&t_full[acc]);
-                    ++it;
-                }
-                commit_2sm(&a_free[ab]);
-            }
-        }
-    } else if (warp < EPI_W0) {
-        // ===================== converters: z fp32 -> fp16 swizzled A tile, |z|^2, range check =====================
-        const int cw = warp - CONV_W0;
-        const uint32_t lead_ready = mapa_cta(a_ready, 0);
-        const int kb = lane >> 3, ch = lane & 7;                  // this lane's 8 elements of a row: k = kb*64 + ch*8 ..
-        const bool lane_ok = lane * 8 < p.D;
-        int tl = 0;
-        for (long long t = pair0; t < p.n_pair_tiles; t += pair_stride, ++tl) {
-            const int ab = tl & 1;
-            mbar_wait(&a_free[ab], ((tl >> 1) & 1) ^ 1, "vq_fused(a_free)");
-            uint8_t* At = sA + ab * A_BYTES;
-            const long long row0 = t * 256 + (long long)rank * TM;
+        return;
+    }
+
+    // ===================== warps 0..7: convert, MMA (warpgroup wg = rows [64 wg, +64)), top-2 per (row, 64-code set), merge ==========
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);     // accumulator rows r0, r0 + 8 (layout: vf_wgmma.cuh)
+    const int c_ln = 2 * (lane & 3);
+    const int my_g = lane & 3;                                   // the 64-code column group whose keys this lane folds
+    const uint32_t esq_a = smem_u32(esq_s), res_a = smem_u32(res_s);
+    const int EMPTY = 0x7fffffff;
+    const int key_mul = p.key_mul;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[TN / 2];
+    for (long long t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
+        named_sync(1, MMA_THREADS);                              // the previous tile's merge is done with sA, zz_s, bad_s, res_s
+        // ---- converters: z fp32 -> fp16 swizzled A tile, |z|^2, range check
+        {
+            const int kb = lane >> 3, ch = lane & 7;              // this lane's 8 elements of a row: k = kb*64 + ch*8 ..
+            const bool lane_ok = lane * 8 < p.D;
+            const long long row0 = t * TM;
 #pragma unroll 1
             for (int rb = 0; rb < TM / NCONV; rb += 4) {           // 4 rows of this warp in flight: 8 x LDG.128 per lane
                 float4 v[4][2];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
-                    const int r = cw + (rb + u) * NCONV;
+                    const int r = warp + (rb + u) * NCONV;
                     const long long gr = row0 + r;
                     if (gr < p.M && lane_ok) {
                         const float4* src = reinterpret_cast<const float4*>(p.z + gr * p.D + lane * 8);
@@ -261,7 +167,7 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
                 }
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
-                    const int r = cw + (rb + u) * NCONV;
+                    const int r = warp + (rb + u) * NCONV;
                     const float e[8] = {v[u][0].x, v[u][0].y, v[u][0].z, v[u][0].w, v[u][1].x, v[u][1].y, v[u][1].z, v[u][1].w};
                     float ss = 0.f;
                     uint32_t w[4];
@@ -273,86 +179,91 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
                         w[q] = *reinterpret_cast<const uint32_t*>(&h);
                     }
                     if (lane_ok)
-                        *reinterpret_cast<uint4*>(At + kb * KB_BYTES + r * 128 + ((ch ^ (r & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
+                        *reinterpret_cast<uint4*>(sA + kb * KB_BYTES + r * 128 + ((ch ^ (r & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
                     ss = warp_sum(ss);
                     if (lane == 0) {
-                        zz_s[(tl & (ZRING - 1)) * TM + r] = ss;
+                        zz_s[r] = ss;
                         // |z|^2 below the cap keeps every element inside the fp16 range and every score inside the fixed-point range;
                         // NaN / inf fail the comparison too.  Rows that fail are decided by the exact pass.
-                        bad_s[(tl & (ZRING - 1)) * TM + r] = !(ss < zz_cap);
+                        bad_s[r] = !(ss < zz_cap);
                     }
                 }
             }
-            fence_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(lead_ready + (uint32_t)(ab * 8));
         }
-    } else {
-        // ===================== epilogue: top-2 per (row, 64-code set) straight from TMEM =====================
-        const int quarter = warp & 3;                             // TMEM lanes [32q, 32q+32)
-        const int grp = (warp - EPI_W0) >> 2;                     // columns [64g, 64g+64) of every sub-tile
-        const int row = quarter * 32 + lane;
-        const uint32_t lead_empty = mapa_cta(t_empty, 0);
-        const uint32_t esq_a = smem_u32(esq_s), res_a = smem_u32(res_s);
-        const int EMPTY = 0x7fffffff;
-        const int key_mul = p.key_mul;
-        int it = 0, tl = 0;
-        for (long long t = pair0; t < p.n_pair_tiles; t += pair_stride, ++tl) {
-            int t1 = EMPTY, t2 = EMPTY, t3 = EMPTY;               // this thread's three best keys over its 4 sets (8-bit index: n | h | j)
-            for (int n = 0; n < p.nsub; ++n) {
-                const int acc = it & 1;
-                mbar_wait(&t_full[acc], (it >> 1) & 1, "vq_fused(t_full)");
-                ++it;
-                tc_fence_after();
-                int m1 = EMPTY, m2 = EMPTY;
+        fence_async_smem();                                      // generic-proxy A tile -> visible to wgmma
+        named_sync(1, MMA_THREADS);
+
+        // ---- S = A . B^T per 256-code sub-tile, then this thread's keys
+        int tk[2][3] = {{EMPTY, EMPTY, EMPTY}, {EMPTY, EMPTY, EMPTY}};     // three best keys of (row r0 + 8 hh, group my_g) over the sets
+        const uint32_t a_addr = smem_u32(sA) + (uint32_t)(wg * 64 * 128);
+        for (int n = 0; n < p.nsub; ++n) {
+            for (int kb = 0; kb < p.kblocks; ++kb) {
+                mbar_wait(&b_full[stage], phase, "vq_fused(b_full)");
+                const uint64_t adesc = sw128_desc(a_addr + kb * KB_BYTES), bdesc = sw128_desc(smem_u32(sB + stage * B_STAGE));
+                wgmma_fence();
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * TN + grp * 64 + h * 32), r);
-                    if (h == 1) {
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster_relaxed(lead_empty + (uint32_t)(acc * 8));
+                for (int k = 0; k < 4; ++k) wgmma_ss<TN, F16>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(acc);
+                mbar_arrive(&b_empty[stage]);
+                if (++stage == B_STAGES) { stage = 0; phase ^= 1; }
+            }
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+                for (int g = 0; g < 4; ++g) {
+                    int m1 = EMPTY, m2 = EMPTY;
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) {
+                        const int col = 64 * g + 8 * jj + c_ln;                                   // column of acc[4 j + 2 hh], j = 8 g + jj
+                        const float2 e = *reinterpret_cast<const float2*>(esq_s + n * TN + col);
+                        const int tb0 = __float_as_int(acc[4 * (8 * g + jj) + 2 * hh] + e.x);     // score + C, one binade
+                        const int tb1 = __float_as_int(acc[4 * (8 * g + jj) + 2 * hh + 1] + e.y);
+                        const int k0 = tb0 * key_mul + (col & 63), k1 = tb1 * key_mul + (col & 63) + 1;    // low byte = index in the set
+                        m2 = min(m2, max(m1, k0));
+                        m1 = min(m1, k0);
+                        m2 = min(m2, max(m1, k1));
+                        m1 = min(m1, k1);
                     }
-                    const uint32_t ea = esq_a + (uint32_t)((n * TN + grp * 64 + h * 32) * 4);
+                    // the set's 64 codes are spread over the 4 lanes of the row: merge their (best, second best) pairs
 #pragma unroll
-                    for (int j4 = 0; j4 < 8; ++j4) {
-                        const float4 e = lds_f4(ea + j4 * 16);
-                        const float ev[4] = {e.x, e.y, e.z, e.w};
+                    for (int o = 1; o < 4; o <<= 1) {
+                        const int b1 = __shfl_xor_sync(0xffffffffu, m1, o), b2 = __shfl_xor_sync(0xffffffffu, m2, o);
+                        m2 = min(max(m1, b1), min(m2, b2));
+                        m1 = min(m1, b1);
+                    }
+                    if (g == my_g) {
+                        // fold the set's two best into the three best of (row, group) (set number into bits 6..7 of the index)
 #pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            const int j = j4 * 4 + q;
-                            const int tb = __float_as_int(__uint_as_float(r[j]) + ev[q]);     // FADD (fma pipe): score + C, one binade
-                            const int k = tb * key_mul + (h * 32 + j);                        // IMAD (fma pipe): low byte = index
-                            m2 = min(m2, max(m1, k));
-                            m1 = min(m1, k);
+                        for (int q = 0; q < 2; ++q) {
+                            const int mk = q ? m2 : m1;
+                            const int k = mk == EMPTY ? EMPTY : (mk | (n << 6));                  // bits 6..7 of the index byte are zero so far
+                            const int a = max(tk[hh][0], k);
+                            tk[hh][0] = min(tk[hh][0], k);
+                            const int b2 = max(tk[hh][1], a);
+                            tk[hh][1] = min(tk[hh][1], a);
+                            tk[hh][2] = min(tk[hh][2], b2);
                         }
                     }
                 }
-                // fold the set's two best into the thread's three best (set number into bits 6..7 of the index)
-#pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    const int mk = q ? m2 : m1;
-                    const int k = mk == EMPTY ? EMPTY : (mk | (n << 6));                      // bits 6..7 of the index byte are zero so far
-                    const int a = max(t1, k);
-                    t1 = min(t1, k);
-                    const int b2 = max(t2, a);
-                    t2 = min(t2, a);
-                    t3 = min(t3, b2);
-                }
             }
-            const uint32_t rbuf = res_a + (uint32_t)((tl & 1) * RES_BYTES);
-            sts_u4(rbuf + (uint32_t)((grp * TM + row) * 16), make_uint4((uint32_t)t1, (uint32_t)t2, (uint32_t)t3, 0u));
-            asm volatile("bar.sync 1, %0;" ::"n"(32 * NEPI) : "memory");                        // the tile's keys are in res_s[tl & 1]
-            if (grp == 0) {
-                const long long gr = t * 256 + (long long)rank * TM + row;
-                if (gr < p.M) {
-                    uint32_t ks[12];
+        }
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        const uint4 v = lds_u4(rbuf + (uint32_t)((g * TM + row) * 16));
-                        ks[3 * g] = v.x; ks[3 * g + 1] = v.y; ks[3 * g + 2] = v.z;
-                    }
+        for (int hh = 0; hh < 2; ++hh)
+            sts_u4(res_a + (uint32_t)((my_g * TM + r0 + 8 * hh) * 16), make_uint4((uint32_t)tk[hh][0], (uint32_t)tk[hh][1], (uint32_t)tk[hh][2], 0u));
+        named_sync(1, MMA_THREADS);                              // the tile's keys are in res_s
+        // ---- merge (threads 0..127, thread = row): best code over the sets; rows whose runner-up is within the bound are queued
+        if (threadIdx.x < TM) {
+            const int row = threadIdx.x;
+            const long long gr = t * TM + row;
+            if (gr < p.M) {
+                uint32_t ks[12];
+#pragma unroll
+                for (int g = 0; g < 4; ++g) {
+                    const uint4 v = lds_u4(res_a + (uint32_t)((g * TM + row) * 16));
+                    ks[3 * g] = v.x; ks[3 * g + 1] = v.y; ks[3 * g + 2] = v.z;
+                }
                     // key -> (value, code, set): value = ((key - key0) >> 8) * G, code = n*256 + g*64 + idx6, set = n*4 + g
                     const float vscale = g_step * 0.00390625f;            // G / 256
                     float bv = __int_as_float(0x7f800000);
@@ -365,8 +276,8 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
                         const int c = n * TN + g * 64 + (int)(k & 63u);
                         if (k != 0x7fffffffu && (v < bv || (v == bv && c < bc))) { bv = v; bc = c; bset = n * 4 + g; }
                     }
-                    const uint32_t zslot = (uint32_t)(((tl & (ZRING - 1)) * TM + row) * 4);
-                    bool bad = *reinterpret_cast<volatile int*>(bad_s + (tl & (ZRING - 1)) * TM + row) != 0;
+                    const uint32_t zslot = (uint32_t)(row * 4);
+                    bool bad = bad_s[row] != 0;
                     if (bset < 0) { bc = 0; bad = true; }
                     const float znorm = sqrtf(lds_f(smem_u32(zz_s) + zslot));
                     const float eb = sqrtf(__ldg(p.esq + bc));
@@ -380,7 +291,7 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
                         const int n = (int)((k >> 6) & 3u), g = i / 3;
                         const int c = n * TN + g * 64 + (int)(k & 63u);
                         if (c == bc) { inside |= 1u << i; continue; }
-                        // truncating TMEM accumulation (2^-16 relative, generous) + the fixed-point step of both scores
+                        // truncating tensor-core accumulation (2^-16 relative, generous) + the fixed-point step of both scores
                         const float slack = 1.52587891e-5f * (fabsf(v) + fabsf(bv)) + 4.0f * g_step;
                         const float tol = p.tol_factor * 0.001953125f * znorm * (eb + sqrtf(__ldg(p.esq + c))) + slack;
                         if (v - bv <= tol) { ++within; inside |= 1u << i; oc = c; oset = n * 4 + g; }
@@ -404,17 +315,8 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
                         if (!pair) p.worklist[p.M - 1 - atomicAdd(p.counter + 1, 1)] = make_int4((int)gr, bc, -1, (int)mask);
                         else p.worklist[atomicAdd(p.counter, 1)] = make_int4((int)gr, bc, oc, 0);
                     }
-                }
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
     }
 }
 
@@ -615,18 +517,17 @@ extern "C" int vf_vq_lookup_fused(const float* z, const void* Eh_f16, const floa
     memset(&prm, 0, sizeof(prm));
     const uint64_t dims[4] = {(uint64_t)D, (uint64_t)K, 1, 1};
     const uint64_t str[3] = {(uint64_t)D * 2, (uint64_t)D * 2 * K, (uint64_t)D * 2 * K};
-    const uint32_t box[4] = {64, 128, 1, 1};
+    const uint32_t box[4] = {64, (uint32_t)TN, 1, 1};
     int rc;
     if ((rc = make_tmap_16bit(&prm.tmB, Eh_f16, dims, str, box)) != VF_OK) return rc;
     prm.z = z; prm.esq = esq; prm.M = M; prm.D = D; prm.K = K;
     prm.kblocks = D / 64; prm.nsub = K / TN;
-    prm.n_pair_tiles = (M + 255) / 256;
+    prm.n_tiles = (M + TM - 1) / TM;
     prm.tol_factor = tol_factor;
     prm.key_mul = 256;
     prm.idx = reinterpret_cast<long long*>(idx);
     prm.worklist = reinterpret_cast<int4*>(worklist);
     prm.counter = counter;
-    prm.idesc = make_idesc_16bit(0, 256, TN);
     cudaError_t e = cudaMemsetAsync(counter, 0, 2 * sizeof(int), st);
     if (e != cudaSuccess) { vf_set_error("vf_vq_lookup_fused: memset: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
     static vf_per_device_flag configured_pd;          // function attributes are per device
@@ -640,24 +541,10 @@ extern "C" int vf_vq_lookup_fused(const float* z, const void* Eh_f16, const floa
     if (num_sms == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
+        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
     }
-    long long pairs = prm.n_pair_tiles < num_sms / 2 ? prm.n_pair_tiles : num_sms / 2;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(2 * pairs));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SMEM;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, vq_lookup_fused_kernel, prm);
-    if (e != cudaSuccess) { vf_set_error("vf_vq_lookup_fused: cluster launch failed: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
+    const unsigned grid = (unsigned)(prm.n_tiles < num_sms ? prm.n_tiles : num_sms);       // persistent CTAs
+    vq_lookup_fused_kernel<<<grid, THREADS, SMEM, st>>>(prm);
     VF_CHECK_LAUNCH("vf_vq_lookup_fused");
     vq_rescue_kernel<<<num_sms * 8, 256, 0, st>>>(z, Et, E_dk, esq, D, K, M, prm.worklist, counter, prm.idx);
     VF_CHECK_LAUNCH("vf_vq_lookup_fused(rescue)");

@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing: one process per GPU, torch.distributed (NCCL on B200, gloo in CPU tests).
+"""Multi-GPU plumbing: one process per GPU, torch.distributed (NCCL on the GPUs, gloo in CPU tests).
 
 Inference shards scenes across ranks with NO data-path collective (scenes are independent, SURVEY.md §8e);
 the only exchange on the hot path is the codebook-EMA statistics of the training step, which the reference

@@ -1,4 +1,4 @@
-"""``generate()`` — the reference's novel-view synthesis entry point, B200-native.
+"""``generate()`` — the reference's novel-view synthesis entry point, H100-native.
 
 Mirrors ``generate_batch_predictions(transformer_model, codebook_model, images, cameras)`` of
 viewformer/evaluate/evaluate_transformer.py:97-146 (same argument meaning, same result dict), so that
@@ -121,7 +121,7 @@ def generate_batch_predictions(transformer_model, codebook_model, images, camera
 
 class GraphedPredictions:
     """``generate_batch_predictions`` for a fixed (scenes, views) shape, captured once into a CUDA graph and replayed: one
-    cudaGraphLaunch per batch instead of ~380 kernel launches (each tcgen05 / streaming kernel is 10-1000 us long, so the
+    cudaGraphLaunch per batch instead of ~380 kernel launches (each tensor-core / streaming kernel is 10-1000 us long, so the
     launch gaps of the eager path are ~5 % of a step).  Inputs are copied into static device buffers (from pinned host memory
     or from device tensors), outputs live in static device tensors that the next call overwrites.
 

@@ -1,4 +1,4 @@
-"""MIGT context-view transformer — B200-native drop-in for the reference's Keras ``MIGT``.
+"""MIGT context-view transformer — H100-native drop-in for the reference's Keras ``MIGT``.
 
 Surface (viewformer/models/migt.py:241-455, 532-533):
     MIGT(config).load_state_dict(sd)
@@ -216,7 +216,7 @@ class MIGT:
         if kv_out is not None:
             kv_out.append((qk, vt))                      # context K (k half of qk) and V^T of this layer: the KV cache
         if ns == 1 and prec.opd == torch.bfloat16 and dh == 64 and self.fused_attention:
-            # single-stream forward (the generate() hot path): one fused tcgen05 kernel, no S x S tensor in HBM
+            # single-stream forward (the generate() hot path): one fused wgmma kernel, no S x S tensor in HBM
             return [L.attn_block_causal(qk, vt, B, S, H, d, Lt)]
         if ns > 1 and prec.opd == torch.bfloat16 and dh == 64 and Lt == 64 and self.fused_attention:
             # 3-stream forward (multi-context generation, localisation): the same fused kernel with the multi-end key-tile schedule

@@ -1,9 +1,9 @@
 """Precision policy + operator dispatch shared by the VQGAN and MIGT host classes.
 
 Three precisions, all of them CUDA (there is no CPU path):
-  * ``bf16``  tensor-core path: bf16 operands, fp32 accumulation in TMEM (tcgen05), fp32 residual stream,
+  * ``bf16``  tensor-core path: bf16 operands, fp32 accumulation in registers (wgmma), fp32 residual stream,
               fp32 norms / softmax / argmin.  This is the benchmarked configuration.
-  * ``tf32``  same kernels with fp32 operands fed to ``tcgen05.mma.kind::tf32`` (the arithmetic the reference
+  * ``tf32``  same kernels with fp32 operands fed to ``wgmma.mma_async ... .tf32`` (the arithmetic the reference
               itself ran on A100 with torch 1.7 / TF 2.4 defaults).
   * ``fp32``  exact CUDA-core path (FFMA), used for strict parity against the oracle.
   * ``x3``    (VQGAN only) fp32-faithful 3x3 convolutions on the tensor cores (split-fp16 operands, 3 MMAs per product,

@@ -17,7 +17,7 @@ twin flat gradient buffer ordered by backward completion (decoder.conv_out first
 Activations needed by the backward pass are kept on a tape; GroupNorm+swish outputs are recomputed from the saved statistics.
 
 Arithmetic: fp32 throughout, as the reference requires.  The 3x3 stride-1 convolutions with tensor-core-sized channel counts run
-their forward pass and their data gradient on the exact split-fp16 tcgen05 kernels (fp32-faithful results from three fp16 MMA passes,
+their forward pass and their data gradient on the exact split-fp16 tensor-core kernels (fp32-faithful results from three fp16 MMA passes,
 DESIGN.md 5.3; ``VF_TRAIN_TC=0`` keeps everything on the CUDA cores), and their weight gradient as nine exact GEMMs over the pixel axis
 (``_lib.conv_wgrad_tc``) when both channel counts are multiples of 128; strided / upsampling convs, 1x1 layers and the remaining weight
 gradients use the fp32 CUDA-core kernels.
@@ -186,7 +186,7 @@ class VQGANTrainer:
                                         L._p(y), L.F32, L._stream()))
         return y
 
-    # 3x3 stride-1 convolutions whose channel counts fit the tcgen05 tiles run on the EXACT split-fp16 tensor-core path (three fp16 MMA
+    # 3x3 stride-1 convolutions whose channel counts fit the tensor-core tiles run on the EXACT split-fp16 tensor-core path (three fp16 MMA
     # passes, chunked accumulation: fp32-faithful results, DESIGN.md 5.3) in the forward pass and in the data gradient; everything else
     # (conv_in / conv_out, stride-2 and upsampling convs, 1x1 layers) and every weight gradient stays on the fp32 CUDA-core kernels.
     def _tc_ok(self, cw, stride, upsample):

@@ -1,4 +1,4 @@
-"""VQGAN codebook model — B200-native drop-in for the reference's torch ``VQGAN``.
+"""VQGAN codebook model — H100-native drop-in for the reference's torch ``VQGAN``.
 
 Surface (same names / argument meaning / return tuples as viewformer/models/vqgan_th.py:321-398):
     VQGAN(config).load_state_dict(sd)         reference key names, [Cout,Cin,kh,kw] conv weights, [D,K] codebook
@@ -66,9 +66,9 @@ class VQGAN:
         self.enc_prec, self.dec_prec = Precision(enc_name), Precision(dec_name)
         self.prec = self.dec_prec                  # quantizer / glue policy
         self.bf16_edges = True                     # bf16 halves only: conv1 -> norm2 activations travel as bf16 (see _resblock)
-        # norm2 + swish fused into conv2's operand path (vf_tc_gemm_t.norm_*): bit-identical to the two-kernel path and tested, but
-        # with two halo buffers the in-place transform serialises with the TMA load (1.53-1.62 ms against 1.25 + 0.43 ms for
-        # conv + vf_groupnorm_apply at 288 x 128^2 x 128), so it is opt-in (VF_NORM_ON_LOAD=1) until a third buffer fits
+        # norm2 + swish fused into conv2's operand path (vf_tc_gemm_t.norm_*, the halo tile is transformed in shared memory):
+        # bit-identical to the two-kernel path and tested; the MMA warpgroups do the transform between their MMAs, so it stays
+        # opt-in (VF_NORM_ON_LOAD=1) until it is measured faster than conv + vf_groupnorm_apply
         self.norm_on_load = os.environ.get("VF_NORM_ON_LOAD", "0") == "1"      # bf16 halves only
         self.encoder_chunk = int(os.environ.get("VF_ENC_CHUNK", "0"))      # images per chunk of the high-resolution encoder levels (0: whole batch)
         self.encoder_chunk_levels = int(os.environ.get("VF_ENC_CHUNK_LEVELS", "2"))
@@ -85,7 +85,7 @@ class VQGAN:
     def to(self, device):
         device = torch.device(device)
         if device.type != "cuda":
-            raise L.LibraryError("viewformer_b200.VQGAN runs on CUDA (sm_100a) only; there is no CPU path")
+            raise L.LibraryError("viewformer_b200.VQGAN runs on CUDA (sm_90a) only; there is no CPU path")
         if self._sd is not None and device != self.device:
             sd = self.state_dict()                 # includes the live quantizer buffers (EMA updates made in train() mode)
             self.device = device
@@ -323,7 +323,7 @@ class VQGAN:
 
     # ------------------------------------------------------------------ building blocks (NHWC f32 in / out)
     def _conv(self, cw, x_opd_or_f32, *, residual=None, stride=1, upsample=False, stats=True, out_dtype=torch.float32):
-        """``stats``: the output feeds a GroupNorm(32) — let the tcgen05 epilogue accumulate its statistics.
+        """``stats``: the output feeds a GroupNorm(32) — let the tensor-core epilogue accumulate its statistics.
         ``out_dtype`` bf16 is only honoured on the tensor-core path (callers check ``cw.tc``)."""
         gn = 32 if stats else 0
         if cw.tc and stride == 2:    # operand is the space-to-depth tensor [N,H/2,W/2,4C]: stride-1 tap-table conv
@@ -503,7 +503,7 @@ class VQGAN:
         """QuantizeEMA.forward (utils_th.py:32-68) on rows [M,D]; returns (quant rows | None, diff, idx)."""
         q = self._w["q"]
         if q["eh"] is not None and os.environ.get("VF_VQ_FUSED", "1") != "0":
-            # fused tcgen05 lookup: z read once, scores never leave TMEM, near-ties settled in fp64: same indices as the fp32 kernel
+            # fused wgmma lookup: z read once, scores never leave registers, near-ties settled in fp64: same indices as the fp32 kernel
             idx, quant, dsum = L.vq_lookup_fused(z_rows, q["et"], q["esq"], q["eh"], emb_dk=q["emb"], want_quant=want_quant, want_diff=True)
         elif q["et3"] is not None and z_rows.shape[1] % 64 == 0:
             # tensor-core distance GEMM (bf16x3) + exact fp64 re-score of every near-minimal candidate: same indices as the fp32 kernel
