@@ -70,7 +70,7 @@ struct TcParams {
 //   x * w  =  hi_x hi_w  +  2^-11 (hi_x lo_w + lo_x hi_w)  +  O(2^-22 |x w|)            -> three fp16 MMAs per product block
 // The tensor cores add into their fp32 accumulators without round-to-nearest, so a long K loop is not fp32-faithful.  The
 // accumulator is therefore drained every `exact_kc` k-blocks (a "chunk" of MMA steps from a ZERO accumulator) and the chunks are
-// summed in the staging tile with round-to-nearest FFMA, scaled by 2^-11 for the cross terms, small terms first.
+// summed in a second register array with round-to-nearest FFMA, scaled by 2^-11 for the cross terms, small terms first.
 constexpr float EXACT_LO_SCALE = 1.0f / 2048.0f;
 
 struct TileInfo {
@@ -175,6 +175,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     constexpr int STG_LD = HALF_N + 4;         // staging row stride (floats): +4 keeps 128-bit row reads conflict-free
     constexpr int STG_BYTES = NUM_EPI_WARPS * 32 * STG_LD * 4;
     constexpr int NACC = kBlockN / 2;          // accumulator registers per thread (64 rows x kBlockN per warpgroup)
+    constexpr bool kExact = kKind == F16;      // fp16 operands are always split-fp16 pairs (TcParams::exact)
 
     extern __shared__ uint8_t smem_raw[];
     // 1024B alignment required by the 128B swizzle atoms
@@ -284,11 +285,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     float* stg = staging + warp * (32 * STG_LD);       // the epilogue's staging tile of this warp [32][STG_LD]
     int stage = 0, ab = 0;
     uint32_t phase = 0, aphase = 0;
-    float acc[NACC];
 
-    // accumulator fragment -> staging: element (r, c) of the 128 x kBlockN tile goes to the staging tile of the epilogue warp that
-    // stores it.  add = 0: dst = acc * sc; add = 1: dst = fma(acc, sc, dst) (exact mode: chunks summed with round-to-nearest)
-    auto to_staging = [&](float sc, bool add) {
+    // fragment -> staging: element (r, c) of the 128 x kBlockN tile goes to the staging tile of the epilogue warp that stores it
+    auto to_staging = [&](const float (&v)[NACC], float sc) {
         const int r_lo = 64 * wg + 16 * (warp & 3) + (lane >> 2);
 #pragma unroll
         for (int j = 0; j < NACC / 4; ++j) {
@@ -296,15 +295,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             for (int h = 0; h < 2; ++h) {
                 const int r = r_lo + 8 * h, c = 8 * j + 2 * (lane & 3);
                 float* dst = staging + ((c / HALF_N) * 4 + (r >> 5)) * (32 * STG_LD) + (r & 31) * STG_LD + (c % HALF_N);
-                float2 v;
-                if (add) {
-                    v = *reinterpret_cast<float2*>(dst);
-                    v.x = fmaf(acc[4 * j + 2 * h], sc, v.x);
-                    v.y = fmaf(acc[4 * j + 2 * h + 1], sc, v.y);
-                } else {
-                    v = make_float2(acc[4 * j + 2 * h] * sc, acc[4 * j + 2 * h + 1] * sc);
-                }
-                *reinterpret_cast<float2*>(dst) = v;
+                *reinterpret_cast<float2*>(dst) = make_float2(v[4 * j + 2 * h] * sc, v[4 * j + 2 * h + 1] * sc);
             }
         }
     };
@@ -312,6 +303,91 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
         const TileInfo ti = decode_tile(p, t, kBlockN);
         if (ti.skip) continue;
+
+        // Declared per tile, so that neither array is live in the epilogue (every tile's first wgmma starts from a zero accumulator).
+        // csum (exact mode): the running sum of the chunks in the accumulator's fragment layout, first chunk acc * sc, then
+        // fma(acc, sc, csum).
+        float acc[NACC];
+        float csum[kExact ? NACC : 1];
+        auto k_loop = [&]() {
+            // ---- phase 1: K loop.  One wgmma group (4 MMA steps of one k-block) stays in flight: once the group of k-block kb is
+            // issued, wait for kb-1's and hand its ring slot back to the producer.
+            const int nkb = p.halo ? 9 * p.cin_blocks : ti.nkb;
+            const int nsmall = p.exact ? 2 * p.exact_kpp / p.exact_kc : 0;     // exact mode: cross-term chunks come first
+            int prev_stage = -1, prev_halo = -1, in_chunk = 0, ck = 0, tap = 0;
+            bool fresh = true;
+            uint32_t a_base = 0;
+            const uint32_t pitch = (uint32_t)(p.TW + 2);
+            auto retire_prev = [&]() {
+                if (prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
+                if (prev_halo >= 0) mbar_arrive(&a_empty_bar[prev_halo]);
+                prev_stage = prev_halo = -1;
+            };
+#pragma unroll 1
+            for (int kb = 0; kb < nkb; ++kb) {
+                uint64_t adesc, bdesc;
+                const int this_halo = (p.halo && tap == 8) ? ab : -1;
+                if (p.halo) {
+                    // tile = TH rows of TW=8 pixels: MMA row group g (8 rows) = image row g of the tile; inside the halo tile
+                    // (pitch TW+2 rows) tap (dy,dx) starts (dy*(TW+2)+dx) rows in, consecutive groups are (TW+2) rows apart
+                    if (tap == 0) {
+                        mbar_wait(&a_full_bar[ab], aphase, "vf_tc_gemm mma(halo)");
+                        a_base = smem_u32(smem + ab * HALO_BYTES);
+                        if (!kExact && p.norm_mr) {  // every thread's MMAs read the whole tile: transform, then publish it to the async proxy
+                            normalise_halo(p, smem + ab * HALO_BYTES, kb / 9, ti.img0, ti.oy0, ti.ox0, threadIdx.x);
+                            fence_async_smem();
+                            named_sync(1, NUM_MMA_THREADS);
+                        }
+                    }
+                    mbar_wait(&full_bar[stage], phase, "vf_tc_gemm mma");
+                    const uint32_t a_addr = a_base + ((uint32_t)(tap / 3) * pitch + (uint32_t)(tap % 3) + (uint32_t)(8 * wg) * pitch) * ROW_BYTES;
+                    adesc = sw128_desc(a_addr, pitch * ROW_BYTES);
+                    bdesc = sw128_desc(smem_u32(halo_b_base + stage * B_STAGE_BYTES));
+                } else {
+                    mbar_wait(&full_bar[stage], phase, "vf_tc_gemm mma");
+                    const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+                    adesc = sw128_desc(sa + (uint32_t)(wg * 64 * ROW_BYTES));
+                    bdesc = sw128_desc(sa + A_STAGE_BYTES);
+                }
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < K_STEPS; ++k)      // +32 bytes along K inside the swizzle atom => +2 in the (addr >> 4) field
+                    wgmma_ss<kBlockN, kKind>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (fresh && k == 0) ? 0u : 1u);
+                wgmma_commit();
+                fresh = false;
+                wgmma_wait<1>();
+                retire_prev();
+                prev_stage = stage;
+                prev_halo = this_halo;
+                if (p.halo) {
+                    if (++stage == NGH) { stage = 0; phase ^= 1; }
+                    if (++tap == 9) { tap = 0; if (++ab == 2) { ab = 0; aphase ^= 1; } }
+                } else {
+                    if (++stage == NG) { stage = 0; phase ^= 1; }
+                }
+                if (kExact && ++in_chunk == p.exact_kc) {
+                    // chunk complete: fold it into the running sum with round-to-nearest FFMA, restart from a zero accumulator
+                    in_chunk = 0;
+                    wgmma_wait<0>();
+                    reg_fence(acc);
+                    const float sc = (ck < nsmall ? EXACT_LO_SCALE : 1.0f) * p.alpha;
+                    if (ck == 0) {
+#pragma unroll
+                        for (int i = 0; i < NACC; ++i) csum[i] = acc[i] * sc;
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < NACC; ++i) csum[i] = fmaf(acc[i], sc, csum[i]);
+                    }
+                    ++ck;
+                    fresh = true;
+                }
+            }
+            wgmma_wait<0>();
+            reg_fence(acc);
+            retire_prev();
+        };
+        // exact mode: the chunk sums take the registers the row bookkeeping, bias and residual would hold during the loop
+        if constexpr (kExact) k_loop();
 
         // row bookkeeping: lane l stores tile row 32*quarter + l
         const int row = quarter * 32 + lane;
@@ -341,97 +417,30 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
         const int c_ln = (lane % VPR) * 4;             // column inside this warp's half
         const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
         // fast path: full-width tile, 16-byte aligned rows -> vector I/O and the whole residual tile prefetched into
-        // registers BEFORE the main loop, so its DRAM latency hides behind this tile's MMAs
+        // registers BEFORE the main loop, so its DRAM latency hides behind this tile's MMAs.  Exact mode keeps the chunk sums in
+        // those registers and reads the residual in the epilogue loop instead.
         const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
-        float4 resv[ITERS];
-        if (fast && p.residual) {
+        auto residual_at = [&](int i) {
+            const int rr = i * RPI + r_sub;
+            const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
+            const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
+            // unconditional load (out-of-range rows read row 0 and are never stored): a predicated load would make
+            // the compiler funnel all 32 loads through one temporary and serialise their DRAM latencies
+            const long long o = ok ? off_row + n_ln : (long long)n_ln;
+            return __ldg(reinterpret_cast<const float4*>(p.residual + o));
+        };
+        float4 resv[kExact ? 1 : ITERS];
+        if (!kExact && fast && p.residual) {
 #pragma unroll
-            for (int i = 0; i < ITERS; ++i) {
-                const int rr = i * RPI + r_sub;
-                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                // unconditional load (out-of-range rows read row 0 and are never stored): a predicated load would make
-                // the compiler funnel all 32 loads through one temporary and serialise their DRAM latencies
-                const long long o = ok ? off_row + n_ln : (long long)n_ln;
-                resv[i] = __ldg(reinterpret_cast<const float4*>(p.residual + o));
-            }
+            for (int i = 0; i < ITERS; ++i) resv[i] = residual_at(i);
         }
         float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (fast && p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
 
-        // ---- phase 1: K loop.  One wgmma group (4 MMA steps of one k-block) stays in flight: once the group of k-block kb is
-        // issued, wait for kb-1's and hand its ring slot back to the producer.
-        const int nkb = p.halo ? 9 * p.cin_blocks : ti.nkb;
-        const int nsmall = p.exact ? 2 * p.exact_kpp / p.exact_kc : 0;     // exact mode: cross-term chunks come first
-        int prev_stage = -1, prev_halo = -1, in_chunk = 0, ck = 0, tap = 0;
-        bool fresh = true;
-        uint32_t a_base = 0;
-        const uint32_t pitch = (uint32_t)(p.TW + 2);
-        auto retire_prev = [&]() {
-            if (prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
-            if (prev_halo >= 0) mbar_arrive(&a_empty_bar[prev_halo]);
-            prev_stage = prev_halo = -1;
-        };
-#pragma unroll 1
-        for (int kb = 0; kb < nkb; ++kb) {
-            uint64_t adesc, bdesc;
-            const int this_halo = (p.halo && tap == 8) ? ab : -1;
-            if (p.halo) {
-                // tile = TH rows of TW=8 pixels: MMA row group g (8 rows) = image row g of the tile; inside the halo tile
-                // (pitch TW+2 rows) tap (dy,dx) starts (dy*(TW+2)+dx) rows in, consecutive groups are (TW+2) rows apart
-                if (tap == 0) {
-                    mbar_wait(&a_full_bar[ab], aphase, "vf_tc_gemm mma(halo)");
-                    a_base = smem_u32(smem + ab * HALO_BYTES);
-                    if (p.norm_mr) {              // every thread's MMAs read the whole tile: transform, then publish it to the async proxy
-                        normalise_halo(p, smem + ab * HALO_BYTES, kb / 9, ti.img0, ti.oy0, ti.ox0, threadIdx.x);
-                        fence_async_smem();
-                        named_sync(1, NUM_MMA_THREADS);
-                    }
-                }
-                mbar_wait(&full_bar[stage], phase, "vf_tc_gemm mma");
-                const uint32_t a_addr = a_base + ((uint32_t)(tap / 3) * pitch + (uint32_t)(tap % 3) + (uint32_t)(8 * wg) * pitch) * ROW_BYTES;
-                adesc = sw128_desc(a_addr, pitch * ROW_BYTES);
-                bdesc = sw128_desc(smem_u32(halo_b_base + stage * B_STAGE_BYTES));
-            } else {
-                mbar_wait(&full_bar[stage], phase, "vf_tc_gemm mma");
-                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-                adesc = sw128_desc(sa + (uint32_t)(wg * 64 * ROW_BYTES));
-                bdesc = sw128_desc(sa + A_STAGE_BYTES);
-            }
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < K_STEPS; ++k)      // +32 bytes along K inside the swizzle atom => +2 in the (addr >> 4) field
-                wgmma_ss<kBlockN, kKind>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (fresh && k == 0) ? 0u : 1u);
-            wgmma_commit();
-            fresh = false;
-            wgmma_wait<1>();
-            retire_prev();
-            prev_stage = stage;
-            prev_halo = this_halo;
-            if (p.halo) {
-                if (++stage == NGH) { stage = 0; phase ^= 1; }
-                if (++tap == 9) { tap = 0; if (++ab == 2) { ab = 0; aphase ^= 1; } }
-            } else {
-                if (++stage == NG) { stage = 0; phase ^= 1; }
-            }
-            if (p.exact && ++in_chunk == p.exact_kc) {
-                // chunk complete: fold it into the staging tile (the first chunk initialises it), restart from a zero accumulator
-                in_chunk = 0;
-                wgmma_wait<0>();
-                reg_fence(acc);
-                if (ck == 0) named_sync(1, NUM_MMA_THREADS);      // the previous tile's epilogue is done with the staging tile
-                to_staging((ck < nsmall ? EXACT_LO_SCALE : 1.0f) * p.alpha, ck > 0);
-                ++ck;
-                fresh = true;
-            }
-        }
-        wgmma_wait<0>();
-        reg_fence(acc);
-        retire_prev();
-        if (!p.exact) {
-            named_sync(1, NUM_MMA_THREADS);                       // the previous tile's epilogue is done with the staging tile
-            to_staging(p.alpha, false);
-        }
+        if constexpr (!kExact) k_loop();
+        named_sync(1, NUM_MMA_THREADS);                           // the previous tile's epilogue is done with the staging tile
+        if constexpr (kExact) to_staging(csum, 1.0f);
+        else to_staging(acc, p.alpha);
         named_sync(1, NUM_MMA_THREADS);                           // staging tile complete
 
         // ---- phase 2: lanes span the columns of a tile row -> fully coalesced stores; bias / activation / residual here
@@ -447,7 +456,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                 if (p.bias_mode == VF_BIAS_N) { v.x += bias4.x; v.y += bias4.y; v.z += bias4.z; v.w += bias4.w; }
                 else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
                 if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
-                if (p.residual) { v.x += resv[i].x; v.y += resv[i].y; v.z += resv[i].z; v.w += resv[i].w; }
+                if (p.residual) {
+                    const float4 r = kExact ? residual_at(i) : resv[i];
+                    v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
+                }
                 if (ok) {
                     gs += (v.x + v.y) + (v.z + v.w);
                     gq += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
