@@ -2,9 +2,9 @@
 
     python scripts/prof_exact_conv.py [n_images]
 
-One line per shape and residual: launch time, executed fp16 MMA rate (three passes per product), and the operand bytes the tile
-schedule moves from L2 into shared memory per launch, both for the tap-box path (a shifted A box per tap and k-block) and, where the
-shape takes it, the halo-tile path (one halo tile per channel block and half per tile).
+One line per shape and residual: launch time, executed fp16 MMA rate (three passes per product), the path the shape takes and the
+operand bytes that path moves from L2 into shared memory per launch: tap-box (a shifted A box per tap and k-block) or halo (Cin <=
+128: one halo tile per channel block and half, resident for the whole tile).  Weight boxes are counted on both paths.
 """
 import os
 import sys
@@ -18,17 +18,15 @@ SHAPES = [(128, 128, 128), (64, 128, 128), (32, 128, 256), (32, 256, 256), (16, 
 
 
 def operand_bytes(n, side, cin, cout):
-    """L2 -> SM bytes per launch: (tap-box, halo or None), from the tile schedule of tc_gemm_kernel (128-pixel tiles, 64-channel
-    k-blocks of 128 bytes per row, 3 product passes)."""
+    """(path, L2 -> SM bytes per launch) of the schedule tc_gemm_kernel runs (128-pixel tiles, 64-channel k-blocks of 128 bytes per
+    row, 3 product passes)."""
     block_n = 128 if cout > 64 else 64
     cbs = cin // 64
     tiles = n * side * side // 128 * (cout // block_n)
     b = 3 * 9 * cbs * block_n * 128                              # weight boxes per tile
-    tapbox = tiles * (3 * 9 * cbs * 128 * 128 + b)
-    halo = None
-    if cin <= 128 and side >= 16:                              # 8 x 16-pixel tiles, one (16+2) x (8+2) halo tile per (half, block)
-        halo = tiles * (2 * cbs * 18 * 10 * 128 + b)
-    return tapbox, halo
+    if cin <= 128 and side >= 16:                              # 16 x 8-pixel tiles, one (8+2) x (16+2) halo tile per (half, block)
+        return "halo", tiles * (2 * cbs * 10 * 18 * 128 + b)
+    return "tap-box", tiles * (3 * 9 * cbs * 128 * 128 + b)
 
 
 def main():
@@ -37,8 +35,8 @@ def main():
     L.load(True)
     dev = "cuda"
     print(f"{torch.cuda.get_device_name(0)}, {n} images per launch")
-    print("| map | Cin->Cout | residual | ms | executed fp16 MMA TFLOP/s | L2->SM GB tap-box | L2->SM GB halo |")
-    print("|---|---|---|---:|---:|---:|---:|")
+    print("| map | Cin->Cout | residual | ms | executed fp16 MMA TFLOP/s | path | L2->SM GB |")
+    print("|---|---|---|---:|---:|---|---:|")
     g = torch.Generator(device=dev).manual_seed(0)
     for side, cin, cout in SHAPES:
         x = torch.randn((n, side, side, cin), device=dev, generator=g)
@@ -50,7 +48,7 @@ def main():
         o = torch.empty((n, side, side, cout), device=dev)
         res = torch.randn((n, side, side, cout), device=dev, generator=g)
         reps = max(5, int(2e10 / (n * side * side * cin * cout * 9)))
-        tb, hb = operand_bytes(n, side, cin, cout)
+        path, nbytes = operand_bytes(n, side, cin, cout)
         for r in (None, res):
             for _ in range(3):
                 L.tc_conv(xs, ws, b, out=o, residual=r, gn_groups=32)
@@ -63,8 +61,7 @@ def main():
             torch.cuda.synchronize()
             ms = e0.elapsed_time(e1) / reps
             fl = 3 * 2.0 * n * side * side * cin * 9 * cout
-            halo = f"{hb / 1e9:.1f}" if hb is not None else "-"
-            print(f"| {side}x{side} | {cin}->{cout} | {'yes' if r is not None else 'no'} | {ms:.3f} | {fl / ms / 1e9:.1f} | {tb / 1e9:.1f} | {halo} |")
+            print(f"| {side}x{side} | {cin}->{cout} | {'yes' if r is not None else 'no'} | {ms:.3f} | {fl / ms / 1e9:.1f} | {path} | {nbytes / 1e9:.1f} |")
         del xs, ws, o, res
         torch.cuda.empty_cache()
 

@@ -49,8 +49,9 @@ struct TcParams {
     __nv_bfloat16* C_bf16;
     long long ldc, c_sb1, c_sb2;
     int vec_ok;                // output/residual/bias addressing is 16-byte friendly -> vector epilogue
-    int halo;                  // conv only: 1 = load one (TH+2)x(TW+2) halo tile per 64-channel block and address the 9 taps
-                               // as row-shifted wgmma descriptors into it (9x fewer A bytes from L2); 0 = one shifted TMA box per tap
+    int halo;                  // conv only: 1 = load one (TH+2)x(TW+2) halo tile per 64-channel block (exact: per block and half)
+                               // and address the 9 taps as row-shifted wgmma descriptors into it (9x fewer A bytes from L2);
+                               // 0 = one shifted TMA box per tap
     double* gn_sums;           // optional fused GroupNorm statistics of the OUTPUT: [images][groups][2] (sum, sum of squares)
     int gn_groups, gn_cpg, gn_rows_per_img;
     int exact;                 // split-fp16 operands (VF_F16X2), three product passes, chunked accumulation (see EXACT_LO_SCALE)
@@ -111,16 +112,34 @@ __device__ __forceinline__ TileInfo decode_tile(const TcParams& p, int t, int bl
 }
 
 constexpr int HALO_BYTES = 23552;  // one (16+2) x (8+2) halo tile of 128-byte rows, rounded up to 1024
-constexpr int HALO_SLOTS = 6;      // weight-tile slots of the halo-mode ring
-__host__ __device__ constexpr int operand_bytes(int stages, int stage_bytes, int b_stage_bytes) {
-    return stages * stage_bytes > 2 * HALO_BYTES + HALO_SLOTS * b_stage_bytes ? stages * stage_bytes
-                                                                               : 2 * HALO_BYTES + HALO_SLOTS * b_stage_bytes;
+// Halo mode carves the operand region into halo buffers followed by a ring of weight-tile slots.  bf16 / TF32: 2 halo buffers
+// (double-buffered over the channel blocks), 6 slots.  Exact: 4 buffers, the lo and hi halves of up to 2 channel blocks, all
+// resident for the whole tile, 4 slots.
+__host__ __device__ constexpr int halo_buffers(bool exact) { return exact ? 4 : 2; }
+__host__ __device__ constexpr int halo_slots(bool exact) { return exact ? 4 : 6; }
+__host__ __device__ constexpr int operand_bytes(int stages, int stage_bytes, int b_stage_bytes, bool exact) {
+    return stages * stage_bytes > halo_buffers(exact) * HALO_BYTES + halo_slots(exact) * b_stage_bytes
+               ? stages * stage_bytes
+               : halo_buffers(exact) * HALO_BYTES + halo_slots(exact) * b_stage_bytes;
 }
 constexpr int MAX_STAGES = 8;
-template <int kBlockN, int kStages>
+template <int kBlockN, int kStages, bool kExact>
 __host__ __device__ constexpr int tc_smem_bytes() {
-    return operand_bytes(kStages, A_STAGE_BYTES + kBlockN * ROW_BYTES, kBlockN * ROW_BYTES) +
-           NUM_EPI_WARPS * 32 * (kBlockN / 2 + 4) * 4 /*epilogue staging*/ + 1024 /*align slack*/ + 8 * (2 * MAX_STAGES + 4) /*barriers*/;
+    return operand_bytes(kStages, A_STAGE_BYTES + kBlockN * ROW_BYTES, kBlockN * ROW_BYTES, kExact) +
+           NUM_EPI_WARPS * 32 * (kBlockN / 2 + 4) * 4 /*epilogue staging*/ + 1024 /*align slack*/ + 8 * (2 * MAX_STAGES + 8) /*barriers*/;
+}
+
+// L2 prefetch of the residual rows a conv tile's epilogue will read: one bulk prefetch per (image, output row) of the tile, spanning
+// its valid pixels from channel n0 on (the columns between the tile's channel slices ride along).
+__device__ __forceinline__ void prefetch_residual_l2(const TcParams& p, const TileInfo& ti, int block_n) {
+    const int tw = min(p.TW, p.OW - ti.ox0);
+    const uint32_t bytes = (uint32_t)(((long long)(tw - 1) * p.ldc + block_n) * 4);
+    for (int r = 0; r < p.TN * p.TH; ++r) {
+        const int img = ti.img0 + r / p.TH, oy = ti.oy0 + r % p.TH;
+        if (img >= p.Nimg || oy >= p.OH) continue;
+        const float* src = p.residual + ((long long)(img * p.OH + oy) * p.OW + ti.ox0) * p.ldc + ti.n0;
+        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+    }
 }
 
 // Normalise-on-load: GroupNorm (+ swish) of the raw halo tile of channel block cb, in place, by the 256 MMA threads.  The tile holds
@@ -180,16 +199,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     extern __shared__ uint8_t smem_raw[];
     // 1024B alignment required by the 128B swizzle atoms
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    constexpr int OPER_BYTES = operand_bytes(kStages, STAGE_BYTES, B_STAGE_BYTES);
+    constexpr int OPER_BYTES = operand_bytes(kStages, STAGE_BYTES, B_STAGE_BYTES, kExact);
     float* staging = reinterpret_cast<float*>(smem + OPER_BYTES);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OPER_BYTES + STG_BYTES);   // [MAX_STAGES]
     uint64_t* empty_bar = full_bar + MAX_STAGES;        // [MAX_STAGES]
-    uint64_t* a_full_bar = empty_bar + MAX_STAGES;      // [2]  halo mode: A halo tiles
-    uint64_t* a_empty_bar = a_full_bar + 2;             // [2]
+    constexpr int NHB = halo_buffers(kExact);
+    uint64_t* a_full_bar = empty_bar + MAX_STAGES;      // [NHB]  halo mode: A halo tiles
+    uint64_t* a_empty_bar = a_full_bar + NHB;           // [NHB]
     constexpr int NG = kStages;                         // ring depth (normal mode)
-    // halo mode carves the same operand region differently: 2 halo buffers, then a ring of B-only slots
-    constexpr int NGH = HALO_SLOTS;
-    uint8_t* halo_b_base = smem + 2 * HALO_BYTES;
+    // halo mode carves the same operand region differently: NHB halo buffers, then a ring of B-only slots
+    constexpr int NGH = halo_slots(kExact);
+    uint8_t* halo_b_base = smem + NHB * HALO_BYTES;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -201,7 +221,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], NUM_MMA_THREADS);     // every MMA thread arrives once its wgmma reading the slot retired
         }
-        for (int a = 0; a < 2; ++a) {
+        for (int a = 0; a < NHB; ++a) {
             mbar_init(&a_full_bar[a], 1);
             mbar_init(&a_empty_bar[a], NUM_MMA_THREADS);
         }
@@ -216,12 +236,39 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             int stage = 0;
             uint32_t phase = 0;
             int ab = 0;
-            uint32_t aphase = 0;
-            for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+            uint32_t aphase = 0, tpar = 0;
+            for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, tpar ^= 1) {
                 const TileInfo ti = decode_tile(p, t, kBlockN);
                 if (ti.skip) continue;
+                const uint32_t halo_bytes = (uint32_t)((p.TW + 2) * (p.TH + 2)) * ROW_BYTES;
+                if (kExact && p.halo) {
+                    // Halo buffer 2 h + cb holds half h (0 = lo, 1 = hi) of channel block cb and is loaded once per tile.  The lo
+                    // halves are read by product pass 0 only, so they load first; the hi halves, still read by the previous
+                    // tile's last pass when this tile starts, load NGH k-blocks into pass 0.
+                    auto load_halves = [&](int h) {
+                        for (int cb = 0; cb < p.cin_blocks; ++cb) {
+                            const int hb = 2 * h + cb;
+                            mbar_wait(&a_empty_bar[hb], tpar ^ 1, "vf_tc_gemm producer(halo)");
+                            mbar_expect_tx(&a_full_bar[hb], halo_bytes);
+                            tma_load_4d(smem + hb * HALO_BYTES, &p.tmA, &a_full_bar[hb], (h ? 0 : p.exact_clog) + cb * p.bk_elems,
+                                        ti.ox0 - 1, ti.oy0 - 1, ti.img0);
+                        }
+                    };
+                    load_halves(0);
+                    if (p.residual && p.vec_ok && ti.n0 + kBlockN <= p.Ncols) prefetch_residual_l2(p, ti, kBlockN);
+                    int j = 0, tap = 0, cb = 0;     // the tap-box walk: product pass, tap, channel block
+                    for (int kb = 0; kb < ti.nkb; ++kb) {
+                        if (kb == NGH) load_halves(1);
+                        mbar_wait(&empty_bar[stage], phase ^ 1, "vf_tc_gemm producer");
+                        mbar_expect_tx(&full_bar[stage], (uint32_t)B_STAGE_BYTES);
+                        tma_load_4d(halo_b_base + stage * B_STAGE_BYTES, &p.tmB, &full_bar[stage],
+                                    ((tap * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb) * p.bk_elems, ti.n0, 0, 0);
+                        if (++cb == p.cin_blocks) { cb = 0; if (++tap == 9) { tap = 0; ++j; } }
+                        if (++stage == NGH) { stage = 0; phase ^= 1; }
+                    }
+                    continue;
+                }
                 if (p.halo) {
-                    const uint32_t halo_bytes = (uint32_t)((p.TW + 2) * (p.TH + 2)) * ROW_BYTES;
                     const int nkb = 9 * p.cin_blocks;
                     int tap = 0, cb = 0;
                     for (int kb = 0; kb < nkb; ++kb) {
@@ -240,6 +287,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                     }
                     continue;
                 }
+                if (kExact && p.conv && p.residual && p.vec_ok && ti.n0 + kBlockN <= p.Ncols) prefetch_residual_l2(p, ti, kBlockN);
                 for (int kb = 0; kb < ti.nkb; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1, "vf_tc_gemm producer");
                     mbar_expect_tx(&full_bar[stage], (uint32_t)STAGE_BYTES);
@@ -284,23 +332,27 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     const int col_half = warp >> 2;                    // ... of column half col_half
     float* stg = staging + warp * (32 * STG_LD);       // the epilogue's staging tile of this warp [32][STG_LD]
     int stage = 0, ab = 0;
-    uint32_t phase = 0, aphase = 0;
+    uint32_t phase = 0, aphase = 0, tpar = 0;
 
-    // fragment -> staging: element (r, c) of the 128 x kBlockN tile goes to the staging tile of the epilogue warp that stores it
+    // fragment -> staging: element (r, c) of the 128 x kBlockN tile goes to the staging tile of the epilogue warp that stores it.
+    // Exact halo mode with 16 x 8-pixel tiles: MMA row group g of warpgroup wg is image row g, columns [8 wg, 8 wg + 8), stored as
+    // tile row 16 g + 8 wg + i, so that every epilogue warp sums the same pixels as on the tap-box path (same GroupNorm partials).
+    const bool col_split = kExact && p.halo && p.TW == 16;
     auto to_staging = [&](const float (&v)[NACC], float sc) {
         const int r_lo = 64 * wg + 16 * (warp & 3) + (lane >> 2);
 #pragma unroll
         for (int j = 0; j < NACC / 4; ++j) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int r = r_lo + 8 * h, c = 8 * j + 2 * (lane & 3);
+                const int r = col_split ? 16 * (2 * (warp & 3) + h) + 8 * wg + (lane >> 2) : r_lo + 8 * h;
+                const int c = 8 * j + 2 * (lane & 3);
                 float* dst = staging + ((c / HALF_N) * 4 + (r >> 5)) * (32 * STG_LD) + (r & 31) * STG_LD + (c % HALF_N);
                 *reinterpret_cast<float2*>(dst) = make_float2(v[4 * j + 2 * h] * sc, v[4 * j + 2 * h + 1] * sc);
             }
         }
     };
 
-    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, tpar ^= 1) {
         const TileInfo ti = decode_tile(p, t, kBlockN);
         if (ti.skip) continue;
 
@@ -312,12 +364,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
         auto k_loop = [&]() {
             // ---- phase 1: K loop.  One wgmma group (4 MMA steps of one k-block) stays in flight: once the group of k-block kb is
             // issued, wait for kb-1's and hand its ring slot back to the producer.
-            const int nkb = p.halo ? 9 * p.cin_blocks : ti.nkb;
+            const int nkb = (p.halo && !kExact) ? 9 * p.cin_blocks : ti.nkb;
             const int nsmall = p.exact ? 2 * p.exact_kpp / p.exact_kc : 0;     // exact mode: cross-term chunks come first
-            int prev_stage = -1, prev_halo = -1, in_chunk = 0, ck = 0, tap = 0;
+            int prev_stage = -1, prev_halo = -1, in_chunk = 0, ck = 0, tap = 0, j = 0, cb = 0;
             bool fresh = true;
             uint32_t a_base = 0;
             const uint32_t pitch = (uint32_t)(p.TW + 2);
+            // halo rows between the two warpgroups' first pixels: TW = 8 -> 8 image rows apart, TW = 16 -> 8 columns apart
+            const uint32_t wg_rows = p.TW == 16 ? 8u : 8u * pitch;
             auto retire_prev = [&]() {
                 if (prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
                 if (prev_halo >= 0) mbar_arrive(&a_empty_bar[prev_halo]);
@@ -326,8 +380,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
 #pragma unroll 1
             for (int kb = 0; kb < nkb; ++kb) {
                 uint64_t adesc, bdesc;
-                const int this_halo = (p.halo && tap == 8) ? ab : -1;
-                if (p.halo) {
+                int this_halo = (p.halo && tap == 8) ? ab : -1;
+                if (kExact && p.halo) {
+                    // the tap-box walk (pass j, tap, channel block cb) over the resident halo tiles: pass 0 reads the lo halves
+                    // (buffers 0, 1), passes 1 and 2 the hi halves (buffers 2, 3); a buffer is released after its last read
+                    const int hb = (j == 0 ? 0 : 2) + cb;
+                    if (tap == 0 && j < 2) mbar_wait(&a_full_bar[hb], tpar, "vf_tc_gemm mma(halo)");
+                    this_halo = (tap == 8 && j != 1) ? hb : -1;
+                    mbar_wait(&full_bar[stage], phase, "vf_tc_gemm mma");
+                    const uint32_t a_addr = smem_u32(smem + hb * HALO_BYTES) +
+                                            ((uint32_t)(tap / 3) * pitch + (uint32_t)(tap % 3) + (uint32_t)wg * wg_rows) * ROW_BYTES;
+                    adesc = sw128_desc(a_addr, pitch * ROW_BYTES);
+                    bdesc = sw128_desc(smem_u32(halo_b_base + stage * B_STAGE_BYTES));
+                } else if (p.halo) {
                     // tile = TH rows of TW=8 pixels: MMA row group g (8 rows) = image row g of the tile; inside the halo tile
                     // (pitch TW+2 rows) tap (dy,dx) starts (dy*(TW+2)+dx) rows in, consecutive groups are (TW+2) rows apart
                     if (tap == 0) {
@@ -359,7 +424,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                 retire_prev();
                 prev_stage = stage;
                 prev_halo = this_halo;
-                if (p.halo) {
+                if (kExact && p.halo) {
+                    if (++stage == NGH) { stage = 0; phase ^= 1; }
+                    if (++cb == p.cin_blocks) { cb = 0; if (++tap == 9) { tap = 0; ++j; } }
+                } else if (p.halo) {
                     if (++stage == NGH) { stage = 0; phase ^= 1; }
                     if (++tap == 9) { tap = 0; if (++ab == 2) { ab = 0; aphase ^= 1; } }
                 } else {
@@ -418,7 +486,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
         const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
         // fast path: full-width tile, 16-byte aligned rows -> vector I/O and the whole residual tile prefetched into
         // registers BEFORE the main loop, so its DRAM latency hides behind this tile's MMAs.  Exact mode keeps the chunk sums in
-        // those registers and reads the residual in the epilogue loop instead.
+        // those registers and loads the residual tile in the epilogue loop, half a tile at a time (a whole tile would spill), from
+        // L2: the producer prefetched it there while the K loop ran.
         const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
         auto residual_at = [&](int i) {
             const int rr = i * RPI + r_sub;
@@ -429,11 +498,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             const long long o = ok ? off_row + n_ln : (long long)n_ln;
             return __ldg(reinterpret_cast<const float4*>(p.residual + o));
         };
-        float4 resv[kExact ? 1 : ITERS];
-        if (!kExact && fast && p.residual) {
+        constexpr int RB = kExact ? ITERS / 2 : ITERS;
+        float4 resv[RB];
+        auto load_residual = [&](int i0) {
+            if (fast && p.residual) {
 #pragma unroll
-            for (int i = 0; i < ITERS; ++i) resv[i] = residual_at(i);
-        }
+                for (int i = 0; i < RB; ++i) resv[i] = residual_at(i0 + i);
+            }
+        };
+        if constexpr (!kExact) load_residual(0);
         float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (fast && p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
 
@@ -448,6 +521,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             float gs = 0.f, gq = 0.f;                 // fused GroupNorm statistics of this lane's 4 channels
 #pragma unroll
             for (int i = 0; i < ITERS; ++i) {
+                if (kExact && i % RB == 0) load_residual(i);
                 const int rr = i * RPI + r_sub;
                 const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
                 const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
@@ -457,7 +531,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                 else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
                 if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
                 if (p.residual) {
-                    const float4 r = kExact ? residual_at(i) : resv[i];
+                    const float4 r = resv[i % RB];
                     v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
                 }
                 if (ok) {
@@ -543,7 +617,7 @@ int make_tmap(CUtensorMap* tm, int dtype, const void* base, const uint64_t dims[
 
 template <int kBlockN, int kStages, WgKind kKind>
 int launch(const TcParams& prm, dim3 grid, cudaStream_t st) {
-    constexpr int smem = tc_smem_bytes<kBlockN, kStages>();
+    constexpr int smem = tc_smem_bytes<kBlockN, kStages, kKind == F16>();
     static_assert(kStages <= MAX_STAGES, "ring depth");
     static_assert(smem <= 232448, "shared memory budget");
     static vf_per_device_flag configured_pd;          // function attributes are per device
@@ -617,10 +691,14 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         int TH = 128 / TW;
         if (TH > q->OH) { TH = 1; while (TH * 2 <= q->OH) TH *= 2; }
         int TN = 128 / (TW * TH);
-        // halo mode: plain stride-1 pad-1 3x3 conv on maps at least 16 rows tall -> 8x16-pixel tiles, one halo load per channel block
-        bool halo = !exact && q->ntaps == 9 && q->Ctot == q->Cin && q->OH == q->H && q->OW == q->W && q->OH >= 16 && q->OW >= 8;
+        // halo mode: plain stride-1 pad-1 3x3 conv on maps at least 16 rows tall -> 8x16-pixel tiles, one halo load per channel block.
+        // Exact mode: one halo per channel block and half, all resident for the tile (so at most 2 channel blocks), on the tap-box
+        // path's own 16x8 or 8x16 tiles, which keeps the fused GroupNorm partial sums of each epilogue warp.
+        bool halo = q->ntaps == 9 && q->OH == q->H && q->OW == q->W &&
+                    (exact ? q->Ctot == 2 * q->Cin && q->Cin <= 2 * bk && TN == 1 && TW >= 8
+                           : q->Ctot == q->Cin && q->OH >= 16 && q->OW >= 8);
         for (int t = 0; halo && t < 9; ++t) halo = q->tap_dy[t] == t / 3 - 1 && q->tap_dx[t] == t % 3 - 1 && q->tap_coff[t] == 0;
-        if (halo) { TW = 8; TH = 16; TN = 1; }
+        if (halo && !exact) { TW = 8; TH = 16; TN = 1; }
         prm.halo = halo ? 1 : 0;
         if (q->norm_mean_rstd) {
             VF_CHECK_ARG(halo && q->ab_dtype == VF_BF16 && q->H >= 32 && q->Ncols % 128 == 0 && q->Cin % 64 == 0,
