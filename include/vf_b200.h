@@ -191,7 +191,8 @@ int vf_attn_block_multiend(const void* qk_bf16, const void* vt_bf16, int B, int 
  *     KH = KW = 1 with so_k = 1, so_n = Cin gives the [Cout, Cin] gradient of a dense layer.
  *   vf_col_sums: out[c] += sum_rows x[row][c]  (bias gradients).
  *   vf_groupnorm_bwd: GroupNorm(groups) [+ swish] backward of y = act(xhat*gamma + beta): dx = rstd (dg gamma - mean - xhat mean2) + add,
- *     dgamma += sum dg xhat, dbeta += sum dg;  mean_rstd from the forward pass; gsums = double [N, groups, 2] scratch.
+ *     dgamma += sum dg xhat, dbeta += sum dg;  mean_rstd from the forward pass; gsums = double [N, groups, 2] scratch;
+ *     dx_bf16 (nullable) receives a second copy of dx rounded to bf16 (nearest even), the operand of the next tensor-core data gradient.
  *   vf_softmax_bwd_rows: dS = P (dP - rowsum(dP P)).   vf_l1_grad: dy = scale * sign(y - x), loss_sum += sum |y - x|.
  *   vf_lincomb3: out = a x + b y + c z (y, z nullable).   vf_sumpool2x2: [N,2H,2W,C] -> [N,H,W,C] (nearest-upsample backward).
  *   vf_adam: torch.optim.Adam step number `step` (>= 1) on flat buffers; the gradient is multiplied by grad_scale first (1 / world size).
@@ -200,7 +201,8 @@ int vf_conv_wgrad(const float* x, const float* dy, int N, int H, int W, int Cin,
                   int pad_t, int pad_l, int upsample2x, int64_t so_k, int64_t so_n, float* dw, vf_stream_t s);
 int vf_col_sums(const float* x, int64_t rows, int C, float* out, vf_stream_t s);
 int vf_groupnorm_bwd(const float* x, const float* dout, const float* mean_rstd, const float* gamma, const float* beta, int N, int HW,
-                     int C, int groups, int swish, const float* add, double* gsums, float* dgamma, float* dbeta, float* dx, vf_stream_t s);
+                     int C, int groups, int swish, const float* add, double* gsums, float* dgamma, float* dbeta, float* dx, void* dx_bf16,
+                     vf_stream_t s);
 int vf_softmax_bwd_rows(const float* P, const float* dP, int64_t rows, int cols, float* dS, vf_stream_t s);
 int vf_l1_grad(const float* x, const float* y, int64_t n, float scale, float* dy, double* loss_sum, vf_stream_t s);
 int vf_lincomb3(float a, const float* x, float b, const float* y, float c, const float* z, int64_t n, float* out, vf_stream_t s);
@@ -214,6 +216,17 @@ int vf_lincomb3(float a, const float* x, float b, const float* y, float c, const
 int vf_pad_transpose_split(const float* x_nhwc, int N, int H, int W, int C, int pitch, int copies, int64_t margin, int64_t L, void* out_f16,
                            vf_stream_t s);
 int vf_sum_splits(const float* partial, int groups, int splits, int64_t n, int accumulate, float* out, vf_stream_t s);
+/* bf16 training step.  vf_pad_transpose_bf16: the single-pass bf16 operand of the same weight-gradient GEMM (vf_tc_gemm, VF_BF16):
+ * bf16 [copies*C][L], the column map of vf_pad_transpose_split with no lo half, over the logical image x (upsample2x = 0) or its nearest x2
+ * upsample (upsample2x = 1: [N,2H,2W,C], pitch >= 2W + 2).  mean_rstd (nullable, [N, groups, 2] from the forward pass) applies
+ * GroupNorm(groups) [+ swish] on the way, with vf_groupnorm_apply's bf16-output arithmetic; the caller clears the buffer.
+ * vf_conv_weights_bf16: one launch over `n` convs (table in device memory) writes the bf16 operands of each from its fp32 master
+ * weights w_kn [9*Cin, Cout]: fw [Cout][9*Cin] (forward conv, also the space-to-depth stride-2 conv) and, when bw_bf16 is not null,
+ * bw [Cin][9*Cout] = the flipped-tap, channel-swapped weights of the data gradient. */
+typedef struct { const float* w_kn; void* fw_bf16; void* bw_bf16; int64_t cin, cout; } vf_conv_weights_bf16_t;
+int vf_pad_transpose_bf16(const float* x_nhwc, int N, int H, int W, int C, int upsample2x, int pitch, int copies, int64_t margin, int64_t L,
+                          const float* mean_rstd, const float* gamma, const float* beta, int groups, int swish, void* out_bf16, vf_stream_t s);
+int vf_conv_weights_bf16(const vf_conv_weights_bf16_t* table, int n, vf_stream_t s);
 int vf_sumpool2x2(const float* x, int N, int H, int W, int C, float* y, vf_stream_t s);
 int vf_adam(float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps, int step,
             float grad_scale, vf_stream_t s);

@@ -25,7 +25,7 @@ EXPORTS = [
     "vf_conv3x3_small_cin", "vf_conv3x3_small_cout", "vf_groupnorm_finalize", "vf_split_f16x2", "vf_attn_block_causal", "vf_attn_block_causal_tail", "vf_attn_block_causal_decode", "vf_attn_block_multiend",
     "vf_vq_split3", "vf_vq_select", "vf_cross_entropy_rows", "vf_pose_loss_rows", "vf_row_mean",
     "vf_vq_prepare_codebook_f16", "vf_vq_lookup_fused", "vf_resize_u8", "vf_image_pair_sums", "vf_ssim_u8", "vf_ssim_u8_k",
-    "vf_conv_wgrad", "vf_pad_transpose_split", "vf_sum_splits", "vf_col_sums", "vf_groupnorm_bwd", "vf_softmax_bwd_rows", "vf_l1_grad", "vf_lincomb3", "vf_sumpool2x2", "vf_adam",
+    "vf_conv_wgrad", "vf_pad_transpose_split", "vf_pad_transpose_bf16", "vf_conv_weights_bf16", "vf_sum_splits", "vf_col_sums", "vf_groupnorm_bwd", "vf_softmax_bwd_rows", "vf_l1_grad", "vf_lincomb3", "vf_sumpool2x2", "vf_adam",
     "vf_layernorm_bwd", "vf_gelu_fwd", "vf_gelu_bwd", "vf_migt_embed_bwd", "vf_cross_entropy_grad", "vf_pose_loss_grad", "vf_adamw_keras", "vf_sumsq", "vf_dropout",
 ]
 
@@ -869,6 +869,80 @@ def dense_wgrad_tc(x_rows, dy_rows, dw_kn, *, accumulate=True):
     return dw_kn
 
 
+def pad_transpose_bf16(x, out, *, pitch, copies, margin, norm=None, upsample=False):
+    """x f32 NHWC -> out bf16 [copies*C, L] (zeroed by the caller): the K-major operand of the bf16 weight-gradient GEMM over the zero-padded
+    pixel grid of the logical image (x, or its nearest x2 upsample), column margin + ((n (H+2) + y + 1) pitch + x + 1) - (k - copies/2) of copy k.
+    ``norm=(mean_rstd, gamma, beta, swish)`` applies GroupNorm(32) [+ swish] first, as vf_groupnorm_apply does for a bf16 output."""
+    lib = load(True)
+    _dev(x, torch.float32); _dev(out, torch.bfloat16)
+    n, h, w, c = x.shape
+    mr, gamma, beta, swish = norm if norm is not None else (None, None, None, False)
+    groups = mr.shape[1] if mr is not None else 0
+    _check(lib.vf_pad_transpose_bf16(_p(x), n, h, w, c, int(upsample), pitch, copies, C.c_int64(margin), C.c_int64(out.shape[-1]), _p(mr), _p(gamma),
+                                     _p(beta), groups, int(swish), _p(out), _stream()))
+    return out
+
+
+def conv_wgrad_bf16_ok(x, dy, kh, stride, upsample):
+    """Shapes conv_wgrad_bf16 takes: those of conv_wgrad_tc, and the upsample convs (x [N,H,W,Cin], dy [N,2H,2W,Cout])."""
+    n, h, w, cin = x.shape
+    up = 2 if upsample else 1
+    return kh == 3 and stride == 1 and cin % 128 == 0 and dy.shape[-1] % 128 == 0 and tuple(dy.shape[1:3]) == (up * h, up * w)
+
+
+def conv_wgrad_bf16(x, dy, dw, *, norm=None, upsample=False, accumulate=True):
+    """Weight gradient of a 3x3 stride-1 pad-1 convolution on the single-pass bf16 tensor-core GEMM: the layout and schedule of
+    conv_wgrad_tc (K = pixels of the zero-padded grid, three horizontal shifts as row blocks, vertical shifts as K offsets, split-K over the
+    SMs, vf_sum_splits), with bf16 operands and fp32 accumulation.  x f32 [N,H,W,Cin] is the conv's input before ``norm`` (see
+    pad_transpose_bf16) and before the nearest x2 upsample when ``upsample``; dy f32 [N,OH,OW,Cout]; dw f32 [9*Cin, Cout]."""
+    lib = load(True)
+    _dev(x, torch.float32); _dev(dy, torch.float32); _dev(dw, torch.float32)
+    n, _, _, cin = x.shape
+    _, h, w, cout = dy.shape                                   # the logical (upsampled) image
+    pitch = (w + 2 + 7) // 8 * 8
+    ppad = n * (h + 2) * pitch
+    tiles = (3 * cin // 128) * (cout // 128)
+    splits = max(1, min(64, (132 + 3 * tiles - 1) // (3 * tiles)))
+    kc = ((ppad + splits - 1) // splits + 63) // 64 * 64
+    kpad = kc * splits
+    margin = pitch + 8
+    la, lb = kpad + 2 * margin, kpad
+    key = ("bf16", x.device, n, h, w, cin, cout)               # buffers cached per shape, borders / padding / margins cleared once
+    bufs = _wgrad_bufs.get(key)
+    if bufs is None:
+        if len(_wgrad_bufs) >= 32:
+            _wgrad_bufs.clear()
+        bufs = (torch.zeros((3 * cin, la), dtype=torch.bfloat16, device=x.device), torch.zeros((cout, lb), dtype=torch.bfloat16, device=x.device),
+                torch.empty((3, splits, 3 * cin, cout), dtype=torch.float32, device=x.device))
+        _wgrad_bufs[key] = bufs
+    at, bt, partial = bufs
+    pad_transpose_bf16(x, at, pitch=pitch, copies=3, margin=margin, norm=norm, upsample=upsample)
+    pad_transpose_bf16(dy, bt, pitch=pitch, copies=1, margin=0)
+    offs = [margin - pitch, margin, margin + pitch]
+    tc_gemm(at, bt, partial, M=3 * cin, N=cout, K=kc, lda=la, ldb=lb, ldc=cout, batch=(3, splits), a_bs=(0, kc), b_bs=(0, kc),
+            c_bs=(splits * 3 * cin * cout, 3 * cin * cout), k_offsets=offs)
+    _check(lib.vf_sum_splits(_p(partial), 3, splits, C.c_int64(3 * cin * cout), int(accumulate), _p(dw), _stream()))
+    return dw
+
+
+def conv_weights_bf16_table(entries, device):
+    """entries: (w_kn f32 [9*Cin, Cout], fw bf16 [Cout, 9*Cin], bw bf16 [Cin, 9*Cout] or None) -> the device table of vf_conv_weights_bf16
+    (int64 [n, 5] = vf_conv_weights_bf16_t).  The tensors must outlive the table."""
+    rows = []
+    for w_kn, fw, bw in entries:
+        _dev(w_kn, torch.float32); _dev(fw, torch.bfloat16)
+        k, cout = w_kn.shape
+        assert k % 9 == 0 and fw.shape == (cout, k) and (bw is None or (bw.dtype == torch.bfloat16 and bw.shape == (k // 9, 9 * cout)))
+        rows.append([w_kn.data_ptr(), fw.data_ptr(), bw.data_ptr() if bw is not None else 0, k // 9, cout])
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 5).to(device)
+
+
+def conv_weights_bf16(table):
+    """Rewrite every conv's bf16 operand copies listed in ``table`` (conv_weights_bf16_table) from its fp32 master weights: one launch."""
+    lib = load(True)
+    _check(lib.vf_conv_weights_bf16(_p(table), table.shape[0], _stream()))
+
+
 def col_sums(x_rows, out):
     lib = load(True)
     _dev(x_rows, torch.float32)
@@ -876,14 +950,18 @@ def col_sums(x_rows, out):
     return out
 
 
-def groupnorm_bwd(x, dout, mean_rstd, gamma, beta, dgamma, dbeta, *, swish, groups=32, add=None):
+def groupnorm_bwd(x, dout, mean_rstd, gamma, beta, dgamma, dbeta, *, swish, groups=32, add=None, out_bf16=False):
+    """dx f32; ``out_bf16`` also writes dx rounded to bf16 from the same pass and attaches it as ``dx._bf16``."""
     lib = load(True)
     _dev(x, torch.float32); _dev(dout, torch.float32)
     n, h, w, c = x.shape
     dx = torch.empty_like(x)
+    dx16 = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if out_bf16 else None
     gs = torch.empty((n, groups, 2), dtype=torch.float64, device=x.device)
     _check(lib.vf_groupnorm_bwd(_p(x), _p(dout), _p(mean_rstd), _p(gamma), _p(beta), n, h * w, c, groups, int(swish), _p(add), _p(gs),
-                                _p(dgamma), _p(dbeta), _p(dx), _stream()))
+                                _p(dgamma), _p(dbeta), _p(dx), _p(dx16), _stream()))
+    if dx16 is not None:
+        dx._bf16 = dx16
     return dx
 
 

@@ -165,7 +165,8 @@ __global__ void __launch_bounds__(256) gn_bwd_stats_kernel(const float* __restri
 __global__ void __launch_bounds__(256) gn_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ dout, const float* __restrict__ mr,
                                                            const float* __restrict__ gamma, const float* __restrict__ beta,
                                                            const double* __restrict__ gsums, const float* __restrict__ add, int HW, int C,
-                                                           int groups, int swish, int pix_per_block, float* __restrict__ dx) {
+                                                           int groups, int swish, int pix_per_block, float* __restrict__ dx,
+                                                           __nv_bfloat16* __restrict__ dx_bf16) {
     const int quads = C >> 2, lanes = 256 / quads;
     const int cq = threadIdx.x % quads, pl = threadIdx.x / quads, n = blockIdx.y, cpg = C / groups;
     if (pl >= lanes) return;
@@ -195,6 +196,13 @@ __global__ void __launch_bounds__(256) gn_bwd_apply_kernel(const float* __restri
             r[j] = rs[j] * (dg * ga[j] - m1[j] - xh * m2[j]) + ae[j];
         }
         *reinterpret_cast<float4*>(dx + o) = make_float4(r[0], r[1], r[2], r[3]);
+        if (dx_bf16) {                  // the tensor-core operand copy of dx (bf16 training step), round to nearest even
+            const __nv_bfloat162 lo = __floats2bfloat162_rn(r[0], r[1]), hi = __floats2bfloat162_rn(r[2], r[3]);
+            uint2 u;
+            u.x = *reinterpret_cast<const uint32_t*>(&lo);
+            u.y = *reinterpret_cast<const uint32_t*>(&hi);
+            *reinterpret_cast<uint2*>(dx_bf16 + o) = u;
+        }
     }
 }
 
@@ -470,6 +478,94 @@ __global__ void __launch_bounds__(256) pad_transpose_split_kernel(const float* _
     }
 }
 
+// bf16 twin of pad_transpose_split_kernel (bf16 training step): out bf16 [copies * C][L], no lo half, same column map.  The logical image
+// is x itself, or its nearest x2 upsample ([N,2H,2W,C], up = 1).  With mr != null every element first goes through GroupNorm(+swish) from
+// the forward pass's (mean, rstd) in vf_groupnorm_apply's bf16-output arithmetic (affine folded to one FMA, ex2/rcp swish), so the operand
+// equals the bf16 activation the forward conv consumed, and is rounded once.
+__global__ void __launch_bounds__(256) pad_transpose_bf16_kernel(const float* __restrict__ x, int N, int H, int W, int C, int up, int pitch,
+                                                                 int copies, long long margin, long long L, const float* __restrict__ mr,
+                                                                 const float* __restrict__ gamma, const float* __restrict__ beta, int groups,
+                                                                 int swish, __nv_bfloat16* __restrict__ out) {
+    __shared__ float tile[64][33];
+    const int LH = H << up, LW = W << up;
+    const long long p0 = (long long)blockIdx.x * 64;
+    const int c0 = blockIdx.y * 32;
+    const long long P = (long long)N * LH * LW;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int c = c0 + lane;
+    float sc = 1.f, sh = 0.f;
+    for (int i = warp; i < 64; i += 8) {
+        const long long pix = p0 + i;
+        float v = 0.f;
+        if (pix < P && c < C) {
+            const int xx = (int)(pix % LW);
+            const long long t = pix / LW;
+            const int yy = (int)(t % LH);
+            const long long n = t / LH;
+            v = __ldg(x + ((n * H + (yy >> up)) * W + (xx >> up)) * C + c);
+            if (mr) {
+                const float2 m = __ldg(reinterpret_cast<const float2*>(mr) + n * groups + c / (C / groups));
+                sc = m.y * __ldg(gamma + c);
+                sh = __ldg(beta + c) - m.x * sc;
+                v = fmaf(v, sc, sh);
+            }
+            if (swish) v = __fdividef(v, 1.0f + __expf(-v));
+        }
+        tile[i][lane] = v;
+    }
+    __syncthreads();
+    for (int cc = warp; cc < 32; cc += 8) {
+        if (c0 + cc >= C) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int i = lane + 32 * h;
+            const long long pix = p0 + i;
+            if (pix >= P) continue;
+            const int xx = (int)(pix % LW);
+            const long long t = pix / LW;
+            const int yy = (int)(t % LH);
+            const long long n = t / LH;
+            const long long q = pitch ? (n * (LH + 2) + yy + 1) * (long long)pitch + xx + 1 : pix;
+            const __nv_bfloat16 v = __float2bfloat16_rn(tile[i][cc]);
+            for (int k = 0; k < copies; ++k) out[((long long)k * C + c0 + cc) * L + margin + q - (k - copies / 2)] = v;
+        }
+    }
+}
+
+// bf16 operand copies of the tensor-core convs' fp32 master weights w_kn [9*Cin, Cout] (k = tap*Cin + ci), all convs in one launch
+// (grid.y = conv).  A block moves a 32 (k) x 32 (co) tile: the data-gradient layout bw[ci][(8 - tap)*Cout + co] is written in read order,
+// the forward layout fw[co][k] through a shared-memory transpose.
+__global__ void __launch_bounds__(256) conv_weights_bf16_kernel(const vf_conv_weights_bf16_t* __restrict__ table) {
+    __shared__ float tile[32][33];
+    const vf_conv_weights_bf16_t d = table[blockIdx.y];
+    const int cin = (int)d.cin, cout = (int)d.cout, K = 9 * cin;
+    const int kt = (K + 31) / 32, ct = (cout + 31) / 32;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    __nv_bfloat16* fw = reinterpret_cast<__nv_bfloat16*>(d.fw_bf16);
+    __nv_bfloat16* bw = reinterpret_cast<__nv_bfloat16*>(d.bw_bf16);
+    for (int tl = blockIdx.x; tl < kt * ct; tl += gridDim.x) {
+        const int k0 = (tl / ct) * 32, co0 = (tl % ct) * 32;
+        for (int i = warp; i < 32; i += 8) {
+            const int k = k0 + i, co = co0 + lane;
+            float v = 0.f;
+            if (k < K && co < cout) {
+                v = __ldg(d.w_kn + (long long)k * cout + co);
+                if (bw) {
+                    const int tap = k / cin, ci = k - tap * cin;
+                    bw[(long long)ci * 9 * cout + (8 - tap) * cout + co] = __float2bfloat16_rn(v);
+                }
+            }
+            tile[i][lane] = v;
+        }
+        __syncthreads();
+        for (int i = warp; i < 32; i += 8) {
+            const int co = co0 + i, k = k0 + lane;
+            if (co < cout && k < K) fw[(long long)co * K + k] = __float2bfloat16_rn(tile[lane][i]);
+        }
+        __syncthreads();
+    }
+}
+
 // out[g * n + i] (+)= sum_s partial[(g * splits + s) * n + i]   — folds the split-K partial products of the weight-gradient GEMM
 __global__ void sum_splits_kernel(const float* __restrict__ partial, int groups, int splits, long long n, int accumulate, float* __restrict__ out) {
     const long long total = (long long)groups * n;
@@ -494,6 +590,29 @@ extern "C" int vf_pad_transpose_split(const float* x, int N, int H, int W, int C
     dim3 grid((unsigned)((P + 63) / 64), (unsigned)((C + 31) / 32));
     pad_transpose_split_kernel<<<grid, 256, 0, vf_s(s)>>>(x, N, H, W, C, pitch, copies, margin, L, reinterpret_cast<__half*>(out_f16));
     VF_CHECK_LAUNCH("vf_pad_transpose_split");
+    return VF_OK;
+}
+extern "C" int vf_pad_transpose_bf16(const float* x, int N, int H, int W, int C, int upsample2x, int pitch, int copies, int64_t margin, int64_t L,
+                                     const float* mean_rstd, const float* gamma, const float* beta, int groups, int swish, void* out_bf16,
+                                     vf_stream_t s) {
+    VF_CHECK_ARG(x && out_bf16 && N > 0 && H > 0 && W > 0 && C > 0 && (upsample2x == 0 || upsample2x == 1), "vf_pad_transpose_bf16: bad args");
+    const int LH = H << upsample2x, LW = W << upsample2x;
+    VF_CHECK_ARG((pitch >= LW + 2 || (pitch == 0 && copies == 1)) && (copies == 1 || copies == 3) && margin >= copies / 2,
+                 "vf_pad_transpose_bf16: pitch / copies / margin");
+    VF_CHECK_ARG(L >= margin + (pitch ? (int64_t)N * (LH + 2) * pitch : (int64_t)N * LH * LW) + copies / 2, "vf_pad_transpose_bf16: row length L too small");
+    VF_CHECK_ARG(!mean_rstd || (gamma && beta && groups > 0 && C % groups == 0), "vf_pad_transpose_bf16: GroupNorm needs gamma, beta and groups dividing C");
+    const long long P = (long long)N * LH * LW;
+    dim3 grid((unsigned)((P + 63) / 64), (unsigned)((C + 31) / 32));
+    pad_transpose_bf16_kernel<<<grid, 256, 0, vf_s(s)>>>(x, N, H, W, C, upsample2x, pitch, copies, margin, L, mean_rstd, gamma, beta, groups, swish,
+                                                         reinterpret_cast<__nv_bfloat16*>(out_bf16));
+    VF_CHECK_LAUNCH("vf_pad_transpose_bf16");
+    return VF_OK;
+}
+extern "C" int vf_conv_weights_bf16(const vf_conv_weights_bf16_t* table, int n, vf_stream_t s) {
+    VF_CHECK_ARG(table && n >= 0 && n <= 65535, "vf_conv_weights_bf16: bad args");
+    if (n == 0) return VF_OK;
+    conv_weights_bf16_kernel<<<dim3(132, (unsigned)n), 256, 0, vf_s(s)>>>(table);
+    VF_CHECK_LAUNCH("vf_conv_weights_bf16");
     return VF_OK;
 }
 extern "C" int vf_sum_splits(const float* partial, int groups, int splits, int64_t n, int accumulate, float* out, vf_stream_t s) {
@@ -537,7 +656,7 @@ extern "C" int vf_col_sums(const float* x, int64_t rows, int C, float* out, vf_s
 
 extern "C" int vf_groupnorm_bwd(const float* x, const float* dout, const float* mean_rstd, const float* gamma, const float* beta, int N,
                                 int HW, int C, int groups, int swish, const float* add, double* gsums, float* dgamma, float* dbeta,
-                                float* dx, vf_stream_t s) {
+                                float* dx, void* dx_bf16, vf_stream_t s) {
     VF_CHECK_ARG(x && dout && mean_rstd && gamma && beta && gsums && dgamma && dbeta && dx, "vf_groupnorm_bwd: null pointer");
     VF_CHECK_ARG(C % groups == 0 && C % 4 == 0 && C / 4 <= 256 && 256 % (C / 4) == 0 && N <= 65535, "vf_groupnorm_bwd: unsupported C=%d groups=%d", C, groups);
     if (N == 0 || HW == 0) return VF_OK;
@@ -552,7 +671,8 @@ extern "C" int vf_groupnorm_bwd(const float* x, const float* dout, const float* 
     int ppb2 = lanes * 16;          // the streaming pass keeps many short blocks in flight
     while (ppb2 > lanes * 4 && (long long)((HW + ppb2 - 1) / ppb2) * N < 132 * 8) ppb2 >>= 1;
     dim3 grid2((HW + ppb2 - 1) / ppb2, N);
-    gn_bwd_apply_kernel<<<grid2, 256, 0, vf_s(s)>>>(x, dout, mean_rstd, gamma, beta, gsums, add, HW, C, groups, swish, ppb2, dx);
+    gn_bwd_apply_kernel<<<grid2, 256, 0, vf_s(s)>>>(x, dout, mean_rstd, gamma, beta, gsums, add, HW, C, groups, swish, ppb2, dx,
+                                                                      reinterpret_cast<__nv_bfloat16*>(dx_bf16));
     VF_CHECK_LAUNCH("vf_groupnorm_bwd(apply)");
     return VF_OK;
 }

@@ -21,6 +21,14 @@ their forward pass and their data gradient on the exact split-fp16 tensor-core k
 DESIGN.md 5.3; ``VF_TRAIN_TC=0`` keeps everything on the CUDA cores), and their weight gradient as nine exact GEMMs over the pixel axis
 (``_lib.conv_wgrad_tc``) when both channel counts are multiples of 128; strided / upsampling convs, 1x1 layers and the remaining weight
 gradients use the fp32 CUDA-core kernels.
+
+``precision="bf16"`` (BASELINE configs[3]: bf16 activations over fp32 master weights) runs every conv that a bf16-built model puts on the
+tensor cores (3x3, Cin % 64 == 0, Cout % 16 == 0, Cout >= 64) as ONE bf16 wgmma pass: forward (stride-2 convs on the space-to-depth
+operand), data gradient (flipped bf16 weights) and weight gradient (``_lib.conv_wgrad_bf16``, bf16 operands transposed with GroupNorm(+swish)
+or the x2 upsample applied on the way).  Accumulation, conv outputs (the residual stream), GroupNorm statistics and backward, the loss, the
+gradient buffers, the all-reduce, Adam and the whole quantizer block stay fp32, as do conv_in / conv_out, the 1x1 layers, the attention
+blocks and the stride-2 convs' gradients.  No loss scaling: bf16 has fp32's exponent range.  The bf16 weight operands are rewritten from
+the fp32 master weights by one kernel after every Adam step.
 """
 import math
 import os
@@ -40,7 +48,11 @@ class _P:
 
 
 class VQGANTrainer:
-    def __init__(self, model, lr=None, betas=(0.5, 0.9), eps=1e-8, bucket_bytes=64 << 20, process_group=None):
+    def __init__(self, model, lr=None, betas=(0.5, 0.9), eps=1e-8, bucket_bytes=64 << 20, process_group=None, precision="fp32"):
+        """``precision``: "fp32" (the reference's arithmetic) or "bf16" (single-pass bf16 tensor-core convs, see the module docstring);
+        either way the model is built with precision="fp32" and its fp32 weights are the master copy."""
+        if precision not in ("fp32", "bf16"):
+            raise ValueError("VQGANTrainer precision must be 'fp32' or 'bf16'")
         if model.enc_prec.name != "fp32" or model.dec_prec.name != "fp32":
             raise ValueError("VQGANTrainer runs the fp32 path (the reference asserts no mixed precision, vqgan_th.py:326): build the model "
                              "with precision='fp32'")
@@ -57,16 +69,22 @@ class VQGANTrainer:
         self.last = {}
         self.use_tc = os.environ.get("VF_TRAIN_TC", "1") != "0"
         self._wsplit = {}
+        self.precision, self.bf16 = precision, precision == "bf16"
+        if self.bf16:
+            self._setup_bf16_weights()
 
     # ------------------------------------------------------------------ parameter registry
     def _collect_params(self):
         w = self.model._w
         ps = []
 
+        self._convs = []
+
         def conv(name, cw):
             key = "w_kn" if hasattr(cw, "w_kn") else None
             if key is None:
                 raise RuntimeError(f"{name}: tensor-core weight layout in an fp32 model")
+            self._convs.append((name, cw))
             ps.append(_P(name + ".weight", cw.w_kn, lambda t, cw=cw: setattr(cw, "w_kn", t), "conv", cin=cw.cin))
             ps.append(_P(name + ".bias", cw.bias, lambda t, cw=cw: setattr(cw, "bias", t), "vec"))
 
@@ -152,6 +170,25 @@ class VQGANTrainer:
         self._bucket_size = [sum(1 for b in self._bucket_of.values() if b == i) for i in range(len(self.buckets))]
         self.model._refresh_decode_table()
 
+    def _setup_bf16_weights(self):
+        """bf16 operand copies of every tensor-core conv's weights: forward [Cout, 9 Cin] and (stride-1 convs) data gradient [Cin, 9 Cout],
+        rewritten from the fp32 master weights in the flat buffer by one launch per step (``_refresh_bf16_weights``)."""
+        dev = self.model.device
+        self._wb16, entries = {}, []
+        for name, cw in self._convs:
+            stride = 2 if name.endswith("downsample.conv") else 1
+            if not self._tc_ok(cw, stride, False):
+                continue
+            fw = torch.empty((cw.cout, 9 * cw.cin), dtype=torch.bfloat16, device=dev)
+            bw = torch.empty((cw.cin, 9 * cw.cout), dtype=torch.bfloat16, device=dev) if stride == 1 else None
+            self._wb16[id(cw)] = (fw, bw)
+            entries.append((cw.w_kn, fw, bw))
+        self._wb16_table = L.conv_weights_bf16_table(entries, dev)
+        self._refresh_bf16_weights()
+
+    def _refresh_bf16_weights(self):
+        L.conv_weights_bf16(self._wb16_table)
+
     # ------------------------------------------------------------------ data-parallel exchange
     def _world(self):
         import torch.distributed as dist
@@ -178,19 +215,26 @@ class VQGANTrainer:
         st = L.gn_mean_rstd(x)
         return st
 
-    def _gn_apply(self, x, st, nw, swish):
+    def _gn_apply(self, x, st, nw, swish, dtype=torch.float32):
         n, h, w, c = x.shape
-        y = torch.empty_like(x)
+        y = torch.empty(x.shape, dtype=dtype, device=x.device)
         lib = L.load(True)
         L._check(lib.vf_groupnorm_apply(L._p(x), L.F32, L._p(st), L._p(nw[0]), L._p(nw[1]), n, h, w, c, 32, L.C.c_float(1e-6), 1, int(swish), 0,
-                                        L._p(y), L.F32, L._stream()))
+                                        L._p(y), L._dt(y), L._stream()))
         return y
+
+    def _act(self, x, st, nw, swish, cw):
+        """GroupNorm(+swish) of x as the operand of conv ``cw``: bf16 when the bf16 step runs that conv on the tensor cores, else fp32."""
+        return self._gn_apply(x, st, nw, swish, torch.bfloat16 if self.bf16 and self._tc_ok(cw, 1, False) else torch.float32)
 
     # 3x3 stride-1 convolutions whose channel counts fit the tensor-core tiles run on the EXACT split-fp16 tensor-core path (three fp16 MMA
     # passes, chunked accumulation: fp32-faithful results, DESIGN.md 5.3) in the forward pass and in the data gradient; everything else
     # (conv_in / conv_out, stride-2 and upsampling convs, 1x1 layers) and every weight gradient stays on the fp32 CUDA-core kernels.
     def _tc_ok(self, cw, stride, upsample):
-        """3x3 stride-1 convs, incl. the Upsample convs (nearest x2, then a stride-1 conv on the doubled map: vqgan_th.py:29-32)."""
+        """3x3 stride-1 convs, incl. the Upsample convs (nearest x2, then a stride-1 conv on the doubled map: vqgan_th.py:29-32).
+        bf16 step: the convs a bf16-built model runs on the tensor cores (_Conv3.tc), stride-2 ones included."""
+        if self.bf16:
+            return cw.k == 3 and cw.cin % 64 == 0 and cw.cout % 16 == 0 and cw.cout >= 64
         return self.use_tc and cw.k == 3 and stride == 1 and cw.cin % 64 == 0 and cw.cout % 64 == 0
 
     def _split_weight(self, key, w_kn, n_out):
@@ -209,7 +253,21 @@ class VQGANTrainer:
         n, h, w, c = x.shape
         return L.split_f16x2(x.reshape(n * h * w, c)).reshape(n, h, w, 2 * c)
 
+    @staticmethod
+    def _b16(t):
+        """The bf16 operand copy of an fp32 gradient: the one its producer wrote alongside (``_bf16``), else one rounding pass."""
+        hit = getattr(t, "_bf16", None)
+        return hit if hit is not None else L.groupnorm(t, None, None, swish=False, out_dtype=torch.bfloat16, normalize=False)
+
     def _conv_fw(self, cw, a, residual=None, stride=1, upsample=False):
+        if self.bf16 and self._tc_ok(cw, stride, upsample):
+            fw = self._wb16[id(cw)][0]
+            if stride == 2:                                     # space-to-depth operand: a stride-1 tap-table conv (as the bf16 model)
+                a16 = L.groupnorm(a, None, None, swish=False, out_dtype=torch.bfloat16, normalize=False, s2d=True)
+                return L.tc_conv(a16, fw, cw.bias, taps=L.TAPS_S2D, coffs=L.s2d_coffs(cw.cin), cin=cw.cin)
+            if upsample or a.dtype != torch.bfloat16:
+                a = L.groupnorm(a, None, None, swish=False, out_dtype=torch.bfloat16, normalize=False, upsample=upsample)
+            return L.tc_conv(a, fw, cw.bias, residual=residual)
         if self._tc_ok(cw, stride, upsample):
             a_split = (L.groupnorm(a, None, None, swish=False, out_dtype=torch.float16, normalize=False, upsample=True) if upsample
                        else self._split_act(a))
@@ -246,6 +304,26 @@ class VQGANTrainer:
         dx = L.simt_conv(dy, wd, None, kh=cw.k, stride=1, pad=(1, 1) if cw.k == 3 else (0, 0))
         return L.sumpool2x2(dx) if upsample else dx
 
+    def _conv_bw16(self, name, cw, x, dy, norm=None, stride=1, upsample=False, need_dx=True):
+        """bf16 step.  x: the conv's fp32 input BEFORE ``norm`` = (mean_rstd, (gamma, beta), swish) and before the x2 upsample; dy fp32.
+        Accumulates dW, db; returns dx (or None)."""
+        if stride == 2 or not self._tc_ok(cw, stride, upsample):     # the fp32 step's kernels
+            a = x if norm is None else self._gn_apply(x, norm[0], norm[1], norm[2])
+            return self._conv_bw(name, cw, a, dy, stride=stride, upsample=upsample, need_dx=need_dx)
+        P = self.P
+        gw = P[name + ".weight"].grad
+        if L.conv_wgrad_bf16_ok(x, dy, cw.k, stride, upsample):
+            L.conv_wgrad_bf16(x, dy, gw, norm=None if norm is None else (norm[0], norm[1][0], norm[1][1], norm[2]), upsample=upsample)
+        else:
+            a = x if norm is None else self._gn_apply(x, norm[0], norm[1], norm[2])
+            L.conv_wgrad(a, dy, gw, kh=cw.k, stride=1, pad=(1, 1), upsample=upsample)
+        L.col_sums(dy.reshape(-1, cw.cout), P[name + ".bias"].grad)
+        self._grad_ready(P[name + ".bias"]); self._grad_ready(P[name + ".weight"])
+        if not need_dx:
+            return None
+        dx = L.tc_conv(self._b16(dy), self._wb16[id(cw)][1], None)
+        return L.sumpool2x2(dx) if upsample else dx
+
     def _lin_bw(self, name, ln, x_rows, dy_rows, residual=None):
         """y = x W^T + b.  Accumulates dW [out,in], db; returns dx = dy W (+ residual)."""
         P = self.P
@@ -261,9 +339,9 @@ class VQGANTrainer:
     def _res_fw(self, r, x, tape, name):
         ex = self.model.exact
         st1 = L.gn_mean_rstd(x)
-        h = self._conv_fw(r["c1"], self._gn_apply(x, st1, r["n1"], True))
+        h = self._conv_fw(r["c1"], self._act(x, st1, r["n1"], True, r["c1"]))
         st2 = L.gn_mean_rstd(h)
-        a2 = self._gn_apply(h, st2, r["n2"], True)
+        a2 = self._act(h, st2, r["n2"], True, r["c2"])
         n, hh, ww, c = x.shape
         res = linear(ex, x.reshape(-1, c), r["sc"], torch.float32).reshape(n, hh, ww, -1) if "sc" in r else x
         y = self._conv_fw(r["c2"], a2, residual=res)
@@ -273,18 +351,26 @@ class VQGANTrainer:
     def _res_bw(self, entry, dy):
         _, name, r, x, st1, h, st2 = entry
         P = self.P
-        a2 = self._gn_apply(h, st2, r["n2"], True)
-        da2 = self._conv_bw(name + ".conv2", r["c2"], a2, dy)
-        dh = L.groupnorm_bwd(h, da2, st2, r["n2"][0], r["n2"][1], P[name + ".norm2.weight"].grad, P[name + ".norm2.bias"].grad, swish=True)
+        if self.bf16:
+            da2 = self._conv_bw16(name + ".conv2", r["c2"], h, dy, norm=(st2, r["n2"], True))
+        else:
+            a2 = self._gn_apply(h, st2, r["n2"], True)
+            da2 = self._conv_bw(name + ".conv2", r["c2"], a2, dy)
+        dh = L.groupnorm_bwd(h, da2, st2, r["n2"][0], r["n2"][1], P[name + ".norm2.weight"].grad, P[name + ".norm2.bias"].grad, swish=True,
+                             out_bf16=self.bf16)
         self._grad_ready(P[name + ".norm2.bias"]); self._grad_ready(P[name + ".norm2.weight"])
-        a1 = self._gn_apply(x, st1, r["n1"], True)
-        da1 = self._conv_bw(name + ".conv1", r["c1"], a1, dh)
+        if self.bf16:
+            da1 = self._conv_bw16(name + ".conv1", r["c1"], x, dh, norm=(st1, r["n1"], True))
+        else:
+            a1 = self._gn_apply(x, st1, r["n1"], True)
+            da1 = self._conv_bw(name + ".conv1", r["c1"], a1, dh)
         n, hh, ww, c = x.shape
         if "sc" in r:
             dres = self._lin_bw(name + ".nin_shortcut", r["sc"], x.reshape(-1, c), dy.reshape(-1, dy.shape[-1])).reshape(x.shape)
         else:
             dres = dy
-        dx = L.groupnorm_bwd(x, da1, st1, r["n1"][0], r["n1"][1], P[name + ".norm1.weight"].grad, P[name + ".norm1.bias"].grad, swish=True, add=dres)
+        dx = L.groupnorm_bwd(x, da1, st1, r["n1"][0], r["n1"][1], P[name + ".norm1.weight"].grad, P[name + ".norm1.bias"].grad, swish=True, add=dres,
+                             out_bf16=self.bf16)
         self._grad_ready(P[name + ".norm1.bias"]); self._grad_ready(P[name + ".norm1.weight"])
         return dx
 
@@ -333,7 +419,7 @@ class VQGANTrainer:
         da = self._lin_bw(name + ".v", aw["v"], a, dv)
         da = self._lin_bw(name + ".qk", aw["qk"], a, dqk, residual=da)
         dx = L.groupnorm_bwd(x, da.reshape(x.shape), st, aw["norm"][0], aw["norm"][1], P[name + ".norm.weight"].grad, P[name + ".norm.bias"].grad,
-                             swish=False, add=dy)
+                             swish=False, add=dy, out_bf16=self.bf16)
         self._grad_ready(P[name + ".norm.bias"]); self._grad_ready(P[name + ".norm.weight"])
         return dx
 
@@ -408,7 +494,8 @@ class VQGANTrainer:
                 dy = self._attn_bw(entry, dy)
             elif kind == "conv":
                 _, name, cw, xin, stride, ups, need_dx = entry
-                dy = self._conv_bw(name, cw, xin, dy, stride=stride, upsample=ups, need_dx=need_dx)
+                conv_bw = self._conv_bw16 if self.bf16 else self._conv_bw
+                dy = conv_bw(name, cw, xin, dy, stride=stride, upsample=ups, need_dx=need_dx)
                 if name == "decoder.conv_in":
                     # through post_quant_conv, the straight-through estimator and the commitment term, quant_conv
                     dq = self._lin_bw("post_quant_conv", w["post_quant_conv"], quant, dy.reshape(-1, dy.shape[-1]))
@@ -427,7 +514,7 @@ class VQGANTrainer:
                 cw = blk["conv_out"]
                 a = self._gn_apply(xin, st, nw, True)
                 da = self._conv_bw(cname, cw, a, dy)
-                dy = L.groupnorm_bwd(xin, da, st, nw[0], nw[1], P[nname + ".weight"].grad, P[nname + ".bias"].grad, swish=True)
+                dy = L.groupnorm_bwd(xin, da, st, nw[0], nw[1], P[nname + ".weight"].grad, P[nname + ".bias"].grad, swish=True, out_bf16=self.bf16)
                 self._grad_ready(P[nname + ".bias"]); self._grad_ready(P[nname + ".weight"])
         model.training = was_training
         if any(self._bucket_left):
@@ -442,6 +529,8 @@ class VQGANTrainer:
         L.adam(self.flat_p, self.flat_g, self.flat_m, self.flat_v, lr=self.lr, beta1=self.betas[0], beta2=self.betas[1], eps=self.eps,
                step=self.step_count, grad_scale=1.0 / self._world())
         self._wsplit = {}                               # split-fp16 operand copies of the conv weights are stale now
+        if self.bf16:
+            self._refresh_bf16_weights()
         if self.model.quantizer == "commit":
             self.model._refresh_codebook()
         else:

@@ -50,14 +50,19 @@ class _Conv3:
 class VQGAN:
     _ignore_checkpoint_attributes = [r"perceptual_loss\..*", r"loss\..*"]
 
-    def __init__(self, config=None, precision="bf16", device="cuda", quantizer="ema", beta=0.25, **config_overrides):
+    def __init__(self, config=None, precision="bf16", device="cuda", quantizer="ema", beta=0.25, train_precision="fp32", **config_overrides):
         """``quantizer``: "ema" = QuantizeEMA (utils_th.py:8-72, what vqgan_th.py:331 instantiates) or "commit" = Quantize
-        (utils_th.py:75-124: the codebook is a gradient-trained parameter, loss = |sg(q) - z|^2 + beta |q - sg(z)|^2)."""
+        (utils_th.py:75-124: the codebook is a gradient-trained parameter, loss = |sg(q) - z|^2 + beta |q - sg(z)|^2).
+        ``train_precision``: arithmetic of configure_optimizers() / training_step() on a model built with precision="fp32" — "fp32" (the
+        reference's) or "bf16" (bf16 tensor-core convs over the fp32 master weights, see viewformer_b200.train)."""
         if config is None:
             config = VQGANConfig(**config_overrides)
         if quantizer not in ("ema", "commit"):
             raise ValueError("quantizer must be 'ema' (QuantizeEMA) or 'commit' (Quantize, beta-weighted commitment loss)")
         self.quantizer, self.beta = quantizer, float(beta)
+        if train_precision not in ("fp32", "bf16"):
+            raise ValueError("train_precision must be 'fp32' or 'bf16'")
+        self.train_precision = train_precision
         self.config = load_config(config)
         # ``mixed``: the encoder (whose output feeds the bit-exact codebook argmin) runs in the fp32-faithful ``exact`` arithmetic,
         # the decoder (pixels within a tolerance) on the bf16 tensor-core path.  One precision name otherwise serves both halves.
@@ -635,7 +640,7 @@ class VQGAN:
         """The trainer object that owns Adam(betas=(0.5, 0.9), lr=config.learning_rate) and the flat parameter / gradient buffers."""
         from .train import VQGANTrainer
         if getattr(self, "_trainer", None) is None:
-            self._trainer = VQGANTrainer(self)
+            self._trainer = VQGANTrainer(self, precision=self.train_precision)
         return self._trainer
 
     @L.on_model_device
