@@ -182,6 +182,18 @@ int vf_attn_block_causal_decode(const void* qk_bf16, const void* vt_bf16, int B,
  * Streams >= 1 need block == 64.  Same fused kernel: the key-tile schedule changes, nothing is materialised in HBM. */
 int vf_attn_block_multiend(const void* qk_bf16, const void* vt_bf16, int B, int S, int n_streams, int stream, int H, int d, int block,
                            void* out_bf16, vf_stream_t s);
+/* Training forward of one stream (bf16 transformer training step): vf_attn_block_multiend plus the natural-log log-sum-exp of every query
+ * row (lse [B, H, S], nullable), an fp32 copy of the output (out_f32 [B*S, d], nullable) and inverted dropout of the probabilities before
+ * the P.V product, with vf_dropout's hash mask over this stream's [B, H, S, cols] probability tensor (cols = S for stream 0, 2S with the
+ * own-stream keys at columns S + j for streams >= 1).  rate 0 and no outputs: the bits of vf_attn_block_multiend. */
+int vf_attn_multiend_train(const void* qk_bf16, const void* vt_bf16, int B, int S, int n_streams, int stream, int H, int d, int block,
+                           float rate, uint64_t seed, float* lse, float* out_f32, void* out_bf16, vf_stream_t s);
+/* Fused backward of the multi-end attention of all n_streams streams: P is recomputed from Q, K and lse ([n_streams, B, H, S]) with the
+ * forward pass's dropout mask (stream s uses seed + s); dout bf16 [n_streams, B*S, d], out fp32 [n_streams, B*S, d] (D = rowsum(dout*out)).
+ * dvqk fp32 [n_streams, B*S, 3d], columns v | q | k (zeroed by the caller): stream-0 keys / values get gradient from every stream's
+ * queries, stream-s keys / values only from stream s.  Head dim 64, block = 64; no S x S tensor in global memory. */
+int vf_attn_multiend_bwd(const void* qk_bf16, const void* vt_bf16, const void* dout_bf16, const float* out, const float* lse, int B, int S,
+                         int n_streams, int H, int d, int block, float rate, uint64_t seed, float* dvqk, vf_stream_t s);
 
 /* ------------------------------------------------------------------------------------------
  * Backward pass of the codebook training step (models/vqgan_th.py:395-423, 443-445), fp32.  Data gradients of convolutions and dense
@@ -252,6 +264,13 @@ int vf_adamw_keras(float* p, const float* g, float* m, float* v, int64_t n, floa
                    float weight_decay, int step, float grad_scale, float clip_scale, vf_stream_t s);
 int vf_sumsq(const float* x, int64_t n, double* out, vf_stream_t s);
 int vf_dropout(const float* x, int64_t n, float rate, uint64_t seed, float* y, vf_stream_t s);
+/* bf16 transformer training step.
+ *   vf_to_bf16: y_bf16 = bf16(dropout(x)) with vf_dropout's mask (rate 0: plain round-to-nearest-even); y (nullable) = the fp32 dropout(x).
+ *   vf_dense_weights_bf16: one launch over `n` dense layers (table in device memory) writes the bf16 operands of each from its fp32 master
+ *     weights w_kn [k, n]: fw [n][k] (the forward GEMM's K-major weights) and bw [k][n] (the data gradient's), either nullable. */
+typedef struct { const float* w_kn; void* fw_bf16; void* bw_bf16; int64_t k, n; } vf_dense_weights_bf16_t;
+int vf_to_bf16(const float* x, int64_t n, float rate, uint64_t seed, float* y, void* y_bf16, vf_stream_t s);
+int vf_dense_weights_bf16(const vf_dense_weights_bf16_t* table, int n, vf_stream_t s);
 
 /* ------------------------------------------------------------------------------------------
  * Evaluation-side kernels (SURVEY.md §8 f2 / f3)

@@ -1,26 +1,55 @@
-"""Full-size transformer training step timing (MIGTConfig defaults: 12 layers, d = 768; B scenes x 20 views x 64 tokens)."""
-import os, sys
+"""Full-size transformer training step timing (MIGTConfig defaults: 12 layers, d = 768; B scenes x T views x 64 tokens), the fp32-faithful and
+the bf16 trainer alternated in one process (three timed runs each, after a warm-up), with each trainer's peak allocated memory.  The default
+B = 5, T = 20 is the InteriorNet recipe's batch of 40 scenes over 8 GPUs.  VF_B / VF_T / VF_STEPS change the shape and the steps per run."""
+import os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
 import torch
 from oracle import synth, migt_oracle as mo
 from viewformer_b200 import MIGT
 from viewformer_b200.config import MIGTConfig
 from viewformer_b200.train_migt import MIGTTrainer
 
-B, T = int(os.environ.get("VF_B", "4")), 20
+B, T, n = int(os.environ.get("VF_B", "5")), int(os.environ.get("VF_T", "20")), int(os.environ.get("VF_STEPS", "3"))
 cfg = MIGTConfig()
 model = MIGT(cfg, precision="fp32").init_weights(0)
-tr = MIGTTrainer(model)
 codes = synth.make_codes(B, T, n_embed=cfg.n_embeddings, seed=1)
 cams = mo.normalize_cameras(mo.to_relative_cameras(synth.make_cameras(B, T, seed=2))[0])
-for _ in range(2):
-    tr.forward_backward(cams, codes); tr.optimizer_step()
-torch.cuda.synchronize()
-e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-e0.record()
-n = 3
-for _ in range(n):
-    loss = tr.forward_backward(cams, codes); tr.optimizer_step()
-e1.record(); torch.cuda.synchronize()
-ms = e0.elapsed_time(e1) / n
-print(f"[migt train step, full size] B={B} T={T}: {ms:.1f} ms/step -> {B * T * 64 / ms * 1e3:.0f} tokens/s; loss {float(loss):.4f}")
+try:
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+except OSError:
+    card = "unknown"
+print(f"[card] {torch.cuda.get_device_name()} | nvidia-smi: {card}")
+
+
+def run(tr, steps):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(steps):
+        loss = tr.forward_backward(cams, codes)
+        tr.optimizer_step()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps, float(loss)
+
+
+trainers, times, peaks, losses = {}, {}, {}, {}
+for prec in ("fp32", "bf16"):
+    trainers[prec] = MIGTTrainer(model, precision=prec)
+    times[prec] = []
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    base = torch.cuda.memory_allocated()                       # the trainers' weights, gradients and moments
+    run(trainers[prec], 2)                                     # warm-up: module loads, operand buffers
+    peaks[prec] = torch.cuda.max_memory_allocated() - base
+for _ in range(3):
+    for prec in ("fp32", "bf16"):
+        ms, losses[prec] = run(trainers[prec], n)
+        times[prec].append(ms)
+for prec in ("fp32", "bf16"):
+    t = np.array(times[prec])
+    med = float(np.median(t))
+    print(f"[migt train step, full size, {prec}] B={B} T={T}: median {med:.1f} ms/step (runs {', '.join(f'{x:.1f}' for x in t)}; "
+          f"spread {t.max() - t.min():.1f} ms) -> {B * T * 64 / med * 1e3:.0f} tokens/s; step peak {peaks[prec] / 2**30:.2f} GiB above the trainers' state; "
+          f"loss {losses[prec]:.4f}")
+print(f"[bf16 vs fp32] {np.median(times['fp32']) / np.median(times['bf16']):.2f}x")

@@ -27,6 +27,7 @@ EXPORTS = [
     "vf_vq_prepare_codebook_f16", "vf_vq_lookup_fused", "vf_resize_u8", "vf_image_pair_sums", "vf_ssim_u8", "vf_ssim_u8_k",
     "vf_conv_wgrad", "vf_pad_transpose_split", "vf_pad_transpose_bf16", "vf_conv_weights_bf16", "vf_sum_splits", "vf_col_sums", "vf_groupnorm_bwd", "vf_softmax_bwd_rows", "vf_l1_grad", "vf_lincomb3", "vf_sumpool2x2", "vf_adam",
     "vf_layernorm_bwd", "vf_gelu_fwd", "vf_gelu_bwd", "vf_migt_embed_bwd", "vf_cross_entropy_grad", "vf_pose_loss_grad", "vf_adamw_keras", "vf_sumsq", "vf_dropout",
+    "vf_attn_multiend_train", "vf_attn_multiend_bwd", "vf_to_bf16", "vf_dense_weights_bf16",
 ]
 
 
@@ -685,6 +686,65 @@ def attn_block_multiend(qk, vt, B, S, n_streams, stream, H, d, block, out=None):
     return out
 
 
+def attn_multiend_train(qk, vt, B, S, n_streams, stream, H, d, block, *, rate=0.0, seed=0, lse=None, out_f32=None, out=None):
+    """Training forward of stream ``stream`` of the multi-end attention: attn_block_multiend plus the per-row log-sum-exp ``lse`` f32 [B,H,S]
+    and an fp32 copy ``out_f32`` [B*S, d] (both optional, written in place) and hash dropout of the probabilities (vf_dropout's mask of the
+    stream's [B,H,S,cols] tensor) -> bf16 [B*S, d]."""
+    lib = load(True)
+    _dev(qk, torch.bfloat16)
+    _dev(vt, torch.bfloat16)
+    if out is None:
+        out = torch.empty((B * S, d), dtype=torch.bfloat16, device=qk.device)
+    for t in (lse, out_f32):
+        if t is not None:
+            _dev(t, torch.float32)
+    _check(lib.vf_attn_multiend_train(_p(qk), _p(vt), B, S, n_streams, stream, H, d, block, C.c_float(rate),
+                                      C.c_uint64(int(seed) & ((1 << 64) - 1)), _p(lse), _p(out_f32), _p(out), _stream()))
+    return out
+
+
+def attn_multiend_bwd(qk, vt, dout, out_f32, lse, B, S, n_streams, H, d, block, *, rate=0.0, seed=0, dvqk=None):
+    """Fused backward of all streams: dout bf16 [ns, B*S, d], out_f32 [ns, B*S, d], lse [ns, B, H, S] -> dvqk f32 [ns, B*S, 3d] (v | q | k).
+    Stream s's dropout seed is seed + s (the sites of the fp32 trainer)."""
+    lib = load(True)
+    for t, dt in ((qk, torch.bfloat16), (vt, torch.bfloat16), (dout, torch.bfloat16), (out_f32, torch.float32), (lse, torch.float32)):
+        _dev(t, dt)
+    if dvqk is None:
+        dvqk = torch.zeros((n_streams, B * S, 3 * d), dtype=torch.float32, device=qk.device)
+    _check(lib.vf_attn_multiend_bwd(_p(qk), _p(vt), _p(dout), _p(out_f32), _p(lse), B, S, n_streams, H, d, block, C.c_float(rate),
+                                    C.c_uint64(int(seed) & ((1 << 64) - 1)), _p(dvqk), _stream()))
+    return dvqk
+
+
+def to_bf16(x, rate=0.0, seed=0, out_f32=False):
+    """bf16(dropout(x)) with vf_dropout's mask (rate 0: the plain rounding); ``out_f32=True`` returns (fp32 dropout(x), bf16) from one pass."""
+    lib = load(True)
+    _dev(x, torch.float32)
+    y16 = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    y = torch.empty_like(x) if out_f32 else None
+    _check(lib.vf_to_bf16(_p(x), C.c_int64(x.numel()), C.c_float(rate), C.c_uint64(int(seed) & ((1 << 64) - 1)), _p(y), _p(y16), _stream()))
+    return (y, y16) if out_f32 else y16
+
+
+def dense_weights_bf16_table(entries, device):
+    """entries: (w_kn f32 [k, n], fw bf16 [n, k] or None, bw bf16 [k, n] or None) -> the device table of vf_dense_weights_bf16
+    (int64 [n, 5] = vf_dense_weights_bf16_t).  The tensors must outlive the table."""
+    rows = []
+    for w_kn, fw, bw in entries:
+        assert w_kn.is_cuda and w_kn.dtype == torch.float32 and w_kn.is_contiguous()
+        k, n = w_kn.shape
+        assert fw is None or (fw.dtype == torch.bfloat16 and fw.is_contiguous() and tuple(fw.shape) == (n, k))
+        assert bw is None or (bw.dtype == torch.bfloat16 and bw.is_contiguous() and tuple(bw.shape) == (k, n))
+        rows.append([w_kn.data_ptr(), fw.data_ptr() if fw is not None else 0, bw.data_ptr() if bw is not None else 0, k, n])
+    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 5).to(device)
+
+
+def dense_weights_bf16(table):
+    """Rewrite every dense layer's bf16 operand copies listed in ``table`` (dense_weights_bf16_table) from its fp32 master weights: one launch."""
+    lib = load(True)
+    _check(lib.vf_dense_weights_bf16(_p(table), table.shape[0], _stream()))
+
+
 def softmax_rows(scores, P, *, rows_total, rows_per_batch, cols, ld_in, ld_out, mask_mode=0, block=0, row0=0):
     lib = load(True)
     _check(lib.vf_softmax_rows(_p(scores), C.c_int64(rows_total), rows_per_batch, cols, C.c_int64(ld_in), mask_mode, block,
@@ -865,6 +925,33 @@ def dense_wgrad_tc(x_rows, dy_rows, dw_kn, *, accumulate=True):
     _check(lib.vf_pad_transpose_split(_p(dy_rows), 1, 1, m, n, 0, 1, C.c_int64(0), C.c_int64(lm), _p(bt), _stream()))
     tc_gemm(at, bt, partial, M=k, N=n, K=kc, lda=2 * lm, ldb=2 * lm, ldc=n, batch=(1, splits), a_bs=(0, kc), b_bs=(0, kc),
             c_bs=(0, k * n), lo_a=lm, lo_b=lm)
+    _check(lib.vf_sum_splits(_p(partial), 1, splits, C.c_int64(k * n), int(accumulate), _p(dw_kn), _stream()))
+    return dw_kn
+
+
+def dense_wgrad_bf16(x_rows, dy_rows, dw_kn, *, accumulate=True):
+    """dW[k, n] (+)= sum_m x[m, k] dy[m, n] on the single-pass bf16 tensor-core GEMM: the schedule of dense_wgrad_tc (row axis split over the
+    SMs, vf_sum_splits) with both fp32 operands rounded once to bf16 by the K-major transposer (vf_pad_transpose_bf16, plain mode)."""
+    lib = load(True)
+    _dev(x_rows, torch.float32); _dev(dy_rows, torch.float32); _dev(dw_kn, torch.float32)
+    m, k = x_rows.shape
+    n = dy_rows.shape[1]
+    tiles = (k // 128) * (n // 128)
+    splits = max(1, min(32, (132 + tiles - 1) // tiles))
+    kc = ((m + splits - 1) // splits + 63) // 64 * 64
+    lm = kc * splits
+    key = ("dense_bf16", x_rows.device, m, k, n)
+    bufs = _wgrad_bufs.get(key)
+    if bufs is None:                                           # the columns past m stay zero: cleared once
+        if len(_wgrad_bufs) >= 32:
+            _wgrad_bufs.clear()
+        bufs = (torch.zeros((k, lm), dtype=torch.bfloat16, device=x_rows.device), torch.zeros((n, lm), dtype=torch.bfloat16, device=x_rows.device),
+                torch.empty((splits, k, n), dtype=torch.float32, device=x_rows.device))
+        _wgrad_bufs[key] = bufs
+    at, bt, partial = bufs
+    pad_transpose_bf16(x_rows.reshape(1, 1, m, k), at, pitch=0, copies=1, margin=0)
+    pad_transpose_bf16(dy_rows.reshape(1, 1, m, n), bt, pitch=0, copies=1, margin=0)
+    tc_gemm(at, bt, partial, M=k, N=n, K=kc, lda=lm, ldb=lm, ldc=n, batch=(1, splits), a_bs=(0, kc), b_bs=(0, kc), c_bs=(0, k * n))
     _check(lib.vf_sum_splits(_p(partial), 1, splits, C.c_int64(k * n), int(accumulate), _p(dw_kn), _stream()))
     return dw_kn
 

@@ -421,16 +421,59 @@ __global__ void sumsq_kernel(const float* __restrict__ x, long long n, double* _
 }
 
 // inverted dropout with a counter-based hash (no state): keep = hash(seed, i) >= rate * 2^32; y = keep ? x / (1 - rate) : 0.
-// The backward pass calls it again on the gradient with the same (seed, offset).
-__device__ __forceinline__ uint32_t mix32(uint64_t k) {
-    k ^= k >> 33; k *= 0xff51afd7ed558ccdULL; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ULL; k ^= k >> 33;
-    return (uint32_t)k;
-}
+// The backward pass calls it again on the gradient with the same (seed, offset).  (mix32: vf_common.cuh)
 __global__ void dropout_kernel(const float* __restrict__ x, long long n, float rate, unsigned long long seed, float* __restrict__ y) {
-    const uint32_t thr = (uint32_t)fminf(rate * 4294967296.0f, 4294967295.0f);
+    const uint32_t thr = vf_drop_threshold(rate);
     const float sc = 1.0f / (1.0f - rate);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        y[i] = mix32(seed * 0x9E3779B97F4A7C15ULL + (unsigned long long)i) >= thr ? x[i] * sc : 0.f;
+        y[i] = vf_drop_keep(seed, (unsigned long long)i, thr) ? x[i] * sc : 0.f;
+}
+
+// bf16 training step: y16 = bf16(dropout(x)) (rate 0: the plain rounding), and y = dropout(x) in fp32 when y is not null — the bf16 operand of
+// a tensor-core GEMM and, where the fp32 value is also needed, its fp32 twin from the same pass, with vf_dropout's mask.
+__global__ void to_bf16_kernel(const float* __restrict__ x, long long n, float rate, unsigned long long seed, float* __restrict__ y,
+                               __nv_bfloat16* __restrict__ y16) {
+    const uint32_t thr = vf_drop_threshold(rate);
+    const float sc = 1.0f / (1.0f - rate);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        float v = x[i];
+        if (rate > 0.f) v = vf_drop_keep(seed, (unsigned long long)i, thr) ? v * sc : 0.f;
+        if (y) y[i] = v;
+        y16[i] = __float2bfloat16_rn(v);
+    }
+}
+
+// bf16 operand copies of the dense layers' fp32 master weights w_kn [k, n] (Conv1D layout), all layers in one launch (grid.y = layer):
+// fw [n][k] (the transpose: forward GEMM, K = k) through a shared-memory transpose and, when not null, bw [k][n] (same layout: data-gradient
+// GEMM, K = n) in read order.
+__global__ void __launch_bounds__(256) dense_weights_bf16_kernel(const vf_dense_weights_bf16_t* __restrict__ table) {
+    __shared__ float tile[32][33];
+    const vf_dense_weights_bf16_t d = table[blockIdx.y];
+    const int K = (int)d.k, N = (int)d.n;
+    const int kt = (K + 31) / 32, nt = (N + 31) / 32;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    __nv_bfloat16* fw = reinterpret_cast<__nv_bfloat16*>(d.fw_bf16);
+    __nv_bfloat16* bw = reinterpret_cast<__nv_bfloat16*>(d.bw_bf16);
+    for (int tl = blockIdx.x; tl < kt * nt; tl += gridDim.x) {
+        const int k0 = (tl / nt) * 32, n0 = (tl % nt) * 32;
+        for (int i = warp; i < 32; i += 8) {
+            const int k = k0 + i, n = n0 + lane;
+            float v = 0.f;
+            if (k < K && n < N) {
+                v = __ldg(d.w_kn + (long long)k * N + n);
+                if (bw) bw[(long long)k * N + n] = __float2bfloat16_rn(v);
+            }
+            tile[i][lane] = v;
+        }
+        __syncthreads();
+        if (fw) {
+            for (int i = warp; i < 32; i += 8) {
+                const int n = n0 + i, k = k0 + lane;
+                if (n < N && k < K) fw[(long long)n * K + k] = __float2bfloat16_rn(tile[lane][i]);
+            }
+        }
+        __syncthreads();
+    }
 }
 
 // ---- operands of the tensor-core weight gradient (vf_tc_gemm, exact split-fp16 GEMM with K = pixels) ----
@@ -801,5 +844,19 @@ extern "C" int vf_dropout(const float* x, int64_t n, float rate, uint64_t seed, 
     if (n == 0) return VF_OK;
     dropout_kernel<<<grid_for(n), 256, 0, vf_s(s)>>>(x, n, rate, seed, y);
     VF_CHECK_LAUNCH("vf_dropout");
+    return VF_OK;
+}
+extern "C" int vf_to_bf16(const float* x, int64_t n, float rate, uint64_t seed, float* y, void* y_bf16, vf_stream_t s) {
+    VF_CHECK_ARG(x && y_bf16 && rate >= 0.f && rate < 1.f, "vf_to_bf16: bad args");
+    if (n == 0) return VF_OK;
+    to_bf16_kernel<<<grid_for(n), 256, 0, vf_s(s)>>>(x, n, rate, seed, y, reinterpret_cast<__nv_bfloat16*>(y_bf16));
+    VF_CHECK_LAUNCH("vf_to_bf16");
+    return VF_OK;
+}
+extern "C" int vf_dense_weights_bf16(const vf_dense_weights_bf16_t* table, int n, vf_stream_t s) {
+    VF_CHECK_ARG(table && n >= 0 && n <= 65535, "vf_dense_weights_bf16: bad args");
+    if (n == 0) return VF_OK;
+    dense_weights_bf16_kernel<<<dim3(132, (unsigned)n), 256, 0, vf_s(s)>>>(table);
+    VF_CHECK_LAUNCH("vf_dense_weights_bf16");
     return VF_OK;
 }

@@ -46,6 +46,17 @@ __device__ __forceinline__ float vf_gelu_erf(float x) {
 }
 __device__ __forceinline__ float vf_swish(float x) { return x / (1.0f + expf(-x)); }
 
+// Stateless dropout hash: element i of a tensor dropped with `seed` is kept when mix32(seed * 0x9E3779B97F4A7C15 + i) >= thr,
+// thr = vf_drop_threshold(rate).  vf_dropout and the fused attention kernels share it, so they drop the same elements.
+__device__ __forceinline__ uint32_t mix32(uint64_t k) {
+    k ^= k >> 33; k *= 0xff51afd7ed558ccdULL; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ULL; k ^= k >> 33;
+    return (uint32_t)k;
+}
+__host__ __device__ __forceinline__ uint32_t vf_drop_threshold(float rate) { return (uint32_t)fminf(rate * 4294967296.0f, 4294967295.0f); }
+__device__ __forceinline__ bool vf_drop_keep(unsigned long long seed, unsigned long long i, uint32_t thr) {
+    return mix32(seed * 0x9E3779B97F4A7C15ULL + i) >= thr;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

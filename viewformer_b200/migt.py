@@ -418,7 +418,11 @@ class MIGT:
 
     # ------------------------------------------------------------------ Keras training surface (migt.py:457-505)
     def compile(self, optimizer=None, **kwargs):
-        """migt.py:457-462: AdamWeightDecay + 2000-step warm-up + cosine decay; the trainer owns the flat parameter / gradient buffers."""
+        """migt.py:457-462: AdamWeightDecay + 2000-step warm-up + cosine decay; the trainer owns the flat parameter / gradient buffers.
+        Keyword arguments go to MIGTTrainer.  ``precision="bf16"`` selects the reference's 16-bit recipe (--fp16): bf16 tensor-core
+        operands for the dense layers and the fused attention forward and backward, fp32 master weights, and dynamic loss scaling
+        (LossScaleOptimizer semantics; ``train_step`` then reports ``loss_scale``).  It needs d_model / n_head == 64 and
+        token_image_size == 8.  ``precision="fp32"`` (the default) is the fp32-faithful step."""
         from .train_migt import MIGTTrainer
         self._trainer = optimizer if optimizer is not None else MIGTTrainer(self, **kwargs)
         return self._trainer

@@ -1,4 +1,4 @@
-"""Transformer training step — MIGT.train_step (viewformer/models/migt.py:464-505) on libvf_b200 kernels, fp32.
+"""Transformer training step — MIGT.train_step (viewformer/models/migt.py:464-505) on libvf_b200 kernels, fp32 or bf16.
 
     forward   three streams as in ``call(compute_losses=True, training=True)`` (migt.py:338-455): tokens + poses, MASK tokens + query
               poses (image generation), tokens + LOC token (localisation); block-causal multi-end attention
@@ -17,6 +17,14 @@
               divided by the world size — see the note in DESIGN.md on MirroredStrategy's per-replica reduce_mean) asynchronously
               while the rest of the backward pass runs.
 
+precision="bf16" (the reference's 16-bit recipes: --fp16 -> mixed-precision policy + LossScaleOptimizer, train_transformer.py:102-104,
+models/utils.py:432-433, migt.py:466-488): every dense GEMM that fits the tensor-core tiles (forward, data and weight gradient) takes bf16
+operands in one wgmma pass; the attention runs forward in the fused multi-end kernel (vf_attn_multiend_train, which also keeps the per-row
+log-sum-exp) and backward in vf_attn_multiend_bwd, which recomputes the probabilities, so no [S, S] tensor is kept or written.  Accumulation,
+the residual stream, LayerNorm, GELU pre-activations, softmax statistics, losses, embeddings, gradients, the all-reduce, clipping and AdamW
+stay fp32; the flat fp32 buffers remain the master copy and bf16 operand copies of the weights are rewritten after every applied step.
+Dynamic loss scaling as TF 2.4's DynamicLossScale: see optimizer_step.
+
 Parameters are kept in the reference's own layouts (Conv1D weight [in, out], bias [1, out]); ``state_dict()`` can be loaded straight
 into ``viewformer_b200.MIGT`` for inference.
 """
@@ -32,11 +40,23 @@ LN_EPS = 1e-5
 
 
 class MIGTTrainer:
+    LOSS_SCALE_INIT = 2.0 ** 15                                    # tf.mixed_precision DynamicLossScale defaults (TF 2.4)
+    LOSS_SCALE_GROWTH_STEPS = 2000
+
     def __init__(self, model, betas=(0.9, 0.999), eps=1e-8, warmup_steps=2000, bucket_bytes=64 << 20, process_group=None, seed=0,
-                 grad_reduce="sum"):
+                 grad_reduce="sum", precision="fp32"):
         cfg = model.config
         if cfg.random_pose_multiplier != 1.0:
             raise NotImplementedError("random_pose_multiplier != 1 (pose-scale augmentation, migt.py:350-353) is not supported")
+        if precision not in ("fp32", "bf16"):
+            raise ValueError(f"precision must be 'fp32' or 'bf16', got {precision!r}")
+        self.precision, self.bf16 = precision, precision == "bf16"
+        if self.bf16 and (cfg.d_model % cfg.n_head or cfg.d_model // cfg.n_head != 64 or cfg.token_image_size != 8):
+            raise NotImplementedError(f"precision='bf16' needs d_model / n_head == 64 and token_image_size == 8 (the fused attention kernels), got "
+                                      f"d_model={cfg.d_model} n_head={cfg.n_head} token_image_size={cfg.token_image_size}")
+        # dynamic loss scaling (bf16 only): the scale multiplies the loss gradient seeds; updates are skipped on non-finite gradients
+        self.loss_scale = self.LOSS_SCALE_INIT if self.bf16 else 1.0
+        self.loss_scale_counter = 0
         self.model, self.cfg, self.device = model, cfg, model.device
         self.betas, self.eps, self.warmup_steps = betas, eps, warmup_steps
         self.group, self.bucket_bytes, self.seed = process_group, bucket_bytes, seed
@@ -45,13 +65,15 @@ class MIGTTrainer:
         assert grad_reduce in ("sum", "mean")
         self.grad_reduce = grad_reduce
         self.iterations = 0                                        # optimizer.iterations (0-based: the schedule sees it BEFORE the increment)
-        self.use_tc = os.environ.get("VF_TRAIN_TC", "1") != "0"
+        self.use_tc = self.bf16 or os.environ.get("VF_TRAIN_TC", "1") != "0"
         self._wsplit = {}                                          # split-fp16 operand copies of the weights, rebuilt after every step
         self.use_loc = model.use_localization
         from .schedules import parse
         self._loc_schedule = parse(cfg.localization_weight).with_total_steps(int(cfg.total_steps))
         self.dynamic_pose = bool(cfg.use_dynamic_pose_loss) and self.use_loc
         self._build(model.state_dict())
+        if self.bf16:
+            self._build_bf16_weights()
 
     @property
     def loc_weight(self):
@@ -97,6 +119,30 @@ class MIGTTrainer:
         self._bucket_size = [sum(1 for b in self._bucket_of.values() if b == i) for i in range(len(self.buckets))]
         # AdamWeightDecay: every variable except the ones whose name contains "bias" (see the module docstring)
         self.decay = {k: ("bias" not in k) for k in order}
+
+    def _build_bf16_weights(self):
+        """bf16 operand copies of every tensor-core dense layer: fw [n, k] (forward, K = k) and bw [k, n] (data gradient, K = n); rewritten
+        from the fp32 master weights by one vf_dense_weights_bf16 launch after every applied step.  The tied head uses wte[:V] as its
+        [k, n] = [V, d] matrix (logits read bw, the data gradient reads fw)."""
+        self._w16, entries = {}, []
+        for name in self.order:
+            if not name.endswith(".weight") or name.startswith("wte") or self.p[name].dim() != 2:
+                continue
+            k, n = self.p[name].shape
+            if self._tc_dense_ok(k, n):
+                layer = name[:-len(".weight")]
+                fw = torch.empty((n, k), dtype=torch.bfloat16, device=self.device)
+                bw = torch.empty((k, n), dtype=torch.bfloat16, device=self.device)
+                self._w16[layer] = (fw, bw)
+                entries.append((self.p[name], fw, bw))
+        V, d = self.cfg.n_embeddings, self.cfg.d_model
+        if self._tc_dense_ok(d, V):
+            fw = torch.empty((d, V), dtype=torch.bfloat16, device=self.device)
+            bw = torch.empty((V, d), dtype=torch.bfloat16, device=self.device)
+            self._w16["wte"] = (fw, bw)
+            entries.append((self.p["wte.weight"][:V], fw, bw))
+        self._w16_table = L.dense_weights_bf16_table(entries, self.device)
+        L.dense_weights_bf16(self._w16_table)
 
     def state_dict(self):
         return OrderedDict((k, self.p[k].detach().cpu().clone()) for k in self.model.param_shapes().keys())
@@ -144,6 +190,12 @@ class MIGTTrainer:
     def _lin(self, x, name, act=L.ACT_NONE, residual=None):
         W, b = self.p[name + ".weight"], self.p[name + ".bias"]
         k, n = W.shape
+        if self.bf16 and act == L.ACT_NONE and self._tc_dense_ok(k, n):
+            x16 = x if x.dtype == torch.bfloat16 else L.to_bf16(x)
+            out = torch.empty((x.shape[0], n), dtype=torch.float32, device=x.device)
+            L.tc_gemm(x16, self._w16[name][0], out, M=x.shape[0], N=n, K=k, lda=k, ldb=k, ldc=n, bias=b.reshape(-1), bias_mode=L.BIAS_N,
+                      residual=residual)
+            return out
         if act == L.ACT_NONE and self._tc_dense_ok(k, n):
             return self._dense_fw_tc(x, ("fw", name), lambda: W.t().contiguous(), n, k, bias=b.reshape(-1), residual=residual)
         out = torch.empty((x.shape[0], n), dtype=torch.float32, device=x.device)
@@ -151,11 +203,24 @@ class MIGTTrainer:
                     act=act, residual=residual)
         return out
 
+    def _dgrad16(self, dy, name, residual=None, out16=None):
+        """bf16 data gradient dx = dy W^T [m, k] fp32 (or, with out16, written as bf16 only)."""
+        k, n = self.p[name + ".weight"].shape
+        m = dy.shape[0]
+        dx = out16 if out16 is not None else torch.empty((m, k), dtype=torch.float32, device=dy.device)
+        L.tc_gemm(L.to_bf16(dy), self._w16[name][1], dx, M=m, N=k, K=n, lda=n, ldb=n, ldc=k, residual=residual)
+        return dx
+
     def _lin_bw(self, x, dy, name, need_dx=True, residual=None):
         W = self.p[name + ".weight"]
         k, n = W.shape
         m = x.shape[0]
         tc = self._tc_dense_ok(k, n)
+        if tc and self.bf16:
+            L.dense_wgrad_bf16(x, dy, self.g[name + ".weight"])
+            L.col_sums(dy, self.g[name + ".bias"].reshape(-1))
+            self._ready(name + ".bias", name + ".weight")
+            return self._dgrad16(dy, name, residual=residual) if need_dx else None
         if tc:
             L.dense_wgrad_tc(x, dy, self.g[name + ".weight"])
         else:
@@ -170,8 +235,8 @@ class MIGTTrainer:
         L.simt_gemm(dy, W, dx, M=m, N=k, K=n, a_strides=(n, 1), b_strides=(1, n), ldc=k, residual=residual)
         return dx
 
-    def _ln(self, x, name):
-        return L.layernorm(x, self.p[name + ".gamma"], self.p[name + ".beta"], torch.float32, eps=LN_EPS)
+    def _ln(self, x, name, dtype=torch.float32):
+        return L.layernorm(x, self.p[name + ".gamma"], self.p[name + ".beta"], dtype, eps=LN_EPS)
 
     def _ln_bw(self, x, dy, name, add=None, last=True):
         dx = L.layernorm_bwd(x, dy, self.p[name + ".gamma"], self.g[name + ".gamma"], self.g[name + ".beta"], eps=LN_EPS, add=add)
@@ -179,11 +244,14 @@ class MIGTTrainer:
             self._ready(name + ".beta", name + ".gamma")
         return dx
 
+    def _drop_seed(self, site):
+        return (self.seed * 1000003 + self.iterations) * 4096 + site
+
     def _drop(self, x, site):
         rate = float(self.cfg.dropout)
         if rate <= 0.0:
             return x
-        return L.dropout(x, rate, (self.seed * 1000003 + self.iterations) * 4096 + site)
+        return L.dropout(x, rate, self._drop_seed(site))
 
     # ------------------------------------------------------------------ attention over the stream list
     def _attention_fw(self, vqk, B, S, Lt, site0):
@@ -238,6 +306,27 @@ class MIGTTrainer:
                             b_bs=(S * 3 * d, dh), c_bs=(S * 3 * d, dh), a_off=half * S, b_off=d, c_off=2 * d, residual=dvqk[ks])
         return dvqk
 
+    def _attention_fw16(self, a16, pre, B, S, Lt, site0):
+        """bf16: a16 per stream [B*S, d] (LayerNorm output) -> q|k [B, ns*S, 2d] and V^T [B, d, ns*S] from the c_attn GEMMs, then the fused
+        training forward per stream.  Returns (outputs bf16 [ns, B*S, d], what the backward pass needs)."""
+        d, H = self.cfg.d_model, self.cfg.n_head
+        ns, dev = len(a16), a16[0].device
+        w16, bias = self._w16[pre + "attn.c_attn"][0], self.p[pre + "attn.c_attn.bias"].reshape(-1)      # [3d, d]: rows v | q | k
+        qk = torch.empty((B, ns * S, 2 * d), dtype=torch.bfloat16, device=dev)
+        vt = torch.empty((B, d, ns * S), dtype=torch.bfloat16, device=dev)
+        for s, a in enumerate(a16):
+            L.tc_gemm(a, w16, qk, M=S, N=2 * d, K=d, lda=d, ldb=d, ldc=2 * d, batch=(B, 1), a_bs=(S * d, 0), c_bs=(ns * S * 2 * d, 0),
+                      b_off=d * d, c_off=s * S * 2 * d, bias=bias[d:], bias_mode=L.BIAS_N)
+            L.tc_gemm(w16, a, vt, M=d, N=S, K=d, lda=d, ldb=d, ldc=ns * S, batch=(B, 1), b_bs=(S * d, 0), c_bs=(d * ns * S, 0),
+                      c_off=s * S, bias=bias[:d], bias_mode=L.BIAS_M)
+        o16 = torch.empty((ns, B * S, d), dtype=torch.bfloat16, device=dev)
+        o32 = torch.empty((ns, B * S, d), dtype=torch.float32, device=dev)
+        lse = torch.empty((ns, B, H, S), dtype=torch.float32, device=dev)
+        rate = float(self.cfg.dropout)
+        for s in range(ns):
+            L.attn_multiend_train(qk, vt, B, S, ns, s, H, d, Lt, rate=rate, seed=self._drop_seed(site0 + s), lse=lse[s], out_f32=o32[s], out=o16[s])
+        return o16, (qk, vt, o32, lse)
+
     # ------------------------------------------------------------------ the step
     def forward_backward(self, poses, tokens):
         cfg, dev, p, g = self.cfg, self.device, self.p, self.g
@@ -265,12 +354,18 @@ class MIGTTrainer:
         for li in range(cfg.n_layer):
             pre = f"h.{li}."
             site = 100 + li * 20
-            a = [self._ln(x, pre + "ln_1") for x in xs]
-            vqk = [self._lin(t, pre + "attn.c_attn") for t in a]
-            outs, probs = self._attention_fw(vqk, B, S, Lt, site)
+            if self.bf16:
+                # outs: bf16 attention outputs (c_proj's operands); vqk: what the fused backward needs in place of the probabilities
+                outs, vqk = self._attention_fw16([self._ln(x, pre + "ln_1", torch.bfloat16) for x in xs], pre, B, S, Lt, site)
+                probs = None
+            else:
+                a = [self._ln(x, pre + "ln_1") for x in xs]
+                vqk = [self._lin(t, pre + "attn.c_attn") for t in a]
+                outs, probs = self._attention_fw(vqk, B, S, Lt, site)
             ys = [self._drop(self._lin(o, pre + "attn.c_proj"), site + 4 + s) for s, o in enumerate(outs)]
             ys = [L.lincomb3(1.0, x, 1.0, y) for x, y in zip(xs, ys)]
-            hm = [self._lin(self._ln(y, pre + "ln_2"), pre + "mlp.c_fc") for y in ys]
+            ln2_dt = torch.bfloat16 if self.bf16 else torch.float32
+            hm = [self._lin(self._ln(y, pre + "ln_2", ln2_dt), pre + "mlp.c_fc") for y in ys]
             zs = [self._drop(self._lin(self._gelu(h), pre + "mlp.c_proj"), site + 8 + s) for s, h in enumerate(hm)]
             zs = [L.lincomb3(1.0, y, 1.0, z) for y, z in zip(ys, zs)]
             tape.append((xs, vqk, probs, outs, ys, hm))
@@ -280,7 +375,10 @@ class MIGTTrainer:
         denom = float(B * (T - skip) * Lt)
         view_ok = (torch.arange(T, device=dev) >= skip).to(torch.float32).repeat_interleave(Lt).repeat(B)        # [B*S] row mask
         head_tc = self._tc_dense_ok(d, V)
-        if head_tc:                                                                                                # tied head, first V rows (:417)
+        if head_tc and self.bf16:
+            logits = torch.empty((B * S, V), dtype=torch.float32, device=dev)
+            L.tc_gemm(L.to_bf16(hn[1]), self._w16["wte"][1], logits, M=B * S, N=V, K=d, lda=d, ldb=d, ldc=V)
+        elif head_tc:                                                                                              # tied head, first V rows (:417)
             logits = self._dense_fw_tc(hn[1], ("fw", "wte"), lambda: wte[:V].contiguous(), V, d)
         else:
             logits = torch.empty((B * S, V), dtype=torch.float32, device=dev)
@@ -290,9 +388,15 @@ class MIGTTrainer:
         loss = ce * float(cfg.image_generation_weight)
         self.last = dict(ce_loss=ce, logits=logits.reshape(B, T, Lt, V))
         dhn = [None] * ns
-        dlog = L.cross_entropy_grad(logits, ids.reshape(-1), (view_ok * (float(cfg.image_generation_weight) / denom)).contiguous(), float(cfg.label_smoothing))
+        ls = self.loss_scale                                                       # gradient seeds carry the loss scale (1 in fp32)
+        dlog = L.cross_entropy_grad(logits, ids.reshape(-1), (view_ok * (float(cfg.image_generation_weight) * ls / denom)).contiguous(),
+                                    float(cfg.label_smoothing))
         # tied LM head backward: d hn1 = dlogits wte[:V];  d wte[:V] += dlogits^T hn1
-        if head_tc:
+        if head_tc and self.bf16:
+            dhn[1] = torch.empty((B * S, d), dtype=torch.float32, device=dev)
+            L.tc_gemm(L.to_bf16(dlog), self._w16["wte"][0], dhn[1], M=B * S, N=d, K=V, lda=V, ldb=V, ldc=d)
+            L.dense_wgrad_bf16(dlog, hn[1], g["wte.weight"][:V])
+        elif head_tc:
             dhn[1] = self._dense_fw_tc(dlog, ("bw", "wte"), lambda: wte[:V].t().contiguous(), d, V)
             L.dense_wgrad_tc(dlog, hn[1], g["wte.weight"][:V])
         else:
@@ -313,14 +417,14 @@ class MIGTTrainer:
                 e0, e1 = math.exp(-float(w01[0])), math.exp(-float(w01[1]))
                 pls, ols = float(pl.double().sum()), float(ol.double().sum())
                 pose_loss = torch.full_like(pl, float(B * (w01[0] + w01[1]) + e0 * pls + e1 * ols))
-                self.g[wkey].copy_(torch.tensor([lw_now * (B - e0 * pls), lw_now * (B - e1 * ols)], dtype=torch.float32))
+                self.g[wkey].copy_(torch.tensor([lw_now * (B - e0 * pls) * ls, lw_now * (B - e1 * ols) * ls], dtype=torch.float32))
                 self._ready(wkey)
                 ps, os_ = e0 * B, e1 * B
             else:
                 pose_loss, ps, os_ = pl + ol, 1.0, 1.0
             loss = loss + pose_loss * lw_now
             self.last.update(pose_pos_loss=pl, pose_ori_loss=ol, pose_loss=pose_loss)
-            draw = L.pose_loss_grad(raw, poses, (view_ok * (lw_now / denom)).contiguous(), Lt, float(cfg.pose_multiplier), ps, os_)
+            draw = L.pose_loss_grad(raw, poses, (view_ok * (lw_now * ls / denom)).contiguous(), Lt, float(cfg.pose_multiplier), ps, os_)
             dg_ = self._lin_bw(self._gelu(pc_h), draw, "pose_classifier.c_proj")
             dhn[2] = self._lin_bw(hn[2], L.gelu_bwd(pc_h, dg_), "pose_classifier.c_fc")
         else:
@@ -342,11 +446,19 @@ class MIGTTrainer:
                 dgel = self._lin_bw_shared(self._gelu(hm[s]), dz, pre + "mlp.c_proj", last)
                 dm = self._lin_bw_shared(self._ln(ys[s], pre + "ln_2"), L.gelu_bwd(hm[s], dgel), pre + "mlp.c_fc", last)
                 dys.append(self._ln_bw(ys[s], dm, pre + "ln_2", add=dxs[s], last=last))
-            dos = []
-            for s in range(ns):
-                dy = self._drop(dys[s], site + 4 + s) if float(cfg.dropout) > 0 else dys[s]
-                dos.append(self._lin_bw_shared(outs[s], dy, pre + "attn.c_proj", s == ns - 1))
-            dvqk = self._attention_bw(vqk, probs, dos, B, S, Lt, site)
+            if self.bf16:
+                qk, vt, o32, lse = vqk
+                do16 = torch.empty((ns, B * S, d), dtype=torch.bfloat16, device=dev)
+                for s in range(ns):
+                    dy = self._drop(dys[s], site + 4 + s) if float(cfg.dropout) > 0 else dys[s]
+                    self._lin_bw_shared(o32[s], dy, pre + "attn.c_proj", s == ns - 1, out16=do16[s])
+                dvqk = L.attn_multiend_bwd(qk, vt, do16, o32, lse, B, S, ns, cfg.n_head, d, Lt, rate=float(cfg.dropout), seed=self._drop_seed(site))
+            else:
+                dos = []
+                for s in range(ns):
+                    dy = self._drop(dys[s], site + 4 + s) if float(cfg.dropout) > 0 else dys[s]
+                    dos.append(self._lin_bw_shared(outs[s], dy, pre + "attn.c_proj", s == ns - 1))
+                dvqk = self._attention_bw(vqk, probs, dos, B, S, Lt, site)
             new_dxs = []
             for s in range(ns):
                 last = s == ns - 1
@@ -374,12 +486,19 @@ class MIGTTrainer:
     def _gelu(self, x):
         return L.gelu(x)
 
-    def _lin_bw_shared(self, x, dy, name, last):
-        """_lin_bw for a layer applied to every stream: the weight-gradient kernels accumulate; readiness is signalled on the last one."""
+    def _lin_bw_shared(self, x, dy, name, last, out16=None):
+        """_lin_bw for a layer applied to every stream: the weight-gradient kernels accumulate; readiness is signalled on the last one.
+        bf16: ``out16`` receives dx as bf16 only (the attention backward's dO operand)."""
         W = self.p[name + ".weight"]
         k, n = W.shape
         m = x.shape[0]
         tc = self._tc_dense_ok(k, n)
+        if tc and self.bf16:
+            L.dense_wgrad_bf16(x, dy, self.g[name + ".weight"])
+            L.col_sums(dy, self.g[name + ".bias"].reshape(-1))
+            if last:
+                self._ready(name + ".bias", name + ".weight")
+            return self._dgrad16(dy, name, out16=out16)
         if tc:
             L.dense_wgrad_tc(x, dy, self.g[name + ".weight"])
         else:
@@ -404,15 +523,34 @@ class MIGTTrainer:
         return init * 0.5 * (1.0 + math.cos(math.pi * t))
 
     def optimizer_step(self):
+        """AdamW on the all-reduced gradients; returns whether the update was applied.
+
+        bf16: Keras LossScaleOptimizer over TF 2.4's DynamicLossScale (migt.py:466-488).  The gradients carry the loss scale; one fp64 sum of
+        squares of the flat gradient decides whether all of them are finite.  Non-finite: no update (weights and moments untouched), the
+        scale halves (not below 1) and the good-step counter resets, but ``iterations`` still advances, as Keras's do_not_apply_fn does, so
+        the learning-rate and localisation schedules move on.  Finite: the update runs on the unscaled gradients (clipping included), and
+        when the counter has reached 1999 the scale doubles (if that is finite) and the counter resets, else the counter counts up."""
         for h in self._handles:
             h.wait()
         self._handles = []
         lr = self.learning_rate()
         self.iterations += 1
         self._wsplit = {}
+        ls = self.loss_scale
+        if self.bf16:
+            if not math.isfinite(float(L.sumsq(self.flat_g))):
+                self.loss_scale = max(ls / 2.0, 1.0)
+                self.loss_scale_counter = 0
+                return False
+            if self.loss_scale_counter == self.LOSS_SCALE_GROWTH_STEPS - 1:
+                if math.isfinite(ls * 2.0):
+                    self.loss_scale = ls * 2.0
+                self.loss_scale_counter = 0
+            else:
+                self.loss_scale_counter += 1
         wd = float(self.cfg.weight_decay)
         clip = float(self.cfg.gradient_clip_val or 0.0)
-        gs = 1.0 / self._world() if self.grad_reduce == "mean" else 1.0
+        gs = (1.0 / self._world() if self.grad_reduce == "mean" else 1.0) / ls
         for k in self.order:
             cs = 1.0
             if clip > 0:                                                  # tf.clip_by_norm: g * clip / max(|g|, clip), per tensor
@@ -422,6 +560,9 @@ class MIGTTrainer:
             L.adamw_keras(self.flat_p[o:o + n], self.flat_g[o:o + n], self.flat_m[o:o + n], self.flat_v[o:o + n], lr=lr, beta1=self.betas[0],
                           beta2=self.betas[1], eps=self.eps, weight_decay=wd if (wd > 0 and self.decay[k]) else 0.0, step=self.iterations,
                           grad_scale=gs, clip_scale=cs)
+        if self.bf16:
+            L.dense_weights_bf16(self._w16_table)
+        return True
 
     def train_step(self, batch):
         """(poses [B,T,7], tokens [B,T,h,w]) -> dict(loss, ce_loss, [pose losses], acc, learning_rate) — migt.py:464-505."""
@@ -437,4 +578,6 @@ class MIGTTrainer:
         skip = self.cfg.n_loss_skip
         out["acc"] = float((pred[:, skip:] == tok.reshape(tok.shape[0], tok.shape[1], -1)[:, skip:]).float().mean())
         out["learning_rate"] = lr
+        if self.bf16:
+            out["loss_scale"] = self.loss_scale
         return out
