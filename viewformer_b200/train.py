@@ -13,7 +13,8 @@ Data layout: every trainable tensor lives in ONE flat fp32 buffer (kernel layout
 twin flat gradient buffer ordered by backward completion (decoder.conv_out first, encoder.conv_in last), so that
   * the data-parallel exchange is a handful of large NCCL all-reduces over contiguous buckets, each launched (async) the moment
     the backward pass has produced its last gradient — the transfers ride under the remaining backward kernels;
-  * Adam is one kernel launch over the whole model.
+  * Adam is one kernel launch over the whole model (``gradient_clip_val`` > 0: the global-norm clip the reference's Lightning trainer
+    applies first, folded into Adam's gradient scale).
 Activations needed by the backward pass are kept on a tape; GroupNorm+swish outputs are recomputed from the saved statistics.
 
 Arithmetic: fp32 throughout, as the reference requires.  The 3x3 stride-1 convolutions with tensor-core-sized channel counts run
@@ -526,8 +527,16 @@ class VQGANTrainer:
             h.wait()
         self._handles = []
         self.step_count += 1
+        gs = 1.0 / self._world()
+        clip = float(self.cfg.gradient_clip_val or 0.0)
+        if clip > 0:
+            # the reference trains under pytorch-lightning (train_codebook_th.py:69), which clips the global L2 norm of all gradients (after
+            # the data-parallel mean) before the optimizer: g *= min(1, clip / (norm + 1e-6)).  flat_g's alignment padding is zero, so one
+            # sum of squares over the whole buffer is that norm; the factor rides on Adam's gradient scale.
+            norm = math.sqrt(float(L.sumsq(self.flat_g))) * gs
+            gs *= min(1.0, clip / (norm + 1e-6))
         L.adam(self.flat_p, self.flat_g, self.flat_m, self.flat_v, lr=self.lr, beta1=self.betas[0], beta2=self.betas[1], eps=self.eps,
-               step=self.step_count, grad_scale=1.0 / self._world())
+               step=self.step_count, grad_scale=gs)
         self._wsplit = {}                               # split-fp16 operand copies of the conv weights are stale now
         if self.bf16:
             self._refresh_bf16_weights()
