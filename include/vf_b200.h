@@ -22,7 +22,8 @@ extern "C" {
 
 typedef void* vf_stream_t; /* cudaStream_t */
 
-enum { VF_F32 = 0, VF_BF16 = 1, VF_F16X2 = 2 /* fp32 value as two fp16: [.., hi(C) | lo(C)], lo = fp16((v - hi) * 2^11); see vf_tc_gemm */ };
+enum { VF_F32 = 0, VF_BF16 = 1, VF_F16X2 = 2 /* fp32 value as two fp16: [.., hi(C) | lo(C)], lo = fp16((v - hi) * 2^11); fp32-faithful for
+                                                   tensors with amax in [2^-10, 2^15], NaN products at |v| >= 65520; see vf_tc_gemm */ };
 enum { VF_ACT_NONE = 0, VF_ACT_GELU_ERF = 1 };
 enum { VF_BIAS_NONE = 0, VF_BIAS_N = 1, VF_BIAS_M = 2 };
 enum { VF_OK = 0, VF_ERR_ARG = -1, VF_ERR_CUDA = -2, VF_ERR_UNSUPPORTED = -3 };
@@ -154,7 +155,11 @@ typedef struct {
        lo.hi), accumulation drained from the accumulators in short chunks and summed with round-to-nearest FFMAs; fp32 output only):
          conv: A = [N,H,W, hi(Cl) | lo(Cl)] with Ctot = 2*Cl, B = [Cout][tap][hi(Cin) | lo(Cin)];
          gemm: a row of A holds hi(K) at column 0 and lo(K) at column exact_lo_a (elements), B rows likewise at exact_lo_b;
-               K %% 64 == 0; lda / ldb are the full row strides. */
+               K %% 64 == 0; lda / ldb are the full row strides.
+       Faithful range: the products are as accurate as an fp32 FFMA chain for operands whose amax lies in [2^-10, 2^15].  Below
+       2^-14 hi is an fp16 subnormal and lo's absolute floor is 2^-36, so relative precision falls below fp32's once a tensor's amax
+       drops under about 2^-12; at |v| >= 65520 hi = inf and the result is NaN (no guard).  Callers keep their operands inside the range
+       (the fp32 trainers scale their gradient seeds, DESIGN.md §6). */
     int64_t exact_lo_a, exact_lo_b;
 } vf_tc_gemm_t;
 int vf_tc_gemm(const vf_tc_gemm_t* p, vf_stream_t s);

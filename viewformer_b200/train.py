@@ -21,7 +21,9 @@ Arithmetic: fp32 throughout, as the reference requires.  The 3x3 stride-1 convol
 their forward pass and their data gradient on the exact split-fp16 tensor-core kernels (fp32-faithful results from three fp16 MMA passes,
 DESIGN.md 5.3; ``VF_TRAIN_TC=0`` keeps everything on the CUDA cores), and their weight gradient as nine exact GEMMs over the pixel axis
 (``_lib.conv_wgrad_tc``) when both channel counts are multiples of 128; strided / upsampling convs, 1x1 layers and the remaining weight
-gradients use the fp32 CUDA-core kernels.
+gradients use the fp32 CUDA-core kernels.  The backward pass runs on loss seeds multiplied by a power of two near the number of output
+elements (``grad_seed_scale``), because the split is only fp32-faithful for operands of magnitude 2^-10 .. 2^15 and the plain seeds
+(1 / numel) are far below that; the gradient buffer is unscaled bucket by bucket, so every result outside the backward pass is unscaled.
 
 ``precision="bf16"`` (BASELINE configs[3]: bf16 activations over fp32 master weights) runs every conv that a bf16-built model puts on the
 tensor cores (3x3, Cin % 64 == 0, Cout % 16 == 0, Cout >= 64) as ONE bf16 wgmma pass: forward (stride-2 convs on the space-to-depth
@@ -49,6 +51,8 @@ class _P:
 
 
 class VQGANTrainer:
+    _seed_scale = 1.0                                   # the gradient-seed scale of the running step (see grad_seed_scale)
+
     def __init__(self, model, lr=None, betas=(0.5, 0.9), eps=1e-8, bucket_bytes=64 << 20, process_group=None, precision="fp32"):
         """``precision``: "fp32" (the reference's arithmetic) or "bf16" (single-pass bf16 tensor-core convs, see the module docstring);
         either way the model is built with precision="fp32" and its fp32 weights are the master copy."""
@@ -71,6 +75,9 @@ class VQGANTrainer:
         self.use_tc = os.environ.get("VF_TRAIN_TC", "1") != "0"
         self._wsplit = {}
         self.precision, self.bf16 = precision, precision == "bf16"
+        # gradient-seed scale: None = 2^round(log2(numel of the reconstruction)), which brings the loss seeds (1 / numel) to about 1 so that
+        # the backward operands sit inside the split-fp16 tensor-core path's faithful range; a number = that fixed power of two (1 = off)
+        self.grad_seed_scale = 1.0 if self.bf16 else None
         if self.bf16:
             self._setup_bf16_weights()
 
@@ -201,9 +208,11 @@ class VQGANTrainer:
         self._bucket_left[b] -= 1
         if self._bucket_left[b] == 0:
             self.launched.append(b)
+            s, e, _ = self.buckets[b]
+            if self._seed_scale != 1.0:                 # divide the seed scale back out (exact: a power of two)
+                L.lincomb3(1.0 / self._seed_scale, self.flat_g[s:e], out=self.flat_g[s:e])
             if self._world() > 1:
                 import torch.distributed as dist
-                s, e, _ = self.buckets[b]
                 self._handles.append(dist.all_reduce(self.flat_g[s:e], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
         elif self._bucket_left[b] < 0:
             raise RuntimeError(f"gradient of {p.name} signalled twice")
@@ -480,7 +489,11 @@ class VQGANTrainer:
         tape.append(("normconv", "decoder.norm_out", "decoder.conv_out", d, g, st))
         dec = self._conv_fw(d["conv_out"], a)
         # ---------------- loss (vqgan_th.py:400-411): mean |x - xrec| + codebook_weight * diff
-        ddec, l1 = L.l1_grad(x, dec, 1.0 / dec.numel())
+        # the backward pass is linear in its seed, so it runs on seeds times a power of two s (exact in fp32: no CUDA-core result changes)
+        # that keeps the split-fp16 operands of the tensor-core convs away from fp16's subnormal range; each gradient bucket is divided
+        # by s when it completes, so flat_g, the all-reduce, clipping and Adam see the unscaled gradient
+        s = self._seed_scale = float(2.0 ** round(math.log2(dec.numel())) if self.grad_seed_scale is None else self.grad_seed_scale)
+        ddec, l1 = L.l1_grad(x, dec, s / dec.numel())
         rec = l1 / dec.numel()
         loss = rec.to(torch.float32).reshape(()) + float(cfg.codebook_weight) * diff
         self.last = dict(rec_loss=rec, quant_loss=diff, codes=idx.reshape(n, zh, zw), reconstruction=dec)
@@ -500,13 +513,14 @@ class VQGANTrainer:
                 if name == "decoder.conv_in":
                     # through post_quant_conv, the straight-through estimator and the commitment term, quant_conv
                     dq = self._lin_bw("post_quant_conv", w["post_quant_conv"], quant, dy.reshape(-1, dy.shape[-1]))
-                    dz = L.lincomb3(1.0, dq, 2.0 * float(cfg.codebook_weight) / z.numel(), z, -2.0 * float(cfg.codebook_weight) / z.numel(), quant)
+                    cz = s * 2.0 * float(cfg.codebook_weight) / z.numel()
+                    dz = L.lincomb3(1.0, dq, cz, z, -cz, quant)
                     if model.quantizer == "commit":
                         # d/dE of beta mean((q - sg(z))^2): column k gets 2 beta / numel * (count_k e_k - sum of the z rows mapped to k);
                         # the straight-through output carries no gradient to E (utils_th.py:117)
                         pe = P["quantize.embeddings"]
                         counts, zsum = L.vq_ema_stats(z, idx, pe.tensor.shape[1])
-                        L.vq_commit_grad(pe.tensor, counts, zsum, 2.0 * model.beta * float(cfg.codebook_weight) / z.numel(), pe.grad)
+                        L.vq_commit_grad(pe.tensor, counts, zsum, s * 2.0 * model.beta * float(cfg.codebook_weight) / z.numel(), pe.grad)
                         self._grad_ready(pe)
                     dy = self._lin_bw("quant_conv", w["quant_conv"], hz.reshape(-1, zc), dz).reshape(hz.shape)
             elif kind == "normconv":

@@ -42,6 +42,7 @@ LN_EPS = 1e-5
 class MIGTTrainer:
     LOSS_SCALE_INIT = 2.0 ** 15                                    # tf.mixed_precision DynamicLossScale defaults (TF 2.4)
     LOSS_SCALE_GROWTH_STEPS = 2000
+    _seed_scale = 1.0                                              # the gradient-seed scale of the running step (see grad_seed_scale)
 
     def __init__(self, model, betas=(0.9, 0.999), eps=1e-8, warmup_steps=2000, bucket_bytes=64 << 20, process_group=None, seed=0,
                  grad_reduce="sum", precision="fp32"):
@@ -57,6 +58,11 @@ class MIGTTrainer:
         # dynamic loss scaling (bf16 only): the scale multiplies the loss gradient seeds; updates are skipped on non-finite gradients
         self.loss_scale = self.LOSS_SCALE_INIT if self.bf16 else 1.0
         self.loss_scale_counter = 0
+        # fp32 gradient-seed scale: None = 2^round(log2(denom)) (denom = the loss's row count), which brings the cross-entropy and pose seeds
+        # (weight / denom) to about 1 so that the backward operands sit inside the split-fp16 tensor-core path's faithful range; a number =
+        # that fixed power of two (1 = off).  Unlike loss_scale it is divided out of each gradient bucket as the bucket completes, so
+        # flat_g, gradients(), the all-reduce, clipping and AdamW see the same values as without it.
+        self.grad_seed_scale = 1.0 if self.bf16 else None
         self.model, self.cfg, self.device = model, cfg, model.device
         self.betas, self.eps, self.warmup_steps = betas, eps, warmup_steps
         self.group, self.bucket_bytes, self.seed = process_group, bucket_bytes, seed
@@ -161,9 +167,11 @@ class MIGTTrainer:
             self._left[b] -= 1
             if self._left[b] == 0:
                 self.launched.append(b)
+                s, e = self.buckets[b]
+                if self._seed_scale != 1.0:                        # divide the seed scale back out (exact: a power of two)
+                    L.lincomb3(1.0 / self._seed_scale, self.flat_g[s:e], out=self.flat_g[s:e])
                 if self._world() > 1:
                     import torch.distributed as dist
-                    s, e = self.buckets[b]
                     self._handles.append(dist.all_reduce(self.flat_g[s:e], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
             elif self._left[b] < 0:
                 raise RuntimeError(f"gradient of {k} signalled twice")
@@ -388,7 +396,8 @@ class MIGTTrainer:
         loss = ce * float(cfg.image_generation_weight)
         self.last = dict(ce_loss=ce, logits=logits.reshape(B, T, Lt, V))
         dhn = [None] * ns
-        ls = self.loss_scale                                                       # gradient seeds carry the loss scale (1 in fp32)
+        self._seed_scale = float(2.0 ** round(math.log2(denom)) if self.grad_seed_scale is None else self.grad_seed_scale)
+        ls = self.loss_scale * self._seed_scale                                    # gradient seeds carry the loss scale (1 in fp32) and the seed scale
         dlog = L.cross_entropy_grad(logits, ids.reshape(-1), (view_ok * (float(cfg.image_generation_weight) * ls / denom)).contiguous(),
                                     float(cfg.label_smoothing))
         # tied LM head backward: d hn1 = dlogits wte[:V];  d wte[:V] += dlogits^T hn1
