@@ -21,8 +21,7 @@ B = 4 * world
 x = vq_images(B, cfg.image_size, 123)
 tr = VQGANTrainer(VQGAN(cfg, precision="fp32", device=f"cuda:{local}").load_state_dict(sd), bucket_bytes=1 << 18)
 loss = tr.forward_backward(x[rank * 4:(rank + 1) * 4])
-for h in tr._handles:
-    h.wait()
+tr.ex.wait()
 g_dp = tr.flat_g.clone() / world                 # the optimizer applies the same 1 / world (DDP gradient average)
 tr.optimizer_step()
 torch.cuda.synchronize()

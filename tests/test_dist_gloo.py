@@ -1,5 +1,5 @@
 """world_size-2 gloo tests (CPU) of the multi-GPU host logic: scene sharding, the packed EMA all-reduce, and the bucketed gradient
-exchange of the two trainers (their own bucket code driven on CPU tensors)."""
+exchange shared by the two trainers (driven on CPU tensors with each trainer's real parameter list)."""
 import os
 
 import torch
@@ -56,11 +56,10 @@ def test_packed_ema_allreduce_equals_reference_two_call_pattern():
 
 # ---------------------------------------------------------------------------------------- gradient buckets of the two trainers
 def _bucket_worker(rank, world, port, q):
-    """Drives the trainers' OWN bucket code (VQGANTrainer._flatten/_grad_ready, MIGTTrainer._build/_ready) on CPU tensors over gloo:
-    the kernels are not involved, only the host logic of the exchange — flat buffer layout in backward order, bucket boundaries,
-    an async all-reduce launched the moment a bucket's last gradient is signalled, SUM semantics (train_codebook_th.py:39-41 DDP;
-    migt.py:471-476 MirroredStrategy)."""
-    from collections import OrderedDict
+    """Drives the shared gradient exchange (dist.GradExchange) as each trainer builds it (VQGANTrainer._flatten, MIGTTrainer._build) on
+    CPU tensors over gloo: the kernels are not involved, only the host logic of the exchange — flat buffer layout in backward order,
+    bucket boundaries, an async all-reduce launched the moment a bucket's last gradient is signalled, SUM semantics
+    (train_codebook_th.py:39-41 DDP; migt.py:471-476 MirroredStrategy)."""
     from types import SimpleNamespace
     from viewformer_b200.train import VQGANTrainer, _P
     from viewformer_b200.train_migt import MIGTTrainer
@@ -87,35 +86,36 @@ def _bucket_worker(rank, world, port, q):
     tr.model = SimpleNamespace(device=torch.device("cpu"), _refresh_decode_table=lambda: None)
     tr.params, tr.bucket_bytes, tr.group = params, 4096, None
     tr._flatten()
+    ex = tr.ex
     check(len(tr.buckets) >= 3, f"expected several buckets, got {tr.buckets}")
-    check(tr.buckets[0][0] == 0 and tr.buckets[-1][1] == tr.flat_g.numel() and all(a[1] == b[0] for a, b in zip(tr.buckets, tr.buckets[1:])),
+    check(tr.buckets[0][0] == 0 and tr.buckets[-1][1] == ex.flat_g.numel() and all(a[1] == b[0] for a, b in zip(tr.buckets, tr.buckets[1:])),
           "buckets do not partition the flat gradient")
-    check([p.name for p in tr.order] == [f"p{i}" for i in reversed(range(len(shapes)))], "flat buffer is not in backward order")
-    check(all(torch.equal(homes[i], originals[i]) and homes[i].data_ptr() == params[i].tensor.data_ptr() for i in range(len(shapes))),
-          "parameters were not re-homed into the flat buffer")
-    check(all(p.offset % 4 == 0 for p in params), "views are not 16-byte aligned")
+    check(ex.order == [f"p{i}" for i in reversed(range(len(shapes)))], "flat buffer is not in backward order")
+    check(all(torch.equal(homes[i], originals[i]) and homes[i].data_ptr() == params[i].tensor.data_ptr() == ex.p[f"p{i}"].data_ptr()
+              for i in range(len(shapes))), "parameters were not re-homed into the flat buffer")
+    check(all(ex.offs[p.name] % 4 == 0 for p in params), "views are not 16-byte aligned")
     for step in range(2):                                            # two steps: the per-step bookkeeping must reset
-        tr.flat_g.zero_()
-        tr._handles, tr.launched, tr._bucket_left = [], [], list(tr._bucket_size)
+        ex.reset()
         gr = torch.Generator().manual_seed(1000 * step + rank)
-        for p in tr.order:                                           # "backward": gradients complete in flat-buffer order
-            p.grad.copy_(torch.randn(p.tensor.shape, generator=gr))
-        want = tr.flat_g.clone()
+        for name in ex.order:                                        # "backward": gradients complete in flat-buffer order
+            ex.g[name].copy_(torch.randn(ex.g[name].shape, generator=gr))
+        want = ex.flat_g.clone()
         dist.all_reduce(want)                                        # what one big all-reduce after backward would give
-        tr.flat_g.zero_()
+        ex.flat_g.zero_()
         gr = torch.Generator().manual_seed(1000 * step + rank)
         seen = 0
-        for p in tr.order:
-            p.grad.copy_(torch.randn(p.tensor.shape, generator=gr))
-            tr._grad_ready(p)
-            check(len(tr._handles) == len(tr.launched) >= seen, "handle bookkeeping")
-            seen = len(tr.launched)
-        check(not any(tr._bucket_left) and tr.launched == list(range(len(tr.buckets))), "buckets not launched in completion order")
-        for h in tr._handles:
-            h.wait()
-        check(torch.equal(tr.flat_g, want), f"codebook trainer: bucketed exchange != plain all-reduce (step {step})")
+        for name in ex.order:
+            ex.g[name].copy_(torch.randn(ex.g[name].shape, generator=gr))
+            ex.ready(name)
+            check(len(ex.handles) == len(ex.launched) >= seen, "handle bookkeeping")
+            seen = len(ex.launched)
+        check(not any(ex._left) and ex.launched == list(range(len(tr.buckets))), "buckets not launched in completion order")
+        ex.check_complete()
+        ex.wait()
+        check(not ex.handles, "wait() leaves handles behind")
+        check(torch.equal(ex.flat_g, want), f"codebook trainer: bucketed exchange != plain all-reduce (step {step})")
     try:
-        tr._grad_ready(tr.order[0])
+        ex.ready(ex.order[0])
         check(False, "a gradient signalled twice must raise")
     except RuntimeError:
         pass
@@ -127,32 +127,32 @@ def _bucket_worker(rank, world, port, q):
     mt = MIGTTrainer.__new__(MIGTTrainer)
     mt.model, mt.cfg, mt.device, mt.bucket_bytes, mt.group = model, cfg, torch.device("cpu"), 32 << 10, None
     mt._build(sd)
+    ex = mt.ex
     names = list(model.param_shapes().keys())
-    check(sorted(mt.order) == sorted(names) and mt.order[-1] == "wte.weight" and mt.order[0].split(".")[0] in ("pose_loss_weighting_criterion", "pose_classifier", "ln_f"),
+    check(sorted(ex.order) == sorted(names) and ex.order[-1] == "wte.weight" and ex.order[0].split(".")[0] in ("pose_loss_weighting_criterion", "pose_classifier", "ln_f"),
           "transformer flat buffer is not in backward-completion order")
-    check(len(mt.buckets) >= 3 and mt.buckets[0][0] == 0 and mt.buckets[-1][1] == mt.flat_g.numel()
-          and all(a[1] == b[0] for a, b in zip(mt.buckets, mt.buckets[1:])), "transformer buckets do not partition the flat gradient")
+    check(len(ex.buckets) >= 3 and ex.buckets[0][0] == 0 and ex.buckets[-1][1] == ex.flat_g.numel()
+          and all(a[1] == b[0] for a, b in zip(ex.buckets, ex.buckets[1:])), "transformer buckets do not partition the flat gradient")
     check(all(torch.equal(mt.p[k], sd[k].float()) for k in names), "transformer parameters not copied into the flat buffer")
     check(all(mt.decay[k] == ("bias" not in k) for k in names), "weight-decay mask")
+    ex.reset()
     gr = torch.Generator().manual_seed(77 + rank)
-    for k in mt.order:
+    for k in ex.order:
         mt.g[k].copy_(torch.randn(mt.g[k].shape, generator=gr))
-    want = mt.flat_g.clone()
+    want = ex.flat_g.clone()
     dist.all_reduce(want)
-    mt._handles, mt.launched, mt._left = [], [], list(mt._bucket_size)
     i = 0
-    while i < len(mt.order):                                         # the step signals groups of names at once (e.g. weight + bias)
-        mt._ready(*mt.order[i:i + 3])
+    while i < len(ex.order):                                         # the step signals groups of names at once (e.g. weight + bias)
+        ex.ready(*ex.order[i:i + 3])
         i += 3
-    check(not any(mt._left) and sorted(mt.launched) == list(range(len(mt.buckets))), "transformer buckets incomplete")
-    for h in mt._handles:
-        h.wait()
-    check(torch.equal(mt.flat_g, want), "transformer trainer: bucketed exchange != plain all-reduce")
+    check(not any(ex._left) and sorted(ex.launched) == list(range(len(ex.buckets))), "transformer buckets incomplete")
+    ex.wait()
+    check(torch.equal(ex.flat_g, want), "transformer trainer: bucketed exchange != plain all-reduce")
     q.put((rank, ok, "; ".join(why)))
     dist.destroy_process_group()
 
 
-def test_gradient_buckets_of_both_trainers_equal_a_plain_allreduce():
+def test_shared_gradient_exchange_of_both_trainers_equals_a_plain_allreduce():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = 31500 + os.getpid() % 2000

@@ -253,24 +253,15 @@ def ssim_u8(a_u8, b_u8, k1=None, k2=None):
 
 
 # ----------------------------------------------------------------------------------------------- norms
-def groupnorm(x, gamma, beta, *, swish, out_dtype, eps=1e-6, groups=32, upsample=False, normalize=True, s2d=False):
-    """x f32|bf16 [N,H,W,C] -> GroupNorm(32) [+swish] [+nearest x2] as out_dtype (vqgan_th.py:11-17,29-30).
-    A bf16 x must carry the statistics its producing conv accumulated (from the fp32 accumulators) in ``_gn_sums``."""
+def groupnorm(x, gamma, beta, *, swish, out_dtype, eps=1e-6, groups=32, upsample=False, normalize=True, s2d=False, stats=None):
+    """x f32|bf16 [N,H,W,C] -> GroupNorm(32) [+swish] [+nearest x2] as out_dtype (vqgan_th.py:11-17,29-30).  The statistics are ``stats``
+    (mean, rstd) [N, groups, 2] when given, else gn_mean_rstd(x): a bf16 x must then carry the statistics its producing conv accumulated
+    (from the fp32 accumulators) in ``_gn_sums``."""
     lib = load(True)
     _dev(x)
     n, h, w, c = x.shape
-    stats = None
-    if normalize:
-        stats = torch.empty((n, groups, 2), dtype=torch.float32, device=x.device)      # (mean, rstd)
-        fused = getattr(x, "_gn_sums", None)        # statistics already accumulated by the producing conv's epilogue
-        if fused is not None and fused[1] == groups:
-            _check(lib.vf_groupnorm_finalize(_p(fused[0]), n * groups, C.c_double(float(h * w * (c // groups))), C.c_float(eps),
-                                             _p(stats), _stream()))
-        else:
-            if x.dtype != torch.float32:
-                raise LibraryError("groupnorm: a bf16 input needs fused statistics from its producer")
-            sums = torch.empty((n, groups, 2), dtype=torch.float64, device=x.device)
-            _check(lib.vf_groupnorm_stats(_p(x), n, h * w, c, groups, C.c_float(eps), _p(sums), _p(stats), _stream()))
+    if normalize and stats is None:
+        stats = gn_mean_rstd(x, groups, eps)
     oshape = (n, 2 * h, 2 * w, c) if upsample else ((n, h // 2, w // 2, 4 * c) if s2d else (n, h, w, c))
     if out_dtype == torch.float16:          # split-fp16 pair [hi | lo] (exact tensor-core operand): twice the channels
         oshape = oshape[:3] + (2 * oshape[3],)
@@ -861,99 +852,93 @@ def conv_wgrad_tc_ok(x, dy, kh, stride, upsample):
     return kh == 3 and stride == 1 and not upsample and cin % 128 == 0 and dy.shape[-1] % 128 == 0 and dy.shape[1:3] == x.shape[1:3]
 
 
+def conv_wgrad_bf16_ok(x, dy, kh, stride, upsample):
+    """Shapes conv_wgrad_bf16 takes: those of conv_wgrad_tc_ok, and the upsample convs (x [N,H,W,Cin], dy [N,2H,2W,Cout])."""
+    n, h, w, cin = x.shape
+    up = 2 if upsample else 1
+    return kh == 3 and stride == 1 and cin % 128 == 0 and dy.shape[-1] % 128 == 0 and tuple(dy.shape[1:3]) == (up * h, up * w)
+
+
 def conv_wgrad_tc(x, dy, dw, *, accumulate=True):
     """Weight gradient of a 3x3 stride-1 pad-1 convolution on the exact split-fp16 tensor-core GEMM.  x [N,H,W,Cin], dy [N,H,W,Cout] fp32;
     dw [9*Cin, Cout] (k = (ky*3 + kx)*Cin + c).  dW[ky,kx][c, co] = sum_q xpad[c, q + (ky-1) pitch + (kx-1)] * dypad[co, q] over the
     zero-padded pixel grid: both operands are transposed to K-major split form, the horizontal shifts are three row blocks of the activation
     operand (M = 3 Cin), the vertical ones are K offsets of whole (8-aligned) rows, the pixel axis is split over the SMs and the partial
     products are folded by vf_sum_splits."""
-    lib = load(True)
-    _dev(x, torch.float32); _dev(dy, torch.float32); _dev(dw, torch.float32)
-    n, h, w, cin = x.shape
-    cout = dy.shape[-1]
-    pitch = (w + 2 + 7) // 8 * 8
-    ppad = n * (h + 2) * pitch
-    tiles = (3 * cin // 128) * (cout // 128)
-    splits = max(1, min(64, (132 + 3 * tiles - 1) // (3 * tiles)))
-    kc = (ppad + splits - 1) // splits
-    kc = (kc + 63) // 64 * 64                                  # the exact GEMM walks K in blocks of 64
-    kpad = kc * splits
-    margin = pitch + 8                                          # multiple of 8, >= pitch + 1
-    la = kpad + 2 * margin
-    lb = kpad
-    # operand buffers are cached per shape: the transposer rewrites every interior position on each call and never touches the zero
-    # borders / pitch padding / margins, so they are cleared once
-    key = (x.device, n, h, w, cin, cout)
-    bufs = _wgrad_bufs.get(key)
-    if bufs is None:
-        if len(_wgrad_bufs) >= 32:
-            _wgrad_bufs.clear()
-        bufs = (torch.zeros((3 * cin, 2, la), dtype=torch.float16, device=x.device), torch.zeros((cout, 2, lb), dtype=torch.float16, device=x.device),
-                torch.empty((3, splits, 3 * cin, cout), dtype=torch.float32, device=x.device))
-        _wgrad_bufs[key] = bufs
-    at, bt, partial = bufs
-    _check(lib.vf_pad_transpose_split(_p(x), n, h, w, cin, pitch, 3, C.c_int64(margin), C.c_int64(la), _p(at), _stream()))
-    _check(lib.vf_pad_transpose_split(_p(dy), n, h, w, cout, pitch, 1, C.c_int64(0), C.c_int64(lb), _p(bt), _stream()))
-    offs = [margin - pitch, margin, margin + pitch]
-    tc_gemm(at, bt, partial, M=3 * cin, N=cout, K=kc, lda=2 * la, ldb=2 * lb, ldc=cout, batch=(3, splits), a_bs=(0, kc), b_bs=(0, kc),
-            c_bs=(splits * 3 * cin * cout, 3 * cin * cout), lo_a=la, lo_b=lb, k_offsets=offs)
-    _check(lib.vf_sum_splits(_p(partial), 3, splits, C.c_int64(3 * cin * cout), int(accumulate), _p(dw), _stream()))
-    return dw
+    return _wgrad_tc(x, dy, dw, bf16=False, conv=True, accumulate=accumulate)
+
+
+def conv_wgrad_bf16(x, dy, dw, *, norm=None, upsample=False, accumulate=True):
+    """conv_wgrad_tc on the single-pass bf16 tensor-core GEMM (bf16 operands, fp32 accumulation).  x f32 [N,H,W,Cin] is the conv's input
+    before ``norm`` (see pad_transpose_bf16) and before the nearest x2 upsample when ``upsample``; dy f32 [N,OH,OW,Cout]; dw f32 [9*Cin, Cout]."""
+    return _wgrad_tc(x, dy, dw, bf16=True, conv=True, norm=norm, upsample=upsample, accumulate=accumulate)
 
 
 def dense_wgrad_tc(x_rows, dy_rows, dw_kn, *, accumulate=True):
     """dW[k, n] (+)= sum_m x[m, k] dy[m, n] on the exact split-fp16 tensor-core GEMM (K = rows): both operands are transposed to K-major
-    split form (vf_pad_transpose_split, plain mode), the row axis is split over the SMs, vf_sum_splits folds the partial products."""
+    split form, the row axis is split over the SMs, vf_sum_splits folds the partial products."""
+    return _wgrad_tc(x_rows, dy_rows, dw_kn, bf16=False, conv=False, accumulate=accumulate)
+
+
+def dense_wgrad_bf16(x_rows, dy_rows, dw_kn, *, accumulate=True):
+    """dense_wgrad_tc on the single-pass bf16 tensor-core GEMM: both fp32 operands rounded once to bf16 by the K-major transposer."""
+    return _wgrad_tc(x_rows, dy_rows, dw_kn, bf16=True, conv=False, accumulate=accumulate)
+
+
+def _wgrad_tc(x, dy, dw, *, bf16, conv, norm=None, upsample=False, accumulate=True):
+    """The split-K weight-gradient GEMM behind conv_wgrad_tc / conv_wgrad_bf16 (``conv``) and dense_wgrad_tc / dense_wgrad_bf16: one plan,
+    the same launches for both operand formats (``bf16``: single-pass bf16, else exact split-fp16)."""
     lib = load(True)
-    _dev(x_rows, torch.float32); _dev(dy_rows, torch.float32); _dev(dw_kn, torch.float32)
-    m, k = x_rows.shape
-    n = dy_rows.shape[1]
-    tiles = (k // 128) * (n // 128)
-    splits = max(1, min(32, (132 + tiles - 1) // tiles))
-    kc = ((m + splits - 1) // splits + 63) // 64 * 64
-    lm = kc * splits
-    key = ("dense", x_rows.device, m, k, n)
+    _dev(x, torch.float32); _dev(dy, torch.float32); _dev(dw, torch.float32)
+    cin, cout = x.shape[-1], dy.shape[-1]
+    key = (bf16, conv, x.device, tuple(dy.shape[:-1]), cin, cout)
+    if conv:                                                   # K = pixels of the zero-padded logical (upsampled) image
+        n, h, w = dy.shape[:3]
+        pitch = (w + 2 + 7) // 8 * 8
+        klen, blocks, max_splits, margin = n * (h + 2) * pitch, 3, 64, pitch + 8        # margin: a multiple of 8, >= pitch + 1
+    else:                                                      # K = rows: one plain row of pixels
+        x, dy = x.reshape(1, 1, -1, cin), dy.reshape(1, 1, -1, cout)
+        pitch, klen, blocks, max_splits, margin = 0, x.shape[2], 1, 32, 0
+    M = blocks * cin
+    tiles = (M // 128) * (cout // 128)
+    splits = max(1, min(max_splits, (132 + blocks * tiles - 1) // (blocks * tiles)))
+    kc = ((klen + splits - 1) // splits + 63) // 64 * 64       # the tensor-core GEMM walks K in blocks of 64
+    kpad = kc * splits
+    la, lb = kpad + 2 * margin, kpad
+    # operand buffers are cached per shape: the transposer rewrites every interior position on each call and never touches the zero
+    # borders / pitch padding / margins / columns past K, so they are cleared once
     bufs = _wgrad_bufs.get(key)
     if bufs is None:
         if len(_wgrad_bufs) >= 32:
             _wgrad_bufs.clear()
-        bufs = (torch.zeros((k, 2, lm), dtype=torch.float16, device=x_rows.device), torch.zeros((n, 2, lm), dtype=torch.float16, device=x_rows.device),
-                torch.empty((splits, k, n), dtype=torch.float32, device=x_rows.device))
+        dt = torch.bfloat16 if bf16 else torch.float16
+
+        def operand(rows, length):                             # a split-fp16 row holds its hi and lo halves
+            return torch.zeros((rows, length) if bf16 else (rows, 2, length), dtype=dt, device=x.device)
+
+        bufs = (operand(M, la), operand(cout, lb), torch.empty(((blocks,) if conv else ()) + (splits, M, cout), dtype=torch.float32, device=x.device))
         _wgrad_bufs[key] = bufs
     at, bt, partial = bufs
-    _check(lib.vf_pad_transpose_split(_p(x_rows), 1, 1, m, k, 0, 1, C.c_int64(0), C.c_int64(lm), _p(at), _stream()))
-    _check(lib.vf_pad_transpose_split(_p(dy_rows), 1, 1, m, n, 0, 1, C.c_int64(0), C.c_int64(lm), _p(bt), _stream()))
-    tc_gemm(at, bt, partial, M=k, N=n, K=kc, lda=2 * lm, ldb=2 * lm, ldc=n, batch=(1, splits), a_bs=(0, kc), b_bs=(0, kc),
-            c_bs=(0, k * n), lo_a=lm, lo_b=lm)
-    _check(lib.vf_sum_splits(_p(partial), 1, splits, C.c_int64(k * n), int(accumulate), _p(dw_kn), _stream()))
-    return dw_kn
+    transpose = pad_transpose_bf16 if bf16 else pad_transpose_split
+    transpose(x, at, pitch=pitch, copies=blocks, margin=margin, norm=norm, upsample=upsample)
+    transpose(dy, bt, pitch=pitch, copies=1, margin=0)
+    ld = 1 if bf16 else 2
+    tc_gemm(at, bt, partial, M=M, N=cout, K=kc, lda=ld * la, ldb=ld * lb, ldc=cout, batch=(blocks, splits), a_bs=(0, kc), b_bs=(0, kc),
+            c_bs=(splits * M * cout if conv else 0, M * cout), lo_a=la, lo_b=lb, k_offsets=[margin - pitch, margin, margin + pitch] if conv else None)
+    _check(lib.vf_sum_splits(_p(partial), blocks, splits, C.c_int64(M * cout), int(accumulate), _p(dw), _stream()))
+    return dw
 
 
-def dense_wgrad_bf16(x_rows, dy_rows, dw_kn, *, accumulate=True):
-    """dW[k, n] (+)= sum_m x[m, k] dy[m, n] on the single-pass bf16 tensor-core GEMM: the schedule of dense_wgrad_tc (row axis split over the
-    SMs, vf_sum_splits) with both fp32 operands rounded once to bf16 by the K-major transposer (vf_pad_transpose_bf16, plain mode)."""
+def pad_transpose_split(x, out, *, pitch, copies, margin, norm=None, upsample=False):
+    """x f32 NHWC -> out split-fp16 [copies*C, 2, L] (zeroed by the caller): the K-major operand of the exact weight-gradient GEMM, the column
+    map of pad_transpose_bf16 with a lo half after the hi one.  The split transposer applies neither GroupNorm nor the x2 upsample."""
+    if norm is not None or upsample:
+        raise ValueError("pad_transpose_split: no GroupNorm or x2 upsample on the split-fp16 operand")
     lib = load(True)
-    _dev(x_rows, torch.float32); _dev(dy_rows, torch.float32); _dev(dw_kn, torch.float32)
-    m, k = x_rows.shape
-    n = dy_rows.shape[1]
-    tiles = (k // 128) * (n // 128)
-    splits = max(1, min(32, (132 + tiles - 1) // tiles))
-    kc = ((m + splits - 1) // splits + 63) // 64 * 64
-    lm = kc * splits
-    key = ("dense_bf16", x_rows.device, m, k, n)
-    bufs = _wgrad_bufs.get(key)
-    if bufs is None:                                           # the columns past m stay zero: cleared once
-        if len(_wgrad_bufs) >= 32:
-            _wgrad_bufs.clear()
-        bufs = (torch.zeros((k, lm), dtype=torch.bfloat16, device=x_rows.device), torch.zeros((n, lm), dtype=torch.bfloat16, device=x_rows.device),
-                torch.empty((splits, k, n), dtype=torch.float32, device=x_rows.device))
-        _wgrad_bufs[key] = bufs
-    at, bt, partial = bufs
-    pad_transpose_bf16(x_rows.reshape(1, 1, m, k), at, pitch=0, copies=1, margin=0)
-    pad_transpose_bf16(dy_rows.reshape(1, 1, m, n), bt, pitch=0, copies=1, margin=0)
-    tc_gemm(at, bt, partial, M=k, N=n, K=kc, lda=lm, ldb=lm, ldc=n, batch=(1, splits), a_bs=(0, kc), b_bs=(0, kc), c_bs=(0, k * n))
-    _check(lib.vf_sum_splits(_p(partial), 1, splits, C.c_int64(k * n), int(accumulate), _p(dw_kn), _stream()))
-    return dw_kn
+    _dev(x, torch.float32); _dev(out, torch.float16)
+    n, h, w, c = x.shape
+    _check(lib.vf_pad_transpose_split(_p(x), n, h, w, c, pitch, copies, C.c_int64(margin), C.c_int64(out.shape[-1]), _p(out), _stream()))
+    return out
 
 
 def pad_transpose_bf16(x, out, *, pitch, copies, margin, norm=None, upsample=False):
@@ -968,48 +953,6 @@ def pad_transpose_bf16(x, out, *, pitch, copies, margin, norm=None, upsample=Fal
     _check(lib.vf_pad_transpose_bf16(_p(x), n, h, w, c, int(upsample), pitch, copies, C.c_int64(margin), C.c_int64(out.shape[-1]), _p(mr), _p(gamma),
                                      _p(beta), groups, int(swish), _p(out), _stream()))
     return out
-
-
-def conv_wgrad_bf16_ok(x, dy, kh, stride, upsample):
-    """Shapes conv_wgrad_bf16 takes: those of conv_wgrad_tc, and the upsample convs (x [N,H,W,Cin], dy [N,2H,2W,Cout])."""
-    n, h, w, cin = x.shape
-    up = 2 if upsample else 1
-    return kh == 3 and stride == 1 and cin % 128 == 0 and dy.shape[-1] % 128 == 0 and tuple(dy.shape[1:3]) == (up * h, up * w)
-
-
-def conv_wgrad_bf16(x, dy, dw, *, norm=None, upsample=False, accumulate=True):
-    """Weight gradient of a 3x3 stride-1 pad-1 convolution on the single-pass bf16 tensor-core GEMM: the layout and schedule of
-    conv_wgrad_tc (K = pixels of the zero-padded grid, three horizontal shifts as row blocks, vertical shifts as K offsets, split-K over the
-    SMs, vf_sum_splits), with bf16 operands and fp32 accumulation.  x f32 [N,H,W,Cin] is the conv's input before ``norm`` (see
-    pad_transpose_bf16) and before the nearest x2 upsample when ``upsample``; dy f32 [N,OH,OW,Cout]; dw f32 [9*Cin, Cout]."""
-    lib = load(True)
-    _dev(x, torch.float32); _dev(dy, torch.float32); _dev(dw, torch.float32)
-    n, _, _, cin = x.shape
-    _, h, w, cout = dy.shape                                   # the logical (upsampled) image
-    pitch = (w + 2 + 7) // 8 * 8
-    ppad = n * (h + 2) * pitch
-    tiles = (3 * cin // 128) * (cout // 128)
-    splits = max(1, min(64, (132 + 3 * tiles - 1) // (3 * tiles)))
-    kc = ((ppad + splits - 1) // splits + 63) // 64 * 64
-    kpad = kc * splits
-    margin = pitch + 8
-    la, lb = kpad + 2 * margin, kpad
-    key = ("bf16", x.device, n, h, w, cin, cout)               # buffers cached per shape, borders / padding / margins cleared once
-    bufs = _wgrad_bufs.get(key)
-    if bufs is None:
-        if len(_wgrad_bufs) >= 32:
-            _wgrad_bufs.clear()
-        bufs = (torch.zeros((3 * cin, la), dtype=torch.bfloat16, device=x.device), torch.zeros((cout, lb), dtype=torch.bfloat16, device=x.device),
-                torch.empty((3, splits, 3 * cin, cout), dtype=torch.float32, device=x.device))
-        _wgrad_bufs[key] = bufs
-    at, bt, partial = bufs
-    pad_transpose_bf16(x, at, pitch=pitch, copies=3, margin=margin, norm=norm, upsample=upsample)
-    pad_transpose_bf16(dy, bt, pitch=pitch, copies=1, margin=0)
-    offs = [margin - pitch, margin, margin + pitch]
-    tc_gemm(at, bt, partial, M=3 * cin, N=cout, K=kc, lda=la, ldb=lb, ldc=cout, batch=(3, splits), a_bs=(0, kc), b_bs=(0, kc),
-            c_bs=(splits * 3 * cin * cout, 3 * cin * cout), k_offsets=offs)
-    _check(lib.vf_sum_splits(_p(partial), 3, splits, C.c_int64(3 * cin * cout), int(accumulate), _p(dw), _stream()))
-    return dw
 
 
 def conv_weights_bf16_table(entries, device):

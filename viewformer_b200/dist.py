@@ -1,12 +1,16 @@
 """Multi-GPU plumbing: one process per GPU, torch.distributed (NCCL on the GPUs, gloo in CPU tests).
 
-Inference shards scenes across ranks with NO data-path collective (scenes are independent, SURVEY.md §8e);
-the only exchange on the hot path is the codebook-EMA statistics of the training step, which the reference
-issues as two blocking all-reduces inside the quantizer forward (viewformer/models/utils_th.py:50-52) and which
-are packed into ONE all-reduce here.
+Inference shards scenes across ranks with NO data-path collective (scenes are independent, SURVEY.md §8e).  The training steps exchange
+two things: the codebook-EMA statistics, which the reference issues as two blocking all-reduces inside the quantizer forward
+(viewformer/models/utils_th.py:50-52) and which are packed into ONE all-reduce here, and the gradients, through ``GradExchange``: one
+flat buffer in backward-completion order, all-reduced bucket by bucket while the backward pass is still running.
 """
+import math
+
 import torch
 import torch.distributed as dist
+
+from . import _lib as L
 
 
 def shard_range(n_items, rank, world):
@@ -24,6 +28,79 @@ def allreduce_ema_stats(counts, embed_sum, group=None):
     packed = torch.cat([counts.reshape(-1), embed_sum.reshape(-1)])
     dist.all_reduce(packed, op=dist.ReduceOp.SUM, group=group)
     return packed[:k].reshape(counts.shape).contiguous(), packed[k:].reshape(embed_sum.shape).contiguous()
+
+
+class GradExchange:
+    """The trainers' parameters, gradients and optimizer moments in flat fp32 buffers, and the data-parallel gradient exchange over them.
+
+    ``entries``: (name, shape) pairs in the order the backward pass completes them.  Each name gets 16-byte aligned views ``p[name]`` /
+    ``g[name]`` at ``offs[name]`` of ``flat_p`` / ``flat_g`` (``flat_m`` / ``flat_v`` share the layout).  A bucket is a contiguous range
+    (start, end, name of its last parameter) of the flat gradient, closed after the parameter that pushes it past ``bucket_bytes``; the
+    last one closes at the end.  Once the backward pass has signalled every gradient of a bucket (``ready``), the bucket is divided by
+    the running step's gradient-seed scale and its asynchronous SUM all-reduce starts, so the transfers ride under the rest of the
+    backward pass."""
+
+    def __init__(self, entries, device, bucket_bytes, group=None):
+        self.group = group
+        self.order, self.offs, n = [name for name, _ in entries], {}, 0
+        sizes = {name: math.prod(shape) for name, shape in entries}
+        for name in self.order:
+            self.offs[name] = n
+            n += (sizes[name] + 3) // 4 * 4                  # 16-byte aligned views
+        self.flat_p = torch.zeros((n,), dtype=torch.float32, device=device)
+        self.flat_g, self.flat_m, self.flat_v = torch.zeros_like(self.flat_p), torch.zeros_like(self.flat_p), torch.zeros_like(self.flat_p)
+        self.p, self.g = {}, {}
+        for name, shape in entries:
+            o = self.offs[name]
+            self.p[name] = self.flat_p[o:o + sizes[name]].view(shape)
+            self.g[name] = self.flat_g[o:o + sizes[name]].view(shape)
+        self.buckets, self._bucket_of, self._bucket_size, start, count = [], {}, [], 0, 0
+        for i, name in enumerate(self.order):
+            self._bucket_of[name] = len(self.buckets)
+            count += 1
+            end = self.offs[name] + (sizes[name] + 3) // 4 * 4
+            if (end - start) * 4 >= bucket_bytes or i == len(self.order) - 1:
+                self.buckets.append((start, end, name))
+                self._bucket_size.append(count)
+                start, count = end, 0
+        self.launched = []                                   # buckets in the order their exchange started; cleared in place every step
+        self.reset()
+
+    def world(self):
+        return dist.get_world_size(self.group) if (dist.is_available() and dist.is_initialized()) else 1
+
+    def reset(self, seed_scale=1.0):
+        """Start a step: zero the gradient, no bucket signalled yet; the backward pass runs on seeds times ``seed_scale`` (a power of two)."""
+        self.flat_g.zero_()
+        self.seed_scale = seed_scale
+        self.handles, self._left = [], list(self._bucket_size)
+        self.launched.clear()
+
+    def ready(self, *names):
+        """The backward pass has finished the gradients of ``names``: unscale and start the all-reduce of every bucket this completes."""
+        for name in names:
+            b = self._bucket_of[name]
+            self._left[b] -= 1
+            if self._left[b] == 0:
+                self.launched.append(b)
+                s, e, _ = self.buckets[b]
+                if self.seed_scale != 1.0:                   # divide the seed scale back out (exact: a power of two)
+                    L.lincomb3(1.0 / self.seed_scale, self.flat_g[s:e], out=self.flat_g[s:e])
+                if self.world() > 1:
+                    self.handles.append(dist.all_reduce(self.flat_g[s:e], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
+            elif self._left[b] < 0:
+                raise RuntimeError(f"gradient of {name} signalled twice")
+
+    def check_complete(self):
+        """End of the backward pass: every bucket must have been signalled."""
+        if any(self._left):
+            raise RuntimeError("backward pass left gradient buckets incomplete: " + str([self.buckets[i][2] for i, n in enumerate(self._left) if n]))
+
+    def wait(self):
+        """Wait for the all-reduces of the step: flat_g then holds the gradient summed over ranks."""
+        for h in self.handles:
+            h.wait()
+        self.handles = []
 
 
 def max_over_ranks(value, device):

@@ -10,7 +10,8 @@ reference requires (vqgan_th.py:326); LPIPS is not available offline, so ``perce
     trainer.export_state_dict()            # reference-keyed weights after the step
 
 Data layout: every trainable tensor lives in ONE flat fp32 buffer (kernel layouts: conv [kh*kw*Cin, Cout], dense [out, in]) with a
-twin flat gradient buffer ordered by backward completion (decoder.conv_out first, encoder.conv_in last), so that
+twin flat gradient buffer ordered by backward completion (decoder.conv_out first, encoder.conv_in last), both owned by the trainers'
+shared gradient exchange (``dist.GradExchange``), so that
   * the data-parallel exchange is a handful of large NCCL all-reduces over contiguous buckets, each launched (async) the moment
     the backward pass has produced its last gradient — the transfers ride under the remaining backward kernels;
   * Adam is one kernel launch over the whole model (``gradient_clip_val`` > 0: the global-norm clip the reference's Lightning trainer
@@ -39,15 +40,15 @@ import os
 import torch
 
 from . import _lib as L
+from .dist import GradExchange
 from .ops import linear
 
 
 class _P:
-    """One trainable tensor: kernel-layout view into the flat parameter buffer + its gradient view, and how to export it."""
+    """One trainable tensor: kernel-layout view into the flat parameter buffer, how to re-home it in the model, and how to export it."""
 
     def __init__(self, name, tensor, setter, kind, part=None, cin=None):
         self.name, self.tensor, self.setter, self.kind, self.part, self.cin = name, tensor, setter, kind, part, cin
-        self.grad = None
 
 
 class VQGANTrainer:
@@ -144,38 +145,15 @@ class VQGANTrainer:
         self.params = ps
 
     def _flatten(self):
-        """Re-home every parameter in one flat buffer, in BACKWARD order; twin flat buffers for the gradient and Adam's moments."""
-        dev = self.model.device
+        """Re-home every parameter in the flat buffers of the gradient exchange, in BACKWARD order (decoder.conv_out first)."""
         order = list(reversed(self.params))
-        offs, n = [], 0
+        ex = self.ex = GradExchange([(p.name, p.tensor.shape) for p in order], self.model.device, self.bucket_bytes, self.group)
+        self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.buckets, self.launched = ex.flat_p, ex.flat_g, ex.flat_m, ex.flat_v, ex.buckets, ex.launched
         for p in order:
-            offs.append(n)
-            n += (p.tensor.numel() + 3) // 4 * 4            # 16-byte aligned views
-        self.flat_p = torch.zeros((n,), dtype=torch.float32, device=dev)
-        self.flat_g = torch.zeros_like(self.flat_p)
-        self.flat_m = torch.zeros_like(self.flat_p)
-        self.flat_v = torch.zeros_like(self.flat_p)
-        for p, o in zip(order, offs):
-            view = self.flat_p[o:o + p.tensor.numel()].view(p.tensor.shape)
+            view = self.ex.p[p.name]
             view.copy_(p.tensor)
             p.setter(view)
-            p.tensor, p.offset = view, o
-            p.grad = self.flat_g[o:o + p.tensor.numel()].view(p.tensor.shape)
-        self.order = order
-        # buckets: contiguous ranges of the flat gradient, closed after the parameter that pushes them past bucket_bytes
-        self.buckets, start = [], 0
-        for i, p in enumerate(order):
-            end = p.offset + (p.tensor.numel() + 3) // 4 * 4
-            if (end - start) * 4 >= self.bucket_bytes or i == len(order) - 1:
-                self.buckets.append((start, end, p.name))
-                start = end
-        self._bucket_of = {}
-        bi = 0
-        for p in order:
-            while p.offset >= self.buckets[bi][1]:
-                bi += 1
-            self._bucket_of[p.name] = bi
-        self._bucket_size = [sum(1 for b in self._bucket_of.values() if b == i) for i in range(len(self.buckets))]
+            p.tensor = view
         self.model._refresh_decode_table()
 
     def _setup_bf16_weights(self):
@@ -197,41 +175,9 @@ class VQGANTrainer:
     def _refresh_bf16_weights(self):
         L.conv_weights_bf16(self._wb16_table)
 
-    # ------------------------------------------------------------------ data-parallel exchange
-    def _world(self):
-        import torch.distributed as dist
-        return dist.get_world_size(self.group) if (dist.is_available() and dist.is_initialized()) else 1
-
-    def _grad_ready(self, p):
-        """Called when the backward pass has finished the gradient of ``p``: if that closes a bucket, start its all-reduce."""
-        b = self._bucket_of[p.name]
-        self._bucket_left[b] -= 1
-        if self._bucket_left[b] == 0:
-            self.launched.append(b)
-            s, e, _ = self.buckets[b]
-            if self._seed_scale != 1.0:                 # divide the seed scale back out (exact: a power of two)
-                L.lincomb3(1.0 / self._seed_scale, self.flat_g[s:e], out=self.flat_g[s:e])
-            if self._world() > 1:
-                import torch.distributed as dist
-                self._handles.append(dist.all_reduce(self.flat_g[s:e], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
-        elif self._bucket_left[b] < 0:
-            raise RuntimeError(f"gradient of {p.name} signalled twice")
-
     # ------------------------------------------------------------------ primitive forward / backward pairs
-    def _pmap(self):
-        return {p.name: p for p in self.params}
-
-    def _gn_fw(self, x, nw):
-        st = L.gn_mean_rstd(x)
-        return st
-
     def _gn_apply(self, x, st, nw, swish, dtype=torch.float32):
-        n, h, w, c = x.shape
-        y = torch.empty(x.shape, dtype=dtype, device=x.device)
-        lib = L.load(True)
-        L._check(lib.vf_groupnorm_apply(L._p(x), L.F32, L._p(st), L._p(nw[0]), L._p(nw[1]), n, h, w, c, 32, L.C.c_float(1e-6), 1, int(swish), 0,
-                                        L._p(y), L._dt(y), L._stream()))
-        return y
+        return L.groupnorm(x, nw[0], nw[1], swish=swish, out_dtype=dtype, stats=st)
 
     def _act(self, x, st, nw, swish, cw):
         """GroupNorm(+swish) of x as the operand of conv ``cw``: bf16 when the bf16 step runs that conv on the tensor cores, else fp32."""
@@ -286,17 +232,17 @@ class VQGANTrainer:
 
     def _conv_bw(self, name, cw, a, dy, stride=1, upsample=False, need_dx=True):
         """a: the conv's input (NHWC f32); dy: gradient of its output.  Accumulates dW, db; returns dx (or None)."""
-        P = self.P
+        G = self.ex.g
         pad = ((1, 1) if stride == 1 else (0, 0)) if cw.k == 3 else (0, 0)
         if self.use_tc and upsample and L.conv_wgrad_tc_ok(dy, dy, cw.k, stride, False) and cw.cin % 128 == 0:
             a_up = L.groupnorm(a, None, None, swish=False, out_dtype=torch.float32, normalize=False, upsample=True)
-            L.conv_wgrad_tc(a_up, dy, P[name + ".weight"].grad)
+            L.conv_wgrad_tc(a_up, dy, G[name + ".weight"])
         elif self.use_tc and L.conv_wgrad_tc_ok(a, dy, cw.k, stride, upsample):
-            L.conv_wgrad_tc(a, dy, P[name + ".weight"].grad)             # exact split-fp16 GEMMs over the pixel axis (K = pixels)
+            L.conv_wgrad_tc(a, dy, G[name + ".weight"])             # exact split-fp16 GEMMs over the pixel axis (K = pixels)
         else:
-            L.conv_wgrad(a, dy, P[name + ".weight"].grad, kh=cw.k, stride=stride, pad=pad, upsample=upsample)
-        L.col_sums(dy.reshape(-1, cw.cout), P[name + ".bias"].grad)
-        self._grad_ready(P[name + ".bias"]); self._grad_ready(P[name + ".weight"])
+            L.conv_wgrad(a, dy, G[name + ".weight"], kh=cw.k, stride=stride, pad=pad, upsample=upsample)
+        L.col_sums(dy.reshape(-1, cw.cout), G[name + ".bias"])
+        self.ex.ready(name + ".bias", name + ".weight")
         if not need_dx:
             return None
         wk = cw.w_kn.reshape(cw.k, cw.k, cw.cin, cw.cout)
@@ -320,15 +266,15 @@ class VQGANTrainer:
         if stride == 2 or not self._tc_ok(cw, stride, upsample):     # the fp32 step's kernels
             a = x if norm is None else self._gn_apply(x, norm[0], norm[1], norm[2])
             return self._conv_bw(name, cw, a, dy, stride=stride, upsample=upsample, need_dx=need_dx)
-        P = self.P
-        gw = P[name + ".weight"].grad
+        G = self.ex.g
+        gw = G[name + ".weight"]
         if L.conv_wgrad_bf16_ok(x, dy, cw.k, stride, upsample):
             L.conv_wgrad_bf16(x, dy, gw, norm=None if norm is None else (norm[0], norm[1][0], norm[1][1], norm[2]), upsample=upsample)
         else:
             a = x if norm is None else self._gn_apply(x, norm[0], norm[1], norm[2])
             L.conv_wgrad(a, dy, gw, kh=cw.k, stride=1, pad=(1, 1), upsample=upsample)
-        L.col_sums(dy.reshape(-1, cw.cout), P[name + ".bias"].grad)
-        self._grad_ready(P[name + ".bias"]); self._grad_ready(P[name + ".weight"])
+        L.col_sums(dy.reshape(-1, cw.cout), G[name + ".bias"])
+        self.ex.ready(name + ".bias", name + ".weight")
         if not need_dx:
             return None
         dx = L.tc_conv(self._b16(dy), self._wb16[id(cw)][1], None)
@@ -336,11 +282,11 @@ class VQGANTrainer:
 
     def _lin_bw(self, name, ln, x_rows, dy_rows, residual=None):
         """y = x W^T + b.  Accumulates dW [out,in], db; returns dx = dy W (+ residual)."""
-        P = self.P
+        G = self.ex.g
         m = x_rows.shape[0]
-        L.conv_wgrad(x_rows.reshape(1, m, 1, ln.k), dy_rows.reshape(1, m, 1, ln.n), P[name + ".weight"].grad, kh=1, pad=(0, 0), so=(1, ln.k))
-        L.col_sums(dy_rows, P[name + ".bias"].grad)
-        self._grad_ready(P[name + ".bias"]); self._grad_ready(P[name + ".weight"])
+        L.conv_wgrad(x_rows.reshape(1, m, 1, ln.k), dy_rows.reshape(1, m, 1, ln.n), G[name + ".weight"], kh=1, pad=(0, 0), so=(1, ln.k))
+        L.col_sums(dy_rows, G[name + ".bias"])
+        self.ex.ready(name + ".bias", name + ".weight")
         dx = torch.empty((m, ln.k), dtype=torch.float32, device=x_rows.device)
         L.simt_gemm(dy_rows, ln.w, dx, M=m, N=ln.k, K=ln.n, a_strides=(ln.n, 1), b_strides=(ln.k, 1), ldc=ln.k, residual=residual)
         return dx
@@ -360,15 +306,15 @@ class VQGANTrainer:
 
     def _res_bw(self, entry, dy):
         _, name, r, x, st1, h, st2 = entry
-        P = self.P
+        G = self.ex.g
         if self.bf16:
             da2 = self._conv_bw16(name + ".conv2", r["c2"], h, dy, norm=(st2, r["n2"], True))
         else:
             a2 = self._gn_apply(h, st2, r["n2"], True)
             da2 = self._conv_bw(name + ".conv2", r["c2"], a2, dy)
-        dh = L.groupnorm_bwd(h, da2, st2, r["n2"][0], r["n2"][1], P[name + ".norm2.weight"].grad, P[name + ".norm2.bias"].grad, swish=True,
+        dh = L.groupnorm_bwd(h, da2, st2, r["n2"][0], r["n2"][1], G[name + ".norm2.weight"], G[name + ".norm2.bias"], swish=True,
                              out_bf16=self.bf16)
-        self._grad_ready(P[name + ".norm2.bias"]); self._grad_ready(P[name + ".norm2.weight"])
+        self.ex.ready(name + ".norm2.bias", name + ".norm2.weight")
         if self.bf16:
             da1 = self._conv_bw16(name + ".conv1", r["c1"], x, dh, norm=(st1, r["n1"], True))
         else:
@@ -379,9 +325,9 @@ class VQGANTrainer:
             dres = self._lin_bw(name + ".nin_shortcut", r["sc"], x.reshape(-1, c), dy.reshape(-1, dy.shape[-1])).reshape(x.shape)
         else:
             dres = dy
-        dx = L.groupnorm_bwd(x, da1, st1, r["n1"][0], r["n1"][1], P[name + ".norm1.weight"].grad, P[name + ".norm1.bias"].grad, swish=True, add=dres,
+        dx = L.groupnorm_bwd(x, da1, st1, r["n1"][0], r["n1"][1], G[name + ".norm1.weight"], G[name + ".norm1.bias"], swish=True, add=dres,
                              out_bf16=self.bf16)
-        self._grad_ready(P[name + ".norm1.bias"]); self._grad_ready(P[name + ".norm1.weight"])
+        self.ex.ready(name + ".norm1.bias", name + ".norm1.weight")
         return dx
 
     def _attn_fw(self, aw, x, tape, name):
@@ -407,7 +353,7 @@ class VQGANTrainer:
 
     def _attn_bw(self, entry, dy):
         _, name, aw, x, st, qk, v, Pm, o = entry
-        P = self.P
+        G = self.ex.g
         n, hh, ww, c = x.shape
         hw = hh * ww
         scale = float(int(c) ** (-0.5))
@@ -428,19 +374,15 @@ class VQGANTrainer:
         a = self._gn_apply(x, st, aw["norm"], False).reshape(n * hw, c)
         da = self._lin_bw(name + ".v", aw["v"], a, dv)
         da = self._lin_bw(name + ".qk", aw["qk"], a, dqk, residual=da)
-        dx = L.groupnorm_bwd(x, da.reshape(x.shape), st, aw["norm"][0], aw["norm"][1], P[name + ".norm.weight"].grad, P[name + ".norm.bias"].grad,
+        dx = L.groupnorm_bwd(x, da.reshape(x.shape), st, aw["norm"][0], aw["norm"][1], G[name + ".norm.weight"], G[name + ".norm.bias"],
                              swish=False, add=dy, out_bf16=self.bf16)
-        self._grad_ready(P[name + ".norm.bias"]); self._grad_ready(P[name + ".norm.weight"])
+        self.ex.ready(name + ".norm.bias", name + ".norm.weight")
         return dx
 
     # ------------------------------------------------------------------ the step
     def forward_backward(self, x_nchw):
-        """x f32 NCHW in [-1,1] -> loss (python float).  Leaves the gradient (summed over ranks once the handles complete) in flat_g."""
+        """x f32 NCHW in [-1,1] -> loss (python float).  Leaves the gradient (summed over ranks once the exchange is waited for) in flat_g."""
         model, cfg, w = self.model, self.cfg, self.model._w
-        self.P = self._pmap()
-        self.flat_g.zero_()
-        self._handles, self.launched = [], []
-        self._bucket_left = list(self._bucket_size)
         was_training = model.training
         model.training = True                                      # QuantizeEMA.forward: EMA statistics + codebook overwrite (utils_th.py:46-64)
         x = L.nchw_to_nhwc(model._in(x_nchw))
@@ -493,13 +435,14 @@ class VQGANTrainer:
         # that keeps the split-fp16 operands of the tensor-core convs away from fp16's subnormal range; each gradient bucket is divided
         # by s when it completes, so flat_g, the all-reduce, clipping and Adam see the unscaled gradient
         s = self._seed_scale = float(2.0 ** round(math.log2(dec.numel())) if self.grad_seed_scale is None else self.grad_seed_scale)
+        self.ex.reset(s)
         ddec, l1 = L.l1_grad(x, dec, s / dec.numel())
         rec = l1 / dec.numel()
         loss = rec.to(torch.float32).reshape(()) + float(cfg.codebook_weight) * diff
         self.last = dict(rec_loss=rec, quant_loss=diff, codes=idx.reshape(n, zh, zw), reconstruction=dec)
         # ---------------- backward
         dy = ddec
-        P = self.P
+        G = self.ex.g
         for entry in reversed(tape):
             kind = entry[0]
             if kind == "res":
@@ -518,10 +461,10 @@ class VQGANTrainer:
                     if model.quantizer == "commit":
                         # d/dE of beta mean((q - sg(z))^2): column k gets 2 beta / numel * (count_k e_k - sum of the z rows mapped to k);
                         # the straight-through output carries no gradient to E (utils_th.py:117)
-                        pe = P["quantize.embeddings"]
-                        counts, zsum = L.vq_ema_stats(z, idx, pe.tensor.shape[1])
-                        L.vq_commit_grad(pe.tensor, counts, zsum, s * 2.0 * model.beta * float(cfg.codebook_weight) / z.numel(), pe.grad)
-                        self._grad_ready(pe)
+                        emb = self.ex.p["quantize.embeddings"]
+                        counts, zsum = L.vq_ema_stats(z, idx, emb.shape[1])
+                        L.vq_commit_grad(emb, counts, zsum, s * 2.0 * model.beta * float(cfg.codebook_weight) / z.numel(), G["quantize.embeddings"])
+                        self.ex.ready("quantize.embeddings")
                     dy = self._lin_bw("quant_conv", w["quant_conv"], hz.reshape(-1, zc), dz).reshape(hz.shape)
             elif kind == "normconv":
                 _, nname, cname, blk, xin, st = entry
@@ -529,19 +472,16 @@ class VQGANTrainer:
                 cw = blk["conv_out"]
                 a = self._gn_apply(xin, st, nw, True)
                 da = self._conv_bw(cname, cw, a, dy)
-                dy = L.groupnorm_bwd(xin, da, st, nw[0], nw[1], P[nname + ".weight"].grad, P[nname + ".bias"].grad, swish=True, out_bf16=self.bf16)
-                self._grad_ready(P[nname + ".bias"]); self._grad_ready(P[nname + ".weight"])
+                dy = L.groupnorm_bwd(xin, da, st, nw[0], nw[1], G[nname + ".weight"], G[nname + ".bias"], swish=True, out_bf16=self.bf16)
+                self.ex.ready(nname + ".bias", nname + ".weight")
         model.training = was_training
-        if any(self._bucket_left):
-            raise RuntimeError("backward pass left gradient buckets incomplete: " + str([self.buckets[i][2] for i, n in enumerate(self._bucket_left) if n]))
+        self.ex.check_complete()
         return loss
 
     def optimizer_step(self):
-        for h in self._handles:
-            h.wait()
-        self._handles = []
+        self.ex.wait()
         self.step_count += 1
-        gs = 1.0 / self._world()
+        gs = 1.0 / self.ex.world()
         clip = float(self.cfg.gradient_clip_val or 0.0)
         if clip > 0:
             # the reference trains under pytorch-lightning (train_codebook_th.py:69), which clips the global L2 norm of all gradients (after
@@ -592,7 +532,7 @@ class VQGANTrainer:
 
     def export_gradients(self):
         """Gradient of the last forward_backward (already summed over ranks if the handles were waited for), reference layouts."""
-        return self._export(lambda p: p.grad)
+        return self._export(lambda p: self.ex.g[p.name])
 
     def export_state_dict(self):
         """Reference-keyed state_dict after training; also refreshes the model's host copy."""

@@ -13,9 +13,9 @@
               decoupled decay lr*wd*p for every variable whose name has no "bias" (models/utils.py:424, 507-515 — LayerNorm gamma /
               beta ARE decayed: their Keras names are ln_1/gamma ..., which match none of the exclusion patterns), learning rate
               = 2000-step linear warm-up then cosine decay to 0 (migt.py:457-462, models/utils.py:310-416; the first step runs at lr 0)
-    exchange  gradients live in one flat buffer ordered by backward completion; contiguous buckets are all-reduced (SUM, then
-              divided by the world size — see the note in DESIGN.md on MirroredStrategy's per-replica reduce_mean) asynchronously
-              while the rest of the backward pass runs.
+    exchange  the codebook trainer's ``dist.GradExchange``: gradients live in one flat buffer ordered by backward completion;
+              contiguous buckets are all-reduced (SUM; grad_reduce="mean" divides by the world size — see the note in DESIGN.md on
+              MirroredStrategy's per-replica reduce_mean) asynchronously while the rest of the backward pass runs.
 
 precision="bf16" (the reference's 16-bit recipes: --fp16 -> mixed-precision policy + LossScaleOptimizer, train_transformer.py:102-104,
 models/utils.py:432-433, migt.py:466-488): every dense GEMM that fits the tensor-core tiles (forward, data and weight gradient) takes bf16
@@ -35,6 +35,7 @@ from collections import OrderedDict
 import torch
 
 from . import _lib as L
+from .dist import GradExchange
 
 LN_EPS = 1e-5
 
@@ -97,32 +98,11 @@ class MIGTTrainer:
             order += [k for k in names if k.startswith(f"h.{i}.")]
         order += [k for k in names if k.startswith("pose_embedding.")] + ["wpe.embeddings", "wte.weight"]
         assert sorted(order) == sorted(names)
-        offs, n = {}, 0
+        ex = self.ex = GradExchange([(k, sd[k].shape) for k in order], self.device, self.bucket_bytes, self.group)
+        self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.p, self.g = ex.flat_p, ex.flat_g, ex.flat_m, ex.flat_v, ex.p, ex.g
+        self.order, self.offs, self.buckets, self.launched = ex.order, ex.offs, ex.buckets, ex.launched
         for k in order:
-            offs[k] = n
-            n += (sd[k].numel() + 3) // 4 * 4
-        dev = self.device
-        self.flat_p = torch.zeros((n,), dtype=torch.float32, device=dev)
-        self.flat_g, self.flat_m, self.flat_v = torch.zeros_like(self.flat_p), torch.zeros_like(self.flat_p), torch.zeros_like(self.flat_p)
-        self.p, self.g = OrderedDict(), OrderedDict()
-        for k in order:
-            t = sd[k].to(torch.float32)
-            self.p[k] = self.flat_p[offs[k]:offs[k] + t.numel()].view(t.shape)
-            self.p[k].copy_(t)
-            self.g[k] = self.flat_g[offs[k]:offs[k] + t.numel()].view(t.shape)
-        self.order, self.offs = order, offs
-        self.buckets, start = [], 0
-        for i, k in enumerate(order):
-            end = offs[k] + (sd[k].numel() + 3) // 4 * 4
-            if (end - start) * 4 >= self.bucket_bytes or i == len(order) - 1:
-                self.buckets.append((start, end))
-                start = end
-        self._bucket_of, bi = {}, 0
-        for k in order:
-            while offs[k] >= self.buckets[bi][1]:
-                bi += 1
-            self._bucket_of[k] = bi
-        self._bucket_size = [sum(1 for b in self._bucket_of.values() if b == i) for i in range(len(self.buckets))]
+            self.p[k].copy_(sd[k].to(torch.float32))
         # AdamWeightDecay: every variable except the ones whose name contains "bias" (see the module docstring)
         self.decay = {k: ("bias" not in k) for k in order}
 
@@ -155,26 +135,6 @@ class MIGTTrainer:
 
     def gradients(self):
         return OrderedDict((k, self.g[k].detach().cpu().clone()) for k in self.model.param_shapes().keys())
-
-    # ------------------------------------------------------------------ exchange
-    def _world(self):
-        import torch.distributed as dist
-        return dist.get_world_size(self.group) if (dist.is_available() and dist.is_initialized()) else 1
-
-    def _ready(self, *names):
-        for k in names:
-            b = self._bucket_of[k]
-            self._left[b] -= 1
-            if self._left[b] == 0:
-                self.launched.append(b)
-                s, e = self.buckets[b]
-                if self._seed_scale != 1.0:                        # divide the seed scale back out (exact: a power of two)
-                    L.lincomb3(1.0 / self._seed_scale, self.flat_g[s:e], out=self.flat_g[s:e])
-                if self._world() > 1:
-                    import torch.distributed as dist
-                    self._handles.append(dist.all_reduce(self.flat_g[s:e], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
-            elif self._left[b] < 0:
-                raise RuntimeError(f"gradient of {k} signalled twice")
 
     # ------------------------------------------------------------------ dense layer (Conv1D: x @ W[in,out] + b[1,out])
     # Dense layers whose sizes fit the tensor-core tiles run forward, data gradient and weight gradient on the exact split-fp16 GEMM
@@ -219,24 +179,25 @@ class MIGTTrainer:
         L.tc_gemm(L.to_bf16(dy), self._w16[name][1], dx, M=m, N=k, K=n, lda=n, ldb=n, ldc=k, residual=residual)
         return dx
 
-    def _lin_bw(self, x, dy, name, need_dx=True, residual=None):
+    def _lin_bw(self, x, dy, name, *, need_dx=True, residual=None, last=True, out16=None):
+        """Accumulates dW, db of x @ W + b and returns dx = dy W^T (+ residual).  A layer applied to every stream is called once per stream:
+        the weight-gradient kernels accumulate, and readiness is signalled on the ``last`` call.  bf16: ``out16`` receives dx as bf16 only
+        (the attention backward's dO operand)."""
         W = self.p[name + ".weight"]
         k, n = W.shape
         m = x.shape[0]
         tc = self._tc_dense_ok(k, n)
-        if tc and self.bf16:
-            L.dense_wgrad_bf16(x, dy, self.g[name + ".weight"])
-            L.col_sums(dy, self.g[name + ".bias"].reshape(-1))
-            self._ready(name + ".bias", name + ".weight")
-            return self._dgrad16(dy, name, residual=residual) if need_dx else None
         if tc:
-            L.dense_wgrad_tc(x, dy, self.g[name + ".weight"])
+            (L.dense_wgrad_bf16 if self.bf16 else L.dense_wgrad_tc)(x, dy, self.g[name + ".weight"])
         else:
             L.conv_wgrad(x.reshape(1, m, 1, k), dy.reshape(1, m, 1, n), self.g[name + ".weight"], kh=1, pad=(0, 0), so=(n, 1))
         L.col_sums(dy, self.g[name + ".bias"].reshape(-1))
-        self._ready(name + ".bias", name + ".weight")
+        if last:
+            self.ex.ready(name + ".bias", name + ".weight")
         if not need_dx:
             return None
+        if tc and self.bf16:
+            return self._dgrad16(dy, name, residual=residual, out16=out16)
         if tc:                                  # dx = dy W^T: W [k, n] is already K-major for this product
             return self._dense_fw_tc(dy, ("bw", name), lambda: W.contiguous(), k, n, residual=residual)
         dx = torch.empty((m, k), dtype=torch.float32, device=x.device)
@@ -249,7 +210,7 @@ class MIGTTrainer:
     def _ln_bw(self, x, dy, name, add=None, last=True):
         dx = L.layernorm_bwd(x, dy, self.p[name + ".gamma"], self.g[name + ".gamma"], self.g[name + ".beta"], eps=LN_EPS, add=add)
         if last:
-            self._ready(name + ".beta", name + ".gamma")
+            self.ex.ready(name + ".beta", name + ".gamma")
         return dx
 
     def _drop_seed(self, site):
@@ -303,8 +264,7 @@ class MIGTTrainer:
                             b_bs=(S * 3 * d, dh), c_bs=pb, c_off=half * S)
                 L.simt_gemm(Pd, do, dvqk[ks], M=S, N=dh, K=S, a_strides=(1, cols), b_strides=(d, 1), ldc=3 * d, batch=(B, H), a_bs=pb, b_bs=(S * d, dh),
                             c_bs=(S * 3 * d, dh), a_off=half * S, residual=dvqk[ks])
-            if float(self.cfg.dropout) > 0:
-                dP = self._drop(dP, site0 + s)                      # same mask and scale as the forward pass
+            dP = self._drop(dP, site0 + s)                          # same mask and scale as the forward pass
             dS = L.softmax_bwd_rows(P, dP)
             for half, ks in ((0, 0),) if s == 0 else ((0, 0), (1, s)):
                 # dq_s += dS[:, half] k_ks ;  dk_ks += dS[:, half]^T q_s
@@ -338,8 +298,6 @@ class MIGTTrainer:
     # ------------------------------------------------------------------ the step
     def forward_backward(self, poses, tokens):
         cfg, dev, p, g = self.cfg, self.device, self.p, self.g
-        self.flat_g.zero_()
-        self._handles, self.launched, self._left = [], [], list(self._bucket_size)
         tokens = torch.as_tensor(tokens)
         B, T = tokens.shape[:2]
         Lt, d, V = self.model.n_image_tokens, cfg.d_model, cfg.n_embeddings
@@ -397,6 +355,7 @@ class MIGTTrainer:
         self.last = dict(ce_loss=ce, logits=logits.reshape(B, T, Lt, V))
         dhn = [None] * ns
         self._seed_scale = float(2.0 ** round(math.log2(denom)) if self.grad_seed_scale is None else self.grad_seed_scale)
+        self.ex.reset(self._seed_scale)
         ls = self.loss_scale * self._seed_scale                                    # gradient seeds carry the loss scale (1 in fp32) and the seed scale
         dlog = L.cross_entropy_grad(logits, ids.reshape(-1), (view_ok * (float(cfg.image_generation_weight) * ls / denom)).contiguous(),
                                     float(cfg.label_smoothing))
@@ -427,7 +386,7 @@ class MIGTTrainer:
                 pls, ols = float(pl.double().sum()), float(ol.double().sum())
                 pose_loss = torch.full_like(pl, float(B * (w01[0] + w01[1]) + e0 * pls + e1 * ols))
                 self.g[wkey].copy_(torch.tensor([lw_now * (B - e0 * pls) * ls, lw_now * (B - e1 * ols) * ls], dtype=torch.float32))
-                self._ready(wkey)
+                self.ex.ready(wkey)
                 ps, os_ = e0 * B, e1 * B
             else:
                 pose_loss, ps, os_ = pl + ol, 1.0, 1.0
@@ -437,7 +396,7 @@ class MIGTTrainer:
             dg_ = self._lin_bw(self._gelu(pc_h), draw, "pose_classifier.c_proj")
             dhn[2] = self._lin_bw(hn[2], L.gelu_bwd(pc_h, dg_), "pose_classifier.c_fc")
         else:
-            self._ready(*[k for k in self.order if k.startswith("pose_classifier.") or k.startswith("pose_loss_weighting_criterion.")])
+            self.ex.ready(*[k for k in self.order if k.startswith("pose_classifier.") or k.startswith("pose_loss_weighting_criterion.")])
         # ln_f backward (shared parameters: accumulate over the streams that carry a loss)
         dxs = [torch.zeros_like(xs[0])] + [None] * (ns - 1)
         live = [s for s in range(ns) if dhn[s] is not None]
@@ -450,33 +409,30 @@ class MIGTTrainer:
             xin, vqk, probs, outs, ys, hm = tape[li]
             dys = []
             for s in range(ns):
-                dz = self._drop(dxs[s], site + 8 + s) if float(cfg.dropout) > 0 else dxs[s]
+                dz = self._drop(dxs[s], site + 8 + s)
                 last = s == ns - 1
-                dgel = self._lin_bw_shared(self._gelu(hm[s]), dz, pre + "mlp.c_proj", last)
-                dm = self._lin_bw_shared(self._ln(ys[s], pre + "ln_2"), L.gelu_bwd(hm[s], dgel), pre + "mlp.c_fc", last)
+                dgel = self._lin_bw(self._gelu(hm[s]), dz, pre + "mlp.c_proj", last=last)
+                dm = self._lin_bw(self._ln(ys[s], pre + "ln_2"), L.gelu_bwd(hm[s], dgel), pre + "mlp.c_fc", last=last)
                 dys.append(self._ln_bw(ys[s], dm, pre + "ln_2", add=dxs[s], last=last))
             if self.bf16:
                 qk, vt, o32, lse = vqk
                 do16 = torch.empty((ns, B * S, d), dtype=torch.bfloat16, device=dev)
                 for s in range(ns):
-                    dy = self._drop(dys[s], site + 4 + s) if float(cfg.dropout) > 0 else dys[s]
-                    self._lin_bw_shared(o32[s], dy, pre + "attn.c_proj", s == ns - 1, out16=do16[s])
+                    self._lin_bw(o32[s], self._drop(dys[s], site + 4 + s), pre + "attn.c_proj", last=s == ns - 1, out16=do16[s])
                 dvqk = L.attn_multiend_bwd(qk, vt, do16, o32, lse, B, S, ns, cfg.n_head, d, Lt, rate=float(cfg.dropout), seed=self._drop_seed(site))
             else:
                 dos = []
                 for s in range(ns):
-                    dy = self._drop(dys[s], site + 4 + s) if float(cfg.dropout) > 0 else dys[s]
-                    dos.append(self._lin_bw_shared(outs[s], dy, pre + "attn.c_proj", s == ns - 1))
+                    dos.append(self._lin_bw(outs[s], self._drop(dys[s], site + 4 + s), pre + "attn.c_proj", last=s == ns - 1))
                 dvqk = self._attention_bw(vqk, probs, dos, B, S, Lt, site)
             new_dxs = []
             for s in range(ns):
                 last = s == ns - 1
-                da = self._lin_bw_shared(self._ln(xin[s], pre + "ln_1"), dvqk[s], pre + "attn.c_attn", last)
+                da = self._lin_bw(self._ln(xin[s], pre + "ln_1"), dvqk[s], pre + "attn.c_attn", last=last)
                 new_dxs.append(self._ln_bw(xin[s], da, pre + "ln_1", add=dys[s], last=last))
             dxs = new_dxs
         # ---------------- embeddings backward
-        if float(cfg.dropout) > 0:
-            dxs = [self._drop(dx, 10 + s) for s, dx in enumerate(dxs)]
+        dxs = [self._drop(dx, 10 + s) for s, dx in enumerate(dxs)]
         dpe = torch.zeros((B * T, d), dtype=torch.float32, device=dev)
         L.migt_embed_bwd(dxs[0], ids, 0, B * T, Lt, g["wte.weight"], g["wpe.embeddings"], dpe)
         L.migt_embed_bwd(dxs[1], None, self.model.mask_token, B * T, Lt, g["wte.weight"], g["wpe.embeddings"], dpe)
@@ -486,40 +442,13 @@ class MIGTTrainer:
             L.col_sums(dloc, g["wte.weight"][self.model.localization_token])
         dh_ = self._lin_bw(self._gelu(pe_h), dpe, "pose_embedding.c_proj")
         self._lin_bw(pin, L.gelu_bwd(pe_h, dh_), "pose_embedding.c_fc", need_dx=False)
-        self._ready("wpe.embeddings", "wte.weight")
-        if any(self._left):
-            raise RuntimeError("backward pass left gradient buckets incomplete: " + str([i for i, n in enumerate(self._left) if n]))
+        self.ex.ready("wpe.embeddings", "wte.weight")
+        self.ex.check_complete()
         self.last["loss_per_scene"] = loss
         return loss.mean()
 
     def _gelu(self, x):
         return L.gelu(x)
-
-    def _lin_bw_shared(self, x, dy, name, last, out16=None):
-        """_lin_bw for a layer applied to every stream: the weight-gradient kernels accumulate; readiness is signalled on the last one.
-        bf16: ``out16`` receives dx as bf16 only (the attention backward's dO operand)."""
-        W = self.p[name + ".weight"]
-        k, n = W.shape
-        m = x.shape[0]
-        tc = self._tc_dense_ok(k, n)
-        if tc and self.bf16:
-            L.dense_wgrad_bf16(x, dy, self.g[name + ".weight"])
-            L.col_sums(dy, self.g[name + ".bias"].reshape(-1))
-            if last:
-                self._ready(name + ".bias", name + ".weight")
-            return self._dgrad16(dy, name, out16=out16)
-        if tc:
-            L.dense_wgrad_tc(x, dy, self.g[name + ".weight"])
-        else:
-            L.conv_wgrad(x.reshape(1, m, 1, k), dy.reshape(1, m, 1, n), self.g[name + ".weight"], kh=1, pad=(0, 0), so=(n, 1))
-        L.col_sums(dy, self.g[name + ".bias"].reshape(-1))
-        if last:
-            self._ready(name + ".bias", name + ".weight")
-        if tc:
-            return self._dense_fw_tc(dy, ("bw", name), lambda: W.contiguous(), k, n)
-        dx = torch.empty((m, k), dtype=torch.float32, device=x.device)
-        L.simt_gemm(dy, W, dx, M=m, N=k, K=n, a_strides=(n, 1), b_strides=(1, n), ldc=k)
-        return dx
 
     # ------------------------------------------------------------------ schedule + optimizer (models/utils.py:310-564)
     def learning_rate(self, step=None):
@@ -539,9 +468,7 @@ class MIGTTrainer:
         scale halves (not below 1) and the good-step counter resets, but ``iterations`` still advances, as Keras's do_not_apply_fn does, so
         the learning-rate and localisation schedules move on.  Finite: the update runs on the unscaled gradients (clipping included), and
         when the counter has reached 1999 the scale doubles (if that is finite) and the counter resets, else the counter counts up."""
-        for h in self._handles:
-            h.wait()
-        self._handles = []
+        self.ex.wait()
         lr = self.learning_rate()
         self.iterations += 1
         self._wsplit = {}
@@ -559,7 +486,7 @@ class MIGTTrainer:
                 self.loss_scale_counter += 1
         wd = float(self.cfg.weight_decay)
         clip = float(self.cfg.gradient_clip_val or 0.0)
-        gs = (1.0 / self._world() if self.grad_reduce == "mean" else 1.0) / ls
+        gs = (1.0 / self.ex.world() if self.grad_reduce == "mean" else 1.0) / ls
         for k in self.order:
             cs = 1.0
             if clip > 0:                                                  # tf.clip_by_norm: g * clip / max(|g|, clip), per tensor
