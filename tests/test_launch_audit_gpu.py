@@ -1,0 +1,198 @@
+"""Every GEMM, convolution, attention, weight-gradient and codebook-lookup launch of the real workloads, checked against fp64 on its own
+operands (tests/launch_checks.py: references and bars).  The kernel tests pin each entry point at a few hand-picked shapes; the workloads
+call the same entry points at dozens of others (tile shapes, tails, split-K and tile walks all depend on the shape), which were otherwise
+only held by loose end-to-end bars.
+
+Each wrapped call snapshots what it overwrites, runs the real wrapper, and is checked at once on the same stream, before later launches
+reuse its buffers.  Sampling keeps full size cheap: GEMMs up to 3 batch indices x (first 128, last 128, 64 random rows) x all columns;
+convs 3 images (first, last, one random) x all pixels; attention 3 (batch, head) pairs x all rows and streams; weight gradients in full.
+Calls made while a CUDA graph is being captured are counted and skipped (all workloads here are eager).
+
+Measured on an H100 80GB HBM3 (700 W power limit), worst ratio to the bar per workload (the file runs in about 30 s of pytest time):
+  mixed generate, 3 scenes x 10 views (VF_NORM_ON_LOAD 0 and 1 alike): tc_gemm bf16 0.989 (bf16-output GEMMs: the output rounding bound
+      itself), tc_conv bf16 0.84, attn_block_causal 0.64, simt_gemm 0.11, conv3x3_small_cin 0.089, tc_gemm split 0.047, tc_conv split 0.010,
+      vq_lookup_fused 1e-4.
+  tf32 encode + decode_code: conv3x3_small_cin 0.10, tc_gemm tf32 0.062, tc_conv tf32 0.011.
+  C5 KV cache (19 context views, empty slot): tc_gemm bf16 0.89, attn_block_causal 0.66.
+  bf16 codebook step, medium / full size: conv3x3_small_cin 0.075 / 0.12, simt_conv 0.066 / 0.068, conv_wgrad_bf16 0.0037 / 0.035,
+      conv_wgrad_tc 0.0013 / 0.020, tc_gemm bf16 0.018 / 0.019, tc_conv bf16 0.0031 / 0.0035.
+  bf16 transformer step, small (dropout 0.1) / full size: tc_gemm bf16 0.97 / 0.89, attn_multiend_train 0.54 / 0.61, attn_multiend_bwd
+      0.32 / 0.70, conv_wgrad 0.17 / 0.26, dense_wgrad_bf16 0.093 / 0.20.
+  fp32 trainers, small: simt_gemm 0.076 / 0.23, dense_wgrad_tc 0.22, conv_wgrad 0.026 / 0.18, tc_gemm split 0.051, tc_conv split 0.0029.
+"""
+import os
+import random
+import statistics
+import sys
+from collections import defaultdict
+
+import pytest
+import torch
+
+import launch_checks as lc
+from oracle import synth, migt_oracle as mo
+from oracle.make_golden import vq_images, SMALL_VQ, MIGT_TRAIN
+from viewformer_b200.config import VQGANConfig, MIGTConfig
+
+pytestmark = pytest.mark.gpu
+
+_SKIP_FILES = ("_lib.py", "ops.py", "launch_checks.py", os.path.basename(__file__))
+
+
+@pytest.fixture(scope="module")
+def L(lib):
+    from viewformer_b200 import _lib
+    _lib.load(require_device=True)
+    return _lib
+
+
+class Audit:
+    """Wraps every checked ``_lib`` wrapper; records (calls, worst ratio) per (wrapper, operand dtype, caller file:line)."""
+
+    def __init__(self, L, monkeypatch, seed=0):
+        self.rec = defaultdict(list)
+        self.skipped = 0
+        self.rng = random.Random(seed)
+        orig = {name: getattr(L, name) for name in lc.CHECKERS}
+        groupnorm, dropout = L.groupnorm, L.dropout
+        monkeypatch.setitem(lc.HOOKS, "gn_apply_bf16", lambda x, mr, gamma, beta, swish: groupnorm(
+            x.contiguous(), gamma, beta, swish=swish, out_dtype=torch.bfloat16, stats=mr.contiguous(), groups=mr.shape[1]))
+        monkeypatch.setitem(lc.HOOKS, "dropout_mask", lambda shape, rate, seed, device: dropout(
+            torch.ones(shape, dtype=torch.float32, device=device), rate, seed))
+        monkeypatch.setitem(lc.HOOKS, "ref_lookup", lambda z, et, esq: orig["vq_lookup"](z, et, esq, want_quant=False, want_diff=False)[0])
+        for name, fn in orig.items():
+            monkeypatch.setattr(L, name, self._wrap(name, fn))
+
+    @staticmethod
+    def _site():
+        f = sys._getframe(2)
+        while f is not None and os.path.basename(f.f_code.co_filename) in _SKIP_FILES:
+            f = f.f_back
+        return "?" if f is None else f"{os.path.basename(f.f_code.co_filename)}:{f.f_lineno}"
+
+    def _wrap(self, name, fn):
+        def call(*a, **k):
+            if torch.cuda.is_current_stream_capturing():
+                self.skipped += 1
+                return fn(*a, **k)
+            first = a[0] if a else next(iter(k.values()))
+            dtype = str(first.dtype).replace("torch.", "")
+            with torch.no_grad():
+                result, r = lc.run_check(name, fn, a, k, self.rng)
+            self.rec[(name, dtype, self._site())].append(r)
+            return result
+        return call
+
+    def report(self, tag):
+        print(f"\n[audit {tag}] {'wrapper':<20} {'dtype':<9} {'site':<22} {'calls':>5} {'worst':>8} {'median':>8}")
+        bad = []
+        for (name, dtype, site), rs in sorted(self.rec.items()):
+            worst = max(rs)
+            print(f"[audit {tag}] {name:<20} {dtype:<9} {site:<22} {len(rs):>5} {worst:>8.3g} {statistics.median(rs):>8.3g}"
+                  + ("  <-- over its bar" if worst > 1.0 else ""))
+            if worst > 1.0:
+                bad.append(f"{name} {dtype} {site}: worst ratio {worst:.3g} over {len(rs)} calls")
+        per = defaultdict(float)
+        for (name, dtype, _), rs in self.rec.items():
+            per[(name, dtype)] = max(per[(name, dtype)], max(rs))
+        print(f"[audit {tag}] worst per wrapper: " + ", ".join(f"{n}/{d} {v:.3g}" for (n, d), v in sorted(per.items()))
+              + f"; skipped while capturing: {self.skipped}")
+        return bad
+
+    def reached(self):
+        return {(name, dtype) for name, dtype, _ in self.rec}
+
+
+def _mixed_generate(monkeypatch, L, norm_on_load):
+    import bench
+    from viewformer_b200 import VQGAN, MIGT, generate_batch_predictions
+    monkeypatch.setenv("VF_NORM_ON_LOAD", norm_on_load)
+    vcfg, tcfg = VQGANConfig(), MIGTConfig(localization_weight="0")
+    cb = VQGAN(vcfg, precision="mixed").load_state_dict(synth.make_vqgan_state_dict(vcfg, 0))
+    tr = MIGT(tcfg, precision="bf16").load_state_dict(synth.make_migt_state_dict(tcfg, 0))
+    images, cams = bench.synth_inputs(3, 1234)
+    generate_batch_predictions(tr, cb, images, cams)
+
+
+def _tf32_codec(monkeypatch, L):
+    from viewformer_b200 import VQGAN
+    cfg = VQGANConfig()
+    model = VQGAN(cfg, precision="tf32").load_state_dict(synth.make_vqgan_state_dict(cfg, 1))
+    codes = model.encode(vq_images(2, cfg.image_size, 21))[2]
+    model.decode_code(codes)
+
+
+def _kv_cache(monkeypatch, L):
+    from viewformer_b200 import MIGT
+    cfg = MIGTConfig(localization_weight="0")
+    model = MIGT(cfg, precision="bf16").load_state_dict(synth.make_migt_state_dict(cfg, 5))
+    B, T = 2, 20
+    codes = synth.make_codes(B, T, seed=31)
+    cams = mo.normalize_cameras(mo.to_relative_cameras(synth.make_cameras(B, T, seed=32))[0])
+    cache = model.prefill_context(codes[:, :-1], cams[:, :-1].contiguous())
+    model.query(cache, cams[:, -1].contiguous(), return_logits=True)
+
+
+def _vq_step(cfg_kw, n, precision, seed):
+    from viewformer_b200 import VQGAN
+    from viewformer_b200.train import VQGANTrainer
+    cfg = VQGANConfig(**cfg_kw)
+    model = VQGAN(cfg, precision="fp32").load_state_dict(synth.make_vqgan_state_dict(cfg, 5))
+    VQGANTrainer(model, precision=precision).forward_backward(vq_images(n, cfg.image_size, seed))
+
+
+def _migt_step(cfg_kw, B, T, precision, seed):
+    from viewformer_b200 import MIGT
+    from viewformer_b200.train_migt import MIGTTrainer
+    cfg = MIGTConfig(**cfg_kw)
+    model = MIGT(cfg, precision="fp32").load_state_dict(synth.make_migt_state_dict(cfg, 9))
+    codes = synth.make_codes(B, T, n_embed=cfg.n_embeddings, seed=seed)
+    cams = mo.normalize_cameras(mo.to_relative_cameras(synth.make_cameras(B, T, seed=seed + 1))[0])
+    MIGTTrainer(model, seed=seed, precision=precision).forward_backward(cams, codes)
+
+
+MEDIUM_VQ = dict(ch=128, ch_mult=[1, 2], attn_resolutions=[16], image_size=32, n_embed=256, perceptual_weight=0.0)
+SMALL_MIGT_BF16 = dict(n_layer=2, d_model=256, n_head=4, token_image_size=8, n_loss_skip=1, weight_decay=0.01, total_steps=100, learning_rate=1e-3,
+                       label_smoothing=0.05, localization_weight="0.5", image_generation_weight=0.8, pose_multiplier=1.0, dropout=0.1)
+FULL_MIGT_TRAIN = dict(dropout=0.0, label_smoothing=0.1, localization_weight="0.7", total_steps=100, learning_rate=1e-4)
+
+VQ_BF16_STEP = {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("conv_wgrad_bf16", "float32"),
+                ("conv_wgrad_tc", "float32"), ("simt_conv_dgrad_s2", "float32"), ("vq_lookup", "float32")}
+
+# workload -> (run, the (wrapper, operand dtype) pairs it is known to reach)
+WORKLOADS = {
+    "mixed-generate-norm0": (lambda mp, L: _mixed_generate(mp, L, "0"),
+                             {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("attn_block_causal", "bfloat16"),
+                              ("vq_lookup_fused", "float32")}),
+    "mixed-generate-norm1": (lambda mp, L: _mixed_generate(mp, L, "1"),
+                             {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("attn_block_causal", "bfloat16"),
+                              ("vq_lookup_fused", "float32")}),
+    "tf32-codec": (_tf32_codec, {("tc_conv", "float32"), ("tc_gemm", "float32"), ("vq_lookup_fused", "float32")}),
+    "kv-cache-c5": (_kv_cache, {("attn_block_causal", "bfloat16"), ("tc_gemm", "bfloat16")}),
+    "vq-step-bf16-medium": (lambda mp, L: _vq_step(MEDIUM_VQ, 4, "bf16", 4100), VQ_BF16_STEP),
+    "vq-step-bf16-full": (lambda mp, L: _vq_step(dict(perceptual_weight=0.0), 2, "bf16", 4200), VQ_BF16_STEP),
+    "migt-step-bf16-small": (lambda mp, L: _migt_step(SMALL_MIGT_BF16, 2, 5, "bf16", 4300),
+                             {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")}),
+    "migt-step-bf16-full": (lambda mp, L: _migt_step(FULL_MIGT_TRAIN, 1, 5, "bf16", 4400),
+                            {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")}),
+    "vq-step-fp32-small": (lambda mp, L: _vq_step(dict(SMALL_VQ, perceptual_weight=0.0), 3, "fp32", 4500),
+                           {("simt_gemm", "float32"), ("simt_conv", "float32"), ("simt_conv_dgrad_s2", "float32"), ("conv_wgrad", "float32"),
+                            ("tc_conv", "float16"), ("vq_lookup", "float32")}),
+    "migt-step-fp32-small": (lambda mp, L: _migt_step(MIGT_TRAIN, 2, 4, "fp32", 4600),
+                             {("tc_gemm", "float16"), ("simt_gemm", "float32"), ("dense_wgrad_tc", "float32"), ("conv_wgrad", "float32")}),
+}
+
+
+@pytest.mark.parametrize("workload", list(WORKLOADS))
+def test_launch_audit(L, monkeypatch, workload):
+    """One eager run of the workload with every checked launch held to its fp64 bar (ratio <= 1) and the expected wrappers reached."""
+    run, expected = WORKLOADS[workload]
+    audit = Audit(L, monkeypatch)
+    run(monkeypatch, L)
+    torch.cuda.synchronize()
+    bad = audit.report(workload)
+    missing = expected - audit.reached()
+    torch.cuda.empty_cache()
+    assert not missing, f"{workload}: the audit never saw {sorted(missing)}"
+    assert not bad, "launches outside their bar:\n  " + "\n  ".join(bad)
+
