@@ -30,6 +30,7 @@ and of the bf16 weight-gradient transposer, the dropout mask of the attention ke
 import math
 import random
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -58,6 +59,7 @@ HOOKS = {
     "gn_apply_bf16": _gn_apply_bf16_torch,       # (x [n,h,w,c], mean_rstd [n,g,2], gamma, beta, swish) -> bf16 operand
     "dropout_mask": _dropout_mask_missing,       # (shape, rate, seed, device) -> fp32 multipliers (0 or 1 / (1 - rate))
     "ref_lookup": None,                          # (z_rows, et, esq) -> int64 indices, or None: fp64 argmin with a near-tie tolerance
+    "gn_mean_rstd": None,                        # (x, groups, eps) -> the (mean, rstd) groupnorm computes when not given stats
 }
 
 
@@ -670,6 +672,799 @@ def check_vq_lookup(ba, result, st):
     return check_lookup(ba, result, st, use_hook=False)
 
 
+# ----------------------------------------------------------------------------------------------- normalisation
+GN_COND = []          # mean^2 / var of every GroupNorm group whose statistics were checked (the audit prints the largest)
+GN_USED = {}          # (x.data_ptr(), groups) -> the (mean, rstd) the last checked gn_mean_rstd call returned (what groupnorm then consumes)
+
+
+def f32(x):
+    """A hyperparameter as the kernel receives it (a C float), in fp64."""
+    return float(np.float32(x))
+
+
+def _gn_stats64(x, groups):
+    """fp64 (mean, var, mean |x|, mean x^2) [N, groups] of the stored x [N,H,W,C]."""
+    n = x.shape[0]
+    xg = x.double().reshape(n, -1, groups, x.shape[-1] // groups)
+    m = xg.mean((1, 3))
+    return m, (xg * xg).mean((1, 3)) - m * m, xg.abs().mean((1, 3)), (xg * xg).mean((1, 3))
+
+
+def gn_stats_chain(n, hw, c):
+    """Longest fp32 chain of vf_groupnorm_stats: a thread sums ceil(ppb / lanes) pixels of its channel quad, then folds the quad (+2); the
+    block's threads and the chunks then meet in fp64 atomics."""
+    lanes = 256 // (c // 4)
+    chunks = max(1, min((hw + 63) // 64, (132 * 8 + n - 1) // n))
+    ppb = (hw + chunks - 1) // chunks
+    return (ppb + lanes - 1) // lanes + 2
+
+
+def before_gn_mean_rstd(ba, rng):
+    x = ba["x"]
+    fused = getattr(x, "_gn_sums", None)
+    return dict(fused=fused is not None and fused[1] == ba["groups"])
+
+
+def check_gn_mean_rstd(ba, result, st):
+    """mean / rstd against the fp64 statistics of the stored x.  Sums with relative error t (of sum |x| and sum x^2) give
+    |mean err| <= t mean|x| + u |mean| and |var err| <= (2t + t^2) E x^2 + 2 t |mean| mean|x| + t^2 (mean|x|)^2, so rstd is within var_err / (2 (var + eps)) + 2u
+    relatively: the conditioning factor E x^2 / var = 1 + mean^2 / var appears explicitly.  t = 1e-5 for fused sums of an fp32 output,
+    2^-8 for a bf16 one (as _gn_ratio), and (K + 1) u for the statistics pass (K = gn_stats_chain; the squares round once).  Every
+    checked call appends its largest mean^2 / var to GN_COND."""
+    x, groups, eps = ba["x"], ba["groups"], f32(ba["eps"])
+    m, v, am, m2 = _gn_stats64(x, groups)
+    n, h, w, c = x.shape
+    if st["fused"]:
+        t = BF16_OUT if x.dtype == torch.bfloat16 else 1e-5
+    else:
+        t = (gn_stats_chain(n, h * w, c) + 1) * U
+    got = result.double()
+    verr = (2 * t + t * t) * m2 + 2 * t * m.abs() * am + t * t * am * am
+    r64 = 1.0 / torch.sqrt(v.clamp_min(0) + eps)
+    GN_COND.append(float((m * m / v.clamp_min(1e-300)).max()))
+    if len(GN_USED) > 64:
+        GN_USED.clear()
+    GN_USED[(x.data_ptr(), groups)] = result
+    return max(ratio((got[..., 0] - m).abs(), t * am + U * m.abs()),
+               ratio((got[..., 1] - r64).abs(), r64 * (verr / (2 * (v.clamp_min(0) + eps)) + 2 * U)))
+
+
+def _unlayout(y, n, h, w, c, upsample, s2d):
+    """fp64 [N,H,W,C] view(s) of a groupnorm output: the 4 copies of the x2 upsample, the space-to-depth blocks, split pairs decoded."""
+    if y.dtype == torch.float16:
+        cl = y.shape[-1] // 2
+        y = y[..., :cl].double() + y[..., cl:].double() / 2048.0
+    else:
+        y = y.double()
+    if upsample:
+        y6 = y.reshape(n, h, 2, w, 2, c)
+        return [y6[:, :, a, :, b] for a in (0, 1) for b in (0, 1)]
+    if s2d:
+        return [y.reshape(n, h // 2, w // 2, 2, 2, c).permute(0, 1, 3, 2, 4, 5).reshape(n, h, w, c)]
+    return [y]
+
+
+def before_groupnorm(ba, rng):
+    return dict(images=pick(ba["x"].shape[0], rng))
+
+
+def _groupnorm_stats(ba):
+    """The (mean, rstd) groupnorm consumed: the given ``stats``, else what its own gn_mean_rstd call returned (recorded by
+    check_gn_mean_rstd when that call is audited), else HOOKS['gn_mean_rstd']."""
+    if ba["stats"] is not None:
+        return ba["stats"]
+    used = GN_USED.pop((ba["x"].data_ptr(), ba["groups"]), None)
+    return used if used is not None else HOOKS["gn_mean_rstd"](ba["x"], ba["groups"], ba["eps"])
+
+
+def check_groupnorm(ba, result, st):
+    """y = ((x - mean) rstd) gamma + beta [swish] from the given (mean, rstd): 4 u (|xhat gamma| + |mean rstd gamma| + |beta|) (the
+    rounded operations, and the bf16 path's folded shift beta - mean rstd gamma), times 1.1 (the largest slope of swish) + 8 u |y| (its exp
+    and division); a bf16 output adds 2^-8 |y|, a split pair 2^-21 |y| + 2^-36 (hi + lo 2^-11 carries 22 bits)."""
+    x = ba["x"]
+    n, h, w, c = x.shape
+    imgs = torch.tensor(st["images"], device=x.device)
+    xv = x[imgs].double()
+    if ba["normalize"]:
+        g = ba["groups"]
+        mr = _groupnorm_stats(ba)[imgs].double()
+        cidx = torch.arange(c, device=x.device) // (c // g)
+        mu, rs = mr[:, cidx, 0][:, None, None], mr[:, cidx, 1][:, None, None]
+        ga, be = ba["gamma"].double(), ba["beta"].double()
+        ref = (xv - mu) * rs * ga + be
+        bar = 4 * U * (((xv - mu) * rs * ga).abs() + (mu * rs * ga).abs() + be.abs())
+    else:
+        ref, bar = xv, torch.zeros_like(xv)
+    if ba["swish"]:
+        ref = ref * torch.sigmoid(ref)
+        bar = 1.1 * bar + 8 * U * ref.abs()
+    if result.dtype == torch.bfloat16:
+        bar = (1 + BF16_OUT) * bar + BF16_OUT * ref.abs()
+    elif result.dtype == torch.float16:
+        bar = bar + 2.0 ** -21 * ref.abs() + 2.0 ** -36
+    worst = 0.0
+    for got in _unlayout(result[imgs], len(imgs), h, w, c, ba["upsample"], ba["s2d"]):
+        worst = max(worst, ratio((got - ref).abs(), bar))
+    return worst
+
+
+def before_layernorm(ba, rng):
+    x = ba["x"]
+    return dict(rows=pick_rows(x.numel() // x.shape[-1], rng))
+
+
+def check_layernorm(ba, result, st):
+    """Two fp32 passes per row (one warp): K = ceil(d / 128) quads per lane (+2 for the quad fold) + 5 shuffle levels.  The fp32 mean carries
+    K u mean|x|, which every x - mean inherits: |y - y64| <= 2 (K + 4) u (|xhat| + rstd mean|x|) |gamma| + 2 u |beta| (+ 2^-8 |y| for bf16);
+    an rstd off by the conditioning factor 1 + mean^2 / var would not fit (tests/test_norm_stats_gpu.py)."""
+    x, d = ba["x"], ba["x"].shape[-1]
+    rows = st["rows"].to(x.device)
+    xv = x.reshape(-1, d)[rows].double()
+    mu = xv.mean(1, keepdim=True)
+    rs = 1.0 / torch.sqrt(xv.var(1, unbiased=False, keepdim=True) + f32(ba["eps"]))
+    xh = (xv - mu) * rs
+    ga, be = ba["gamma"].double(), ba["beta"].double()
+    ref = xh * ga + be
+    K = (d + 127) // 128 + 7
+    bar = 2 * (K + 4) * U * (xh.abs() + rs * xv.abs().mean(1, keepdim=True)) * ga.abs() + 2 * U * be.abs()
+    if result.dtype == torch.bfloat16:
+        bar = (1 + BF16_OUT) * bar + BF16_OUT * ref.abs()
+    return ratio((result.reshape(-1, d)[rows].double() - ref).abs(), bar)
+
+
+def _gn_bwd_chains(n, hw, c):
+    """(K of the group sums, K of dgamma / dbeta) of vf_groupnorm_bwd: a thread sums ppb / lanes pixels of its quad in fp32 (the group sums
+    then meet in fp64); dgamma / dbeta then add the block's lanes in shared fp32 atomics and the N x chunks blocks in global ones, onto
+    the value held before."""
+    lanes = 256 // (c // 4)
+    ppb = lanes * 128
+    while ppb > lanes * 4 and ((hw + ppb - 1) // ppb) * n < 132 * 4:
+        ppb >>= 1
+    per = ppb // lanes
+    return per + 2, per + lanes + n * ((hw + ppb - 1) // ppb) + 1
+
+
+def before_groupnorm_bwd(ba, rng):
+    return dict(dgamma=ba["dgamma"].clone(), dbeta=ba["dbeta"].clone())
+
+
+def check_groupnorm_bwd(ba, result, st):
+    """dx = rstd (g gamma - mean(g gamma) - xhat mean(g gamma xhat)) [+ add], g = dout [x swish'], from the given (mean, rstd); dgamma /
+    dbeta added onto their snapshots.  The sum|terms| expressions of tests/test_backward_kernels_gpu.py::test_groupnorm_bwd with this
+    kernel's chains (_gn_bwd_chains) for K; the bf16 copy must be dx rounded to nearest even, bit for bit."""
+    x, dout, mr, gamma, beta, groups = ba["x"], ba["dout"], ba["mean_rstd"], ba["gamma"], ba["beta"], ba["groups"]
+    n, h, w, c = x.shape
+    cidx = torch.arange(c, device=x.device) // (c // groups)
+    mu_c, rs_c = mr.double()[:, cidx, 0].reshape(n, 1, 1, c), mr.double()[:, cidx, 1].reshape(n, 1, 1, c)
+    xh = (x.double() - mu_c) * rs_c
+    g = dout.double()
+    if ba["swish"]:
+        z = xh * gamma.double() + beta.double()
+        sg = torch.sigmoid(z)
+        g = g * sg * (1 + z * (1 - sg))
+    gg_ = g * gamma.double()
+    m1 = gg_.reshape(n, -1, groups, c // groups).mean((1, 3))[:, cidx].reshape(n, 1, 1, c)
+    m2 = (gg_ * xh).reshape(n, -1, groups, c // groups).mean((1, 3))[:, cidx].reshape(n, 1, 1, c)
+    add = ba["add"]
+    ref = rs_c * (gg_ - m1 - xh * m2) + (0.0 if add is None else add.double())
+    xh_err = xh.abs() + rs_c * mu_c.abs() + 1.0
+    dgg = gg_.abs()
+    A1 = dgg.reshape(n, -1, groups, c // groups).mean((1, 3))[:, cidx].reshape(n, 1, 1, c)
+    A2 = (dgg * xh_err).reshape(n, -1, groups, c // groups).mean((1, 3))[:, cidx].reshape(n, 1, 1, c)
+    Kg, Kc = _gn_bwd_chains(n, h * w, c)
+    s_dx = rs_c * (dgg * xh_err + A1 + xh_err * A2) + (0.0 if add is None else add.double().abs())
+    worst = ratio((result.double() - ref).abs(), 4 * (Kg + 8) * U * s_dx)
+    dg0, db0 = st["dgamma"].double(), st["dbeta"].double()
+    worst = max(worst, ratio((ba["dgamma"].double() - dg0 - (g * xh).sum((0, 1, 2))).abs(),
+                             4 * (Kc + 8) * U * (g.abs() * xh_err).sum((0, 1, 2)) + 2 * U * dg0.abs()))
+    worst = max(worst, ratio((ba["dbeta"].double() - db0 - g.sum((0, 1, 2))).abs(), 4 * (Kc + 8) * U * g.abs().sum((0, 1, 2)) + 2 * U * db0.abs()))
+    if ba["out_bf16"]:
+        worst = max(worst, bits_equal(result._bf16, result.to(torch.bfloat16)))
+    return worst
+
+
+def before_layernorm_bwd(ba, rng):
+    return dict(dgamma=ba["dgamma"].clone(), dbeta=ba["dbeta"].clone())
+
+
+def check_layernorm_bwd(ba, result, st):
+    """tests/test_backward_kernels_gpu.py::test_layernorm_bwd's bars with this kernel's chains: a row's statistics and mean(dy gamma),
+    mean(dy gamma xhat) are one warp's (K = ceil(d / 32) + 5); dgamma / dbeta meet the block's 8 rows in shared fp32 atomics, then
+    ceil(rows / 8) blocks in global ones, onto the snapshot (Kc = 8 + ceil(rows / 8) + 1)."""
+    x, dy, gamma = ba["x"], ba["dy"], ba["gamma"]
+    d = x.shape[-1]
+    xv, dv = x.reshape(-1, d).double(), dy.reshape(-1, d).double()
+    rows = xv.shape[0]
+    mu = xv.mean(1, keepdim=True)
+    rs = 1.0 / torch.sqrt(xv.var(1, unbiased=False, keepdim=True) + f32(ba["eps"]))
+    xh = (xv - mu) * rs
+    dg = dv * gamma.double()
+    ref = rs * (dg - dg.mean(1, keepdim=True) - xh * (dg * xh).mean(1, keepdim=True))
+    add = ba["add"]
+    if add is not None:
+        ref = ref + add.reshape(-1, d).double()
+    K = (d + 31) // 32 + 5
+    xh_err = xh.abs() + rs * xv.abs().mean(1, keepdim=True) + 1.0
+    dgg = dg.abs()
+    s_dx = rs * (dgg * xh_err + dgg.mean(1, keepdim=True) + xh_err * (dgg * xh_err).mean(1, keepdim=True))
+    if add is not None:
+        s_dx = s_dx + add.reshape(-1, d).double().abs()
+    worst = ratio((result.reshape(-1, d).double() - ref).abs(), 4 * (K + 8) * U * s_dx)
+    Kc = 8 + (rows + 7) // 8 + 1 + K
+    dg0, db0 = st["dgamma"].double(), st["dbeta"].double()
+    worst = max(worst, ratio((ba["dgamma"].double() - dg0 - (dv * xh).sum(0)).abs(), 4 * Kc * U * (dv.abs() * xh_err).sum(0) + 2 * U * dg0.abs()))
+    worst = max(worst, ratio((ba["dbeta"].double() - db0 - dv.sum(0)).abs(), 4 * Kc * U * dv.abs().sum(0) + 2 * U * db0.abs()))
+    return worst
+
+
+# ----------------------------------------------------------------------------------------------- reductions
+def col_sums_chain(rows):
+    """K of vf_col_sums: ceil(rpb / 8) rows per thread, 8 warps folded, the row chunks' atomics, the value held before."""
+    chunks = min((rows + 1023) // 1024, 1024)
+    rpb = (rows + chunks - 1) // chunks
+    chunks = (rows + rpb - 1) // rpb
+    return (rpb + 7) // 8 + 8 + chunks + 1
+
+
+def before_col_sums(ba, rng):
+    return dict(out=ba["out"].clone())
+
+
+def check_col_sums(ba, result, st):
+    """out += column sums of x [rows, C], against the snapshot: 2 K u (sum |x| + |out0|), K = col_sums_chain(rows)."""
+    x = ba["x_rows"]
+    c = x.shape[-1]
+    xv = x.reshape(-1, c).double()
+    K = col_sums_chain(xv.shape[0])
+    o0 = st["out"].double()
+    return ratio((result.double() - o0 - xv.sum(0)).abs(), 2 * K * U * (xv.abs().sum(0) + o0.abs()))
+
+
+def check_softmax_bwd_rows(ba, result, st):
+    """dS = P (dP - sum_j P_j dP_j), one warp per row: 2 (K + 2) u P (|dP| + sum|P dP|), K = ceil(cols / 32) + 5."""
+    P, dP = ba["P"], ba["dP"]
+    cols = P.shape[-1]
+    rows = st["rows"].to(P.device)
+    p, d = P.reshape(-1, cols)[rows].double(), dP.reshape(-1, cols)[rows].double()
+    K = (cols + 31) // 32 + 5
+    ref = p * (d - (p * d).sum(-1, keepdim=True))
+    return ratio((result.reshape(-1, cols)[rows].double() - ref).abs(), 2 * (K + 2) * U * p * (d.abs() + (p * d).abs().sum(-1, keepdim=True)))
+
+
+def before_rows(key):
+    def before(ba, rng):
+        t = ba[key]
+        return dict(rows=pick_rows(t.numel() // t.shape[-1], rng))
+    return before
+
+
+def check_cross_entropy_grad(ba, result, st):
+    """w (softmax - (1 - s) onehot - s / cols), one warp per row: 2 u w ((K + 8) p + 4 y) with K = ceil(cols / 32) + 5 (the row sum of
+    exponentials) and y the smoothed target (tests/test_backward_kernels_gpu.py::test_cross_entropy_grad with this kernel's K)."""
+    lg, lab, w = ba["logits_rows"], ba["labels_i32"], ba["row_weight"]
+    cols = lg.shape[-1]
+    rows = st["rows"].to(lg.device)
+    s = f32(ba["smoothing"])
+    x = lg[rows].double()
+    p = torch.softmax(x, -1)
+    y = F.one_hot(lab[rows].long(), cols).double() * (1 - s) + s / cols
+    wr = w[rows].double()[:, None]
+    K = (cols + 31) // 32 + 5
+    return ratio((result[rows].double() - wr * (p - y)).abs(), 2 * U * wr.abs() * ((K + 8) * p + 4 * y) + 1e-38)
+
+
+def check_sumsq(ba, result, st):
+    """sum x^2 in fp64 (squares exact): per-thread chains over a grid-stride loop, 5 shuffle levels, 8 warps, one fp64 atomic per block:
+    2 K 2^-53 sum x^2."""
+    x = ba["x"]
+    n = x.numel()
+    blocks = min((n + 255) // 256, 132 * 16)
+    K = (n + blocks * 256 - 1) // (blocks * 256) + 5 + 8 + blocks
+    want = (x.double() ** 2).sum()
+    return ratio((result.double().reshape(-1)[:1] - want).abs(), torch.full((1,), 2 * K * 2.0 ** -53 * float(want) + 1e-300,
+                                                                           dtype=torch.float64, device=x.device))
+
+
+def before_migt_embed_bwd(ba, rng):
+    return {k: (None if ba[k] is None else ba[k].clone()) for k in ("dwte", "dwpe", "dpose")}
+
+
+def check_migt_embed_bwd(ba, result, st):
+    """dwte[id] += dh (id = ids, or fixed_token where ids is null or < 0), dwpe[l] += dh, dpose[bt] += dh, onto the snapshots.  Every
+    token adds with one fp32 atomic, so an element's chain is the number of tokens that hit it, plus the value held before:
+    2 (hits + 1) u (|snapshot| + sum |dh|)."""
+    dh, ids, BT, Lt = ba["dh"], ba["ids_i32"], ba["BT"], ba["L"]
+    d = dh.shape[-1]
+    tok = BT * Lt
+    hd = dh.reshape(tok, d).double()
+    dev = dh.device
+    idx = torch.full((tok,), int(ba["fixed_token"]), dtype=torch.long, device=dev) if ids is None else ids.long().reshape(-1)
+    if ids is not None:
+        idx = torch.where(idx < 0, torch.full_like(idx, int(ba["fixed_token"])), idx)
+    worst = 0.0
+    for key, index in (("dwte", idx), ("dwpe", torch.arange(tok, device=dev) % Lt), ("dpose", torch.arange(tok, device=dev) // Lt)):
+        if st[key] is None:
+            continue
+        b0 = st[key].double()
+        want = b0.index_add(0, index, hd)
+        hits = torch.zeros(b0.shape[0], dtype=torch.float64, device=dev).index_add_(0, index, torch.ones(tok, dtype=torch.float64, device=dev))
+        absum = b0.abs().index_add(0, index, hd.abs())
+        worst = max(worst, ratio((ba[key].double() - want).abs(), 2 * (hits[:, None] + 1) * U * absum))
+    return worst
+
+
+# ----------------------------------------------------------------------------------------------- elementwise
+def _ranges(n, rng, block=4096):
+    """Sampled flat ranges of a buffer of n elements: the first block, the last block, and 3 random blocks."""
+    nb = (n + block - 1) // block
+    return [slice(b * block, min(n, (b + 1) * block)) for b in pick(nb, rng, extra=3)]
+
+
+def _snap(ba, keys, rng, n):
+    rs = _ranges(n, rng)
+    return dict(ranges=rs, snap={k: [None if ba[k] is None else ba[k].reshape(-1)[r].clone() for r in rs] for k in keys})
+
+
+def before_elementwise(*keys, size="x"):
+    def before(ba, rng):
+        return _snap(ba, keys, rng, ba[size].numel())
+    return before
+
+
+def check_gelu(ba, result, st):
+    """x Phi(x): 4 u |y| + 4 u |x| (erff's error on 1 + erf, which cancels for negative x) (tests/test_backward_kernels_gpu.py)."""
+    worst = 0.0
+    for r, x in zip(st["ranges"], st["snap"]["x"]):
+        xd = x.double()
+        want = xd * 0.5 * (1 + torch.erf(xd / math.sqrt(2)))
+        worst = max(worst, ratio((result.reshape(-1)[r].double() - want).abs(), 4 * U * want.abs() + 4 * U * xd.abs() + 1e-38))
+    return worst
+
+
+def check_gelu_bwd(ba, result, st):
+    """dy (Phi(x) + x phi(x)): 4 u |ref| + 4 u |dy| (1 + |x phi(x)|) (tests/test_backward_kernels_gpu.py)."""
+    worst = 0.0
+    for r, x, dy in zip(st["ranges"], st["snap"]["pre"], st["snap"]["dy"]):
+        xd = x.double()
+        cdf = 0.5 * (1 + torch.erf(xd / math.sqrt(2)))
+        pdf = torch.exp(-0.5 * xd * xd) / math.sqrt(2 * math.pi)
+        want = dy.double() * (cdf + xd * pdf)
+        worst = max(worst, ratio((result.reshape(-1)[r].double() - want).abs(), 4 * U * want.abs() + 4 * U * dy.double().abs() * (1 + (xd * pdf).abs())))
+    return worst
+
+
+def check_lincomb3(ba, result, st):
+    """a x + b y + c z (null operands dropped), from the snapshots (``out`` may alias ``x``): one product and two fmas, 4 u sum|terms|."""
+    worst = 0.0
+    for i, r in enumerate(st["ranges"]):
+        terms = [f32(ba["a"]) * st["snap"]["x"][i].double()]
+        for k, cf in (("y", "b"), ("z", "c")):
+            if st["snap"][k][i] is not None:
+                terms.append(f32(ba[cf]) * st["snap"][k][i].double())
+        worst = max(worst, ratio((result.reshape(-1)[r].double() - sum(terms)).abs(), 4 * U * sum(t.abs() for t in terms) + 1e-38))
+    return worst
+
+
+def _update_bar(scale, m, v, gi, m1, v1, den, sq_bc2):
+    """Bar of scale m1 / den: m1 and v1 are within em = 4 u (|m| + |g|) and ev = 4 u (|v| + g^2) (3 roundings each, and the rounded
+    gradient), den moves by ev / (2 sqrt(v1) sq_bc2); 8 u |update| for the quotient, the scale and the square root."""
+    em, ev = 4 * U * (m.abs() + gi.abs()), 4 * U * (v.abs() + gi * gi)
+    dden = torch.where(v1 > 0, ev / (2 * v1.sqrt().clamp_min(1e-300) * sq_bc2), ev.sqrt() / sq_bc2)
+    return abs(scale) * (em / den + m1.abs() * dden / (den * den)) + 8 * U * (scale * m1 / den).abs()
+
+
+def _pow32(b, t):
+    return float(np.float32(1.0) - np.float32(b) ** np.float32(t))
+
+
+def keras_lr_t(lr, b1, b2, t):
+    """lr sqrt(1 - b2^t) / (1 - b1^t) in fp32, as vf_adamw_keras's host code and TF 2.4's Adam evaluate it (1 - b2^t cancels)."""
+    one = np.float32(1.0)
+    return float(np.float32(lr) * np.sqrt(one - np.float32(b2) ** np.float32(t)) / (one - np.float32(b1) ** np.float32(t)))
+
+
+def check_adam(ba, result, st):
+    """torch.optim.Adam's step in fp64 from the snapshots of p, m, v (sampled ranges), hyperparameters as fp32, the bias corrections
+    1 - beta^t in fp32 (as the host code): m, v within 4 u of their terms, p within 2 u |p| + 16 u |update|."""
+    b1, b2, eps, lr, gs, t = f32(ba["beta1"]), f32(ba["beta2"]), f32(ba["eps"]), f32(ba["lr"]), f32(ba["grad_scale"]), int(ba["step"])
+    bc1, bc2 = _pow32(b1, t), _pow32(b2, t)
+    worst = 0.0
+    for i, r in enumerate(st["ranges"]):
+        p, g, m, v = (st["snap"][k][i].double() for k in ("p", "g", "m", "v"))
+        gi = g * gs
+        m1 = m + (1 - b1) * (gi - m)
+        v1 = b2 * v + (1 - b2) * gi * gi
+        den = v1.sqrt() / math.sqrt(bc2) + eps
+        upd = lr / bc1 * m1 / den
+        ubar = _update_bar(lr / bc1, m, v, gi, m1, v1, den, math.sqrt(bc2))
+        worst = max(worst, ratio((ba["m"].reshape(-1)[r].double() - m1).abs(), 4 * U * (m.abs() + gi.abs()) + 1e-38),
+                    ratio((ba["v"].reshape(-1)[r].double() - v1).abs(), 4 * U * (v.abs() + gi * gi) + 1e-38),
+                    ratio((ba["p"].reshape(-1)[r].double() - (p - upd)).abs(), 2 * U * p.abs() + ubar + 1e-38))
+    return worst
+
+
+def check_adamw_keras(ba, result, st):
+    """The Keras AdamWeightDecay step in fp64 from the snapshots: p -= lr wd p; m += (g - m)(1 - b1); v += (g^2 - v)(1 - b2);
+    p -= lr_t m / (sqrt(v) + eps) with g = grad grad_scale clip_scale and lr_t = keras_lr_t (fp32).  Bars as check_adam, plus 2 u |lr wd p|."""
+    b1, b2, eps, lr, wd = f32(ba["beta1"]), f32(ba["beta2"]), f32(ba["eps"]), f32(ba["lr"]), f32(ba["weight_decay"])
+    lr_t = keras_lr_t(ba["lr"], ba["beta1"], ba["beta2"], int(ba["step"]))
+    worst = 0.0
+    for i, r in enumerate(st["ranges"]):
+        p, g, m, v = (st["snap"][k][i].double() for k in ("p", "g", "m", "v"))
+        gi = g * f32(ba["grad_scale"]) * f32(ba["clip_scale"])
+        p1 = p - f32(np.float32(lr) * np.float32(wd)) * p
+        m1 = m + (gi - m) * (1 - b1)
+        v1 = v + (gi * gi - v) * (1 - b2)
+        den = v1.sqrt() + eps
+        upd = lr_t * m1 / den
+        ubar = _update_bar(lr_t, m, v, gi, m1, v1, den, 1.0)
+        worst = max(worst, ratio((ba["m"].reshape(-1)[r].double() - m1).abs(), 4 * U * (m.abs() + gi.abs()) + 1e-38),
+                    ratio((ba["v"].reshape(-1)[r].double() - v1).abs(), 4 * U * (v.abs() + gi * gi) + 1e-38),
+                    ratio((ba["p"].reshape(-1)[r].double() - (p1 - upd)).abs(), 2 * U * p.abs() + 2 * U * (lr * wd * p).abs() + ubar + 1e-38))
+    return worst
+
+
+# ----------------------------------------------------------------------------------------------- bit-exact conversions, dropout
+def before_none(ba, rng):
+    return {}
+
+
+def check_split_f16x2(ba, result, st):
+    """[hi | lo] with hi = fp16(v), lo = fp16((v - hi) 2^11), bit for bit."""
+    hi, lo = split_pair(ba["x_rows"])
+    return bits_equal(result, torch.cat([hi, lo], 1))
+
+
+def _dropped(x, rate, seed):
+    """fp32 dropout(x) with the kernels' mask: x times the multiplier (0 or fp32(1 / (1 - rate))), one fp32 product."""
+    if rate <= 0:
+        return x.float()
+    return x.float() * HOOKS["dropout_mask"](tuple(x.shape), rate, seed, x.device).float()
+
+
+def check_to_bf16(ba, result, st):
+    """bf16(dropout(x)) rounded to nearest even, and the fp32 dropout(x) when requested, bit for bit."""
+    y = _dropped(ba["x"], float(ba["rate"]), int(ba["seed"]))
+    if ba["out_f32"]:
+        return max(bits_equal(result[0], y), bits_equal(result[1], y.to(torch.bfloat16)))
+    return bits_equal(result, y.to(torch.bfloat16))
+
+
+def check_dropout(ba, result, st):
+    """The mask is a hash of (seed, index) with no independent reference, so only its form is checked: every element is exactly 0 or
+    x fp32(1 / (1 - rate)), and rate 0 is the identity.  A wrong keep fraction or a mask shifted between sites is invisible here (the
+    kernel test checks the fraction; the attention checkers read the same mask)."""
+    x, rate = ba["x"], float(ba["rate"])
+    if rate <= 0:
+        return bits_equal(result, x)
+    sc = np.float32(1.0) / (np.float32(1.0) - np.float32(rate))
+    ok = (result == 0) | (result == x * float(sc))
+    return 0.0 if bool(ok.all()) else math.inf
+
+
+# ----------------------------------------------------------------------------------------------- pixels, layouts, glue (bit-exact)
+def check_u8_to_unit(ba, result, st):
+    """(x fp32(1/255)) 2 - 1, op by op in fp32, bit for bit; ``first_views=n`` reads views 0..n-1 of every scene."""
+    x, fv = ba["x_u8"], ba["first_views"]
+    if fv is not None:
+        x = x[:, :fv].reshape((-1,) + tuple(x.shape[2:]))
+    k = torch.tensor(1.0 / 255.0, dtype=torch.float32, device=x.device)
+    return bits_equal(result, (x.float() * k) * 2.0 - 1.0)
+
+
+def check_unit_to_u8(ba, result, st):
+    """clamp(x, -1, 1) 0.5 + 0.5, times 255.5, clamped to [0, 255], truncated, op by op in fp32, bit for bit."""
+    v = ba["x"].float().clamp(-1.0, 1.0) * 0.5 + 0.5
+    return bits_equal(result, (v * 255.5).clamp(0.0, 255.0).to(torch.uint8))
+
+
+def check_nchw_to_nhwc(ba, result, st):
+    return bits_equal(result, ba["x"].permute(0, 2, 3, 1).contiguous())
+
+
+def check_nhwc_to_nchw(ba, result, st):
+    return bits_equal(result, ba["x"].permute(0, 3, 1, 2).contiguous())
+
+
+def check_gather_rows(ba, result, st):
+    """table[idx], the index clamped into the table, bit for bit."""
+    t = ba["table"]
+    return bits_equal(result, t[ba["idx"].clamp(0, t.shape[0] - 1)])
+
+
+def check_vq_split3(ba, result, st):
+    """hi = bf16(v), lo = bf16(v - hi), rows [hi | hi | lo] (queries) or [hi | lo | hi] (codebook), bit for bit."""
+    v = ba["x"].float()
+    hi = v.to(torch.bfloat16)
+    lo = (v - hi.float()).to(torch.bfloat16)
+    return bits_equal(result, torch.cat([hi, lo, hi] if ba["codebook"] else [hi, hi, lo], 1))
+
+
+def check_vq_prepare_codebook_f16(ba, result, st):
+    """fp16(-2 e) of the codebook rows Et [K, D] (-2 e is exact in fp32), bit for bit."""
+    return bits_equal(result, (-2.0 * ba["et"].float()).half())
+
+
+def check_vq_prepare_codebook(ba, result, st):
+    """Et = emb^T bit for bit; |e|^2 a sequential fp32 sum of D rounded squares: 2 (D + 1) u sum e^2."""
+    emb = ba["emb_dk"]
+    et, esq = result
+    e = emb.double()
+    want = (e * e).sum(0)
+    return max(bits_equal(et, emb.t().contiguous()), ratio((esq.double() - want).abs(), 2 * (emb.shape[0] + 1) * U * want + 1e-300))
+
+
+def check_migt_embed(ba, result, st):
+    """(wte[id] + wpe[l]) + pose[bt] in fp32, in the reference's order, bit for bit (id = ids, or fixed_token where null or < 0)."""
+    ids, wte, wpe, pose, BT, Lt = ba["ids_i32"], ba["wte"], ba["wpe"], ba["pose_rows"], ba["BT"], ba["L"]
+    tok = BT * Lt
+    dev = wte.device
+    fixed = torch.full((tok,), int(ba["fixed_token"]), dtype=torch.long, device=dev)
+    idx = fixed if ids is None else torch.where(ids.long().reshape(-1) < 0, fixed, ids.long().reshape(-1))
+    ar = torch.arange(tok, device=dev)
+    return bits_equal(result, (wte[idx] + wpe[ar % Lt]) + pose[ar // Lt])
+
+
+def check_argmax_rows(ba, result, st):
+    """Index of the row maximum, ties to the first index, exactly."""
+    return bits_equal(result, torch.argmax(ba["x_rows"], 1))
+
+
+def check_image_pair_sums(ba, result, st):
+    """(sum |a - b|, sum (a - b)^2) per image in int64, exactly."""
+    a, b = ba["a_u8"], ba["b_u8"]
+    d = (a.long() - b.long()).reshape(a.shape[0], -1)
+    return bits_equal(result, torch.stack([d.abs().sum(1), (d * d).sum(1)], 1))
+
+
+def check_sumpool2x2(ba, result, st):
+    """(x00 + x01) + (x10 + x11) per 2 x 2 window: 2 u sum|terms| (bit-exact where the sums are exact)."""
+    x = ba["x"]
+    n, h2, w2, c = x.shape
+    xw = x.double().reshape(n, h2 // 2, 2, w2 // 2, 2, c)
+    return ratio((result.double() - xw.sum((2, 4))).abs(), 2 * U * xw.abs().sum((2, 4)))
+
+
+def check_l1_grad(ba, result, st):
+    """dy = scale sign(y - x) bit for bit (the fp32 difference keeps the sign and is 0 only where y == x); the fp64 loss sum within
+    (u + K 2^-53) sum |y - x| (the fp32 subtraction, then an fp64 chain: per-thread + 5 shuffles + 8 warps + the blocks)."""
+    x, y = ba["x"], ba["y"]
+    dy, ls = result
+    d = y.double() - x.double()
+    sc = torch.tensor(f32(ba["scale"]), dtype=torch.float32, device=x.device)
+    want_dy = torch.sign(d).float() * sc
+    n = y.numel()
+    blocks = min((n + 255) // 256, 132 * 16)
+    K = (n + blocks * 256 - 1) // (blocks * 256) + 13 + blocks
+    s = d.abs().sum()
+    return max(bits_equal(dy, want_dy + 0.0), ratio((ls.double().reshape(-1)[:1] - s).abs(), ((U + K * 2.0 ** -53) * s + 1e-300).reshape(1)))
+
+
+def check_row_mean(ba, result, st):
+    """mean of x[b, start:]: one block per row, ceil((n - start) / 256) terms per thread, 5 shuffles, 8 warps, then the division:
+    2 (K + 1) u mean|x|."""
+    x, start = ba["x_rows"], int(ba["start"])
+    xs = x[:, start:].double()
+    K = (xs.shape[1] + 255) // 256 + 13
+    return ratio((result.double() - xs.mean(1)).abs(), 2 * (K + 1) * U * xs.abs().mean(1) + 1e-300)
+
+
+# ----------------------------------------------------------------------------------------------- softmax, losses, poses
+def before_softmax_rows(ba, rng):
+    return dict(rows=pick_rows(int(ba["rows_total"]), rng))
+
+
+def check_softmax_rows(ba, result, st):
+    """Masked row softmax (one warp per row; row r of its batch at position r + row0, view = position // block): mode 0 all columns,
+    mode 1 columns < (view + 1) block, mode 2 columns < view block of the first half and the view's own block of the second half.  Masked
+    columns exactly 0.  Visible: 2 (K + 8) u p (+ 2^-8 p for bf16), K = ceil(visible / 32) + 5 (the sum of exponentials; expf and the
+    reciprocal a few ulps)."""
+    rows = st["rows"].to(ba["scores"].device)
+    cols, mode, blk = int(ba["cols"]), int(ba["mask_mode"]), int(ba["block"])
+    rt = int(ba["rows_total"])
+    sc = view(ba["scores"], 0, (rt, cols), (int(ba["ld_in"]), 1))[rows].double()
+    got = view(result, 0, (rt, cols), (int(ba["ld_out"]), 1))[rows].double()
+    pos = rows % int(ba["rows_per_batch"]) + int(ba["row0"])
+    c = torch.arange(cols, device=sc.device)[None, :]
+    vw = (pos // blk if blk > 0 else torch.zeros_like(pos))[:, None]
+    if mode == 1:
+        vis = c < ((vw + 1) * blk).clamp(max=cols)
+    elif mode == 2:
+        half = cols // 2
+        vis = (c < (vw * blk).clamp(max=half)) | ((c >= half + vw * blk) & (c < half + (vw + 1) * blk))
+    else:
+        vis = c >= 0
+    p = torch.softmax(sc.masked_fill(~vis, -math.inf), 1).masked_fill(~vis, 0.0)
+    K = (vis.sum(1, keepdim=True).double() + 31) // 32 + 5
+    bar = 2 * (K + 8) * U * p
+    if result.dtype == torch.bfloat16:
+        bar = bar + BF16_OUT * p
+    return ratio((got - p).abs(), bar)
+
+
+def check_cross_entropy_rows(ba, result, st):
+    """(1 - s) (lse - x_label) + s (lse - mean x), one warp per row: lse carries K u (the sum of exponentials, K = ceil(cols / 32) + 5)
+    plus a few ulps of |lse|, the row sum K u sum|x|: 4 (K + 4) u (1 + |lse| + |x_label| + mean|x|)."""
+    lg, lab = ba["logits_rows"], ba["labels_i32"]
+    cols = lg.shape[-1]
+    rows = st["rows"].to(lg.device)
+    x = lg[rows].double()
+    s = f32(ba["smoothing"])
+    lse = torch.logsumexp(x, 1)
+    xl = x.gather(1, lab[rows].long()[:, None])[:, 0]
+    want = (1 - s) * (lse - xl) + s * (lse - x.mean(1))
+    K = (cols + 31) // 32 + 5
+    return ratio((result[rows].double() - want).abs(), 4 * (K + 4) * U * (1 + lse.abs() + xl.abs() + x.abs().mean(1)))
+
+
+def _pose_target(ba, rows):
+    return ba["poses_bt7"].reshape(-1, 7)[rows // int(ba["tokens_per_view"])].double()
+
+
+def check_pose_loss_rows(ba, result, st):
+    """pos = mean_3 (y m - r)^2, ori = mean_4 (y - r)^2 per row (y the pose of the row's view): 8 u mean (|y m| + |r|)^2."""
+    raw = ba["raw_rows"]
+    rows = torch.arange(raw.shape[0], device=raw.device)
+    y, r = _pose_target(ba, rows), raw.double()
+    m = f32(ba["mult"])
+    pos, ori = result
+    ym = y[:, :3] * m
+    return max(ratio((pos.double() - ((ym - r[:, :3]) ** 2).mean(1)).abs(), 8 * U * ((ym.abs() + r[:, :3].abs()) ** 2).mean(1) + 1e-38),
+               ratio((ori.double() - ((y[:, 3:] - r[:, 3:]) ** 2).mean(1)).abs(), 8 * U * ((y[:, 3:].abs() + r[:, 3:].abs()) ** 2).mean(1) + 1e-38))
+
+
+def check_pose_loss_grad(ba, result, st):
+    """d/draw of sum w (ps mean_3 (y m - r)^2 + os mean_4 (y - r)^2): 8 u w scale (|y m| + |r|) (tests/test_backward_kernels_gpu.py)."""
+    raw, w = ba["raw_rows"], ba["row_weight"].double()[:, None]
+    rows = torch.arange(raw.shape[0], device=raw.device)
+    y, r = _pose_target(ba, rows), raw.double()
+    mv = torch.tensor([f32(ba["mult"])] * 3 + [1.0] * 4, dtype=torch.float64, device=raw.device)
+    scl = torch.tensor([f32(ba["pos_scale"]) * 2 / 3] * 3 + [f32(ba["ori_scale"]) * 2 / 4] * 4, dtype=torch.float64, device=raw.device)
+    want = -w * scl * (y * mv - r)
+    return ratio((result.double() - want).abs(), 8 * U * w.abs() * scl * ((y * mv).abs() + r.abs()) + 1e-38)
+
+
+def _quat_unit(q):
+    q = q / q.norm(dim=-1, keepdim=True).clamp_min(1e-6)
+    return q * torch.where(q[..., :1] >= 0, 1.0, -1.0)
+
+
+def check_pose_postprocess(ba, result, st):
+    """xyz / mult (one rounding: u |xyz / mult|), the quaternion normalised with w >= 0: its squared norm is a 4-term chain (4 u relative),
+    rsqrtf is within 2 ulp (4 u), the product rounds once (u), and the result may be one rounding of the stored unit value away (u):
+    16 u absolute on each unit-quaternion component."""
+    raw = ba["raw_rows"].double()
+    want = torch.cat([raw[:, :3] / f32(ba["mult"]), _quat_unit(raw[:, 3:])], 1)
+    bar = torch.cat([U * want[:, :3].abs(), torch.full_like(want[:, 3:], 16 * U)], 1)
+    return ratio((result.double() - want).abs(), bar + 1e-38)
+
+
+def _qmul(a, b):
+    aw, ax, ay, az = a.unbind(-1)
+    bw, bx, by, bz = b.unbind(-1)
+    return torch.stack([aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+                        aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw], -1)
+
+
+def _conj(q):
+    return q * torch.tensor([1.0, -1.0, -1.0, -1.0], dtype=q.dtype, device=q.device)
+
+
+def check_cameras_prepare(ba, result, st):
+    """relative: xyz - xyz0 rotated by conj(q0), q = conj(q0) q; then q normalised with w >= 0; the transform is view 0's camera bit for
+    bit.  Bars: 16 u (|xyz| + |xyz0|) on positions (two quaternion products), 16 u on the unit quaternion."""
+    cams = ba["cams"].double()
+    out, tr = result
+    p, q = cams[..., :3], cams[..., 3:]
+    worst = 0.0
+    if ba["relative"]:
+        inv = _conj(q[:, :1])
+        d = torch.cat([torch.zeros_like(p[..., :1]), p - p[:, :1]], -1)
+        p = _qmul(_qmul(inv.expand_as(q), d), _conj(inv).expand_as(q))[..., 1:]
+        q = _qmul(inv.expand_as(q), q)
+        worst = bits_equal(tr, ba["cams"][:, 0].contiguous())
+    want = torch.cat([p, _quat_unit(q)], -1)
+    sc = (cams[..., :3].abs().sum(-1, keepdim=True) + cams[:, :1, :3].abs().sum(-1, keepdim=True)) * (cams[..., 3:].abs().sum(-1, keepdim=True) ** 2)
+    bar = torch.cat([16 * U * sc.expand_as(p), torch.full_like(q, 16 * U)], -1)
+    return max(worst, ratio((out.double() - want).abs(), bar + 1e-38))
+
+
+def check_cameras_from_relative(ba, result, st):
+    """q = qt q, xyz = qt xyz conj(qt) + t (the inverse of the relative transform): 16 u (|xyz| |qt|^2 + |t|), 8 u |qt| |q| on q."""
+    c, t = ba["cams"].double(), ba["transform"].double()[:, None]
+    tq = t[..., 3:].expand(c.shape[:-1] + (4,))
+    q = _qmul(tq, c[..., 3:])
+    pp = torch.cat([torch.zeros_like(c[..., :1]), c[..., :3]], -1)
+    xyz = _qmul(_qmul(tq, pp), _conj(tq))[..., 1:] + t[..., :3]
+    want = torch.cat([xyz, q], -1)
+    n2 = tq.abs().sum(-1, keepdim=True)
+    bar = torch.cat([16 * U * (c[..., :3].abs().sum(-1, keepdim=True) * n2 * n2 + t[..., :3].abs()).expand_as(xyz),
+                     8 * U * (n2 * c[..., 3:].abs().sum(-1, keepdim=True)).expand_as(q)], -1)
+    return ratio((result.double() - want).abs(), bar + 1e-38)
+
+
+# ----------------------------------------------------------------------------------------------- quantizer
+def check_vq_ema_stats(ba, result, st):
+    """counts exact (integers below 2^24); esum [D, K] = sum of the z rows mapped to each code, one fp32 atomic per row: an element's
+    chain is its code's count, 2 (count + 1) u sum |z|."""
+    z, idx, k = ba["z_rows"], ba["idx"], int(ba["k"])
+    counts, esum = result
+    cnt = torch.bincount(idx, minlength=k).float()
+    zs = torch.zeros(k, z.shape[1], dtype=torch.float64, device=z.device).index_add_(0, idx, z.double()).t()
+    za = torch.zeros(k, z.shape[1], dtype=torch.float64, device=z.device).index_add_(0, idx, z.double().abs()).t()
+    return max(bits_equal(counts, cnt), ratio((esum.double() - zs).abs(), 2 * (cnt.double() + 1) * U * za + 1e-38))
+
+
+def check_vq_commit_grad(ba, result, st):
+    """coef (count_k e - esum) from the given counts and row sums, three roundings: 4 u |coef| (count |e| + |esum|)."""
+    emb, counts, esum = ba["emb_dk"].double(), ba["counts"].double(), ba["esum"].double()
+    c = f32(ba["coef"])
+    want = c * (counts * emb - esum)
+    return ratio((result.double() - want).abs(), 4 * U * abs(c) * (counts * emb.abs() + esum.abs()) + 1e-38)
+
+
+def before_vq_ema_update(ba, rng):
+    return dict(cs=ba["cs_hidden"].clone(), dw=ba["dw_hidden"].clone())
+
+
+def check_vq_ema_update(ba, result, st):
+    """QuantizeEMA's update in fp64 from the snapshots of the hidden EMAs: cs' = cs + a (counts - cs), n = sum cs' / corr (fp32 chain
+    Kn = ceil(K / 1024) + 10), cluster = (cs' / corr + eps) / (n + K eps) n, dw' = dw + a (esum - dw), e = (dw' / corr) / cluster written
+    to emb [D, K] and (bit for bit the same values) Et [K, D], |e|^2 a chain of D fmas.  Bars: cs', dw' 4 u of their terms;
+    e 2 (Kn + 12) u |e| + the dw' error / (corr cluster); |e|^2 2 (D + 2) u sum e^2 + 2 |e| that bar."""
+    a, corr, eps = f32(ba["alpha"]), f32(ba["corr"]), f32(ba["eps"])
+    counts, esum = ba["counts"].double(), ba["esum"].double()
+    cs0, dw0 = st["cs"].double(), st["dw"].double()
+    k = cs0.shape[0]
+    cs1 = cs0 + a * (counts - cs0)
+    n = (cs1 / corr).sum()
+    cluster = (cs1 / corr + eps) / (n + k * eps) * n
+    dw1 = dw0 + a * (esum - dw0)
+    e = (dw1 / corr) / cluster[None, :]
+    Kn = (k + 1023) // 1024 + 10
+    ebar = 2 * (Kn + 12) * U * e.abs() + 4 * U * (dw0.abs() + a * esum.abs()) / (corr * cluster.abs()[None, :])
+    emb, et, esq = ba["emb_dk"], ba["et"], ba["esq"]
+    worst = max(ratio((ba["cs_hidden"].double() - cs1).abs(), 4 * U * (cs0.abs() + a * counts.abs()) + 1e-38),
+                ratio((ba["dw_hidden"].double() - dw1).abs(), 4 * U * (dw0.abs() + a * esum.abs()) + 1e-38),
+                ratio((emb.double() - e).abs(), ebar + 1e-38), bits_equal(et, emb.t().contiguous()))
+    sq = (e * e).sum(0)
+    return max(worst, ratio((esq.double() - sq).abs(), 2 * (emb.shape[0] + 2) * U * sq + 2 * (e.abs() * ebar).sum(0) + 1e-38))
+
+
+# ----------------------------------------------------------------------------------------------- evaluation
+def check_resize_u8(ba, result, st):
+    """fp64 restatement of the nearest / bilinear (align_corners=False) resize of x / 255, times 255, truncated; the source indices and
+    interpolation weights are formed in fp32 as the kernel forms them.  Bit-exact, except where
+    the fp64 value lies within 64 u (of 255) of an integer: there the kernel's fp32 rounding may land on either side, so k or k - 1 is
+    accepted for a value within that distance of k."""
+    x, size = ba["x_u8"], int(ba["size"])
+    n, h, w, c = x.shape
+    if h == size and w == size:
+        return 0.0 if result is x else math.inf
+    method = ba["method"] or ("nearest" if size > w else "bilinear")
+    xv = x.double() / 255.0
+    sh, sw = f32(np.float32(h) / np.float32(size)), f32(np.float32(w) / np.float32(size))
+    o = torch.arange(size, device=x.device, dtype=torch.float32)          # source indices and weights in fp32, as the kernel forms them
+    if method == "nearest":
+        sy = torch.floor(o * sh).long().clamp(max=h - 1)
+        sx = torch.floor(o * sw).long().clamp(max=w - 1)
+        v = xv[:, sy][:, :, sx]
+    else:
+        fy, fx = ((o + 0.5) * sh - 0.5).clamp_min(0), ((o + 0.5) * sw - 0.5).clamp_min(0)
+        y0, x0 = fy.long(), fx.long()
+        y1, x1 = (y0 + 1).clamp(max=h - 1), (x0 + 1).clamp(max=w - 1)
+        ly, lx = (fy - y0).double()[None, :, None, None], (fx - x0).double()[None, None, :, None]
+        g = lambda yy, xx: xv[:, yy][:, :, xx]
+        v = (1 - ly) * ((1 - lx) * g(y0, x0) + lx * g(y0, x1)) + ly * ((1 - lx) * g(y1, x0) + lx * g(y1, x1))
+    t = v.clamp(0, 1) * 255.0
+    k = torch.floor(t)
+    near_up = (torch.ceil(t) - t) <= 64 * U * 255
+    near_dn = (t - k) <= 64 * U * 255
+    got = result.double()
+    ok = (got == k) | (near_up & (got == k + 1)) | (near_dn & (got == k - 1))
+    return 0.0 if bool(ok.all()) else math.inf
+
+
 # ----------------------------------------------------------------------------------------------- registry
 CHECKERS = {
     "tc_gemm": (before_tc_gemm, check_tc_gemm),
@@ -691,6 +1486,64 @@ CHECKERS = {
     "vq_lookup": (before_lookup, check_vq_lookup),
     "vq_lookup_fused": (before_lookup, check_lookup),
     "vq_lookup_tc": (before_lookup, check_lookup),
+    "gn_mean_rstd": (before_gn_mean_rstd, check_gn_mean_rstd),
+    "groupnorm": (before_groupnorm, check_groupnorm),
+    "layernorm": (before_layernorm, check_layernorm),
+    "groupnorm_bwd": (before_groupnorm_bwd, check_groupnorm_bwd),
+    "layernorm_bwd": (before_layernorm_bwd, check_layernorm_bwd),
+    "col_sums": (before_col_sums, check_col_sums),
+    "softmax_bwd_rows": (before_rows("P"), check_softmax_bwd_rows),
+    "cross_entropy_grad": (before_rows("logits_rows"), check_cross_entropy_grad),
+    "sumsq": (before_none, check_sumsq),
+    "migt_embed_bwd": (before_migt_embed_bwd, check_migt_embed_bwd),
+    "gelu": (before_elementwise("x"), check_gelu),
+    "gelu_bwd": (before_elementwise("pre", "dy", size="pre"), check_gelu_bwd),
+    "lincomb3": (before_elementwise("x", "y", "z"), check_lincomb3),
+    "adam": (before_elementwise("p", "g", "m", "v", size="p"), check_adam),
+    "adamw_keras": (before_elementwise("p", "g", "m", "v", size="p"), check_adamw_keras),
+    "split_f16x2": (before_none, check_split_f16x2),
+    "to_bf16": (before_none, check_to_bf16),
+    "dropout": (before_none, check_dropout),
+    "u8_to_unit": (before_none, check_u8_to_unit),
+    "unit_to_u8": (before_none, check_unit_to_u8),
+    "nchw_to_nhwc": (before_none, check_nchw_to_nhwc),
+    "nhwc_to_nchw": (before_none, check_nhwc_to_nchw),
+    "gather_rows": (before_none, check_gather_rows),
+    "vq_split3": (before_none, check_vq_split3),
+    "vq_prepare_codebook_f16": (before_none, check_vq_prepare_codebook_f16),
+    "vq_prepare_codebook": (before_none, check_vq_prepare_codebook),
+    "migt_embed": (before_none, check_migt_embed),
+    "argmax_rows": (before_none, check_argmax_rows),
+    "image_pair_sums": (before_none, check_image_pair_sums),
+    "sumpool2x2": (before_none, check_sumpool2x2),
+    "l1_grad": (before_none, check_l1_grad),
+    "row_mean": (before_none, check_row_mean),
+    "softmax_rows": (before_softmax_rows, check_softmax_rows),
+    "cross_entropy_rows": (before_rows("logits_rows"), check_cross_entropy_rows),
+    "pose_loss_rows": (before_none, check_pose_loss_rows),
+    "pose_loss_grad": (before_none, check_pose_loss_grad),
+    "pose_postprocess": (before_none, check_pose_postprocess),
+    "cameras_prepare": (before_none, check_cameras_prepare),
+    "cameras_from_relative": (before_none, check_cameras_from_relative),
+    "vq_ema_stats": (before_none, check_vq_ema_stats),
+    "vq_commit_grad": (before_none, check_vq_commit_grad),
+    "vq_ema_update": (before_vq_ema_update, check_vq_ema_update),
+    "resize_u8": (before_none, check_resize_u8),
+}
+
+# Launching wrappers without a checker of their own, each with the reason.  test_every_launching_wrapper_has_a_checker allows exactly these.
+UNCHECKED = {
+    "pad_transpose_split": "internal operand builder of the split-fp16 weight gradient (_wgrad_tc): a misplaced or non-zero border value "
+                           "changes dW, which check_conv_wgrad_tc / check_dense_wgrad_tc restate from x and dy directly",
+    "pad_transpose_bf16": "internal operand builder of the bf16 weight gradient (_wgrad_tc), held the same way by check_conv_wgrad_bf16 / "
+                          "check_dense_wgrad_bf16 (GroupNorm operand through HOOKS['gn_apply_bf16'])",
+    "dense_weights_bf16": "its table holds raw device pointers, which a device-agnostic checker cannot dereference; the bf16 copies it "
+                          "writes are the operands every bf16 dense tc_gemm check reads, and tests/test_train_migt_bf16_gpu.py pins them "
+                          "bit for bit against torch",
+    "conv_weights_bf16": "raw device pointers in its table, as dense_weights_bf16; its copies are the operands of the bf16 tc_conv checks "
+                         "and are pinned bit for bit in tests/test_train_bf16_gpu.py",
+    "ssim_u8": "the per-window fp32 bar (cancellation in E[x^2] - E[x]^2) is not derived yet; tests/test_eval_gpu.py compares it with the "
+               "reference metric",
 }
 
 

@@ -1,5 +1,6 @@
-"""Every GEMM, convolution, attention, weight-gradient and codebook-lookup launch of the real workloads, checked against fp64 on its own
-operands (tests/launch_checks.py: references and bars).  The kernel tests pin each entry point at a few hand-picked shapes; the workloads
+"""Every GEMM, convolution, attention, weight-gradient and codebook-lookup launch of the real workloads, and every GroupNorm / LayerNorm
+(forward, statistics, backward), column-sum, softmax-backward, cross-entropy-gradient, embedding-gradient, GELU, lincomb3, Adam, Keras AdamW,
+sumsq, split / bf16 conversion and dropout launch, checked against fp64 on its own operands (tests/launch_checks.py: references and bars).  The kernel tests pin each entry point at a few hand-picked shapes; the workloads
 call the same entry points at dozens of others (tile shapes, tails, split-K and tile walks all depend on the shape), which were otherwise
 only held by loose end-to-end bars.
 
@@ -19,6 +20,19 @@ Measured on an H100 80GB HBM3 (700 W power limit), worst ratio to the bar per wo
   bf16 transformer step, small (dropout 0.1) / full size: tc_gemm bf16 0.97 / 0.89, attn_multiend_train 0.54 / 0.61, attn_multiend_bwd
       0.32 / 0.70, conv_wgrad 0.17 / 0.26, dense_wgrad_bf16 0.093 / 0.20.
   fp32 trainers, small: simt_gemm 0.076 / 0.23, dense_wgrad_tc 0.22, conv_wgrad 0.026 / 0.18, tc_gemm split 0.051, tc_conv split 0.0029.
+Normalisation, reduction, optimizer and elementwise wrappers (same card; the 14 workloads and tests/test_norm_stats_gpu.py: about 45 s):
+  generate / codec / KV cache: groupnorm 0.996 (bf16 outputs: the output rounding itself), layernorm 0.995 (bf16), gn_mean_rstd 0.15 (fused
+      sums of a bf16 output) / 0.0096 (statistics pass), split_f16x2 bit-exact.  Largest GroupNorm mean^2 / var: 1.14.
+  codebook steps (fp32 small, bf16 medium / full; full training_step with clipping): gn_mean_rstd 0.14 (statistics pass), groupnorm 0.996,
+      lincomb3 0.47, adam 0.48, softmax_bwd_rows 0.15, groupnorm_bwd 0.056, col_sums 0.053, sumsq 0.0042.  Largest mean^2 / var: 4.59.
+  transformer steps (fp32 small, bf16 small / full; train_step with clipping): layernorm 0.996 (bf16), migt_embed_bwd 0.32, gelu_bwd 0.32,
+      layernorm_bwd 0.25, lincomb3 0.25, gelu 0.24, cross_entropy_grad 0.22, col_sums 0.12, softmax_bwd_rows 0.09, sumsq 0.06,
+      adamw_keras 0.024; to_bf16 and dropout bit-exact / exact in form.
+  softmax_rows 0.995 (bf16 output, generate) / 0.18 (fp32, mask modes 0, 1, 2), sumpool2x2 0.975, pose_loss_rows 0.51, vq_commit_grad
+      0.34, pose_loss_grad 0.29, vq_ema_update 0.25, vq_ema_stats 0.20, pose_postprocess 0.12, cameras_prepare 0.089, vq_prepare_codebook
+      0.078, row_mean 0.052, cameras_from_relative 0.037, cross_entropy_rows 0.011, l1_grad 0.011; bit-exact: u8_to_unit, unit_to_u8, the
+      layout conversions, gather_rows, vq_split3, vq_prepare_codebook_f16, migt_embed, argmax_rows, image_pair_sums, resize_u8 (evaluation).
+  The whole file (17 workloads) runs in about 40 s.  The largest GroupNorm mean^2 / var above comes from synthetic random-weight models.
 """
 import os
 import random
@@ -60,6 +74,8 @@ class Audit:
         monkeypatch.setitem(lc.HOOKS, "dropout_mask", lambda shape, rate, seed, device: dropout(
             torch.ones(shape, dtype=torch.float32, device=device), rate, seed))
         monkeypatch.setitem(lc.HOOKS, "ref_lookup", lambda z, et, esq: orig["vq_lookup"](z, et, esq, want_quant=False, want_diff=False)[0])
+        monkeypatch.setitem(lc.HOOKS, "gn_mean_rstd", orig["gn_mean_rstd"])
+        lc.GN_COND.clear()
         for name, fn in orig.items():
             monkeypatch.setattr(L, name, self._wrap(name, fn))
 
@@ -75,8 +91,8 @@ class Audit:
             if torch.cuda.is_current_stream_capturing():
                 self.skipped += 1
                 return fn(*a, **k)
-            first = a[0] if a else next(iter(k.values()))
-            dtype = str(first.dtype).replace("torch.", "")
+            first = next((v for v in list(a) + list(k.values()) if isinstance(v, torch.Tensor)), None)
+            dtype = "-" if first is None else str(first.dtype).replace("torch.", "")
             with torch.no_grad():
                 result, r = lc.run_check(name, fn, a, k, self.rng)
             self.rec[(name, dtype, self._site())].append(r)
@@ -97,6 +113,8 @@ class Audit:
             per[(name, dtype)] = max(per[(name, dtype)], max(rs))
         print(f"[audit {tag}] worst per wrapper: " + ", ".join(f"{n}/{d} {v:.3g}" for (n, d), v in sorted(per.items()))
               + f"; skipped while capturing: {self.skipped}")
+        if lc.GN_COND:
+            print(f"[audit {tag}] largest GroupNorm mean^2/var: {max(lc.GN_COND):.3g} over {len(lc.GN_COND)} statistics calls")
         return bad
 
     def reached(self):
@@ -133,22 +151,69 @@ def _kv_cache(monkeypatch, L):
     model.query(cache, cams[:, -1].contiguous(), return_logits=True)
 
 
-def _vq_step(cfg_kw, n, precision, seed):
+def _vq_step(cfg_kw, n, precision, seed, full=False):
+    """forward_backward, or with ``full`` the whole training_step (the quantizer's EMA update, the clipped Adam step)."""
     from viewformer_b200 import VQGAN
     from viewformer_b200.train import VQGANTrainer
     cfg = VQGANConfig(**cfg_kw)
     model = VQGAN(cfg, precision="fp32").load_state_dict(synth.make_vqgan_state_dict(cfg, 5))
-    VQGANTrainer(model, precision=precision).forward_backward(vq_images(n, cfg.image_size, seed))
+    tr = VQGANTrainer(model, precision=precision)
+    x = vq_images(n, cfg.image_size, seed)
+    tr.training_step(x) if full else tr.forward_backward(x)
 
 
-def _migt_step(cfg_kw, B, T, precision, seed):
+def _migt_step(cfg_kw, B, T, precision, seed, full=False):
+    """forward_backward, or with ``full`` the whole train_step (per-tensor clipping, Keras AdamW, the accuracy's argmax)."""
     from viewformer_b200 import MIGT
     from viewformer_b200.train_migt import MIGTTrainer
     cfg = MIGTConfig(**cfg_kw)
     model = MIGT(cfg, precision="fp32").load_state_dict(synth.make_migt_state_dict(cfg, 9))
     codes = synth.make_codes(B, T, n_embed=cfg.n_embeddings, seed=seed)
     cams = mo.normalize_cameras(mo.to_relative_cameras(synth.make_cameras(B, T, seed=seed + 1))[0])
-    MIGTTrainer(model, seed=seed, precision=precision).forward_backward(cams, codes)
+    tr = MIGTTrainer(model, seed=seed, precision=precision)
+    tr.train_step((cams, codes)) if full else tr.forward_backward(cams, codes)
+
+
+_EMA_KEYS = {"quantize.counter", "quantize.ema_cluster_size_hidden", "quantize.ema_dw_hidden"}
+
+
+def _vq_commit_step(monkeypatch, L):
+    """A full codebook training step with the commitment quantizer (Quantize): reaches vq_ema_stats + vq_commit_grad."""
+    from viewformer_b200 import VQGAN
+    from viewformer_b200.train import VQGANTrainer
+    cfg = VQGANConfig(**dict(SMALL_VQ, perceptual_weight=0.0, gradient_clip_val=0.5))
+    sd = {k: v for k, v in synth.make_vqgan_state_dict(cfg, 5).items() if k not in _EMA_KEYS}        # Quantize has no EMA buffers
+    model = VQGAN(cfg, precision="fp32", quantizer="commit").load_state_dict(sd)
+    VQGANTrainer(model, precision="fp32").training_step(vq_images(3, cfg.image_size, 5100))
+
+
+def _fp32_inference(monkeypatch, L):
+    """fp32 models: the codec (AttnBlock softmax), the transformer's teacher-forced 3-stream forward with its losses (test_step: mask modes
+    1 and 2, cross_entropy_rows, pose_loss_rows, row_mean, argmax_rows), and the KV-cache query of an fp32 model (mask mode 0)."""
+    from viewformer_b200 import VQGAN, MIGT
+    vcfg = VQGANConfig(**dict(SMALL_VQ, perceptual_weight=0.0))
+    codec = VQGAN(vcfg, precision="fp32").load_state_dict(synth.make_vqgan_state_dict(vcfg, 2))
+    codec.decode_code(codec.encode(vq_images(2, vcfg.image_size, 5200))[2])
+    cfg = MIGTConfig(**dict(MIGT_TRAIN, localization_weight="0.5"))
+    model = MIGT(cfg, precision="fp32").load_state_dict(synth.make_migt_state_dict(cfg, 9))
+    B, T = 2, 4
+    codes = synth.make_codes(B, T, n_embed=cfg.n_embeddings, seed=5300)
+    cams = mo.normalize_cameras(mo.to_relative_cameras(synth.make_cameras(B, T, seed=5301))[0])
+    model.test_step((cams, codes))
+    cache = model.prefill_context(codes[:, :-1], cams[:, :-1].contiguous())
+    model.query(cache, cams[:, -1].contiguous(), return_logits=True)
+
+
+def _evaluation(monkeypatch, L):
+    """metrics.Evaluator at 128 x 128 (the reference's resize rules and SSIM K1 = 1): a 160 x 160 ground truth shrunk bilinearly, a 96 x 96
+    generated view grown bilinearly, then the exact pair sums and SSIM."""
+    from viewformer_b200.metrics import Evaluator
+    g = torch.Generator().manual_seed(5400)
+    base = torch.rand(4, 3, 20, 20, generator=g)
+    gt = (torch.nn.functional.interpolate(base, size=(160, 160), mode="bilinear") * 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
+    gen = (torch.nn.functional.interpolate(base + 0.05 * torch.rand(4, 3, 20, 20, generator=g), size=(96, 96), mode="bilinear").clamp(0, 1)
+           * 255).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
+    Evaluator(image_size=128).update_with_image(gt.cuda(), gen.cuda())
 
 
 MEDIUM_VQ = dict(ch=128, ch_mult=[1, 2], attn_resolutions=[16], image_size=32, n_embed=256, perceptual_weight=0.0)
@@ -156,30 +221,55 @@ SMALL_MIGT_BF16 = dict(n_layer=2, d_model=256, n_head=4, token_image_size=8, n_l
                        label_smoothing=0.05, localization_weight="0.5", image_generation_weight=0.8, pose_multiplier=1.0, dropout=0.1)
 FULL_MIGT_TRAIN = dict(dropout=0.0, label_smoothing=0.1, localization_weight="0.7", total_steps=100, learning_rate=1e-4)
 
+MIXED_NORMS = {("gn_mean_rstd", "bfloat16"), ("gn_mean_rstd", "float32"), ("groupnorm", "bfloat16"), ("groupnorm", "float32"), ("layernorm", "float32"),
+               ("split_f16x2", "float32")}
+VQ_BWD = {("gn_mean_rstd", "float32"), ("groupnorm", "float32"), ("groupnorm_bwd", "float32"), ("col_sums", "float32"), ("lincomb3", "float32"),
+          ("softmax_bwd_rows", "float32")}
+MIGT_BWD = {("layernorm", "float32"), ("layernorm_bwd", "float32"), ("gelu", "float32"), ("gelu_bwd", "float32"), ("cross_entropy_grad", "float32"),
+            ("migt_embed_bwd", "float32"), ("col_sums", "float32"), ("lincomb3", "float32")}
 VQ_BF16_STEP = {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("conv_wgrad_bf16", "float32"),
-                ("conv_wgrad_tc", "float32"), ("simt_conv_dgrad_s2", "float32"), ("vq_lookup", "float32")}
+                ("conv_wgrad_tc", "float32"), ("simt_conv_dgrad_s2", "float32"), ("vq_lookup", "float32")} | VQ_BWD | {("split_f16x2", "float32")}
 
 # workload -> (run, the (wrapper, operand dtype) pairs it is known to reach)
 WORKLOADS = {
     "mixed-generate-norm0": (lambda mp, L: _mixed_generate(mp, L, "0"),
                              {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("attn_block_causal", "bfloat16"),
-                              ("vq_lookup_fused", "float32")}),
+                              ("vq_lookup_fused", "float32")} | MIXED_NORMS),
     "mixed-generate-norm1": (lambda mp, L: _mixed_generate(mp, L, "1"),
                              {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("attn_block_causal", "bfloat16"),
-                              ("vq_lookup_fused", "float32")}),
-    "tf32-codec": (_tf32_codec, {("tc_conv", "float32"), ("tc_gemm", "float32"), ("vq_lookup_fused", "float32")}),
-    "kv-cache-c5": (_kv_cache, {("attn_block_causal", "bfloat16"), ("tc_gemm", "bfloat16")}),
+                              ("vq_lookup_fused", "float32")} | MIXED_NORMS),
+    "tf32-codec": (_tf32_codec, {("tc_conv", "float32"), ("tc_gemm", "float32"), ("vq_lookup_fused", "float32"), ("gn_mean_rstd", "float32"),
+                                 ("groupnorm", "float32")}),
+    "kv-cache-c5": (_kv_cache, {("attn_block_causal", "bfloat16"), ("tc_gemm", "bfloat16"), ("layernorm", "float32")}),
     "vq-step-bf16-medium": (lambda mp, L: _vq_step(MEDIUM_VQ, 4, "bf16", 4100), VQ_BF16_STEP),
     "vq-step-bf16-full": (lambda mp, L: _vq_step(dict(perceptual_weight=0.0), 2, "bf16", 4200), VQ_BF16_STEP),
     "migt-step-bf16-small": (lambda mp, L: _migt_step(SMALL_MIGT_BF16, 2, 5, "bf16", 4300),
-                             {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")}),
+                             {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")} | MIGT_BWD | {("to_bf16", "float32")}),
     "migt-step-bf16-full": (lambda mp, L: _migt_step(FULL_MIGT_TRAIN, 1, 5, "bf16", 4400),
-                            {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")}),
+                            {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")} | MIGT_BWD | {("to_bf16", "float32")}),
     "vq-step-fp32-small": (lambda mp, L: _vq_step(dict(SMALL_VQ, perceptual_weight=0.0), 3, "fp32", 4500),
                            {("simt_gemm", "float32"), ("simt_conv", "float32"), ("simt_conv_dgrad_s2", "float32"), ("conv_wgrad", "float32"),
-                            ("tc_conv", "float16"), ("vq_lookup", "float32")}),
+                            ("tc_conv", "float16"), ("vq_lookup", "float32")} | VQ_BWD),
     "migt-step-fp32-small": (lambda mp, L: _migt_step(MIGT_TRAIN, 2, 4, "fp32", 4600),
-                             {("tc_gemm", "float16"), ("simt_gemm", "float32"), ("dense_wgrad_tc", "float32"), ("conv_wgrad", "float32")}),
+                             {("tc_gemm", "float16"), ("simt_gemm", "float32"), ("dense_wgrad_tc", "float32"), ("conv_wgrad", "float32")} | MIGT_BWD
+                             | {("softmax_bwd_rows", "float32")}),
+    "vq-train-fp32-small": (lambda mp, L: _vq_step(dict(SMALL_VQ, perceptual_weight=0.0, gradient_clip_val=0.5), 3, "fp32", 4700, full=True),
+                           {("adam", "float32"), ("sumsq", "float32"), ("vq_ema_update", "float32"), ("vq_ema_stats", "float32"),
+                            ("softmax_rows", "float32")} | VQ_BWD),
+    "vq-train-bf16-medium": (lambda mp, L: _vq_step(dict(MEDIUM_VQ, gradient_clip_val=0.5), 4, "bf16", 4800, full=True),
+                             {("adam", "float32"), ("sumsq", "float32"), ("vq_ema_update", "float32"), ("vq_ema_stats", "float32"),
+                              ("vq_prepare_codebook", "float32")} | VQ_BF16_STEP),
+    "vq-train-commit-fp32-small": (_vq_commit_step, {("vq_commit_grad", "float32"), ("vq_ema_stats", "float32"), ("adam", "float32"),
+                                                     ("sumsq", "float32"), ("vq_prepare_codebook", "float32")} | VQ_BWD),
+    "fp32-inference": (_fp32_inference, {("softmax_rows", "float32"), ("cross_entropy_rows", "float32"), ("pose_loss_rows", "float32"),
+                                         ("row_mean", "float32"), ("argmax_rows", "float32"), ("migt_embed", "int32"),
+                                         ("pose_postprocess", "float32"), ("layernorm", "float32"), ("gn_mean_rstd", "float32"),
+                                         ("groupnorm", "float32")}),
+    "evaluation": (_evaluation, {("resize_u8", "uint8"), ("image_pair_sums", "uint8")}),
+    "migt-train-fp32-small": (lambda mp, L: _migt_step(dict(MIGT_TRAIN, gradient_clip_val=1.0), 2, 4, "fp32", 4900, full=True),
+                              {("adamw_keras", "float32"), ("sumsq", "float32")}),
+    "migt-train-bf16-small": (lambda mp, L: _migt_step(dict(SMALL_MIGT_BF16, gradient_clip_val=1.0), 2, 5, "bf16", 5000, full=True),
+                              {("adamw_keras", "float32"), ("sumsq", "float32")}),
 }
 
 

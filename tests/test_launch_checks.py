@@ -4,7 +4,9 @@ column window, a zeroed last image, swapped heads, a missing max rescale, a shif
 one).  So a checker that stopped looking at part of its output would fail here, before any GPU run."""
 import math
 import random
+import re
 
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -486,14 +488,586 @@ def test_removing_the_residual_from_the_reference_is_caught(monkeypatch):
 
 
 def test_every_launching_wrapper_has_a_checker():
-    """Every _lib function that launches a GEMM, conv, attention, weight-gradient or lookup kernel, or calls a checked wrapper (the
-    tensor-core weight gradients and lookup do), has a checker: a new wrapper cannot bypass the launch audit."""
+    """Every public _lib function whose code names a vf_* entry point or a checked wrapper has a checker, or is listed in
+    launch_checks.UNCHECKED with its reason: a new wrapper cannot bypass the launch audit."""
     import inspect
-    import re
-    pat = re.compile(r"^(vf_(tc_gemm|simt_gemm|attn_\w+|conv_wgrad|conv3x3_small_\w+|vq_lookup\w*)|tc_gemm|_wgrad_tc)$")
+    pat = re.compile(r"^vf_\w+$")
+    checked = set(lc.CHECKERS)
     public = {name for name, fn in vars(L).items() if inspect.isfunction(fn) and fn.__module__ == L.__name__ and not name.startswith("_")
-              and any(pat.match(n) for n in fn.__code__.co_names)}
-    assert {"tc_gemm", "tc_conv", "vq_lookup_tc", "conv_wgrad_bf16", "attn_multiend_bwd", "conv3x3_small_cin"} <= public
-    missing = sorted(public - set(lc.CHECKERS))
-    print(f"[completeness] {len(public)} launching wrappers: {sorted(public)}")
-    assert not missing, f"_lib wrappers that launch checked kernels without a checker in tests/launch_checks.py: {missing}"
+              and any(pat.match(n) or n in checked or n == "_wgrad_tc" for n in fn.__code__.co_names)}
+    public -= {"load"}                                         # dlopen and the device check: launches nothing
+    assert {"tc_gemm", "groupnorm", "softmax_rows", "vq_ema_update", "resize_u8", "ssim_u8", "pad_transpose_bf16"} <= public
+    missing = sorted(public - checked - set(lc.UNCHECKED))
+    stale = sorted(set(lc.UNCHECKED) & checked)
+    print(f"[completeness] {len(public)} launching wrappers, {len(public & checked)} checked; unchecked with a reason: {sorted(lc.UNCHECKED)}")
+    assert not missing, f"_lib wrappers that launch kernels without a checker in tests/launch_checks.py: {missing}"
+    assert not stale, f"UNCHECKED lists wrappers that have a checker: {stale}"
+    assert all(len(r) > 40 for r in lc.UNCHECKED.values())
+
+
+# ----------------------------------------------------------------------------------------------- normalisation
+def _gn_input(n, hw, c, ratio=3.0, seed=100):
+    g = gen(seed)
+    return (ratio * torch.randn(n, 1, 1, c, generator=g) + torch.randn(n, hw, 1, c, generator=g)).contiguous()
+
+
+def _mr64(x, groups=32, eps=1e-6):
+    m, v, _, _ = lc._gn_stats64(x, groups)
+    return torch.stack([m, 1.0 / torch.sqrt(v + eps)], -1).float()
+
+
+def test_gn_mean_rstd_stats_pass_and_fused_sums():
+    """The stats pass at a 128 x 128 x 128 map (65 536 terms per group): a group shifted by one channel quad is caught; fused sums with
+    one group's sum of squares off by 1e-4 are caught."""
+    x = _gn_input(1, 128 * 128, 128)
+    good = _mr64(x)
+    xs = torch.roll(x, 4, -1)
+    assert_pass_and_catch("gn_mean_rstd", L.gn_mean_rstd, lambda ba: good.clone(), lambda ba: _mr64(xs), x)
+    xf = _gn_input(2, 256, 128, seed=101)
+    xg = xf.double().reshape(2, 256, 32, 4)
+    xf._gn_sums = (torch.stack([xg.sum((1, 3)), (xg * xg).sum((1, 3))], -1), 32)
+    bad = xf.double().reshape(2, 256, 32, 4).clone()
+    bad[1, :, 31] *= 1.0 + 1e-4
+    badm = torch.stack([bad.mean((1, 3)), 1 / torch.sqrt(bad.var((1, 3), unbiased=False) + 1e-6)], -1).float()
+    assert_pass_and_catch("gn_mean_rstd", L.gn_mean_rstd, lambda ba: _mr64(xf), lambda ba: badm, xf)
+
+
+def _gn_apply64(x, mr, gamma, beta, swish):
+    n, h, w, c = x.shape
+    cidx = torch.arange(c) // (c // mr.shape[1])
+    mu, rs = mr.double()[:, cidx, 0][:, None, None], mr.double()[:, cidx, 1][:, None, None]
+    y = (x.double() - mu) * rs * gamma.double() + beta.double()
+    return y * torch.sigmoid(y) if swish else y
+
+
+@pytest.mark.parametrize("layout", ["plain_f32", "plain_bf16", "upsample_bf16", "s2d_split"])
+def test_groupnorm_apply(layout, monkeypatch):
+    """groupnorm with given and with computed statistics; faults: the last pixel chunk not written, groups shifted by one quad, a bf16
+    output rounded toward zero."""
+    n, h, w, c = 2, 8, 6, 128
+    x = _gn_input(n, h * w, c, seed=102).reshape(n, h, w, c)
+    g = gen(103)
+    gamma, beta = torch.rand(c, generator=g) + 0.5, torch.randn(c, generator=g)
+    mr = _mr64(x)
+    monkeypatch.setitem(lc.HOOKS, "gn_mean_rstd", lambda x_, groups, eps: _mr64(x_, groups, eps))
+    ref = _gn_apply64(x, mr, gamma, beta, True)
+    kw = dict(swish=True, stats=None if layout == "plain_bf16" else mr)
+    if layout == "plain_f32":
+        kw["out_dtype"] = torch.float32
+        bad_ref = ref.clone()
+        bad_ref[:, -1, -1] = 0
+        good, bad = ref.float(), bad_ref.float()
+    elif layout == "plain_bf16":
+        kw["out_dtype"] = torch.bfloat16
+        good = ref.float().to(torch.bfloat16)
+        f = ref.float()
+        bad = (f.view(torch.int32) & ~0xFFFF).view(torch.float32).to(torch.bfloat16)       # truncated toward zero
+    elif layout == "upsample_bf16":
+        kw.update(out_dtype=torch.bfloat16, upsample=True)
+        up = ref.repeat_interleave(2, 1).repeat_interleave(2, 2)
+        good = up.float().to(torch.bfloat16)
+        bad = _gn_apply64(x, torch.roll(mr, 1, 1), gamma, beta, True).repeat_interleave(2, 1).repeat_interleave(2, 2).float().to(torch.bfloat16)
+    else:
+        kw.update(out_dtype=torch.float16, s2d=True)
+
+        def s2d(t):
+            v = t.float().reshape(n, h // 2, 2, w // 2, 2, c).permute(0, 1, 3, 2, 4, 5).reshape(n, h // 2, w // 2, 4 * c)
+            hi, lo = lc.split_pair(v)
+            return torch.cat([hi, lo], -1)
+        good = s2d(ref)
+        flat = ref.clone()
+        flat[:, :, :, :4] = ref[:, :, :, 4:8]                                           # one channel quad read from its neighbour
+        bad = s2d(flat)
+    assert_pass_and_catch("groupnorm", L.groupnorm, lambda ba: good, lambda ba: bad, x, gamma, beta, **kw)
+
+
+def test_layernorm_row_tail():
+    rows, d = 301, 768
+    g = gen(104)
+    x = 30.0 * torch.randn(rows, 1, generator=g) + torch.randn(rows, d, generator=g)
+    gamma, beta = torch.rand(d, generator=g) + 0.5, torch.randn(d, generator=g)
+    y = F.layer_norm(x.double(), (d,), gamma.double(), beta.double(), 1e-5).float()
+    bad = y.clone()
+    bad[-1, -4:] = 0                                                                    # the last quad of the last row
+    assert_pass_and_catch("layernorm", L.layernorm, lambda ba: y, lambda ba: bad, x, gamma, beta, torch.float32)
+
+
+def _gn_bwd64(x, dout, mr, gamma, beta, swish, add):
+    n, h, w, c = x.shape
+    cidx = torch.arange(c) // (c // 32)
+    mu, rs = mr.double()[:, cidx, 0].reshape(n, 1, 1, c), mr.double()[:, cidx, 1].reshape(n, 1, 1, c)
+    xd = x.double().requires_grad_(True)
+    ga, be = gamma.double().requires_grad_(True), beta.double().requires_grad_(True)
+    # autograd of the normalisation with the given statistics treated as functions of x (the kernel's formula)
+    xg = xd.reshape(n, h * w, 32, c // 32)
+    m = xg.mean((1, 3))[:, cidx].reshape(n, 1, 1, c)
+    v = ((xg - xg.mean((1, 3), keepdim=True)) ** 2).mean((1, 3))[:, cidx].reshape(n, 1, 1, c)
+    xh = (xd - m) / torch.sqrt(v + 1e-6)
+    xh = xh + (((x.double() - mu) * rs) - xh).detach()                                  # values from the given statistics
+    y = xh * ga + be
+    if swish:
+        y = y * torch.sigmoid(y)
+    y.backward(dout.double())
+    return xd.grad + (0.0 if add is None else add.double()), ga.grad, be.grad
+
+
+@pytest.mark.parametrize("fault", ["add_ignored", "dgamma_overwritten", "bf16_toward_zero"])
+def test_groupnorm_bwd(fault):
+    n, h, w, c = 2, 16, 16, 128
+    g = gen(105)
+    x = _gn_input(n, h * w, c, seed=106).reshape(n, h, w, c)
+    dout = torch.randn(n, h, w, c, generator=g)
+    add = torch.randn(n, h, w, c, generator=g)
+    gamma, beta = torch.rand(c, generator=g) + 0.5, torch.randn(c, generator=g) * 0.3
+    mr = _mr64(x)
+    dx, dg, db = _gn_bwd64(x, dout, mr, gamma, beta, True, add)
+    dg0, db0 = torch.randn(c, generator=g), torch.randn(c, generator=g)
+    dgam, dbet = dg0.clone(), db0.clone()
+
+    def write(bad):
+        def w_(ba):
+            out = (dx - (add.double() if bad == "add_ignored" else 0.0)).float()
+            dgam.copy_((dg + (0 if bad == "dgamma_overwritten" else dg0.double())).float())
+            dbet.copy_((db + db0.double()).float())
+            out._bf16 = ((out.view(torch.int32) & ~0xFFFF).view(torch.float32) if bad == "bf16_toward_zero" else out).to(torch.bfloat16)
+            return out
+        return w_
+
+    def reset_and(f):
+        def w_(ba):
+            dgam.copy_(dg0)
+            dbet.copy_(db0)
+            return f(ba)
+        return w_
+    kw = dict(swish=True, add=add, out_bf16=True)
+    r_good = run("groupnorm_bwd", L.groupnorm_bwd, reset_and(write(None)), x, dout, mr, gamma, beta, dgam, dbet, **kw)
+    dgam.copy_(dg0), dbet.copy_(db0)
+    r_bad = run("groupnorm_bwd", L.groupnorm_bwd, reset_and(write(fault)), x, dout, mr, gamma, beta, dgam, dbet, **kw)
+    print(f"[groupnorm_bwd {fault}] clean {r_good:.3g}  mutated {r_bad:.3g}")
+    assert r_good <= 1.0 and r_bad > 1.0
+
+
+def test_layernorm_bwd_dgamma_accumulates():
+    rows, d = 3 * 2 * 64, 768
+    g = gen(107)
+    x = torch.randn(rows, d, generator=g) * 1.5 + 0.3
+    dy = torch.randn(rows, d, generator=g)
+    gamma = torch.rand(d, generator=g) + 0.5
+    add = torch.randn(rows, d, generator=g)
+    xd, gd = x.double().requires_grad_(True), gamma.double().requires_grad_(True)
+    bd = torch.zeros(d, dtype=torch.float64, requires_grad=True)
+    F.layer_norm(xd, (d,), gd, bd, 1e-5).backward(dy.double())
+    dg0, db0 = torch.randn(d, generator=g), torch.randn(d, generator=g)
+    dgam, dbet = dg0.clone(), db0.clone()
+
+    def write(overwrite):
+        def w_(ba):
+            dgam.copy_((gd.grad + (0 if overwrite else dg0.double())).float())
+            dbet.copy_((bd.grad + db0.double()).float())
+            return (xd.grad + add.double()).float()
+        return w_
+    r_good = run("layernorm_bwd", L.layernorm_bwd, write(False), x, dy, gamma, dgam, dbet, add=add)
+    dgam.copy_(dg0), dbet.copy_(db0)
+    r_bad = run("layernorm_bwd", L.layernorm_bwd, write(True), x, dy, gamma, dgam, dbet, add=add)
+    print(f"[layernorm_bwd] clean {r_good:.3g}  mutated {r_bad:.3g}")
+    assert r_good <= 1.0 and r_bad > 1.0
+
+
+# ----------------------------------------------------------------------------------------------- reductions
+def test_col_sums_dropped_chunk_at_500k_rows():
+    """500 000 rows (489 row chunks of 1023): K = ceil(1023 / 8) + 8 + 489 + 1 = 626, not 500 000.  The bar 2 K u sum|x| sees a dropped
+    chunk whose column sum exceeds it: here rows with a mean of 0.5 per column (as a bias gradient has), so the last chunk (776 rows) adds
+    about 388 against a bar of about 33.  A chunk of zero-mean noise (its sum ~ sqrt(776) ~ 28) would sit at the bar and is not seen."""
+    rows, c = 500_000, 3
+    x = torch.randn(rows, c, generator=gen(108)) + 0.5
+    o0 = torch.randn(c, generator=gen(109))
+    out = o0.clone()
+    assert lc.col_sums_chain(rows) == 626
+    full = (o0.double() + x.double().sum(0)).float()
+    rpb = (rows + 488) // 489
+    last = (rows - 1) // rpb * rpb
+    drop = (o0.double() + x[:last].double().sum(0)).float()
+
+    def write(v):
+        def w(ba):
+            return out.copy_(v)
+        return w
+    r_good = run("col_sums", L.col_sums, write(full), x, out)
+    out.copy_(o0)                                              # the mutated run snapshots the value held before, as the kernel sees it
+    r_bad = run("col_sums", L.col_sums, write(drop), x, out)
+    print(f"[col_sums] clean {r_good:.3g}  mutated {r_bad:.3g}")
+    assert r_good <= 1.0 and r_bad > 1.0
+
+
+def test_softmax_bwd_and_cross_entropy_grad_tails():
+    rows, cols = 37, 1024
+    g = gen(110)
+    logits = torch.randn(rows, cols, generator=g) * 3.0
+    labels = torch.randint(0, cols, (rows,), generator=g, dtype=torch.int32)
+    w = torch.rand(rows, generator=g)
+    s = 0.1
+    ld = logits.double().requires_grad_(True)
+    y = F.one_hot(labels.long(), cols).double() * (1 - lc.f32(s)) + lc.f32(s) / cols
+    (-(y * F.log_softmax(ld, -1)).sum(-1) * w.double()).sum().backward()
+    good = ld.grad.float()
+    y0 = F.one_hot(labels.long(), cols).double()
+    ld0 = logits.double().requires_grad_(True)
+    (-(y0 * F.log_softmax(ld0, -1)).sum(-1) * w.double()).sum().backward()              # label smoothing missing
+    assert_pass_and_catch("cross_entropy_grad", L.cross_entropy_grad, lambda ba: good, lambda ba: ld0.grad.float(), logits, labels, w, s)
+    P = torch.softmax(logits, -1)
+    dP = torch.randn(rows, cols, generator=g)
+    Pd, dPd = P.double(), dP.double()
+    ref = (Pd * (dPd - (Pd * dPd).sum(-1, keepdim=True))).float()
+    bad = (Pd * (dPd - (Pd[:, :-32] * dPd[:, :-32]).sum(-1, keepdim=True))).float()      # the last 32 columns left out of the row sum
+    assert_pass_and_catch("softmax_bwd_rows", L.softmax_bwd_rows, lambda ba: ref, lambda ba: bad, P, dP)
+
+
+def test_sumsq_dropped_block():
+    n = 1_000_000
+    x = torch.randn(n, generator=gen(111))
+    want = torch.tensor([(x.double() ** 2).sum()])
+    bad = torch.tensor([(x[:-256].double() ** 2).sum()])
+    assert_pass_and_catch("sumsq", L.sumsq, lambda ba: want, lambda ba: bad, x)
+
+
+def test_migt_embed_bwd_collisions_and_fixed_token():
+    """1024 codes, 3 streams of 2 x 64 tokens with heavy code collisions; the fault scatters every token to fixed_token."""
+    BT, Lt, d, V = 6, 64, 96, 1025
+    g = gen(112)
+    dh = torch.randn(BT * Lt, d, generator=g)
+    ids = torch.randint(0, 40, (BT * Lt,), generator=g, dtype=torch.int32)
+    fixed = 1024
+    w0, p0, q0 = torch.randn(V, d, generator=g), torch.randn(Lt, d, generator=g), torch.randn(BT, d, generator=g)
+    dwte, dwpe, dpose = w0.clone(), p0.clone(), q0.clone()
+
+    def write(index):
+        def w_(ba):
+            dwte.copy_(w0.double().index_add(0, index, dh.double()).float())
+            dwpe.copy_(p0.double().index_add(0, torch.arange(BT * Lt) % Lt, dh.double()).float())
+            dpose.copy_(q0.double().index_add(0, torch.arange(BT * Lt) // Lt, dh.double()).float())
+        return w_
+    r_good = run("migt_embed_bwd", L.migt_embed_bwd, write(ids.long()), dh, ids, fixed, BT, Lt, dwte, dwpe, dpose)
+    for t, t0 in ((dwte, w0), (dwpe, p0), (dpose, q0)):
+        t.copy_(t0)
+    r_bad = run("migt_embed_bwd", L.migt_embed_bwd, write(torch.full((BT * Lt,), fixed)), dh, ids, fixed, BT, Lt, dwte, dwpe, dpose)
+    print(f"[migt_embed_bwd] clean {r_good:.3g}  mutated {r_bad:.3g}")
+    assert r_good <= 1.0 and r_bad > 1.0
+
+
+# ----------------------------------------------------------------------------------------------- elementwise
+def test_gelu_and_gelu_bwd():
+    x = torch.randn(20000, generator=gen(113)) * 3
+    dy = torch.randn(20000, generator=gen(114))
+    xd = x.double()
+    cdf = 0.5 * (1 + torch.erf(xd / math.sqrt(2)))
+    pdf = torch.exp(-0.5 * xd * xd) / math.sqrt(2 * math.pi)
+    y = (xd * cdf).float()
+    tanh = F.gelu(x, approximate="tanh")
+    assert_pass_and_catch("gelu", L.gelu, lambda ba: y, lambda ba: tanh, x)
+    db = (dy.double() * (cdf + xd * pdf)).float()
+    assert_pass_and_catch("gelu_bwd", L.gelu_bwd, lambda ba: db, lambda ba: (dy.double() * cdf).float(), x, dy)
+
+
+def test_lincomb3_in_place_bucket_rescale():
+    """out aliasing x (the gradient bucket rescaled in place): the snapshot, not the overwritten x, is the reference."""
+    x = torch.randn(50000, generator=gen(115))
+    x0 = x.clone()
+    a = 1.0 / 1024
+
+    def good(ba):
+        return x.copy_((lc.f32(a) * x0.double()).float())
+
+    def tail(ba):
+        good(ba)
+        x[-100:] = x0[-100:]                                   # the tail of the buffer left unscaled
+        return x
+    r_good = run("lincomb3", L.lincomb3, good, a, x, out=x)
+    x.copy_(x0)
+    r_bad = run("lincomb3", L.lincomb3, tail, a, x, out=x)
+    print(f"[lincomb3] clean {r_good:.3g}  mutated {r_bad:.3g}")
+    assert r_good <= 1.0 and r_bad > 1.0
+
+
+def _adam_ref(p, g, m, v, lr, b1, b2, eps, t, gs):
+    b1, b2, eps, lr = lc.f32(b1), lc.f32(b2), lc.f32(eps), lc.f32(lr)
+    gi = g.double() * lc.f32(gs)
+    m1 = m.double() + (1 - b1) * (gi - m.double())
+    v1 = b2 * v.double() + (1 - b2) * gi * gi
+    bc1, bc2 = lc._pow32(b1, t), lc._pow32(b2, t)
+    return p.double() - lr / bc1 * m1 / (v1.sqrt() / math.sqrt(bc2) + eps), m1, v1
+
+
+@pytest.mark.parametrize("opt", ["adam", "adamw_keras"])
+def test_optimizers_step_count_and_decay_order(opt):
+    """A 1 M-element flat buffer, sampled ranges.  adam: the step count off by one (bias corrections of t + 1); adamw_keras: the weight
+    decay applied after the update instead of before."""
+    n = 1 << 20
+    g_ = gen(116)
+    p0, g, m0, v0 = torch.randn(n, generator=g_), torch.randn(n, generator=g_) * 1e-3, torch.randn(n, generator=g_) * 1e-3, torch.rand(n, generator=g_) * 1e-6
+    p, m, v = p0.clone(), m0.clone(), v0.clone()
+    t = 3
+    if opt == "adam":
+        kw = dict(lr=1e-4, beta1=0.5, beta2=0.9, eps=1e-8, step=t, grad_scale=0.5)
+
+        def write(tt):
+            def w_(ba):
+                pr, mr, vr = _adam_ref(p0, g, m0, v0, 1e-4, 0.5, 0.9, 1e-8, tt, 0.5)
+                p.copy_(pr.float()), m.copy_(mr.float()), v.copy_(vr.float())
+            return w_
+        good, bad, fn = write(t), write(t + 1), L.adam
+    else:
+        kw = dict(lr=1e-4, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.05, step=t, grad_scale=1.0, clip_scale=0.5)
+
+        def write(after):
+            def w_(ba):
+                gi = g.double() * 0.5
+                mr = m0.double() + (gi - m0.double()) * (1 - lc.f32(0.9))
+                vr = v0.double() + (gi * gi - v0.double()) * (1 - lc.f32(0.999))
+                upd = lc.keras_lr_t(1e-4, 0.9, 0.999, t) * mr / (vr.sqrt() + lc.f32(1e-8))
+                wd = lc.f32(np.float32(1e-4) * np.float32(0.05))
+                pr = (p0.double() - upd) * (1 - wd) if after else p0.double() * (1 - wd) - upd
+                p.copy_(pr.float()), m.copy_(mr.float()), v.copy_(vr.float())
+            return w_
+        good, bad, fn = write(False), write(True), L.adamw_keras
+    r_good = run(opt, fn, good, p, g, m, v, **kw)
+    p.copy_(p0), m.copy_(m0), v.copy_(v0)
+    r_bad = run(opt, fn, bad, p, g, m, v, **kw)
+    print(f"[{opt}] clean {r_good:.3g}  mutated {r_bad:.3g}")
+    assert r_good <= 1.0 and r_bad > 1.0
+
+
+# ----------------------------------------------------------------------------------------------- bit-exact conversions, dropout
+def test_split_to_bf16_and_dropout():
+    x = torch.randn(300, 64, generator=gen(117)) * 100
+    hi, lo = lc.split_pair(x)
+    good = torch.cat([hi, lo], 1)
+    bad = torch.cat([hi, (((x - hi.float()) * 1024.0).half())], 1)                     # lo without the 2^11
+    assert_pass_and_catch("split_f16x2", L.split_f16x2, lambda ba: good, lambda ba: bad, x)
+    rate, seed = 0.1, 5
+    y = x * lc.HOOKS["dropout_mask"](tuple(x.shape), rate, seed, "cpu").float()
+    shifted = x * lc.HOOKS["dropout_mask"](tuple(x.shape), rate, seed + 1, "cpu").float()
+    assert_pass_and_catch("to_bf16", L.to_bf16, lambda ba: (y, y.to(torch.bfloat16)), lambda ba: (y, shifted.to(torch.bfloat16)), x, rate, seed,
+                          out_f32=True)
+    trunc = (x.view(torch.int32) & ~0xFFFF).view(torch.float32).to(torch.bfloat16)
+    assert_pass_and_catch("to_bf16", L.to_bf16, lambda ba: x.to(torch.bfloat16), lambda ba: trunc, x)
+    sc = float(np.float32(1.0) / np.float32(1.0 - np.float32(rate)))
+    keep = torch.rand(x.shape, generator=gen(118)) >= rate
+    assert_pass_and_catch("dropout", L.dropout, lambda ba: torch.where(keep, x * sc, torch.zeros_like(x)),
+                          lambda ba: torch.where(keep, x / (1 - rate), torch.zeros_like(x)).double().float() * (1 + 2 ** -20), x, rate, seed)
+    assert_pass_and_catch("dropout", L.dropout, lambda ba: x.clone(), lambda ba: x * sc, x, 0.0, seed)
+
+
+# ----------------------------------------------------------------------------------------------- pixels, layouts, glue, losses, quantizer
+def _last_changed(t):
+    """t with its last element changed (a dropped tail)."""
+    b = t.clone()
+    flat = b.reshape(-1)
+    if b.dtype == torch.uint8:
+        flat[-1] = (int(flat[-1]) + 1) % 256
+    elif b.dtype == torch.bfloat16 or b.dtype == torch.float16:
+        flat[-1] = -flat[-1] if float(flat[-1]) != 0 else 1.0
+    elif b.is_floating_point():
+        flat[-1] = flat[-1] * 1.01 + 1.0
+    else:
+        flat[-1] += 1
+    return b
+
+
+def _bitexact_cases():
+    g = gen(120)
+    u8 = torch.randint(0, 256, (2, 3, 5, 6, 3), generator=g, dtype=torch.uint8)
+    x = torch.randn(2, 3, 5, 8, generator=g) * 3
+    table, idx = torch.randn(40, 16, generator=g), torch.randint(-2, 45, (70,), generator=g)
+    et = torch.randn(64, 32, generator=g)
+    ids = torch.randint(-1, 30, (6 * 16,), generator=g, dtype=torch.int32)
+    wte, wpe, pose = torch.randn(33, 32, generator=g), torch.randn(16, 32, generator=g), torch.randn(6, 32, generator=g)
+    logits = torch.randn(37, 1024, generator=g)
+    logits[5, 3] = logits[5, 900] = 50.0                       # a tie: the first index wins
+    a8, b8 = torch.randint(0, 256, (3, 8, 8, 3), generator=g, dtype=torch.uint8), torch.randint(0, 256, (3, 8, 8, 3), generator=g, dtype=torch.uint8)
+    ar = torch.arange(96)
+    emb = torch.where(ids.long() < 0, 0, ids.long())
+    k = torch.tensor(1.0 / 255.0, dtype=torch.float32)
+    return [
+        ("u8_to_unit", L.u8_to_unit, (u8,), dict(first_views=2), (u8[:, :2].reshape(4, 5, 6, 3).float() * k) * 2.0 - 1.0),
+        ("unit_to_u8", L.unit_to_u8, (x.clamp(-1.2, 1.2),), {}, ((x.clamp(-1, 1) * 0.5 + 0.5) * 255.5).clamp(0, 255).to(torch.uint8)),
+        ("nchw_to_nhwc", L.nchw_to_nhwc, (x,), {}, x.permute(0, 2, 3, 1).contiguous()),
+        ("nhwc_to_nchw", L.nhwc_to_nchw, (x,), {}, x.permute(0, 3, 1, 2).contiguous()),
+        ("gather_rows", L.gather_rows, (table, idx), {}, table[idx.clamp(0, 39)]),
+        ("vq_split3", L.vq_split3, (table, True), {},
+         torch.cat([table.bfloat16(), (table - table.bfloat16().float()).bfloat16(), table.bfloat16()], 1)),
+        ("vq_prepare_codebook_f16", L.vq_prepare_codebook_f16, (et,), {}, (-2.0 * et).half()),
+        ("migt_embed", L.migt_embed, (ids, 32, wte, wpe, pose, 6, 16), {}, (wte[torch.where(ids.long() < 0, 32, emb)] + wpe[ar % 16]) + pose[ar // 16]),
+        ("argmax_rows", L.argmax_rows, (logits,), {}, torch.argmax(logits, 1)),
+        ("image_pair_sums", L.image_pair_sums, (a8, b8), {},
+         torch.stack([(a8.long() - b8.long()).abs().reshape(3, -1).sum(1), ((a8.long() - b8.long()) ** 2).reshape(3, -1).sum(1)], 1)),
+    ]
+
+
+@pytest.mark.parametrize("case", range(10))
+def test_bit_exact_wrappers(case):
+    """The bit-exact checkers accept the restatement and reject it with its last element changed (a dropped tail)."""
+    name, fn, a, k, good = _bitexact_cases()[case]
+    assert_pass_and_catch(name, fn, lambda ba: good, lambda ba: _last_changed(good), *a, **k)
+
+
+def test_migt_embed_fixed_token_and_argmax_tie():
+    g = gen(121)
+    ids = torch.randint(0, 30, (96,), generator=g, dtype=torch.int32)
+    wte, wpe, pose = torch.randn(33, 32, generator=g), torch.randn(16, 32, generator=g), torch.randn(6, 32, generator=g)
+    ar = torch.arange(96)
+    good = (wte[ids.long()] + wpe[ar % 16]) + pose[ar // 16]
+    bad = (wte[torch.full((96,), 32)] + wpe[ar % 16]) + pose[ar // 16]
+    assert_pass_and_catch("migt_embed", L.migt_embed, lambda ba: good, lambda ba: bad, ids, 32, wte, wpe, pose, 6, 16)
+    x = torch.zeros(4, 300)
+    x[:, 7] = x[:, 250] = 1.0
+    assert_pass_and_catch("argmax_rows", L.argmax_rows, lambda ba: torch.full((4,), 7), lambda ba: torch.full((4,), 250), x)
+
+
+def test_sumpool_l1_row_mean():
+    g = gen(122)
+    x = torch.randn(2, 6, 10, 5, generator=g)
+    good = x.double().reshape(2, 3, 2, 5, 2, 5).sum((2, 4)).float()
+    bad = x.double().reshape(2, 3, 2, 5, 2, 5)[:, :, :, :, :1].sum((2, 4)).float()
+    assert_pass_and_catch("sumpool2x2", L.sumpool2x2, lambda ba: good, lambda ba: bad, x)
+    a, b = torch.randn(5000, generator=g), torch.randn(5000, generator=g)
+    d = b.double() - a.double()
+    want = (torch.sign(d).float() * lc.f32(0.25) + 0.0, d.abs().sum().reshape(1))
+    assert_pass_and_catch("l1_grad", L.l1_grad, lambda ba: want, lambda ba: (want[0], d[:-1].abs().sum().reshape(1)), a, b, 0.25)
+    r = torch.randn(6, 3 * 64, generator=g) + 2.0
+    assert_pass_and_catch("row_mean", L.row_mean, lambda ba: r[:, 64:].double().mean(1).float(), lambda ba: r.double().mean(1).float(), r, 64)
+
+
+def _masked_softmax(sc, rows_per_batch, mode, block, row0=0, shift=0):
+    rows, cols = sc.shape
+    pos = torch.arange(rows) % rows_per_batch + row0
+    vw = (pos // block)[:, None] + shift
+    c = torch.arange(cols)[None, :]
+    if mode == 1:
+        vis = c < ((vw + 1) * block).clamp(max=cols)
+    else:
+        half = cols // 2
+        vis = (c < (vw * block).clamp(max=half)) | ((c >= half + vw * block) & (c < half + (vw + 1) * block))
+    return torch.softmax(sc.double().masked_fill(~vis, -math.inf), 1).masked_fill(~vis, 0).float()
+
+
+@pytest.mark.parametrize("fault", ["mode2_view_off_by_one", "row0_ignored"])
+def test_softmax_rows_masks(fault):
+    S, blk = 4 * 16, 16
+    sc = torch.randn(2 * S, 2 * S, generator=gen(123)) * 3
+    kw = dict(rows_total=2 * S, rows_per_batch=S, cols=2 * S, ld_in=2 * S, ld_out=2 * S, block=blk)
+    P = torch.empty(2 * S, 2 * S)
+    if fault == "mode2_view_off_by_one":
+        kw["mask_mode"] = 2
+        good, bad = _masked_softmax(sc, S, 2, blk), _masked_softmax(sc, S, 2, blk, shift=1)
+    else:
+        kw.update(mask_mode=1, row0=blk, cols=2 * S)
+        good, bad = _masked_softmax(sc, S, 1, blk, row0=blk), _masked_softmax(sc, S, 1, blk)
+    assert_pass_and_catch("softmax_rows", L.softmax_rows, lambda ba: P.copy_(good), lambda ba: P.copy_(bad), sc, P, **kw)
+
+
+def test_cross_entropy_and_pose_losses():
+    g = gen(124)
+    rows, cols, s = 37, 1024, 0.1
+    lg = torch.randn(rows, cols, generator=g) * 3
+    lab = torch.randint(0, cols, (rows,), generator=g, dtype=torch.int32)
+    x = lg.double()
+    lse = torch.logsumexp(x, 1)
+    xl = x.gather(1, lab.long()[:, None])[:, 0]
+    good = ((1 - lc.f32(s)) * (lse - xl) + lc.f32(s) * (lse - x.mean(1))).float()
+    assert_pass_and_catch("cross_entropy_rows", L.cross_entropy_rows, lambda ba: good, lambda ba: (lse - xl).float(), lg, lab, s)
+    tpv, views = 16, 5
+    raw, poses, w = torch.randn(tpv * views, 7, generator=g), torch.randn(views, 7, generator=g), torch.rand(tpv * views, generator=g)
+    y = poses.double().repeat_interleave(tpv, 0)
+    m = 2.5
+    pos = ((y[:, :3] * lc.f32(m) - raw.double()[:, :3]) ** 2).mean(1).float()
+    ori = ((y[:, 3:] - raw.double()[:, 3:]) ** 2).mean(1).float()
+    y1 = poses.double().roll(1, 0).repeat_interleave(tpv, 0)                                   # the previous view's pose
+    bad = ((y1[:, :3] * lc.f32(m) - raw.double()[:, :3]) ** 2).mean(1).float()
+    assert_pass_and_catch("pose_loss_rows", L.pose_loss_rows, lambda ba: (pos, ori), lambda ba: (bad, ori), raw, poses, tpv, m)
+    mv = torch.tensor([lc.f32(m)] * 3 + [1.0] * 4, dtype=torch.float64)
+    scl = torch.tensor([lc.f32(0.6) * 2 / 3] * 3 + [lc.f32(1.7) * 2 / 4] * 4, dtype=torch.float64)
+    gr = (-w.double()[:, None] * scl * (y * mv - raw.double())).float()
+    bad = (-w.double()[:, None] * scl * (y - raw.double())).float()                           # multiplier left out
+    assert_pass_and_catch("pose_loss_grad", L.pose_loss_grad, lambda ba: gr, lambda ba: bad, raw, poses, w, tpv, m, 0.6, 1.7)
+    pp = torch.cat([raw[:, :3].double() / lc.f32(m), lc._quat_unit(raw[:, 3:].double())], 1).float()
+    assert_pass_and_catch("pose_postprocess", L.pose_postprocess, lambda ba: pp, lambda ba: torch.cat([pp[:, :3], -pp[:, 3:]], 1), raw, m)
+
+
+def test_cameras():
+    g = gen(125)
+    cams = torch.randn(2, 5, 7, generator=g)
+    c = cams.double()
+    inv = lc._conj(c[:, :1, 3:])
+    d = torch.cat([torch.zeros_like(c[..., :1]), c[..., :3] - c[:, :1, :3]], -1)
+    p = lc._qmul(lc._qmul(inv.expand(2, 5, 4), d), lc._conj(inv).expand(2, 5, 4))[..., 1:]
+    q = lc._quat_unit(lc._qmul(inv.expand(2, 5, 4), c[..., 3:]))
+    out = torch.cat([p, q], -1).float()
+    tr = cams[:, 0].contiguous()
+    bad = torch.cat([(c[..., :3] - c[:, :1, :3]), q], -1).float()                              # translation not rotated
+    assert_pass_and_catch("cameras_prepare", L.cameras_prepare, lambda ba: (out, tr), lambda ba: (bad, tr), cams, True)
+    t = torch.randn(2, 7, generator=g).double()
+    tq = t[:, None, 3:].expand(2, 5, 4)
+    pq = torch.cat([torch.zeros_like(c[..., :1]), c[..., :3]], -1)
+    back = torch.cat([lc._qmul(lc._qmul(tq, pq), lc._conj(tq))[..., 1:] + t[:, None, :3], lc._qmul(tq, c[..., 3:])], -1).float()
+    bad = torch.cat([c[..., :3] + t[:, None, :3], lc._qmul(tq, c[..., 3:])], -1).float()
+    assert_pass_and_catch("cameras_from_relative", L.cameras_from_relative, lambda ba: back, lambda ba: bad, cams, t.float())
+
+
+def test_quantizer_ema_and_commit():
+    """EMA statistics with colliding codes; the commitment gradient; the EMA update with a code getting eps twice (codes 0..15 unused,
+    so their cluster size is eps-dominated and the doubled eps is an O(1) change)."""
+    g = gen(126)
+    D, K, m = 16, 64, 600
+    z = torch.randn(m, D, generator=g)
+    idx = torch.randint(16, K, (m,), generator=g)
+    cnt = torch.bincount(idx, minlength=K).float()
+    zs = torch.zeros(K, D, dtype=torch.float64).index_add_(0, idx, z.double()).t().float().contiguous()
+    bad_zs = zs.clone()
+    bad_zs[:, -1] = 0
+    assert_pass_and_catch("vq_ema_stats", L.vq_ema_stats, lambda ba: (cnt, zs), lambda ba: (cnt, bad_zs), z, idx, K)
+    emb = torch.randn(D, K, generator=g)
+    coef = 0.5 / (m * D)
+    good = (lc.f32(coef) * (cnt.double() * emb.double() - zs.double())).float()
+    assert_pass_and_catch("vq_commit_grad", L.vq_commit_grad, lambda ba: good, lambda ba: (lc.f32(coef) * (emb.double() - zs.double())).float(),
+                          emb, cnt, zs, coef, torch.empty(D, K))
+    a, corr, eps = 0.01, 1 - 0.99 ** 3, 1e-5
+    cs0, dw0 = torch.rand(K, generator=g) * 1e-6, torch.randn(D, K, generator=g)
+    cs, dw, e_out, et, esq = cs0.clone(), dw0.clone(), torch.empty(D, K), torch.empty(K, D), torch.empty(K)
+
+    def write(eps2):
+        def w_(ba):
+            fa, fc, fe = lc.f32(a), lc.f32(corr), lc.f32(eps)
+            cs1 = cs0.double() + fa * (cnt.double() - cs0.double())
+            n = (cs1 / fc).sum()
+            cl = (cs1 / fc + fe * eps2) / (n + K * fe) * n
+            dw1 = dw0.double() + fa * (zs.double() - dw0.double())
+            e = (dw1 / fc) / cl[None, :]
+            cs.copy_(cs1.float()), dw.copy_(dw1.float()), e_out.copy_(e.float()), et.copy_(e_out.t()), esq.copy_((e * e).sum(0).float())
+        return w_
+    args = (cnt, zs, a, corr, eps, cs, dw, e_out, et, esq)
+    r_good = run("vq_ema_update", L.vq_ema_update, write(1.0), *args)
+    cs.copy_(cs0), dw.copy_(dw0)
+    r_bad = run("vq_ema_update", L.vq_ema_update, write(2.0), *args)
+    print(f"[vq_ema_update] clean {r_good:.3g}  mutated {r_bad:.3g}")
+    assert r_good <= 1.0 and r_bad > 1.0
+    et2 = emb.t().contiguous()
+    sq = (emb.double() ** 2).sum(0).float()
+    assert_pass_and_catch("vq_prepare_codebook", L.vq_prepare_codebook, lambda ba: (et2, sq), lambda ba: (et2, (emb.double()[:-1] ** 2).sum(0).float()), emb)
+
+
+@pytest.mark.parametrize("method", ["nearest", "bilinear"])
+def test_resize_u8(method):
+    """The fp64 restatement accepts torch's uint8 resize of the same image (nearest: F.interpolate; bilinear: the same formula) and rejects
+    the image shifted by one source row."""
+    g = gen(127)
+    h = 48 if method == "bilinear" else 12
+    x = torch.randint(0, 256, (2, h, h, 3), generator=g, dtype=torch.uint8)
+    size = 32
+    v = x.permute(0, 3, 1, 2).float() / 255.0
+    if method == "nearest":
+        y = F.interpolate(v, size=(size, size), mode="nearest")
+    else:
+        y = F.interpolate(v, size=(size, size), mode="bilinear", align_corners=False)
+    good = (y.clamp(0, 1) * 255.0).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
+    bad = torch.roll(good, 1, 1)
+    assert_pass_and_catch("resize_u8", L.resize_u8, lambda ba: good, lambda ba: bad, x, size, method)
