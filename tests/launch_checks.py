@@ -25,7 +25,8 @@ Bars, elementwise (u = 2^-24):
       hook is set), quant == z + (e - z) bit for bit, the distance sum within 1e-6 relative.
 
 The checkers are device-agnostic torch code.  Device-specific pieces are the HOOKS: the bf16 GroupNorm+swish operand of the fused-norm conv
-and of the bf16 weight-gradient transposer, the dropout mask of the attention kernels, and the reference lookup.
+and of the bf16 weight-gradient transposer, the dropout mask of the attention kernels, the reference lookup, and the number of resident
+CTAs of the persistent attention kernel (which (batch, head) pairs a CTA computes as its second or later work item).
 """
 import math
 import random
@@ -60,6 +61,7 @@ HOOKS = {
     "dropout_mask": _dropout_mask_missing,       # (shape, rate, seed, device) -> fp32 multipliers (0 or 1 / (1 - rate))
     "ref_lookup": None,                          # (z_rows, et, esq) -> int64 indices, or None: fp64 argmin with a near-tie tolerance
     "gn_mean_rstd": None,                        # (x, groups, eps) -> the (mean, rstd) groupnorm computes when not given stats
+    "attn_resident": None,                       # (train) -> CTAs of the persistent attention kernel resident at once, or None
 }
 
 
@@ -492,9 +494,55 @@ def check_dense_wgrad_bf16(ba, result, st):
 
 
 # ----------------------------------------------------------------------------------------------- attention
-def _heads(B, H, rng):
+ATTN_QT, ATTN_KT = 128, 64         # query rows per work item and keys per tile of attn_block_causal_kernel
+
+
+def attn_items(B, H, S, first_query=0):
+    """Work items of one persistent attention launch (attn_launch): B H n_qtiles, n_qtiles = ceil(S / 128) - first_query / 128."""
+    return B * H * (-(-S // ATTN_QT) - first_query // ATTN_QT)
+
+
+def attn_item(item, B, H, S, block, first_query=0, stream=0, skip_view=-1):
+    """(b, h, n_kt) of work item ``item`` (item_coords of vf_attn_fused.cu): heaviest query tile first, then batch * head; n_kt = the key
+    tiles the item walks (stream >= 1: q0/64 + 3, or + 1 when the tile holds one view; an empty view slot of the KV cache is not walked)."""
+    qt0 = first_query // ATTN_QT
+    n_qt = -(-S // ATTN_QT) - qt0
+    BH = B * H
+    q0 = (qt0 + n_qt - 1 - item // BH) * ATTN_QT
+    last_q = min(q0 + ATTN_QT, S) - 1
+    n_kt = -(-min(S, (last_q // block + 1) * block) // ATTN_KT)
+    if stream > 0:
+        n_kt = q0 // ATTN_KT + (3 if q0 + ATTN_KT < S else 1)
+    elif 0 <= skip_view < n_kt:
+        n_kt -= 1
+    bh = item % BH
+    return bh // H, bh % H, n_kt
+
+
+def attn_walk_pairs(B, H, S, block, resident, rng, first_query=0, stream=0, skip_view=-1):
+    """(b, h) pairs a persistent launch computes as some CTA's second or later work item (CTA c walks items c, c + grid, ...): the last
+    item in walk order (always (B - 1, H - 1), which the plain sample holds as well), and one seeded item whose CTA walked an item with
+    a different n_kt before it, so the K / V ring counters and parities it starts from were carried across items of different lengths
+    (any later item when every item has the same n_kt).  Empty when no CTA walks a second item or ``resident`` is None."""
+    items = attn_items(B, H, S, first_query)
+    if resident is None or items <= resident:
+        return []
+    coords = [attn_item(i, B, H, S, block, first_query, stream, skip_view) for i in range(items)]
+    later = [i for i in range(resident, items) if any(coords[j][2] != coords[i][2] for j in range(i % resident, i, resident))]
+    later = later or list(range(resident, items))
+    return [coords[-1][:2], coords[later[rng.randrange(len(later))]][:2]]
+
+
+def _heads(ba, rng, train):
+    """The (batch, head) pairs an attention check covers: first, last and one random pair, and the attn_walk_pairs of the launch (of the
+    training instance's stream-0 launch for the backward, which is not persistent but reads that forward's lse and out_f32)."""
+    B, H = ba["B"], ba["H"]
     pairs = [(b, h) for b in range(B) for h in range(H)]
-    return [pairs[i] for i in pick(len(pairs), rng)]
+    sampled = {pairs[i] for i in pick(len(pairs), rng)}
+    resident = None if HOOKS["attn_resident"] is None else HOOKS["attn_resident"](train)
+    walk = attn_walk_pairs(B, H, ba["S"], ba["block"], resident, rng, first_query=int(ba.get("first_query", 0)),
+                           stream=int(ba.get("stream", 0)), skip_view=int(ba.get("skip_view", -1)))
+    return sorted(sampled | set(walk))
 
 
 def _stream_qkv(qk, vt, s, S, d, b, h):
@@ -565,11 +613,15 @@ def _attn_forward(ba, st, S, stream, block, out_rows, skip_view=-1, rate=0.0, se
     return worst
 
 
-def before_attn(ba, rng):
-    st = dict(heads=_heads(ba["B"], ba["H"], rng))
+def before_attn(ba, rng, train=False):
+    st = dict(heads=_heads(ba, rng, train))
     if ba.get("out") is not None:
         st["out"] = ba["out"].clone()
     return st
+
+
+def before_attn_train(ba, rng):
+    return before_attn(ba, rng, train=True)
 
 
 def check_attn_block_causal(ba, result, st):
@@ -592,7 +644,7 @@ def check_attn_multiend_train(ba, result, st):
 
 
 def before_attn_bwd(ba, rng):
-    st = dict(heads=_heads(ba["B"], ba["H"], rng))
+    st = dict(heads=_heads(ba, rng, True))
     st["dvqk"] = None if ba["dvqk"] is None else ba["dvqk"].clone()
     return st
 
@@ -1481,7 +1533,7 @@ CHECKERS = {
     "dense_wgrad_bf16": (before_wgrad, check_dense_wgrad_bf16),
     "attn_block_causal": (before_attn, check_attn_block_causal),
     "attn_block_multiend": (before_attn, check_attn_block_multiend),
-    "attn_multiend_train": (before_attn, check_attn_multiend_train),
+    "attn_multiend_train": (before_attn_train, check_attn_multiend_train),
     "attn_multiend_bwd": (before_attn_bwd, check_attn_multiend_bwd),
     "vq_lookup": (before_lookup, check_vq_lookup),
     "vq_lookup_fused": (before_lookup, check_lookup),

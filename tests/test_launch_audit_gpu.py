@@ -6,7 +6,9 @@ only held by loose end-to-end bars.
 
 Each wrapped call snapshots what it overwrites, runs the real wrapper, and is checked at once on the same stream, before later launches
 reuse its buffers.  Sampling keeps full size cheap: GEMMs up to 3 batch indices x (first 128, last 128, 64 random rows) x all columns;
-convs 3 images (first, last, one random) x all pixels; attention 3 (batch, head) pairs x all rows and streams; weight gradients in full.
+convs 3 images (first, last, one random) x all pixels; attention 3 (batch, head) pairs x all rows and streams, plus, when the persistent
+kernel's CTAs walk more than one item, the pair of the last item and of a CTA's later item after a change of n_kt (launch_checks.
+attn_walk_pairs, from this GPU's SM count); weight gradients in full.
 Calls made while a CUDA graph is being captured are counted and skipped (all workloads here are eager).
 
 Measured on an H100 80GB HBM3 (700 W power limit), worst ratio to the bar per workload (the file runs in about 30 s of pytest time):
@@ -19,6 +21,11 @@ Measured on an H100 80GB HBM3 (700 W power limit), worst ratio to the bar per wo
       conv_wgrad_tc 0.0013 / 0.020, tc_gemm bf16 0.018 / 0.019, tc_conv bf16 0.0031 / 0.0035.
   bf16 transformer step, small (dropout 0.1) / full size: tc_gemm bf16 0.97 / 0.89, attn_multiend_train 0.54 / 0.61, attn_multiend_bwd
       0.32 / 0.70, conv_wgrad 0.17 / 0.26, dense_wgrad_bf16 0.093 / 0.20.
+  At the benchmarked sizes, where attention CTAs walk several items (together about 14 s):
+  mixed generate, the bench's 32 scenes (attention: 1920 items on 264 CTAs): tc_gemm bf16 0.989, groupnorm 0.996 (bf16), tc_conv bf16
+      0.84, attn_block_causal 0.60, tc_gemm split 0.054, tc_conv split 0.011.
+  bf16 transformer step at scripts/bench_migt_train.py's size (B = 5, T = 20, dropout 0.1; 600 items per stream on 132 CTAs): tc_gemm
+      bf16 0.90, attn_multiend_train 0.73, attn_multiend_bwd 0.72, migt_embed_bwd 0.33, gelu_bwd 0.32, dense_wgrad_bf16 0.026.
   fp32 trainers, small: simt_gemm 0.076 / 0.23, dense_wgrad_tc 0.22, conv_wgrad 0.026 / 0.18, tc_gemm split 0.051, tc_conv split 0.0029.
 Normalisation, reduction, optimizer and elementwise wrappers (same card; the 14 workloads and tests/test_norm_stats_gpu.py: about 45 s):
   generate / codec / KV cache: groupnorm 0.996 (bf16 outputs: the output rounding itself), layernorm 0.995 (bf16), gn_mean_rstd 0.15 (fused
@@ -32,7 +39,7 @@ Normalisation, reduction, optimizer and elementwise wrappers (same card; the 14 
       0.34, pose_loss_grad 0.29, vq_ema_update 0.25, vq_ema_stats 0.20, pose_postprocess 0.12, cameras_prepare 0.089, vq_prepare_codebook
       0.078, row_mean 0.052, cameras_from_relative 0.037, cross_entropy_rows 0.011, l1_grad 0.011; bit-exact: u8_to_unit, unit_to_u8, the
       layout conversions, gather_rows, vq_split3, vq_prepare_codebook_f16, migt_embed, argmax_rows, image_pair_sums, resize_u8 (evaluation).
-  The whole file (17 workloads) runs in about 40 s.  The largest GroupNorm mean^2 / var above comes from synthetic random-weight models.
+  The whole file (19 workloads) runs in about 55 s.  The largest GroupNorm mean^2 / var above comes from synthetic random-weight models.
 """
 import os
 import random
@@ -75,6 +82,8 @@ class Audit:
             torch.ones(shape, dtype=torch.float32, device=device), rate, seed))
         monkeypatch.setitem(lc.HOOKS, "ref_lookup", lambda z, et, esq: orig["vq_lookup"](z, et, esq, want_quant=False, want_diff=False)[0])
         monkeypatch.setitem(lc.HOOKS, "gn_mean_rstd", orig["gn_mean_rstd"])
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        monkeypatch.setitem(lc.HOOKS, "attn_resident", lambda train: (1 if train else 2) * sms)
         lc.GN_COND.clear()
         for name, fn in orig.items():
             monkeypatch.setattr(L, name, self._wrap(name, fn))
@@ -121,14 +130,14 @@ class Audit:
         return {(name, dtype) for name, dtype, _ in self.rec}
 
 
-def _mixed_generate(monkeypatch, L, norm_on_load):
+def _mixed_generate(monkeypatch, L, norm_on_load, scenes=3):
     import bench
     from viewformer_b200 import VQGAN, MIGT, generate_batch_predictions
     monkeypatch.setenv("VF_NORM_ON_LOAD", norm_on_load)
     vcfg, tcfg = VQGANConfig(), MIGTConfig(localization_weight="0")
     cb = VQGAN(vcfg, precision="mixed").load_state_dict(synth.make_vqgan_state_dict(vcfg, 0))
     tr = MIGT(tcfg, precision="bf16").load_state_dict(synth.make_migt_state_dict(tcfg, 0))
-    images, cams = bench.synth_inputs(3, 1234)
+    images, cams = bench.synth_inputs(scenes, 1234)
     generate_batch_predictions(tr, cb, images, cams)
 
 
@@ -238,6 +247,9 @@ WORKLOADS = {
     "mixed-generate-norm1": (lambda mp, L: _mixed_generate(mp, L, "1"),
                              {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("attn_block_causal", "bfloat16"),
                               ("vq_lookup_fused", "float32")} | MIXED_NORMS),
+    "mixed-generate-bench": (lambda mp, L: _mixed_generate(mp, L, "0", scenes=32),
+                             {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("attn_block_causal", "bfloat16"),
+                              ("vq_lookup_fused", "float32")} | MIXED_NORMS),
     "tf32-codec": (_tf32_codec, {("tc_conv", "float32"), ("tc_gemm", "float32"), ("vq_lookup_fused", "float32"), ("gn_mean_rstd", "float32"),
                                  ("groupnorm", "float32")}),
     "kv-cache-c5": (_kv_cache, {("attn_block_causal", "bfloat16"), ("tc_gemm", "bfloat16"), ("layernorm", "float32")}),
@@ -247,6 +259,9 @@ WORKLOADS = {
                              {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")} | MIGT_BWD | {("to_bf16", "float32")}),
     "migt-step-bf16-full": (lambda mp, L: _migt_step(FULL_MIGT_TRAIN, 1, 5, "bf16", 4400),
                             {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")} | MIGT_BWD | {("to_bf16", "float32")}),
+    "migt-step-bf16-bench": (lambda mp, L: _migt_step(dict(FULL_MIGT_TRAIN, dropout=0.1), 5, 20, "bf16", 5500),
+                             {("attn_multiend_train", "bfloat16"), ("attn_multiend_bwd", "bfloat16"), ("tc_gemm", "bfloat16")} | MIGT_BWD
+                             | {("to_bf16", "float32")}),
     "vq-step-fp32-small": (lambda mp, L: _vq_step(dict(SMALL_VQ, perceptual_weight=0.0), 3, "fp32", 4500),
                            {("simt_gemm", "float32"), ("simt_conv", "float32"), ("simt_conv_dgrad_s2", "float32"), ("conv_wgrad", "float32"),
                             ("tc_conv", "float16"), ("vq_lookup", "float32")} | VQ_BWD),

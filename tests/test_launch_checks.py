@@ -419,6 +419,66 @@ def test_attn_multiend_and_train_dropout():
                           rate=rate, seed=seed, lse=lse, out_f32=o32)
 
 
+def _walk_by_cta(B, H, S, block, resident, first_query=0, stream=0, skip_view=-1):
+    """The persistent kernel's walk, restated from the visible keys: all items in walk order as ((b, h), key tiles walked), and per CTA
+    its items in order.  Query tiles run from the last (most keys) to the first computed one; within a tile b-major, then h; CTA c takes
+    items c, c + grid, ..."""
+    per_qt = []
+    for qt in reversed(range(first_query // 128, -(-S // 128))):
+        q0, q1 = qt * 128, min(qt * 128 + 128, S)
+        if stream == 0:
+            keys = [j for j in range(0, S, 64) if j < (q1 - 1) // block * block + block and j // 64 != skip_view]
+            tiles = len(keys)
+        else:                              # stream-0 keys of the views before the tile, the tile's first view twice, its own views
+            views = (q1 - q0) // 64
+            tiles = q0 // 64 + (3 if views == 2 else 1)
+        per_qt += [((b, h), tiles) for b in range(B) for h in range(H)]
+    grid = min(len(per_qt), resident)
+    return per_qt, [per_qt[c::grid] for c in range(grid)]
+
+
+@pytest.mark.parametrize("sms,train,B,H,T,kw", [
+    (132, False, 32, 12, 10, {}),                                                  # the benchmark's attention: 1920 items on 264 CTAs
+    (132, False, 32, 12, 9, dict(stream=1)),                                       # odd T: the last tile holds one view
+    (132, True, 5, 12, 20, dict(stream=2)),                                        # the transformer step: 600 items on 132 CTAs
+    (132, False, 32, 12, 11, dict(first_query=640, skip_view=9)),                  # KV-cache decode, empty slot: every n_kt alike
+    (4, False, 2, 3, 7, {}),
+    (132, False, 3, 12, 10, {}),                                                   # 180 items, one per CTA: nothing added
+])
+def test_attn_head_sampler_covers_later_items(monkeypatch, sms, train, B, H, T, kw):
+    """With the resident CTA count known, the attention checks also cover the last item in walk order and an item that a CTA walks after
+    one with a different number of key tiles."""
+    S = T * 64
+    monkeypatch.setitem(lc.HOOKS, "attn_resident", lambda tr: (1 if tr else 2) * sms)
+    fn = L.attn_multiend_train if train else (L.attn_block_multiend if "stream" in kw else L.attn_block_causal)
+    qk = torch.empty(0)
+    if fn is L.attn_block_causal:
+        ba = lc.bind(fn, qk, qk, B, S, H, H * 64, 64, **kw)
+    else:
+        ba = lc.bind(fn, qk, qk, B, S, 3, kw["stream"], H, H * 64, 64)
+    before = lc.before_attn_train if train else lc.before_attn
+    order, walk = _walk_by_cta(B, H, S, 64, (1 if train else 2) * sms, **kw)
+    mixed = {pair for items in walk for k, (pair, n) in enumerate(items) if k > 0 and any(m != n for _, m in items[:k])}
+    later = mixed or {pair for items in walk for pair, _ in items[1:]}
+    walks = max(len(items) for items in walk) > 1
+    for seed in range(5):
+        monkeypatch.setitem(lc.HOOKS, "attn_resident", None)
+        plain = set(before(ba, random.Random(seed))["heads"])
+        monkeypatch.setitem(lc.HOOKS, "attn_resident", lambda tr: (1 if tr else 2) * sms)
+        heads = set(before(ba, random.Random(seed))["heads"])
+        rng = random.Random(seed)
+        lc.pick(B * H, rng)                                        # the sampler draws its three pairs first
+        added = lc.attn_walk_pairs(B, H, S, 64, (1 if train else 2) * sms, rng, **kw)
+        assert len(plain) == min(3, B * H) and plain | set(added) == heads
+        if not walks:
+            assert added == [] and heads == plain
+            continue
+        assert added[0] == order[-1][0], f"the last item in walk order is {order[-1][0]}, not {added[0]}"
+        assert added[1] in later, f"{added[1]} is not a later item of a CTA whose walk changes n_kt"
+        print(f"[sampler {sms} SMs, B {B} H {H} T {T} {kw}] plain {sorted(plain)} + walk {added}; "
+              f"{len(mixed)} pairs own a later item after a change of n_kt")
+
+
 def test_attn_multiend_bwd_stream_swap():
     B, S, H, ns, rate, seed = 1, 128, 1, 3, 0.1, 90
     d = H * 64
