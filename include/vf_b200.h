@@ -163,6 +163,10 @@ typedef struct {
     int64_t exact_lo_a, exact_lo_b;
 } vf_tc_gemm_t;
 int vf_tc_gemm(const vf_tc_gemm_t* p, vf_stream_t s);
+/* The tiling vf_tc_gemm chooses for p, without launching or reading any operand: plan[8] = {block_n, TW, TH, TN, halo, exact,
+   tiles, CTAs} (TW / TH / TN / halo are 0 for a GEMM).  The persistent grid is CTAs = min(tiles, SMs); CTA c walks tiles c, c + CTAs, ..
+   with the n tile fastest, then the m tile (conv: x tile, y tile, image tile), then the batch. */
+int vf_tc_gemm_plan(const vf_tc_gemm_t* p, int* plan);
 
 /* ------------------------------------------------------------------------------------------
  * Fused block-causal attention on wgmma (single-stream forward):  out = softmax(mask(Q K^T)) V, no 1/sqrt(dh) scale

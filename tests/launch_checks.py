@@ -26,7 +26,8 @@ Bars, elementwise (u = 2^-24):
 
 The checkers are device-agnostic torch code.  Device-specific pieces are the HOOKS: the bf16 GroupNorm+swish operand of the fused-norm conv
 and of the bf16 weight-gradient transposer, the dropout mask of the attention kernels, the reference lookup, and the number of resident
-CTAs of the persistent attention kernel (which (batch, head) pairs a CTA computes as its second or later work item).
+CTAs of the persistent attention and tensor-core GEMM / conv kernels (which (batch, head) pairs, batch entries and images a CTA computes
+as its second or later work item).
 """
 import math
 import random
@@ -62,6 +63,7 @@ HOOKS = {
     "ref_lookup": None,                          # (z_rows, et, esq) -> int64 indices, or None: fp64 argmin with a near-tie tolerance
     "gn_mean_rstd": None,                        # (x, groups, eps) -> the (mean, rstd) groupnorm computes when not given stats
     "attn_resident": None,                       # (train) -> CTAs of the persistent attention kernel resident at once, or None
+    "tc_ctas": None,                             # () -> CTAs of the persistent tensor-core GEMM / conv kernel (the SM count), or None
 }
 
 
@@ -186,10 +188,69 @@ def _snapshot_if_aliased(res, out):
     return res
 
 
+# ----------------------------------------------------------------------------------------------- tensor-core walk
+TC_BM = 128            # output rows (GEMM) or pixels (conv) per tile of tc_gemm_kernel
+
+
+def tc_block_n(ncols):
+    """Output columns per tile: 128 when Ncols > 64, else 64."""
+    return 128 if ncols > 64 else 64
+
+
+def tc_conv_tiling(h, w, ctot, cin, oh, ow, taps, coffs, exact, tf32):
+    """(TW, TH, TN, halo) the vf_tc_gemm launcher picks for a conv: a tile of TN images x TH rows x TW columns = 128 pixels; halo for
+    the plain 3x3 stride-1 pad-1 conv (exact: <= 2 channel blocks of [hi | lo] channels, one image per tile; bf16 / TF32: maps >= 16 rows,
+    which then take 8 x 16-pixel tiles)."""
+    tw = 16 if ow >= 16 else 8 if ow >= 8 else 4 if ow >= 4 else 2 if ow >= 2 else 1
+    th = 128 // tw
+    if th > oh:
+        th = 1
+        while th * 2 <= oh:
+            th *= 2
+    tn = 128 // (tw * th)
+    bk = 32 if tf32 else 64
+    halo = len(taps) == 9 and (oh, ow) == (h, w) and (
+        (ctot == 2 * cin and cin <= 2 * bk and tn == 1 and tw >= 8) if exact else (ctot == cin and oh >= 16 and ow >= 8))
+    halo = halo and all(tuple(taps[t]) == (t // 3 - 1, t % 3 - 1) and (coffs is None or coffs[t] == 0) for t in range(9))
+    if halo and not exact:
+        tw, th, tn = 8, 16, 1
+    return tw, th, tn, halo
+
+
+def tc_conv_geometry(ba):
+    """(tiles_x, tiles_y, image tiles, n tiles, TN) of a tc_conv call; its tile t is (image tile, y tile, x tile, n tile), n fastest."""
+    n, h, w, ctot = ba["x"].shape
+    split = ba["x"].dtype == torch.float16
+    cin = ctot // (2 if split else 1) if ba["cin"] is None else ba["cin"]
+    oh, ow = (h, w) if ba["out_hw"] is None else ba["out_hw"]
+    tw, th, tn, _ = tc_conv_tiling(h, w, ctot, cin, oh, ow, ba["taps"], ba["coffs"], split, ba["x"].dtype == torch.float32)
+    return -(-ow // tw), -(-oh // th), -(-n // tn), -(-ba["w_nk"].shape[0] // tc_block_n(ba["w_nk"].shape[0])), tn
+
+
+def tc_walk_tiles(total, ctas, rng):
+    """Tiles of a persistent tc_gemm_kernel launch (CTA c walks tiles c, c + grid, ..., grid = min(total, ctas)) that a CTA computes as
+    its second or later tile: the last tile in walk order and one seeded tile from the second round on.  Empty when no CTA walks a second
+    tile or ``ctas`` is None."""
+    if ctas is None or total <= ctas:
+        return []
+    return [total - 1, rng.randrange(ctas, total)]
+
+
 # ----------------------------------------------------------------------------------------------- tensor-core GEMM
 def before_tc_gemm(ba, rng):
+    """Up to 3 batch entries and pick_rows, plus the batch entry and 128-row block of each tc_walk_tiles tile."""
     b1, b2 = ba["batch"]
-    return dict(batches=pick(b1 * b2, rng), rows=pick_rows(ba["M"], rng), res=_snapshot_if_aliased(ba["residual"], ba["out"]),
+    batches, rows = set(pick(b1 * b2, rng)), pick_rows(ba["M"], rng)
+    tiles_m, tiles_n = -(-ba["M"] // TC_BM), -(-ba["N"] // tc_block_n(ba["N"]))
+    walk = tc_walk_tiles(tiles_m * tiles_n * b1 * b2, HOOKS["tc_ctas"] and HOOKS["tc_ctas"](), rng)
+    extra = []
+    for t in walk:
+        batches.add(t // (tiles_n * tiles_m))
+        m0 = (t // tiles_n) % tiles_m * TC_BM
+        extra += range(m0, min(m0 + TC_BM, ba["M"]))
+    if extra:
+        rows = torch.tensor(sorted(set(rows.tolist()) | set(extra)))
+    return dict(batches=sorted(batches), rows=rows, res=_snapshot_if_aliased(ba["residual"], ba["out"]),
                 gn_prev=getattr(ba["out"], "_gn_sums", None))
 
 
@@ -255,8 +316,13 @@ def check_tc_gemm(ba, result, st):
 
 # ----------------------------------------------------------------------------------------------- tensor-core conv
 def before_tc_conv(ba, rng):
+    """First, last and one random image, plus the first image of each tc_walk_tiles tile."""
     n = ba["x"].shape[0]
-    return dict(images=pick(n, rng), res=_snapshot_if_aliased(ba["residual"], ba["out"]), gn_prev=getattr(ba["out"], "_gn_sums", None))
+    images = set(pick(n, rng))
+    tiles_x, tiles_y, tiles_img, tiles_n, tn = tc_conv_geometry(ba)
+    for t in tc_walk_tiles(tiles_x * tiles_y * tiles_img * tiles_n, HOOKS["tc_ctas"] and HOOKS["tc_ctas"](), rng):
+        images.add(t // tiles_n // (tiles_x * tiles_y) * tn)
+    return dict(images=sorted(images), res=_snapshot_if_aliased(ba["residual"], ba["out"]), gn_prev=getattr(ba["out"], "_gn_sums", None))
 
 
 def _tap_conv(xv, w, taps, coffs, cin, oh, ow):

@@ -194,8 +194,9 @@ def test_tc_gemm_epilogues_bf16(L):
 
 
 def test_tc_gemm_wide_tiles(L):
-    """un-batched bf16 GEMMs with >= 256 rows and N % 128 == 0 take the wide-tile kernel (128 features x 256 rows per tile,
-    register epilogue): row tails, K tails, every epilogue combination, and a contiguous batch that flattens."""
+    """un-batched bf16 GEMMs with >= 256 rows and N > 64, so several 128 x 128 tiles (block_n 128) per launch: row tails, K tails, every
+    epilogue combination (bias, GELU with fp32 and bf16 outputs, residual with alpha), and a batch with shared weights whose entries are
+    contiguous."""
     _tc_case(L, torch.bfloat16, 256, 128, 64, seed=40)
     _tc_case(L, torch.bfloat16, 1000, 768, 776, bias_mode=1, residual=True, seed=41)               # M tail (1000 = 3*256+232), K tail
     _tc_case(L, torch.bfloat16, 300, 256, 512, bias_mode=1, act=1, out_dtype=torch.bfloat16, seed=42)   # GELU -> bf16 (fast erf)
@@ -280,8 +281,9 @@ def test_tc_conv3x3(L, dtype, cin, cout, n, hw):
                                                           (3, 32, 8, 256, 128, False, True), (1, 128, 128, 128, 128, True, False),
                                                           (2, 33, 9, 64, 128, False, False)])
 def test_tc_conv3x3_wide_tiles(L, n, H, W, cin, cout, res, out_bf16):
-    """maps >= 32 rows tall take the wide-tile kernel (weights on the M side, 8x32-pixel patches on the N side, direct epilogue):
-    ragged heights / widths, channel tiles, residual, bf16 output and the fused GroupNorm statistics."""
+    """bf16 3x3 convs on maps >= 16 rows tall take the halo path (8 x 16-pixel tiles, one halo tile per 64-channel block, the 9 taps
+    as shifted descriptors into it): ragged heights / widths, one to four channel blocks, two n tiles, residual, bf16 output and the
+    fused GroupNorm statistics."""
     x = torch.randn(n, cin, H, W, generator=g(H + W)).bfloat16()
     w = (torch.randn(cout, cin, 3, 3, generator=g(43)) / (9 * cin) ** 0.5).bfloat16()
     b = torch.randn(cout, generator=g(44))

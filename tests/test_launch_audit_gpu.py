@@ -84,6 +84,7 @@ class Audit:
         monkeypatch.setitem(lc.HOOKS, "gn_mean_rstd", orig["gn_mean_rstd"])
         sms = torch.cuda.get_device_properties(0).multi_processor_count
         monkeypatch.setitem(lc.HOOKS, "attn_resident", lambda train: (1 if train else 2) * sms)
+        monkeypatch.setitem(lc.HOOKS, "tc_ctas", lambda: sms)
         lc.GN_COND.clear()
         for name, fn in orig.items():
             monkeypatch.setattr(L, name, self._wrap(name, fn))

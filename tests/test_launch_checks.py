@@ -479,6 +479,84 @@ def test_attn_head_sampler_covers_later_items(monkeypatch, sms, train, B, H, T, 
               f"{len(mixed)} pairs own a later item after a change of n_kt")
 
 
+def _tc_walk_by_cta(order, ctas):
+    """Per CTA, its tiles in walk order: CTA c takes tiles c, c + grid, ..., grid = min(tiles, ctas)."""
+    grid = min(len(order), ctas)
+    return [order[c::grid] for c in range(grid)]
+
+
+_S2D = dict(taps=L.TAPS_S2D, coffs=L.s2d_coffs(128), cin=128)
+
+
+@pytest.mark.parametrize("sms,n,hw,ctot,cout,dtype,kw,tiling", [
+    (132, 3, (128, 128), 256, 128, torch.float16, {}, (16, 8, 1, True)),          # exact halo: 384 tiles, 3 per CTA
+    (132, 288, (128, 128), 256, 128, torch.float16, {}, (16, 8, 1, True)),        # the benchmark's roofline conv: 36 864 tiles
+    (132, 17, (32, 32), 256, 256, torch.float16, {}, (16, 8, 1, True)),          # two n tiles
+    (132, 67, (8, 8), 512, 512, torch.float16, {}, (8, 8, 2, False)),            # exact tap-box, two images per tile, the last half empty
+    (132, 34, (32, 32), 1024, 128, torch.float16, _S2D, (16, 8, 1, False)),      # exact stride-2 Downsample (space-to-depth taps)
+    (132, 3, (128, 128), 64, 128, torch.bfloat16, {}, (8, 16, 1, True)),         # bf16 halo
+    (132, 9, (64, 64), 128, 128, torch.float32, {}, (8, 16, 1, True)),           # TF32 halo
+    (4, 2, (40, 20), 64, 256, torch.bfloat16, {}, (8, 16, 1, True)),             # ragged borders on a 4-SM device
+    (132, 1, (32, 32), 256, 128, torch.float16, {}, (16, 8, 1, True)),           # 8 tiles, one per CTA: nothing added
+])
+def test_tc_conv_image_sampler_covers_later_tiles(monkeypatch, sms, n, hw, ctot, cout, dtype, kw, tiling):
+    """With the SM count known, the conv check also covers the image of the last tile in walk order and the image of a tile that its CTA
+    walks second or later; the tiling it assumes is the launcher's (stated here per case)."""
+    h, w = hw
+    x = torch.empty(1, dtype=dtype).expand(n, h, w, ctot)              # bind reads shapes only
+    wn = torch.empty(1, dtype=dtype).expand(cout, 1)
+    ba = lc.bind(L.tc_conv, x, wn, None, **kw)
+    cin = kw.get("cin", ctot // (2 if dtype == torch.float16 else 1))
+    assert lc.tc_conv_tiling(h, w, ctot, cin, h, w, ba["taps"], ba["coffs"], dtype == torch.float16, dtype == torch.float32) == tiling
+    tw, th, tn, _ = tiling
+    bn = 128 if cout > 64 else 64
+    order = [it * tn for it in range(-(-n // tn)) for _ in range(-(-h // th)) for _ in range(-(-w // tw)) for _ in range(-(-cout // bn))]
+    walk = _tc_walk_by_cta(order, sms)
+    later = {img for tiles in walk for img in tiles[1:]}
+    for seed in range(5):
+        monkeypatch.setitem(lc.HOOKS, "tc_ctas", None)
+        plain = set(lc.before_tc_conv(ba, random.Random(seed))["images"])
+        monkeypatch.setitem(lc.HOOKS, "tc_ctas", lambda: sms)
+        images = set(lc.before_tc_conv(ba, random.Random(seed))["images"])
+        rng = random.Random(seed)
+        lc.pick(n, rng)                                                   # the sampler draws its three images first
+        added = [order[t] for t in lc.tc_walk_tiles(len(order), sms, rng)]
+        assert plain == set(lc.pick(n, random.Random(seed))) and images == plain | set(added)
+        if len(walk[0]) == 1:
+            assert added == [] and images == plain
+            continue
+        assert added[0] == order[-1] and added[1] in later, f"{added} are not the last tile's image and a later tile's image"
+        print(f"[tc sampler {sms} SMs, {n} x {hw} {ctot}->{cout} {dtype}] {len(order)} tiles, up to {len(walk[0])} per CTA: "
+              f"plain {sorted(plain)} + walk {added}")
+
+
+@pytest.mark.parametrize("sms,M,N,batch", [(132, 1024, 256, (3, 3)), (132, 1024, 1024, (3, 1)), (132, 1024, 64, (20, 1)),
+                                           (4, 300, 200, (1, 2)), (132, 512, 256, (2, 1))])
+def test_tc_gemm_batch_sampler_covers_later_tiles(monkeypatch, sms, M, N, batch):
+    """With the SM count known, the GEMM check also covers the batch entry and the 128-row block of the last tile in walk order and of a
+    tile that its CTA walks second or later."""
+    A = torch.empty(1, dtype=torch.bfloat16).expand(M, 64)
+    ba = lc.bind(L.tc_gemm, A, A, torch.empty(1).expand(M, N), M=M, N=N, K=64, lda=64, ldb=64, ldc=N, batch=batch)
+    bn = 128 if N > 64 else 64
+    order = [(b, m0) for b in range(batch[0] * batch[1]) for m0 in range(0, M, 128) for _ in range(-(-N // bn))]
+    walk = _tc_walk_by_cta(order, sms)
+    later = {tile for tiles in walk for tile in tiles[1:]}
+    for seed in range(5):
+        monkeypatch.setitem(lc.HOOKS, "tc_ctas", lambda: sms)
+        st = lc.before_tc_gemm(ba, random.Random(seed))
+        rng = random.Random(seed)
+        plain_b, plain_rows = lc.pick(batch[0] * batch[1], rng), lc.pick_rows(M, rng)
+        added = [order[t] for t in lc.tc_walk_tiles(len(order), sms, rng)]
+        rows = set(plain_rows.tolist()) | {r for _, m0 in added for r in range(m0, min(m0 + 128, M))}
+        assert st["batches"] == sorted(set(plain_b) | {b for b, _ in added}) and set(st["rows"].tolist()) == rows
+        if len(walk[0]) == 1:
+            assert added == []
+            continue
+        assert added[0] == order[-1] and added[1] in later
+        print(f"[tc sampler {sms} SMs, gemm {M} x {N} batch {batch}] {len(order)} tiles, up to {len(walk[0])} per CTA: "
+              f"batches {st['batches']}, walk tiles (batch, m0) {added}")
+
+
 def test_attn_multiend_bwd_stream_swap():
     B, S, H, ns, rate, seed = 1, 128, 1, 3, 0.1, 90
     d = H * 64

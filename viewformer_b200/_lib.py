@@ -19,7 +19,7 @@ BIAS_NONE, BIAS_N, BIAS_M = 0, 1, 2
 EXPORTS = [
     "vf_last_error", "vf_version", "vf_sizeof_simt_gemm", "vf_sizeof_tc_gemm", "vf_device_check", "vf_u8_to_unit_f32", "vf_unit_f32_to_u8",
     "vf_nchw_to_nhwc_f32", "vf_nhwc_to_nchw_f32", "vf_groupnorm_stats", "vf_groupnorm_apply", "vf_layernorm",
-    "vf_simt_gemm", "vf_tc_gemm", "vf_vq_lookup", "vf_gather_rows", "vf_vq_ema_stats", "vf_vq_ema_update", "vf_vq_commit_grad",
+    "vf_simt_gemm", "vf_tc_gemm", "vf_tc_gemm_plan", "vf_vq_lookup", "vf_gather_rows", "vf_vq_ema_stats", "vf_vq_ema_update", "vf_vq_commit_grad",
     "vf_vq_prepare_codebook", "vf_migt_embed", "vf_softmax_rows", "vf_argmax_rows", "vf_pose_postprocess",
     "vf_cameras_prepare", "vf_cameras_from_relative",
     "vf_conv3x3_small_cin", "vf_conv3x3_small_cout", "vf_groupnorm_finalize", "vf_split_f16x2", "vf_attn_block_causal", "vf_attn_block_causal_tail", "vf_attn_block_causal_decode", "vf_attn_block_multiend",
@@ -346,12 +346,25 @@ def simt_gemm(A, B, out, *, M, N, K, a_strides, b_strides, ldc, batch=(1, 1), a_
     return out
 
 
+_PLAN_KEYS = ("block_n", "TW", "TH", "TN", "halo", "exact", "tiles", "ctas")
+
+
+def _plan(p):
+    """vf_tc_gemm_plan: the tiling vf_tc_gemm would launch for parameter block p, as a dict of _PLAN_KEYS (nothing is launched)."""
+    plan = (C.c_int * len(_PLAN_KEYS))()
+    rc = load(True).vf_tc_gemm_plan(C.byref(p), plan)
+    if rc != 0:
+        raise LibraryError(f"libvf_b200 error {rc}: {_lib.vf_last_error().decode()}")
+    return dict(zip(_PLAN_KEYS, plan))
+
+
 def tc_gemm(A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0), b_bs=(0, 0), c_bs=(0, 0), alpha=1.0,
             bias=None, bias_mode=BIAS_NONE, act=ACT_NONE, residual=None, a_off=0, b_off=0, c_off=0, causal_block=0,
-            causal_skip_n=False, out2=None, gn_rows_per_img=0, gn_groups=32, lo_a=None, lo_b=None, k_offsets=None):
+            causal_skip_n=False, out2=None, gn_rows_per_img=0, gn_groups=32, lo_a=None, lo_b=None, k_offsets=None, plan=False):
     """Tensor-core (wgmma) GEMM: C[m,n] = act(alpha*sum_k A[m,k] B[n,k] + bias) + residual; A,B K-major bf16 (or f32 -> TF32).
     ``out2`` optionally receives a second copy in the other dtype (f32 + bf16 from one epilogue).
-    float16 operands = split-fp16 pairs (exact mode): a row holds hi(K) at column 0 and lo(K) at column ``lo_a`` / ``lo_b``."""
+    float16 operands = split-fp16 pairs (exact mode): a row holds hi(K) at column 0 and lo(K) at column ``lo_a`` / ``lo_b``.
+    ``plan=True`` launches nothing and returns the tiling this call would take (see _plan)."""
     lib = load(True)
     assert A.dtype == B.dtype
     p = TcGemm()
@@ -383,6 +396,8 @@ def tc_gemm(A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0), b_b
         else:
             p.C_bf16 = o.data_ptr() + c_off * 2
     p.ldc = ldc
+    if plan:
+        return _plan(p)
     sums = None
     if gn_rows_per_img and batch == (1, 1) and gn_fusable(N, gn_groups, M, gn_rows_per_img, ldc):
         sums = torch.empty((M // gn_rows_per_img, gn_groups, 2), dtype=torch.float64, device=out.device)
@@ -464,10 +479,11 @@ def gn_mean_rstd(x, groups=32, eps=1e-6):
 
 
 def tc_conv(x, w_nk, bias, *, taps=TAPS_3x3, coffs=None, cin=None, out_hw=None, residual=None, out=None,
-            out_dtype=torch.float32, out2=None, gn_groups=0, norm=None):
+            out_dtype=torch.float32, out2=None, gn_groups=0, norm=None, plan=False):
     """Tensor-core (wgmma) implicit-GEMM conv.  x [N,H,W,Ctot] bf16|f32 NHWC; w_nk [Cout, ntaps*Cin] (K-major, same dtype).
     ``norm=(mean_rstd, gamma, beta, groups, swish)``: x is the RAW activation and GroupNorm(+swish) is applied to it inside the
-    kernel (only for ``conv_norm_fusable`` shapes)."""
+    kernel (only for ``conv_norm_fusable`` shapes).  ``plan=True`` launches nothing and returns the tiling this call would take
+    (see _plan)."""
     lib = load(True)
     _dev(x)
     n, h, w, ctot = x.shape
@@ -498,6 +514,8 @@ def tc_conv(x, w_nk, bias, *, taps=TAPS_3x3, coffs=None, cin=None, out_hw=None, 
         else:
             p.C_bf16 = o.data_ptr()
     p.ldc = cout
+    if plan:
+        return _plan(p)
     sums = None
     if gn_groups and gn_fusable(cout, gn_groups, n * oh * ow, oh * ow, cout):
         sums = torch.empty((n, gn_groups, 2), dtype=torch.float64, device=out.device)

@@ -639,7 +639,59 @@ int launch_kind(const TcParams& prm, WgKind kind, dim3 grid, cudaStream_t st) {
     return launch<kBlockN, kStages, BF16>(prm, grid, st);
 }
 
+// Output tile of a convolution, TN images x TH rows x TW cols = 128 pixels, and whether it takes the halo path (returned).
+bool conv_tiling(const vf_tc_gemm_t* q, bool exact, int bk, int* TWo, int* THo, int* TNo) {
+    int TW = q->OW >= 16 ? 16 : (q->OW >= 8 ? 8 : (q->OW >= 4 ? 4 : (q->OW >= 2 ? 2 : 1)));
+    int TH = 128 / TW;
+    if (TH > q->OH) { TH = 1; while (TH * 2 <= q->OH) TH *= 2; }
+    int TN = 128 / (TW * TH);
+    // halo mode: plain stride-1 pad-1 3x3 conv on maps at least 16 rows tall -> 8x16-pixel tiles, one halo load per channel block.
+    // Exact mode: one halo per channel block and half, all resident for the tile (so at most 2 channel blocks), on the tap-box
+    // path's own 16x8 or 8x16 tiles, which keeps the fused GroupNorm partial sums of each epilogue warp.
+    bool halo = q->ntaps == 9 && q->OH == q->H && q->OW == q->W &&
+                (exact ? q->Ctot == 2 * q->Cin && q->Cin <= 2 * bk && TN == 1 && TW >= 8
+                       : q->Ctot == q->Cin && q->OH >= 16 && q->OW >= 8);
+    for (int t = 0; halo && t < 9; ++t) halo = q->tap_dy[t] == t / 3 - 1 && q->tap_dx[t] == t % 3 - 1 && q->tap_coff[t] == 0;
+    if (halo && !exact) { TW = 8; TH = 16; TN = 1; }
+    *TWo = TW; *THo = TH; *TNo = TN;
+    return halo;
+}
+
+// Persistent CTAs of a launch: one per SM (the device's count, read once).
+int persistent_ctas() {
+    static int num_sms = 0;
+    if (num_sms == 0) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
+    }
+    return num_sms;
+}
+
 }  // namespace
+
+extern "C" int vf_tc_gemm_plan(const vf_tc_gemm_t* q, int* plan) {
+    VF_CHECK_ARG(q && plan, "vf_tc_gemm_plan: null argument");
+    const bool exact = q->ab_dtype == VF_F16X2;
+    const int bk = ROW_BYTES / (q->ab_dtype == VF_F32 ? 4 : 2);
+    const int block_n = (q->Ncols > 64) ? 128 : 64;
+    int TW = 0, TH = 0, TN = 0, halo = 0;
+    long long tiles_m;
+    if (q->conv) {
+        VF_CHECK_ARG(q->ntaps >= 1 && q->ntaps <= 9 && q->OW > 0 && q->OH > 0 && q->N > 0, "vf_tc_gemm_plan: conv shape");
+        halo = conv_tiling(q, exact, bk, &TW, &TH, &TN) ? 1 : 0;
+        tiles_m = (long long)((q->OW + TW - 1) / TW) * ((q->OH + TH - 1) / TH) * ((q->N + TN - 1) / TN);
+    } else {
+        VF_CHECK_ARG(q->M > 0 && q->batch1 > 0 && q->batch2 > 0, "vf_tc_gemm_plan: gemm shape");
+        tiles_m = (long long)((q->M + BLOCK_M - 1) / BLOCK_M) * q->batch1 * q->batch2;
+    }
+    const long long total = tiles_m * ((q->Ncols + block_n - 1) / block_n);
+    VF_CHECK_ARG(total > 0 && total < (1ll << 31), "vf_tc_gemm_plan: tile count out of range");
+    const int ctas = persistent_ctas();
+    const int vals[8] = {block_n, TW, TH, TN, halo, exact ? 1 : 0, (int)total, (int)(total < ctas ? total : ctas)};
+    for (int i = 0; i < 8; ++i) plan[i] = vals[i];
+    return VF_OK;
+}
 
 extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     VF_CHECK_ARG(q && q->A && q->B, "vf_tc_gemm: null operand");
@@ -686,19 +738,8 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         VF_CHECK_ARG(q->ntaps >= 1 && q->ntaps <= 9, "vf_tc_gemm: ntaps");
         VF_CHECK_ARG(q->Cin % bk == 0 && q->Ctot % (16 / es) == 0, "vf_tc_gemm: conv Cin=%d must be a multiple of %d", q->Cin, bk);
         VF_CHECK_ARG(q->causal_block == 0, "vf_tc_gemm: causal with conv");
-        // output tile = TN images x TH rows x TW cols = 128 pixels
-        int TW = q->OW >= 16 ? 16 : (q->OW >= 8 ? 8 : (q->OW >= 4 ? 4 : (q->OW >= 2 ? 2 : 1)));
-        int TH = 128 / TW;
-        if (TH > q->OH) { TH = 1; while (TH * 2 <= q->OH) TH *= 2; }
-        int TN = 128 / (TW * TH);
-        // halo mode: plain stride-1 pad-1 3x3 conv on maps at least 16 rows tall -> 8x16-pixel tiles, one halo load per channel block.
-        // Exact mode: one halo per channel block and half, all resident for the tile (so at most 2 channel blocks), on the tap-box
-        // path's own 16x8 or 8x16 tiles, which keeps the fused GroupNorm partial sums of each epilogue warp.
-        bool halo = q->ntaps == 9 && q->OH == q->H && q->OW == q->W &&
-                    (exact ? q->Ctot == 2 * q->Cin && q->Cin <= 2 * bk && TN == 1 && TW >= 8
-                           : q->Ctot == q->Cin && q->OH >= 16 && q->OW >= 8);
-        for (int t = 0; halo && t < 9; ++t) halo = q->tap_dy[t] == t / 3 - 1 && q->tap_dx[t] == t % 3 - 1 && q->tap_coff[t] == 0;
-        if (halo && !exact) { TW = 8; TH = 16; TN = 1; }
+        int TW, TH, TN;
+        const bool halo = conv_tiling(q, exact, bk, &TW, &TH, &TN);
         prm.halo = halo ? 1 : 0;
         if (q->norm_mean_rstd) {
             VF_CHECK_ARG(halo && q->ab_dtype == VF_BF16 && q->H >= 32 && q->Ncols % 128 == 0 && q->Cin % 64 == 0,
@@ -793,12 +834,7 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     const long long total = (long long)prm.tiles_m * grid.y * grid.z;
     VF_CHECK_ARG(total > 0 && total < (1ll << 31), "vf_tc_gemm: tile count out of range");
     prm.total_tiles = (int)total;
-    static int num_sms = 0;
-    if (num_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
-    }
+    const int num_sms = persistent_ctas();
     const dim3 pgrid((unsigned)(total < num_sms ? total : num_sms), 1, 1);      // persistent CTAs
     {
         auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
