@@ -84,16 +84,14 @@ class VQGANTrainer:
 
     # ------------------------------------------------------------------ parameter registry
     def _collect_params(self):
+        """The trainable tensors in the order of the model's layout: encoder, quantizer block, decoder."""
         w = self.model._w
-        ps = []
+        ps, self._convs = [], []
 
-        self._convs = []
-
-        def conv(name, cw):
-            key = "w_kn" if hasattr(cw, "w_kn") else None
-            if key is None:
+        def conv(name, cw, stride=1):
+            if not hasattr(cw, "w_kn"):
                 raise RuntimeError(f"{name}: tensor-core weight layout in an fp32 model")
-            self._convs.append((name, cw))
+            self._convs.append((cw, stride))
             ps.append(_P(name + ".weight", cw.w_kn, lambda t, cw=cw: setattr(cw, "w_kn", t), "conv", cin=cw.cin))
             ps.append(_P(name + ".bias", cw.bias, lambda t, cw=cw: setattr(cw, "bias", t), "vec"))
 
@@ -105,43 +103,29 @@ class VQGANTrainer:
             ps.append(_P(name + ".weight", d[key][0], lambda t, d=d, key=key: d.__setitem__(key, (t, d[key][1])), "vec"))
             ps.append(_P(name + ".bias", d[key][1], lambda t, d=d, key=key: d.__setitem__(key, (d[key][0], t)), "vec"))
 
-        def rb(name, r):
-            norm(name + ".norm1", r, "n1"); conv(name + ".conv1", r["c1"]); norm(name + ".norm2", r, "n2"); conv(name + ".conv2", r["c2"])
-            if "sc" in r:
-                lin(name + ".nin_shortcut", r["sc"])
+        def stages(built):
+            for st, sw in built:
+                n = st.name
+                if st.kind == "res":
+                    norm(n + ".norm1", sw, "n1"); conv(n + ".conv1", sw["c1"]); norm(n + ".norm2", sw, "n2"); conv(n + ".conv2", sw["c2"])
+                    if "sc" in sw:
+                        lin(n + ".nin_shortcut", sw["sc"])
+                elif st.kind == "attn":
+                    norm(n + ".norm", sw, "norm")
+                    lin(n + ".qk", sw["qk"], parts=(n + ".q", n + ".k"))
+                    lin(n + ".v", sw["v"]); lin(n + ".proj_out", sw["proj"])
+                elif st.kind == "out":
+                    norm(n + ".norm_out", sw, "norm"); conv(n + ".conv_out", sw["conv"])
+                else:
+                    conv(n, sw, st.stride)
 
-        def at(name, a):
-            norm(name + ".norm", a, "norm")
-            lin(name + ".qk", a["qk"], parts=(name + ".q", name + ".k"))
-            lin(name + ".v", a["v"]); lin(name + ".proj_out", a["proj"])
-
-        e, d = w["enc"], w["dec"]
-        conv("encoder.conv_in", e["conv_in"])
-        for lv, lvw in enumerate(e["levels"]):
-            for b, r in enumerate(lvw["blocks"]):
-                rb(f"encoder.down.{lv}.block.{b}", r)
-                if lvw["attns"]:
-                    at(f"encoder.down.{lv}.attn.{b}", lvw["attns"][b])
-            if lvw["down"] is not None:
-                conv(f"encoder.down.{lv}.downsample.conv", lvw["down"])
-        rb("encoder.mid.block_1", e["mid1"]); at("encoder.mid.attn_1", e["mida"]); rb("encoder.mid.block_2", e["mid2"])
-        norm("encoder.norm_out", e, "norm_out"); conv("encoder.conv_out", e["conv_out"])
+        stages(w["enc"])
         lin("quant_conv", w["quant_conv"])
         if self.model.quantizer == "commit":          # Quantize (utils_th.py:75-124): the codebook is an ordinary parameter
             q = w["q"]
             ps.append(_P("quantize.embeddings", q["emb"], lambda t, q=q: q.__setitem__("emb", t), "vec"))
         lin("post_quant_conv", w["post_quant_conv"])
-        conv("decoder.conv_in", d["conv_in"])
-        rb("decoder.mid.block_1", d["mid1"]); at("decoder.mid.attn_1", d["mida"]); rb("decoder.mid.block_2", d["mid2"])
-        for lv in reversed(range(len(self.cfg.ch_mult))):
-            lvw = d["levels"][lv]
-            for b, r in enumerate(lvw["blocks"]):
-                rb(f"decoder.up.{lv}.block.{b}", r)
-                if lvw["attns"]:
-                    at(f"decoder.up.{lv}.attn.{b}", lvw["attns"][b])
-            if lvw["up"] is not None:
-                conv(f"decoder.up.{lv}.upsample.conv", lvw["up"])
-        norm("decoder.norm_out", d, "norm_out"); conv("decoder.conv_out", d["conv_out"])
+        stages(w["dec"])
         self.params = ps
 
     def _flatten(self):
@@ -161,8 +145,7 @@ class VQGANTrainer:
         rewritten from the fp32 master weights in the flat buffer by one launch per step (``_refresh_bf16_weights``)."""
         dev = self.model.device
         self._wb16, entries = {}, []
-        for name, cw in self._convs:
-            stride = 2 if name.endswith("downsample.conv") else 1
+        for cw, stride in self._convs:
             if not self._tc_ok(cw, stride, False):
                 continue
             fw = torch.empty((cw.cout, 9 * cw.cin), dtype=torch.bfloat16, device=dev)
@@ -292,7 +275,7 @@ class VQGANTrainer:
         return dx
 
     # ------------------------------------------------------------------ blocks
-    def _res_fw(self, r, x, tape, name):
+    def _res_fw(self, stage, r, x, tape):
         ex = self.model.exact
         st1 = L.gn_mean_rstd(x)
         h = self._conv_fw(r["c1"], self._act(x, st1, r["n1"], True, r["c1"]))
@@ -301,12 +284,11 @@ class VQGANTrainer:
         n, hh, ww, c = x.shape
         res = linear(ex, x.reshape(-1, c), r["sc"], torch.float32).reshape(n, hh, ww, -1) if "sc" in r else x
         y = self._conv_fw(r["c2"], a2, residual=res)
-        tape.append(("res", name, r, x, st1, h, st2))
+        tape.append((self._res_bw, stage, r, x, st1, h, st2))
         return y
 
-    def _res_bw(self, entry, dy):
-        _, name, r, x, st1, h, st2 = entry
-        G = self.ex.g
+    def _res_bw(self, dy, stage, r, x, st1, h, st2):
+        name, G = stage.name, self.ex.g
         if self.bf16:
             da2 = self._conv_bw16(name + ".conv2", r["c2"], h, dy, norm=(st2, r["n2"], True))
         else:
@@ -330,7 +312,7 @@ class VQGANTrainer:
         self.ex.ready(name + ".norm1.bias", name + ".norm1.weight")
         return dx
 
-    def _attn_fw(self, aw, x, tape, name):
+    def _attn_fw(self, stage, aw, x, tape):
         ex = self.model.exact
         n, hh, ww, c = x.shape
         hw = hh * ww
@@ -348,12 +330,11 @@ class VQGANTrainer:
         L.simt_gemm(Pm, v, o, M=hw, N=c, K=hw, a_strides=(hw, 1), b_strides=(c, 1), ldc=c, batch=(n, 1), a_bs=(hw * hw, 0), b_bs=(hw * c, 0),
                     c_bs=(hw * c, 0))
         y = linear(ex, o, aw["proj"], torch.float32, residual=x.reshape(n * hw, c)).reshape(x.shape)
-        tape.append(("attn", name, aw, x, st, qk, v, Pm, o))
+        tape.append((self._attn_bw, stage, aw, x, st, qk, v, Pm, o))
         return y
 
-    def _attn_bw(self, entry, dy):
-        _, name, aw, x, st, qk, v, Pm, o = entry
-        G = self.ex.g
+    def _attn_bw(self, dy, stage, aw, x, st, qk, v, Pm, o):
+        name, G = stage.name, self.ex.g
         n, hh, ww, c = x.shape
         hw = hh * ww
         scale = float(int(c) ** (-0.5))
@@ -386,50 +367,15 @@ class VQGANTrainer:
         was_training = model.training
         model.training = True                                      # QuantizeEMA.forward: EMA statistics + codebook overwrite (utils_th.py:46-64)
         x = L.nchw_to_nhwc(model._in(x_nchw))
-        tape = []
-        e, d = w["enc"], w["dec"]
-        # ---------------- encoder
-        h = self._conv_fw(e["conv_in"], x)
-        tape.append(("conv", "encoder.conv_in", e["conv_in"], x, 1, False, False))
-        for lv, lvw in enumerate(e["levels"]):
-            for b, r in enumerate(lvw["blocks"]):
-                h = self._res_fw(r, h, tape, f"encoder.down.{lv}.block.{b}")
-                if lvw["attns"]:
-                    h = self._attn_fw(lvw["attns"][b], h, tape, f"encoder.down.{lv}.attn.{b}")
-            if lvw["down"] is not None:
-                tape.append(("conv", f"encoder.down.{lv}.downsample.conv", lvw["down"], h, 2, False, True))
-                h = self._conv_fw(lvw["down"], h, stride=2)
-        h = self._res_fw(e["mid1"], h, tape, "encoder.mid.block_1")
-        h = self._attn_fw(e["mida"], h, tape, "encoder.mid.attn_1")
-        h = self._res_fw(e["mid2"], h, tape, "encoder.mid.block_2")
-        st = L.gn_mean_rstd(h)
-        a = self._gn_apply(h, st, e["norm_out"], True)
-        tape.append(("normconv", "encoder.norm_out", "encoder.conv_out", e, h, st))
-        hz = self._conv_fw(e["conv_out"], a)
+        tape = []                                                  # (backward function, its saved arguments) per stage
+        hz = self._walk_fw(w["enc"], x, tape)
         n, zh, zw, zc = hz.shape
         # ---------------- quantizer (utils_th.py:32-68): z rows, nearest code, straight-through
         z = linear(model.exact, hz.reshape(-1, zc), w["quant_conv"], torch.float32)
         quant, diff, idx = model._quantize(z, want_quant=True)      # training: EMA update + packed all-reduce inside
         pq = linear(model.exact, quant, w["post_quant_conv"], torch.float32).reshape(n, zh, zw, -1)
-        # ---------------- decoder
-        g = self._conv_fw(d["conv_in"], pq)
-        tape.append(("conv", "decoder.conv_in", d["conv_in"], pq, 1, False, True))
-        g = self._res_fw(d["mid1"], g, tape, "decoder.mid.block_1")
-        g = self._attn_fw(d["mida"], g, tape, "decoder.mid.attn_1")
-        g = self._res_fw(d["mid2"], g, tape, "decoder.mid.block_2")
-        for lv in reversed(range(len(cfg.ch_mult))):
-            lvw = d["levels"][lv]
-            for b, r in enumerate(lvw["blocks"]):
-                g = self._res_fw(r, g, tape, f"decoder.up.{lv}.block.{b}")
-                if lvw["attns"]:
-                    g = self._attn_fw(lvw["attns"][b], g, tape, f"decoder.up.{lv}.attn.{b}")
-            if lvw["up"] is not None:
-                tape.append(("conv", f"decoder.up.{lv}.upsample.conv", lvw["up"], g, 1, True, True))
-                g = self._conv_fw(lvw["up"], g, upsample=True)
-        st = L.gn_mean_rstd(g)
-        a = self._gn_apply(g, st, d["norm_out"], True)
-        tape.append(("normconv", "decoder.norm_out", "decoder.conv_out", d, g, st))
-        dec = self._conv_fw(d["conv_out"], a)
+        tape.append((self._quant_bw, hz, z, quant, idx))
+        dec = self._walk_fw(w["dec"], pq, tape)
         # ---------------- loss (vqgan_th.py:400-411): mean |x - xrec| + codebook_weight * diff
         # the backward pass is linear in its seed, so it runs on seeds times a power of two s (exact in fp32: no CUDA-core result changes)
         # that keeps the split-fp16 operands of the tensor-core convs away from fp16's subnormal range; each gradient bucket is divided
@@ -442,41 +388,55 @@ class VQGANTrainer:
         self.last = dict(rec_loss=rec, quant_loss=diff, codes=idx.reshape(n, zh, zw), reconstruction=dec)
         # ---------------- backward
         dy = ddec
-        G = self.ex.g
-        for entry in reversed(tape):
-            kind = entry[0]
-            if kind == "res":
-                dy = self._res_bw(entry, dy)
-            elif kind == "attn":
-                dy = self._attn_bw(entry, dy)
-            elif kind == "conv":
-                _, name, cw, xin, stride, ups, need_dx = entry
-                conv_bw = self._conv_bw16 if self.bf16 else self._conv_bw
-                dy = conv_bw(name, cw, xin, dy, stride=stride, upsample=ups, need_dx=need_dx)
-                if name == "decoder.conv_in":
-                    # through post_quant_conv, the straight-through estimator and the commitment term, quant_conv
-                    dq = self._lin_bw("post_quant_conv", w["post_quant_conv"], quant, dy.reshape(-1, dy.shape[-1]))
-                    cz = s * 2.0 * float(cfg.codebook_weight) / z.numel()
-                    dz = L.lincomb3(1.0, dq, cz, z, -cz, quant)
-                    if model.quantizer == "commit":
-                        # d/dE of beta mean((q - sg(z))^2): column k gets 2 beta / numel * (count_k e_k - sum of the z rows mapped to k);
-                        # the straight-through output carries no gradient to E (utils_th.py:117)
-                        emb = self.ex.p["quantize.embeddings"]
-                        counts, zsum = L.vq_ema_stats(z, idx, emb.shape[1])
-                        L.vq_commit_grad(emb, counts, zsum, s * 2.0 * model.beta * float(cfg.codebook_weight) / z.numel(), G["quantize.embeddings"])
-                        self.ex.ready("quantize.embeddings")
-                    dy = self._lin_bw("quant_conv", w["quant_conv"], hz.reshape(-1, zc), dz).reshape(hz.shape)
-            elif kind == "normconv":
-                _, nname, cname, blk, xin, st = entry
-                nw = blk["norm_out"]
-                cw = blk["conv_out"]
-                a = self._gn_apply(xin, st, nw, True)
-                da = self._conv_bw(cname, cw, a, dy)
-                dy = L.groupnorm_bwd(xin, da, st, nw[0], nw[1], G[nname + ".weight"], G[nname + ".bias"], swish=True, out_bf16=self.bf16)
-                self.ex.ready(nname + ".bias", nname + ".weight")
+        for bw, *saved in reversed(tape):
+            dy = bw(dy, *saved)
         model.training = was_training
         self.ex.check_complete()
         return loss
+
+    def _walk_fw(self, stages, h, tape):
+        """Forward pass of one half's built stages (as VQGAN._walk, fp32 activations); each stage leaves its backward on the tape."""
+        for st, sw in stages:
+            if st.kind == "res":
+                h = self._res_fw(st, sw, h, tape)
+            elif st.kind == "attn":
+                h = self._attn_fw(st, sw, h, tape)
+            elif st.kind == "out":
+                ms = L.gn_mean_rstd(h)
+                a = self._gn_apply(h, ms, sw["norm"], True)
+                tape.append((self._out_bw, st, sw, h, ms))
+                h = self._conv_fw(sw["conv"], a)
+            else:                                                  # the first stage's input is the image: it needs no data gradient
+                tape.append((self._conv_stage_bw, st, sw, h, bool(tape)))
+                h = self._conv_fw(sw, h, stride=st.stride, upsample=st.upsample)
+        return h
+
+    def _conv_stage_bw(self, dy, stage, cw, x, need_dx):
+        conv_bw = self._conv_bw16 if self.bf16 else self._conv_bw
+        return conv_bw(stage.name, cw, x, dy, stride=stage.stride, upsample=stage.upsample, need_dx=need_dx)
+
+    def _out_bw(self, dy, stage, sw, x, ms):
+        """norm_out + swish + conv_out (conv_out on the fp32 step's kernels in both precisions)."""
+        n, G, nw = stage.name, self.ex.g, sw["norm"]
+        da = self._conv_bw(n + ".conv_out", sw["conv"], self._gn_apply(x, ms, nw, True), dy)
+        dx = L.groupnorm_bwd(x, da, ms, nw[0], nw[1], G[n + ".norm_out.weight"], G[n + ".norm_out.bias"], swish=True, out_bf16=self.bf16)
+        self.ex.ready(n + ".norm_out.bias", n + ".norm_out.weight")
+        return dx
+
+    def _quant_bw(self, dy, hz, z, quant, idx):
+        """Through post_quant_conv, the straight-through estimator and the commitment term (and, for Quantize, the codebook), quant_conv."""
+        model, w, G, s = self.model, self.model._w, self.ex.g, self._seed_scale
+        dq = self._lin_bw("post_quant_conv", w["post_quant_conv"], quant, dy.reshape(-1, dy.shape[-1]))
+        cz = s * 2.0 * float(self.cfg.codebook_weight) / z.numel()
+        dz = L.lincomb3(1.0, dq, cz, z, -cz, quant)
+        if model.quantizer == "commit":
+            # d/dE of beta mean((q - sg(z))^2): column k gets 2 beta / numel * (count_k e_k - sum of the z rows mapped to k);
+            # the straight-through output carries no gradient to E (utils_th.py:117)
+            emb = self.ex.p["quantize.embeddings"]
+            counts, zsum = L.vq_ema_stats(z, idx, emb.shape[1])
+            L.vq_commit_grad(emb, counts, zsum, s * 2.0 * model.beta * float(self.cfg.codebook_weight) / z.numel(), G["quantize.embeddings"])
+            self.ex.ready("quantize.embeddings")
+        return self._lin_bw("quant_conv", w["quant_conv"], hz.reshape(-1, hz.shape[-1]), dz).reshape(hz.shape)
 
     def optimizer_step(self):
         self.ex.wait()

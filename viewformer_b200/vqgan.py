@@ -15,6 +15,7 @@ precision's operand dtype.  No torch compute op is on the forward path (torch on
 """
 import re
 from collections import OrderedDict
+from typing import NamedTuple
 
 import os
 
@@ -25,6 +26,60 @@ from .config import VQGANConfig, load_config
 from .ops import Precision, Linear, gemm_nt, linear
 
 _IGNORE = re.compile(r"(perceptual_loss\..*)|(loss\..*)")   # vqgan_th.py:322
+
+
+class Stage(NamedTuple):
+    """One step of the encoder or decoder walk."""
+    kind: str            # conv_in | res | attn | down | up | out (norm_out + swish + conv_out)
+    name: str            # reference key prefix; for "out" the half's own ("encoder" / "decoder")
+    cin: int
+    cout: int
+    exact: bool = False  # encoder.conv_in / decoder.conv_out: always on the exact fp32 kernels
+
+    @property
+    def stride(self):    # Downsample: pad (0,1,0,1), then a VALID stride-2 conv (vqgan_th.py:45-49)
+        return 2 if self.kind == "down" else 1
+
+    @property
+    def upsample(self):  # Upsample: nearest x2, then a stride-1 conv (vqgan_th.py:29-32)
+        return self.kind == "up"
+
+
+def layout(cfg):
+    """Encoder and decoder (vqgan_th.py:147-201, 228-289) as two ordered lists of ``Stage``: conv_in, the resolution levels (res blocks,
+    each followed by an AttnBlock at the attention resolutions, then a Downsample / Upsample), mid block / attention / mid block, out.
+    A pure function of the config and the only place that builds an encoder / decoder key name: the parameter order, the weights, the
+    forward passes and the training step all walk it."""
+    ch, nres = cfg.ch, len(cfg.ch_mult)
+
+    def level(prefix, lv, cin, nblocks):
+        stages, cout = [], ch * cfg.ch_mult[lv]
+        for b in range(nblocks):
+            stages.append(Stage("res", f"{prefix}.block.{b}", cin, cout))
+            cin = cout
+            if cfg.image_size // 2 ** lv in cfg.attn_resolutions:
+                stages.append(Stage("attn", f"{prefix}.attn.{b}", cout, cout))
+        return stages
+
+    def mid(half, c):
+        return [Stage("res", half + ".mid.block_1", c, c), Stage("attn", half + ".mid.attn_1", c, c), Stage("res", half + ".mid.block_2", c, c)]
+
+    enc, c = [Stage("conv_in", "encoder.conv_in", cfg.in_channels, ch, exact=True)], ch
+    for lv in range(nres):
+        enc += level(f"encoder.down.{lv}", lv, c, cfg.num_res_blocks)
+        c = ch * cfg.ch_mult[lv]
+        if lv != nres - 1:
+            enc.append(Stage("down", f"encoder.down.{lv}.downsample.conv", c, c))
+    enc += mid("encoder", c) + [Stage("out", "encoder", c, cfg.z_channels)]
+    c = ch * cfg.ch_mult[-1]
+    dec = [Stage("conv_in", "decoder.conv_in", cfg.z_channels, c)] + mid("decoder", c)
+    for lv in reversed(range(nres)):
+        dec += level(f"decoder.up.{lv}", lv, c, cfg.num_res_blocks + 1)
+        c = ch * cfg.ch_mult[lv]
+        if lv != 0:
+            dec.append(Stage("up", f"decoder.up.{lv}.upsample.conv", c, c))
+    dec.append(Stage("out", "decoder", c, cfg.out_ch, exact=True))
+    return enc, dec
 
 
 class _Conv3:
@@ -75,8 +130,6 @@ class VQGAN:
         # bit-identical to the two-kernel path and tested; the MMA warpgroups do the transform between their MMAs, so it stays
         # opt-in (VF_NORM_ON_LOAD=1) until it is measured faster than conv + vf_groupnorm_apply
         self.norm_on_load = os.environ.get("VF_NORM_ON_LOAD", "0") == "1"      # bf16 halves only
-        self.encoder_chunk = int(os.environ.get("VF_ENC_CHUNK", "0"))      # images per chunk of the high-resolution encoder levels (0: whole batch)
-        self.encoder_chunk_levels = int(os.environ.get("VF_ENC_CHUNK_LEVELS", "2"))
         self.exact = Precision("fp32")
         self.device = torch.device(device)
         self.training = False
@@ -116,8 +169,6 @@ class VQGAN:
         """Ordered {name: shape} of the reference state_dict (vqgan_th.py:147-201, 228-289, 321-336)."""
         cfg = self.config
         out = OrderedDict()
-        nres = len(cfg.ch_mult)
-        res = [cfg.image_size // 2 ** i for i in range(nres)]
 
         def conv(n, cout, cin, k):
             out[n + ".weight"] = (cout, cin, k, k)
@@ -127,46 +178,21 @@ class VQGAN:
             out[n + ".weight"] = (c,)
             out[n + ".bias"] = (c,)
 
-        def rb(n, cin, cout):
-            norm(n + ".norm1", cin); conv(n + ".conv1", cout, cin, 3); norm(n + ".norm2", cout); conv(n + ".conv2", cout, cout, 3)
-            if cin != cout:
-                conv(n + ".nin_shortcut", cout, cin, 1)
-
-        def at(n, c):
-            norm(n + ".norm", c)
-            for p in ("q", "k", "v", "proj_out"):
-                conv(n + "." + p, c, c, 1)
-
-        conv("encoder.conv_in", cfg.ch, cfg.in_channels, 3)
-        cin = cfg.ch
-        for lv in range(nres):
-            cout = cfg.ch * cfg.ch_mult[lv]
-            na = 0
-            for b in range(cfg.num_res_blocks):
-                rb(f"encoder.down.{lv}.block.{b}", cin, cout)
-                cin = cout
-                if res[lv] in cfg.attn_resolutions:
-                    at(f"encoder.down.{lv}.attn.{na}", cin)
-                    na += 1
-            if lv != nres - 1:
-                conv(f"encoder.down.{lv}.downsample.conv", cin, cin, 3)
-        rb("encoder.mid.block_1", cin, cin); at("encoder.mid.attn_1", cin); rb("encoder.mid.block_2", cin, cin)
-        norm("encoder.norm_out", cin); conv("encoder.conv_out", cfg.z_channels, cin, 3)
-        cin = cfg.ch * cfg.ch_mult[-1]
-        conv("decoder.conv_in", cin, cfg.z_channels, 3)
-        rb("decoder.mid.block_1", cin, cin); at("decoder.mid.attn_1", cin); rb("decoder.mid.block_2", cin, cin)
-        for lv in reversed(range(nres)):
-            cout = cfg.ch * cfg.ch_mult[lv]
-            na = 0
-            for b in range(cfg.num_res_blocks + 1):
-                rb(f"decoder.up.{lv}.block.{b}", cin, cout)
-                cin = cout
-                if res[lv] in cfg.attn_resolutions:
-                    at(f"decoder.up.{lv}.attn.{na}", cin)
-                    na += 1
-            if lv != 0:
-                conv(f"decoder.up.{lv}.upsample.conv", cin, cin, 3)
-        norm("decoder.norm_out", cin); conv("decoder.conv_out", cfg.out_ch, cin, 3)
+        enc, dec = layout(cfg)
+        for st in enc + dec:
+            n, cin, cout = st.name, st.cin, st.cout
+            if st.kind == "res":
+                norm(n + ".norm1", cin); conv(n + ".conv1", cout, cin, 3); norm(n + ".norm2", cout); conv(n + ".conv2", cout, cout, 3)
+                if cin != cout:
+                    conv(n + ".nin_shortcut", cout, cin, 1)
+            elif st.kind == "attn":
+                norm(n + ".norm", cin)
+                for p in ("q", "k", "v", "proj_out"):
+                    conv(n + "." + p, cin, cin, 1)
+            elif st.kind == "out":
+                norm(n + ".norm_out", cin); conv(n + ".conv_out", cout, cin, 3)
+            else:
+                conv(n, cout, cin, 3)
         out["quantize.embeddings"] = (cfg.embed_dim, cfg.n_embed)
         if self.quantizer == "ema":
             out["quantize.ema_cluster_size_hidden"] = (cfg.n_embed,)
@@ -243,63 +269,36 @@ class VQGAN:
     def _build(self):
         L.load(require_device=True)
         sd, dev = self._sd, self.device
-        cfg = self.config
-        w = {}
-        prec = None        # set to the half being built (encoder / decoder) before its weights are laid out
 
         def gn(n):
             return (sd[n + ".weight"].to(dev, torch.float32).contiguous(), sd[n + ".bias"].to(dev, torch.float32).contiguous())
 
-        def conv(n, exact=False):
+        def conv(n, prec, exact=False):
             return _Conv3(sd[n + ".weight"], sd[n + ".bias"], prec, dev, exact=exact)
 
-        def lprec():      # precision of the 1x1 convs / attention GEMMs of the half being built
-            return self.exact if (prec.split and os.environ.get("VF_EXACT_GEMM", "1") == "0") else prec
-
-        def lin(n, p=None):
+        def lin(n, prec):
             wt = sd[n + ".weight"]
-            return Linear(wt.reshape(wt.shape[0], wt.shape[1]), sd[n + ".bias"], p or lprec(), dev)
+            return Linear(wt.reshape(wt.shape[0], wt.shape[1]), sd[n + ".bias"], prec, dev)
 
-        def rb(n):
-            d = dict(n1=gn(n + ".norm1"), c1=conv(n + ".conv1"), n2=gn(n + ".norm2"), c2=conv(n + ".conv2"), prec=prec, lprec=lprec())
-            if (n + ".nin_shortcut.weight") in sd:
-                d["sc"] = lin(n + ".nin_shortcut")
-            return d
+        def stage(st, prec):
+            """The stage's weights: a _Conv3 (conv_in / down / up), or a dict of _Conv3, Linear and GroupNorm (weight, bias) tuples."""
+            n, c = st.name, st.cin
+            if st.kind == "res":
+                d = dict(n1=gn(n + ".norm1"), c1=conv(n + ".conv1", prec), n2=gn(n + ".norm2"), c2=conv(n + ".conv2", prec), prec=prec)
+                if st.cin != st.cout:
+                    d["sc"] = lin(n + ".nin_shortcut", prec)
+                return d
+            if st.kind == "attn":
+                wq, wk, wv = (sd[f"{n}.{p}.weight"] for p in ("q", "k", "v"))
+                qk = Linear(torch.cat([wq.reshape(c, c), wk.reshape(c, c)], 0), torch.cat([sd[n + ".q.bias"], sd[n + ".k.bias"]]), prec, dev)
+                return dict(norm=gn(n + ".norm"), qk=qk, v=Linear(wv.reshape(c, c), sd[n + ".v.bias"], prec, dev),
+                            proj=lin(n + ".proj_out", prec), prec=prec)
+            if st.kind == "out":
+                return dict(norm=gn(n + ".norm_out"), conv=conv(n + ".conv_out", prec, st.exact))
+            return conv(n, prec, st.exact)
 
-        def at(n):
-            wq, wk, wv = (sd[f"{n}.{p}.weight"] for p in ("q", "k", "v"))
-            c = wq.shape[0]
-            qk = Linear(torch.cat([wq.reshape(c, c), wk.reshape(c, c)], 0), torch.cat([sd[n + ".q.bias"], sd[n + ".k.bias"]]), lprec(), dev)
-            return dict(norm=gn(n + ".norm"), qk=qk, v=Linear(wv.reshape(c, c), sd[n + ".v.bias"], lprec(), dev),
-                        proj=lin(n + ".proj_out"), c=c, prec=lprec())
-
-        nres = len(cfg.ch_mult)
-        res = [cfg.image_size // 2 ** i for i in range(nres)]
-        prec = self.enc_prec
-        enc = dict(conv_in=conv("encoder.conv_in", exact=True), levels=[], prec=prec)
-        for lv in range(nres):
-            blocks, attns = [], []
-            for b in range(cfg.num_res_blocks):
-                blocks.append(rb(f"encoder.down.{lv}.block.{b}"))
-                if res[lv] in cfg.attn_resolutions:
-                    attns.append(at(f"encoder.down.{lv}.attn.{len(attns)}"))
-            down = conv(f"encoder.down.{lv}.downsample.conv") if lv != nres - 1 else None
-            enc["levels"].append(dict(blocks=blocks, attns=attns, down=down))
-        enc.update(mid1=rb("encoder.mid.block_1"), mida=at("encoder.mid.attn_1"), mid2=rb("encoder.mid.block_2"),
-                   norm_out=gn("encoder.norm_out"), conv_out=conv("encoder.conv_out"))
-        prec = self.dec_prec
-        dec = dict(conv_in=conv("decoder.conv_in"), mid1=rb("decoder.mid.block_1"), mida=at("decoder.mid.attn_1"),
-                   mid2=rb("decoder.mid.block_2"), levels={}, prec=prec)
-        for lv in reversed(range(nres)):
-            blocks, attns = [], []
-            for b in range(cfg.num_res_blocks + 1):
-                blocks.append(rb(f"decoder.up.{lv}.block.{b}"))
-                if res[lv] in cfg.attn_resolutions:
-                    attns.append(at(f"decoder.up.{lv}.attn.{len(attns)}"))
-            up = conv(f"decoder.up.{lv}.upsample.conv") if lv != 0 else None
-            dec["levels"][lv] = dict(blocks=blocks, attns=attns, up=up)
-        dec.update(norm_out=gn("decoder.norm_out"), conv_out=conv("decoder.conv_out", exact=True))
-        w["enc"], w["dec"] = enc, dec
+        enc, dec = layout(self.config)
+        w = dict(enc=[(st, stage(st, self.enc_prec)) for st in enc], dec=[(st, stage(st, self.dec_prec)) for st in dec])
         # 1x1 quant convs always run in exact fp32: their output feeds the bit-exact argmin
         w["quant_conv"] = lin("quant_conv", self.exact)
         w["post_quant_conv"] = lin("post_quant_conv", self.exact)
@@ -367,9 +366,8 @@ class VQGAN:
             a, norm2 = L.groupnorm(h, *rbw["n2"], swish=True, out_dtype=self._act_dtype(rbw["c2"], prec)), None
         if "sc" in rbw:
             n, hh, ww, c = x.shape
-            lp = rbw["lprec"]
-            xs = x if lp.opd == torch.float32 else L.groupnorm(x, None, None, swish=False, out_dtype=lp.opd, normalize=False)
-            res = linear(lp, xs.reshape(n * hh * ww, -1), rbw["sc"], torch.float32).reshape(n, hh, ww, -1)
+            xs = x if prec.opd == torch.float32 else L.groupnorm(x, None, None, swish=False, out_dtype=prec.opd, normalize=False)
+            res = linear(prec, xs.reshape(n * hh * ww, -1), rbw["sc"], torch.float32).reshape(n, hh, ww, -1)
         else:
             res = x
         if norm2 is not None:
@@ -432,76 +430,42 @@ class VQGAN:
         return out4
 
     # ------------------------------------------------------------------ encoder / decoder (NHWC)
-    def _encoder_level(self, lvw, h):
-        for i, rbw in enumerate(lvw["blocks"]):
-            h = self._resblock(rbw, h)
-            if lvw["attns"]:
-                h = self._attn(lvw["attns"][i], h)
-        if lvw["down"] is not None:
-            down = lvw["down"]
-            if down.tc and h.shape[1] % 2 == 0 and h.shape[2] % 2 == 0:
-                hs = L.groupnorm(h, None, None, swish=False, out_dtype=self.enc_prec.opd, normalize=False, s2d=True)
-                h = self._conv(down, hs, stride=2)
-            else:
-                if down.tc:
+    def _walk(self, stages, h, prec):
+        """The built stages of one half, in order, on NHWC f32 activations; ``prec``: that half's precision."""
+        for st, sw in stages:
+            if st.kind == "res":
+                h = self._resblock(sw, h)
+            elif st.kind == "attn":
+                h = self._attn(sw, h)
+            elif st.kind == "conv_in":    # the decoder's z goes to a tensor-core conv_in in the operand dtype
+                zin = h if self._act_dtype(sw, prec) == torch.float32 else L.groupnorm(h, None, None, swish=False, out_dtype=prec.opd, normalize=False)
+                h = self._conv(sw, zin)
+            elif st.kind == "down":
+                if sw.tc and h.shape[1] % 2 == 0 and h.shape[2] % 2 == 0:      # space-to-depth operand for the tensor-core conv
+                    hs = L.groupnorm(h, None, None, swish=False, out_dtype=prec.opd, normalize=False, s2d=True)
+                    h = self._conv(sw, hs, stride=2)
+                elif sw.tc:
                     raise NotImplementedError("odd feature-map size in Downsample on the tensor-core path")
-                h = self._conv(down, h, stride=2)
+                else:
+                    h = self._conv(sw, h, stride=2)
+            elif st.kind == "up":
+                if sw.tc:      # nearest x2 materialised once in the operand dtype, then the tensor-core conv
+                    hu = L.groupnorm(h, None, None, swish=False, out_dtype=prec.opd, normalize=False, upsample=True)
+                    h = self._conv(sw, hu)
+                else:          # exact path: upsampling folded into the conv's address arithmetic
+                    h = self._conv(sw, h, upsample=True)
+            else:              # out: GroupNorm + swish, conv_out (whose output feeds no GroupNorm)
+                a = L.groupnorm(h, *sw["norm"], swish=True, out_dtype=self._act_dtype(sw["conv"], prec))
+                h = self._conv(sw["conv"], a, stats=False)
         return h
 
     def _encoder(self, x):
-        """Encoder.forward (vqgan_th.py:203-225); x f32 [N,H,W,3] -> f32 [N,h,w,z_channels].
-        ``encoder_chunk`` > 0 runs conv_in and the first ``encoder_chunk_levels`` resolution levels in chunks of that many
-        images (images are independent), so that the bf16 activations between producer and consumer kernels stay inside the
-        126 MB L2 instead of streaming through HBM; the low-resolution levels run on the whole batch."""
-        e = self._w["enc"]
-        n = x.shape[0]
-        chunk, nlev = self.encoder_chunk, min(self.encoder_chunk_levels, len(e["levels"]))
-        if chunk > 0 and n > chunk:
-            parts = []
-            for i in range(0, n, chunk):
-                h = self._conv(e["conv_in"], x[i:i + chunk])
-                for lvw in e["levels"][:nlev]:
-                    h = self._encoder_level(lvw, h)
-                parts.append(h)
-            h = torch.cat(parts, 0)
-            if all(hasattr(p, "_gn_sums") for p in parts):          # fused GroupNorm statistics travel with the tensor
-                h._gn_sums = (torch.cat([p._gn_sums[0] for p in parts], 0), parts[0]._gn_sums[1])
-            rest = e["levels"][nlev:]
-        else:
-            h = self._conv(e["conv_in"], x)
-            rest = e["levels"]
-        for lvw in rest:
-            h = self._encoder_level(lvw, h)
-        h = self._resblock(e["mid1"], h)
-        h = self._attn(e["mida"], h)
-        h = self._resblock(e["mid2"], h)
-        a = L.groupnorm(h, *e["norm_out"], swish=True, out_dtype=self._act_dtype(e["conv_out"], self.enc_prec))
-        return self._conv(e["conv_out"], a, stats=False)
+        """Encoder.forward (vqgan_th.py:203-225); x f32 [N,H,W,3] -> f32 [N,h,w,z_channels]."""
+        return self._walk(self._w["enc"], x, self.enc_prec)
 
     def _decoder(self, z):
         """Decoder.forward (vqgan_th.py:291-318); z f32 [N,h,w,z_channels] (post_quant_conv applied) -> f32 [N,H,W,3]."""
-        d = self._w["dec"]
-        cw = d["conv_in"]
-        zin = z if self._act_dtype(cw, self.dec_prec) == torch.float32 else L.groupnorm(z, None, None, swish=False, out_dtype=self.dec_prec.opd, normalize=False)
-        h = self._conv(cw, zin)
-        h = self._resblock(d["mid1"], h)
-        h = self._attn(d["mida"], h)
-        h = self._resblock(d["mid2"], h)
-        for lv in reversed(range(len(self.config.ch_mult))):
-            lvw = d["levels"][lv]
-            for i, rbw in enumerate(lvw["blocks"]):
-                h = self._resblock(rbw, h)
-                if lvw["attns"]:
-                    h = self._attn(lvw["attns"][i], h)
-            if lvw["up"] is not None:
-                up = lvw["up"]
-                if up.tc:      # nearest x2 materialised once in the operand dtype, then the tensor-core conv
-                    hu = L.groupnorm(h, None, None, swish=False, out_dtype=self.dec_prec.opd, normalize=False, upsample=True)
-                    h = self._conv(up, hu)
-                else:          # exact path: upsampling folded into the conv's address arithmetic
-                    h = self._conv(up, h, upsample=True)
-        a = L.groupnorm(h, *d["norm_out"], swish=True, out_dtype=self._act_dtype(d["conv_out"], self.dec_prec))
-        return self._conv(d["conv_out"], a)
+        return self._walk(self._w["dec"], z, self.dec_prec)
 
     # ------------------------------------------------------------------ quantizer
     def _quantize(self, z_rows, want_quant=True):
