@@ -34,7 +34,7 @@ class GradExchange:
     """The trainers' parameters, gradients and optimizer moments in flat fp32 buffers, and the data-parallel gradient exchange over them.
 
     ``entries``: (name, shape) pairs in the order the backward pass completes them.  Each name gets 16-byte aligned views ``p[name]`` /
-    ``g[name]`` at ``offs[name]`` of ``flat_p`` / ``flat_g`` (``flat_m`` / ``flat_v`` share the layout).  A bucket is a contiguous range
+    ``g[name]`` / ``m[name]`` / ``v[name]`` at ``offs[name]`` of ``flat_p`` / ``flat_g`` / ``flat_m`` / ``flat_v``.  A bucket is a contiguous range
     (start, end, name of its last parameter) of the flat gradient, closed after the parameter that pushes it past ``bucket_bytes``; the
     last one closes at the end.  Once the backward pass has signalled every gradient of a bucket (``ready``), the bucket is divided by
     the running step's gradient-seed scale and its asynchronous SUM all-reduce starts, so the transfers ride under the rest of the
@@ -49,11 +49,11 @@ class GradExchange:
             n += (sizes[name] + 3) // 4 * 4                  # 16-byte aligned views
         self.flat_p = torch.zeros((n,), dtype=torch.float32, device=device)
         self.flat_g, self.flat_m, self.flat_v = torch.zeros_like(self.flat_p), torch.zeros_like(self.flat_p), torch.zeros_like(self.flat_p)
-        self.p, self.g = {}, {}
+        self.p, self.g, self.m, self.v = {}, {}, {}, {}
         for name, shape in entries:
             o = self.offs[name]
-            self.p[name] = self.flat_p[o:o + sizes[name]].view(shape)
-            self.g[name] = self.flat_g[o:o + sizes[name]].view(shape)
+            for views, flat in ((self.p, self.flat_p), (self.g, self.flat_g), (self.m, self.flat_m), (self.v, self.flat_v)):
+                views[name] = flat[o:o + sizes[name]].view(shape)
         self.buckets, self._bucket_of, self._bucket_size, start, count = [], {}, [], 0, 0
         for i, name in enumerate(self.order):
             self._bucket_of[name] = len(self.buckets)

@@ -129,9 +129,19 @@ class MIGT:
     # ------------------------------------------------------------------ Keras checkpoint surface (train_transformer.py:106-129)
     def load_weights(self, filepath):
         """Keras ``model.load_weights(<dir>/model)`` of a TF2 object-graph checkpoint (viewformer/utils/tensorflow.py:57-61), read by
-        the pure-Python TensorBundle reader (viewformer_b200/tf_checkpoint.py).  Returns a status object with ``expect_partial()``."""
+        the pure-Python TensorBundle reader (viewformer_b200/tf_checkpoint.py).  Returns a status object with ``expect_partial()``.
+        On a compiled model the weights also go to the trainer and, when the file carries optimizer entries (``save_weights(...,
+        include_optimizer=True)``), so do Adam's moments, the step counters and the loss scale — as Keras restores the optimizer of a
+        compiled model, which finetune_transformer.py:85 relies on."""
         from . import tf_checkpoint
         self.load_state_dict(tf_checkpoint.load_state_dict(filepath, self.expected_keys()))
+        trainer = getattr(self, "_trainer", None)
+        if trainer is not None:
+            trainer.load_state_dict(self._sd)
+            state = tf_checkpoint.load_optimizer_state(filepath, self.expected_keys())
+            if state is not None:
+                trainer.load_optimizer_state(state)
+                self._train_counter = trainer.train_counter
 
         class _Status:
             def expect_partial(self):
@@ -141,10 +151,19 @@ class MIGT:
                 return self
         return _Status()
 
-    def save_weights(self, filepath):
+    def save_weights(self, filepath, include_optimizer=False):
+        """Keras ``model.save_weights``.  ``include_optimizer=True`` (a compiled model) adds what Keras stores for a compiled model — the
+        optimizer's ``iter``, the ``m`` / ``v`` slot of every variable, the schedule's ``offset``, the loss scale (bf16) — so that
+        ``load_weights`` on a compiled model resumes training (tf_checkpoint.OPTIMIZER_SCALARS lists the entries)."""
         from . import tf_checkpoint
         # object paths = the reference model's attribute names (wpe at the root, pose_classifier under pose_criterion): tf_checkpoint.object_paths
-        tf_checkpoint.write_checkpoint(filepath, {tf_checkpoint.object_paths(k)[0]: v.numpy() for k, v in self.state_dict().items()})
+        tensors, slots = {tf_checkpoint.object_paths(k)[0]: v.numpy() for k, v in self.state_dict().items()}, None
+        if include_optimizer:
+            if getattr(self, "_trainer", None) is None:
+                raise RuntimeError("save_weights(include_optimizer=True) needs a compiled model: call compile() first")
+            extra, slots = tf_checkpoint.optimizer_entries(self._trainer.optimizer_state())
+            tensors.update(extra)
+        tf_checkpoint.write_checkpoint(filepath, tensors, slots)
 
     def _build(self):
         L.load(require_device=True)
@@ -435,8 +454,26 @@ class MIGT:
             self.compile()
         out = self._trainer.train_step(batch)
         self.load_state_dict(self._trainer.state_dict())
-        self._train_counter = self._trainer.iterations
+        self._train_counter = self._trainer.train_counter
         return out
+
+    def finetune(self, checkpoint, *, learning_rate, total_steps, **trainer_kwargs):
+        """finetune_transformer.py:72-86: a new optimizer (new peak rate, new horizon) that takes over the moments and ``iterations`` of
+        ``checkpoint`` (written with ``save_weights(..., include_optimizer=True)``) and whose warm-up and decay start at the restored
+        ``iterations`` (``lr_schedule.offset.assign(optimizer.iterations)``); Adam's bias correction and the dropout seed carry on from
+        ``iterations``, the localisation-weight schedule starts again at 0.  Returns the trainer."""
+        import warnings
+        from . import tf_checkpoint
+        self.load_state_dict(tf_checkpoint.load_state_dict(checkpoint, self.expected_keys()))
+        trainer = self.compile(learning_rate=learning_rate, total_steps=total_steps, **trainer_kwargs)
+        state = tf_checkpoint.load_optimizer_state(checkpoint, self.expected_keys())
+        if state is None:
+            warnings.warn(f"{checkpoint} carries no optimizer entries: fine-tuning starts with a fresh optimizer")
+        else:
+            trainer.load_optimizer_state(state)
+        trainer.schedule_offset = trainer.iterations
+        trainer.train_counter = self._train_counter = 0
+        return trainer
 
     # ------------------------------------------------------------------ Keras evaluation steps (migt.py:507-541)
     @L.on_model_device

@@ -27,6 +27,7 @@ _DTYPES = {1: np.float32, 2: np.float64, 3: np.int32, 4: np.uint8, 5: np.int16, 
 _DTYPE_CODES = {np.dtype(v): k for k, v in _DTYPES.items()}
 OBJECT_GRAPH_KEY = "_CHECKPOINTABLE_OBJECT_GRAPH"
 VAR_SUFFIX = "/.ATTRIBUTES/VARIABLE_VALUE"
+SLOT_INFIX = "/.OPTIMIZER_SLOT/"                           # key of a slot variable: <variable path>/.OPTIMIZER_SLOT/<owner path>/<slot name>
 
 
 # ----------------------------------------------------------------------------------------------- varint / protobuf wire helpers
@@ -251,13 +252,14 @@ class Checkpoint:
 
     # --- object graph -----------------------------------------------------------------------------------------
     def object_graph(self):
-        """TrackableObjectGraph -> list of nodes: dict(children={local_name: node_id}, attributes={name: checkpoint_key})."""
+        """TrackableObjectGraph -> list of nodes: dict(children={local_name: node_id}, attributes={name: checkpoint_key},
+        slots={(original_variable_node_id, slot_name): slot_variable_node_id}) — the last on the node that owns the slots (an optimizer)."""
         blob = self.tensor(OBJECT_GRAPH_KEY)
         nodes = []
         for fn, _, v in _fields(blob):
             if fn != 1:
                 continue
-            node = dict(children={}, attributes={})
+            node = dict(children={}, attributes={}, slots={})
             for f2, _, v2 in _fields(v):
                 if f2 == 1:                                   # ObjectReference
                     nid, name = 0, ""
@@ -275,22 +277,45 @@ class Checkpoint:
                         elif f3 == 3:
                             ckey = v3.decode()
                     node["attributes"][aname] = ckey
+                elif f2 == 3:                                 # SlotVariableReference
+                    orig, sname, snid = 0, "", 0
+                    for f3, _, v3 in _fields(v2):
+                        if f3 == 1:
+                            orig = v3
+                        elif f3 == 2:
+                            sname = v3.decode()
+                        elif f3 == 3:
+                            snid = v3
+                    node["slots"][(orig, sname)] = snid
             nodes.append(node)
         return nodes
 
-    def resolve(self, path, nodes=None):
-        """Attribute path ('h/0/attn/c_attn/weight') -> checkpoint key of its VARIABLE_VALUE, via the object graph."""
-        nodes = self.object_graph() if nodes is None else nodes
+    @staticmethod
+    def _walk(path, nodes):
         nid = 0
         for part in path.split("/"):
             ch = nodes[nid]["children"]
             if part not in ch:
                 raise KeyError(f"checkpoint object graph has no '{part}' under '{path}'")
             nid = ch[part]
-        attrs = nodes[nid]["attributes"]
+        return nid
+
+    def resolve(self, path, nodes=None):
+        """Attribute path ('h/0/attn/c_attn/weight') -> checkpoint key of its VARIABLE_VALUE, via the object graph."""
+        nodes = self.object_graph() if nodes is None else nodes
+        attrs = nodes[self._walk(path, nodes)]["attributes"]
         if "VARIABLE_VALUE" not in attrs:
             raise KeyError(f"'{path}' is not a variable in the checkpoint")
         return attrs["VARIABLE_VALUE"]
+
+    def slot(self, path, slot_name, owner="optimizer", nodes=None):
+        """Checkpoint key of the slot variable ``slot_name`` ('m', 'v') that the object at ``owner`` keeps for the variable at ``path``."""
+        nodes = self.object_graph() if nodes is None else nodes
+        ref = (self._walk(path, nodes), slot_name)
+        slots = nodes[self._walk(owner, nodes)]["slots"]
+        if ref not in slots or "VARIABLE_VALUE" not in nodes[slots[ref]]["attributes"]:
+            raise KeyError(f"'{owner}' keeps no slot '{slot_name}' for '{path}'")
+        return nodes[slots[ref]]["attributes"]["VARIABLE_VALUE"]
 
 
 def object_paths(key):
@@ -333,6 +358,76 @@ def load_state_dict(prefix, expected_keys, strict=True):
     return out
 
 
+# ----------------------------------------------------------------------------------------------- optimizer entries
+# Where the reference's compiled Keras model keeps what MIGTTrainer.optimizer_state() holds.  'optimizer' (the model's attribute),
+# 'iter' (OptimizerV2.iterations' weight name), the schedule under 'learning_rate' with WarmUp's 'offset' attribute and the Adam slot
+# names 'm' / 'v' are the names the reference's AdamWeightDecay / WarmUp / MIGT objects carry (tests/test_trainer_state_formats.py walks
+# them).  The names below the wrapper that --fp16 adds (mixed_precision.LossScaleOptimizer: the wrapped optimizer as 'base_optimizer',
+# the scale as 'loss_scale' with weights 'current_loss_scale' / 'good_steps') are TF 2.4's as far as known, and whether TF 2.4 tracks a
+# LearningRateSchedule's variables at all could not be checked either — see INTEGRATION.md.  Keras does not checkpoint the model's
+# _train_counter; it and the dropout seed travel under a child of the root that Keras does not know and skips under expect_partial().
+OPTIMIZER_SCALARS = {                                       # optimizer_state() key -> (path below the Adam optimizer's node, dtype)
+    "iterations": ("iter", np.int64),
+    "schedule_offset": ("learning_rate/offset", np.int64),
+}
+LOSS_SCALE_SCALARS = {                                      # ... -> (path below the LossScaleOptimizer's node, dtype)
+    "loss_scale": ("loss_scale/current_loss_scale", np.float32),
+    "loss_scale_counter": ("loss_scale/good_steps", np.int64),
+}
+EXTRA_SCALARS = {"train_counter": ("viewformer_b200/train_counter", np.int64), "seed": ("viewformer_b200/seed", np.int64)}
+OPTIMIZER_ROOT, BASE_OPTIMIZER, SLOT_NAMES = "optimizer", "base_optimizer", ("m", "v")
+
+
+def optimizer_entries(state):
+    """MIGTTrainer.optimizer_state() -> (tensors, slots) for ``write_checkpoint``, next to the weights written under ``object_paths``."""
+    bf16 = state["precision"] == "bf16"
+    adam = OPTIMIZER_ROOT + ("/" + BASE_OPTIMIZER if bf16 else "")
+    tensors = {adam + "/" + path: np.asarray(state[k], dt) for k, (path, dt) in OPTIMIZER_SCALARS.items()}
+    if bf16:
+        tensors.update({OPTIMIZER_ROOT + "/" + path: np.asarray(state[k], dt) for k, (path, dt) in LOSS_SCALE_SCALARS.items()})
+    tensors.update({path: np.asarray(state[k], dt) for k, (path, dt) in EXTRA_SCALARS.items()})
+    slots = {(adam, slot, object_paths(key)[0]): t.numpy() for slot in SLOT_NAMES for key, t in state[slot].items()}
+    return tensors, slots
+
+
+def load_optimizer_state(prefix, expected_keys):
+    """The optimizer entries of a checkpoint as MIGTTrainer.optimizer_state() lays them out, or None when the file carries none."""
+    import torch
+    ck = Checkpoint(prefix)
+    if OBJECT_GRAPH_KEY not in ck.entries:
+        return None
+    nodes = ck.object_graph()
+
+    def scalar(path):
+        try:
+            return ck.tensor(ck.resolve(path, nodes)).item()
+        except KeyError:
+            return None
+
+    for adam, precision in ((OPTIMIZER_ROOT, "fp32"), (OPTIMIZER_ROOT + "/" + BASE_OPTIMIZER, "bf16")):
+        if scalar(adam + "/" + OPTIMIZER_SCALARS["iterations"][0]) is not None:
+            break
+    else:
+        return None
+    state = dict(precision=precision)
+    tables = [(adam, OPTIMIZER_SCALARS), ("", EXTRA_SCALARS)] + ([(OPTIMIZER_ROOT, LOSS_SCALE_SCALARS)] if precision == "bf16" else [])
+    for base, table in tables:
+        for k, (path, _) in table.items():
+            val = scalar((base + "/" if base else "") + path)
+            if val is not None:
+                state[k] = val
+    for slot in SLOT_NAMES:
+        state[slot] = {}
+        for key in expected_keys:
+            for path in object_paths(key):
+                try:
+                    state[slot][key] = torch.from_numpy(ck.tensor(ck.slot(path, slot, adam, nodes)))
+                    break
+                except KeyError:
+                    continue
+    return state
+
+
 # ----------------------------------------------------------------------------------------------- writer
 def _build_block(items, restart_interval=16):
     out, restarts, prev, n = bytearray(), [], b"", 0
@@ -363,30 +458,46 @@ def _emit_block(f, block):
     return off, len(block)
 
 
-def write_checkpoint(prefix, tensors):
-    """Write {attribute path ('h/0/ln_1/gamma'): numpy array} as a TF2 object-graph checkpoint (<prefix>.index + one data shard)."""
+def write_checkpoint(prefix, tensors, slots=None):
+    """Write {attribute path ('h/0/ln_1/gamma'): numpy array} as a TF2 object-graph checkpoint (<prefix>.index + one data shard).
+    ``slots``: {(owner path, slot name, variable path): numpy array} — slot variables as an optimizer keeps them: a node of its own per
+    slot, reachable only through the owner's ``slot_variables`` (no child edge), stored under the variable's path + SLOT_INFIX + owner +
+    slot name.  Owner and variable must be paths of ``tensors``' graph."""
     os.makedirs(os.path.dirname(os.path.abspath(prefix)), exist_ok=True)
     # object graph: one node per path component, variables are leaf nodes with a VARIABLE_VALUE attribute
-    nodes = [dict(children={}, attributes={})]
+    nodes = [dict(children={}, attributes={}, slots=[])]
 
     def node_for(parts):
         nid = 0
         for p in parts:
             ch = nodes[nid]["children"]
             if p not in ch:
-                nodes.append(dict(children={}, attributes={}))
+                nodes.append(dict(children={}, attributes={}, slots=[]))
                 ch[p] = len(nodes) - 1
             nid = ch[p]
         return nid
 
     entries = {}
     data = bytearray()
-    for path, arr in tensors.items():
+    work = [(path, None, arr) for path, arr in tensors.items()]
+    for path, _, _ in work:                                   # the whole variable graph first, so that slot nodes come after it
+        node_for(path.split("/"))
+    work += [(var + SLOT_INFIX + owner + "/" + name, (owner, name, var), arr) for (owner, name, var), arr in (slots or {}).items()]
+    for path, slot, arr in work:
         arr = np.asarray(arr)
         if arr.ndim and not arr.flags.c_contiguous:
             arr = np.ascontiguousarray(arr)
         key = path + VAR_SUFFIX
-        nodes[node_for(path.split("/"))]["attributes"]["VARIABLE_VALUE"] = key
+        if slot is None:
+            nid = node_for(path.split("/"))
+        else:
+            owner, name, var = slot
+            if var not in tensors or not any(t.startswith(owner + "/") for t in tensors):
+                raise KeyError(f"slot '{name}' of '{var}' kept by '{owner}': both must be paths of the variable graph")
+            nodes.append(dict(children={}, attributes={}, slots=[]))
+            nid = len(nodes) - 1
+            nodes[node_for(owner.split("/"))]["slots"].append((node_for(var.split("/")), name, nid))
+        nodes[nid]["attributes"]["VARIABLE_VALUE"] = key
         raw = arr.tobytes()
         shape = _msg(*[_f_bytes(2, _f_varint(1, d)) for d in arr.shape])
         entries[key] = _msg(_f_varint(1, _DTYPE_CODES[arr.dtype]), _f_bytes(2, shape), _f_varint(4, len(data)) if len(data) else b"",
@@ -399,6 +510,8 @@ def write_checkpoint(prefix, tensors):
             body += _f_bytes(1, _msg(_f_varint(1, nid) if nid else b"", _f_bytes(2, name.encode())))
         for name, key in n["attributes"].items():
             body += _f_bytes(2, _msg(_f_bytes(1, name.encode()), _f_bytes(2, key.encode()), _f_bytes(3, key.encode())))
+        for orig, name, nid in n["slots"]:
+            body += _f_bytes(3, _msg(_f_varint(1, orig), _f_bytes(2, name.encode()), _f_varint(3, nid)))
         graph += _f_bytes(1, body)
     lens = _put_varint(len(graph))
     sraw = lens + struct.pack("<I", masked_crc(lens)) + graph

@@ -34,14 +34,71 @@ gradient buffers, the all-reduce, Adam and the whole quantizer block stay fp32, 
 blocks and the stride-2 convs' gradients.  No loss scaling: bf16 has fp32's exponent range.  The bf16 weight operands are rewritten from
 the fp32 master weights by one kernel after every Adam step.
 """
+import json
 import math
 import os
+import warnings
 
 import torch
 
 from . import _lib as L
 from .dist import GradExchange
 from .ops import linear
+
+
+_REGISTERED = dict(top=("encoder", "decoder", "quantize", "quant_conv", "post_quant_conv"), mid=("block_1", "attn_1", "block_2"),
+                   encoder=("conv_in", "down", "mid", "norm_out", "conv_out"), decoder=("conv_in", "mid", "up", "norm_out", "conv_out"),
+                   level=("block", "attn", "downsample", "upsample"))
+
+
+def _registration_key(name):
+    """Where the reference module tree registers the module that owns ``name`` (vqgan_th.py:159-197, 249-285, 329-333): per resolution
+    level all ResnetBlocks, then all AttnBlocks, then the resampling conv — not the order they run in."""
+    parts = name.split(".")
+    key = [_REGISTERED["top"].index(parts[0])]
+    if parts[0] in ("encoder", "decoder"):
+        key.append(_REGISTERED[parts[0]].index(parts[1]))
+        if parts[1] in ("down", "up"):
+            key += [int(parts[2]), _REGISTERED["level"].index(parts[3])] + ([int(parts[4])] if parts[3] in ("block", "attn") else [])
+        elif parts[1] == "mid":
+            key.append(_REGISTERED["mid"].index(parts[2]))
+    return key
+
+
+def trainable_names(model):
+    """Reference state_dict keys of the tensors Adam updates, in the order of the reference module's ``parameters()`` (encoder, decoder,
+    [Quantize's codebook,] quant_conv, post_quant_conv; QuantizeEMA holds buffers only) — the order ``torch.optim.Adam.state_dict()``
+    numbers them in."""
+    names = [k for k in model.param_shapes() if not (model.quantizer == "ema" and k.startswith("quantize."))]
+    return sorted(names, key=_registration_key)                   # stable: a module's own tensors keep their order
+
+
+def adam_state_dict(names, exp_avg, exp_avg_sq, step, lr, betas, eps):
+    """``torch.optim.Adam.state_dict()`` (what a Lightning checkpoint keeps in ``optimizer_states[i]``) over the parameters ``names``:
+    per-parameter state keyed by the parameter's position, one parameter group."""
+    state = {i: dict(step=torch.tensor(float(step)), exp_avg=exp_avg[k], exp_avg_sq=exp_avg_sq[k]) for i, k in enumerate(names)}
+    group = dict(lr=float(lr), betas=tuple(betas), eps=float(eps), weight_decay=0, amsgrad=False, maximize=False, foreach=None,
+                 capturable=False, differentiable=False, fused=None, params=list(range(len(names))))
+    return dict(state=state, param_groups=[group])
+
+
+def read_adam_state_dict(osd, names):
+    """Inverse of ``adam_state_dict``: dict(exp_avg, exp_avg_sq, step_count, lr, betas, eps).  A state written before the first step has
+    no per-parameter entries: zero moments, step 0."""
+    (group,) = osd["param_groups"]
+    if len(group["params"]) != len(names):
+        raise RuntimeError(f"optimizer state holds {len(group['params'])} parameters, the model has {len(names)}")
+    states = [osd["state"].get(i) for i in group["params"]]
+    if any(st is None for st in states) and any(st is not None for st in states):
+        raise RuntimeError("optimizer state holds moments for some parameters only")
+    steps = {int(st["step"]) for st in states if st is not None} or {0}
+    if len(steps) != 1:
+        raise RuntimeError(f"optimizer state holds different step counts {sorted(steps)}")
+    out = dict(step_count=steps.pop(), lr=float(group["lr"]), betas=tuple(group["betas"]), eps=float(group["eps"]), exp_avg={}, exp_avg_sq={})
+    for k, st in zip(names, states):
+        if st is not None:
+            out["exp_avg"][k], out["exp_avg_sq"][k] = st["exp_avg"], st["exp_avg_sq"]
+    return out
 
 
 class _P:
@@ -451,6 +508,10 @@ class VQGANTrainer:
             gs *= min(1.0, clip / (norm + 1e-6))
         L.adam(self.flat_p, self.flat_g, self.flat_m, self.flat_v, lr=self.lr, beta1=self.betas[0], beta2=self.betas[1], eps=self.eps,
                step=self.step_count, grad_scale=gs)
+        self._weights_changed()
+
+    def _weights_changed(self):
+        """flat_p has new values: everything derived from it is rebuilt."""
         self._wsplit = {}                               # split-fp16 operand copies of the conv weights are stale now
         if self.bf16:
             self._refresh_bf16_weights()
@@ -489,6 +550,123 @@ class VQGANTrainer:
                 else:
                     out[p.name] = tc
         return out
+
+    def _import(self, tensors, what, strict):
+        """Inverse of ``_export``: reference-keyed, reference-layout tensors -> {parameter name: kernel-layout fp32 host tensor}.  Raises on
+        a wrong shape and (strict) on a missing key; nothing on the device is touched."""
+        shapes = self.model.param_shapes()
+
+        def take(key):
+            if key not in tensors:
+                if strict:
+                    raise RuntimeError(f"{what}: missing key {key}")
+                return None
+            t = torch.as_tensor(tensors[key]).detach().to("cpu", torch.float32)
+            if tuple(t.shape) != tuple(shapes[key]):
+                raise RuntimeError(f"{what}: {key} has shape {tuple(t.shape)}, expected {tuple(shapes[key])}")
+            return t
+
+        out = {}
+        for p in self.params:
+            suffix = ".weight" if p.kind == "dense" else ".bias"
+            parts = [take(n + suffix) for n in p.part] if p.part else [take(p.name)]
+            if any(t is None for t in parts):
+                continue
+            t = torch.cat(parts, 0)
+            if p.kind == "conv":
+                t = t.permute(2, 3, 1, 0).reshape(-1, t.shape[0])
+            elif p.kind == "dense":
+                t = t.reshape(t.shape[0], t.shape[1])
+            out[p.name] = t.contiguous()
+        return out
+
+    # ------------------------------------------------------------------ resume: everything a step reads besides the batch
+    def optimizer_state(self):
+        """Host copies of what ``export_state_dict()`` leaves out: Adam's moments under the reference's keys and layouts (the names of
+        ``torch.optim.Adam``'s state) and the scalars.  Every rank of a data-parallel run holds the same state."""
+        return dict(exp_avg=self._export(lambda p: self.ex.m[p.name]), exp_avg_sq=self._export(lambda p: self.ex.v[p.name]),
+                    step_count=self.step_count, lr=self.lr, betas=tuple(self.betas), eps=self.eps, precision=self.precision)
+
+    def load_optimizer_state(self, state, strict=True):
+        """Inverse of ``optimizer_state()``; state saved by a trainer of the other precision loads too (the master copy is fp32)."""
+        m, v = self._import(state["exp_avg"], "exp_avg", strict), self._import(state["exp_avg_sq"], "exp_avg_sq", strict)
+        absent = [k for k in ("step_count", "lr", "betas", "eps") if k not in state]
+        if strict and absent:
+            raise RuntimeError(f"VQGANTrainer.load_optimizer_state: missing {absent}")
+        for views, src in ((self.ex.m, m), (self.ex.v, v)):
+            for k, t in src.items():
+                views[k].copy_(t)
+        self.step_count = int(state.get("step_count", self.step_count))
+        self.lr, self.eps = float(state.get("lr", self.lr)), float(state.get("eps", self.eps))
+        self.betas = tuple(state.get("betas", self.betas))
+        return self
+
+    def load_state_dict(self, state_dict, strict=True):
+        """Reference-keyed weights (the keys of ``export_state_dict()``, EMA buffers included) into the fp32 master copy and the model's
+        quantizer, then what an applied step does to the derived copies."""
+        from .vqgan import _IGNORE
+        model, shapes = self.model, self.model.param_shapes()
+        sd = {k: v for k, v in state_dict.items() if not _IGNORE.match(k)}
+        unknown = [k for k in sd if k not in shapes]
+        if strict and unknown:
+            raise RuntimeError(f"VQGANTrainer.load_state_dict: unexpected keys {unknown[:8]}")
+        new = self._import(sd, "VQGANTrainer.load_state_dict", strict)
+        buffers = {}
+        if model.quantizer == "ema":
+            for key, slot in (("quantize.embeddings", "emb"), ("quantize.ema_cluster_size_hidden", "cs"), ("quantize.ema_dw_hidden", "dw")):
+                if key in sd:
+                    t = torch.as_tensor(sd[key]).detach().to("cpu", torch.float32)
+                    if tuple(t.shape) != tuple(shapes[key]):
+                        raise RuntimeError(f"VQGANTrainer.load_state_dict: {key} has shape {tuple(t.shape)}, expected {tuple(shapes[key])}")
+                    buffers[slot] = t
+                elif strict:
+                    raise RuntimeError(f"VQGANTrainer.load_state_dict: missing key {key}")
+            if strict and "quantize.counter" not in sd:
+                raise RuntimeError("VQGANTrainer.load_state_dict: missing key quantize.counter")
+        for k, t in new.items():
+            self.ex.p[k].copy_(t)
+        q = model._w["q"]
+        for slot, t in buffers.items():
+            q[slot].copy_(t)
+        if model.quantizer == "ema":
+            q["counter"] = int(sd.get("quantize.counter", q["counter"]))
+            model._refresh_codebook()                   # the EMA codebook is no parameter: re-derive its copies as load time does
+        self._weights_changed()
+        model._sd.update({k: torch.as_tensor(v).detach().to("cpu").clone() for k, v in sd.items() if k in shapes})
+        return self
+
+    def save_checkpoint(self, path, epoch=0):
+        """A torch pickle in the pytorch-lightning layout the reference's loaders read (utils/torch.py:9-17 takes ``state_dict``; Lightning's
+        ``resume_from_checkpoint`` also ``optimizer_states``, ``global_step`` and ``epoch``), with ``config.json`` next to it as the
+        reference's checkpoint callback writes it (train/logging_utils_th.py:316-341).  What Lightning has no slot for sits under
+        ``viewformer_b200``.  Under data parallelism call it on rank 0."""
+        st = self.optimizer_state()
+        ckpt = dict(state_dict=dict(self.export_state_dict()), global_step=self.step_count, epoch=int(epoch),
+                    optimizer_states=[adam_state_dict(trainable_names(self.model), st["exp_avg"], st["exp_avg_sq"], self.step_count, self.lr,
+                                                      self.betas, self.eps)],
+                    lr_schedulers=[], viewformer_b200=dict(precision=self.precision, quantizer=self.model.quantizer))
+        os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+        with open(os.path.join(os.path.dirname(os.path.abspath(path)), "config.json"), "w") as f:
+            json.dump(self.cfg.asdict(), f)
+        torch.save(ckpt, path)
+
+    def load_checkpoint(self, path):
+        """Inverse of ``save_checkpoint``.  A file with ``state_dict`` only (what ``registry.load_model`` needs) restores the weights and
+        leaves the optimizer as it is, with a warning.  Returns the checkpoint's ``epoch``."""
+        ckpt = torch.load(path, map_location="cpu")
+        state = None
+        if ckpt.get("optimizer_states"):
+            state = read_adam_state_dict(ckpt["optimizer_states"][0], trainable_names(self.model))
+            # both halves are checked against this model before either is written
+            self._import(state["exp_avg"], "exp_avg", True), self._import(state["exp_avg_sq"], "exp_avg_sq", True)
+        self.load_state_dict(ckpt["state_dict"])
+        if state is None:
+            warnings.warn(f"{path} holds no optimizer state: weights restored, Adam starts from zero moments")
+        else:
+            if not state["exp_avg"]:                    # saved before the first step: Adam had created no moments yet
+                self.flat_m.zero_(), self.flat_v.zero_()
+            self.load_optimizer_state(state, strict=bool(state["exp_avg"]))
+        return int(ckpt.get("epoch", 0))
 
     def export_gradients(self):
         """Gradient of the last forward_backward (already summed over ranks if the handles were waited for), reference layouts."""

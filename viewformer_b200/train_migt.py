@@ -40,13 +40,26 @@ from .dist import GradExchange
 LN_EPS = 1e-5
 
 
+def warmup_cosine(step, init, warm, total_steps, offset=0):
+    """create_optimizer's WarmUp(CosineDecay) (models/utils.py:310-416) at optimizer step ``step``: the schedule runs on
+    ``max(step - offset, 0)`` (WarmUp.__call__, :344-358; ``offset`` is what fine-tuning sets to the restored ``iterations``)."""
+    step = max(step - offset, 0)
+    if warm and step < warm:
+        return init * (step / float(warm))
+    decay_steps = max(1, total_steps - warm)
+    t = min(max(step - warm, 0), decay_steps) / float(decay_steps)
+    return init * 0.5 * (1.0 + math.cos(math.pi * t))
+
+
 class MIGTTrainer:
     LOSS_SCALE_INIT = 2.0 ** 15                                    # tf.mixed_precision DynamicLossScale defaults (TF 2.4)
     LOSS_SCALE_GROWTH_STEPS = 2000
     _seed_scale = 1.0                                              # the gradient-seed scale of the running step (see grad_seed_scale)
 
     def __init__(self, model, betas=(0.9, 0.999), eps=1e-8, warmup_steps=2000, bucket_bytes=64 << 20, process_group=None, seed=0,
-                 grad_reduce="sum", precision="fp32"):
+                 grad_reduce="sum", precision="fp32", learning_rate=None, total_steps=None):
+        """``learning_rate`` / ``total_steps``: peak rate and horizon of the learning-rate schedule when they differ from the config's (the
+        optimizer a fine-tuning run builds, finetune_transformer.py:81-83); the localisation-weight schedule keeps the config's horizon."""
         cfg = model.config
         if cfg.random_pose_multiplier != 1.0:
             raise NotImplementedError("random_pose_multiplier != 1 (pose-scale augmentation, migt.py:350-353) is not supported")
@@ -72,6 +85,10 @@ class MIGTTrainer:
         assert grad_reduce in ("sum", "mean")
         self.grad_reduce = grad_reduce
         self.iterations = 0                                        # optimizer.iterations (0-based: the schedule sees it BEFORE the increment)
+        self.init_lr = float(cfg.learning_rate if learning_rate is None else learning_rate)
+        self.total_steps = int(cfg.total_steps if total_steps is None else total_steps)
+        self.schedule_offset = 0                                   # WarmUp.offset (models/utils.py:342-346): the schedule runs on iterations - offset
+        self._train_counter_base = 0                               # see train_counter
         self.use_tc = self.bf16 or os.environ.get("VF_TRAIN_TC", "1") != "0"
         self._wsplit = {}                                          # split-fp16 operand copies of the weights, rebuilt after every step
         self.use_loc = model.use_localization
@@ -83,9 +100,20 @@ class MIGTTrainer:
             self._build_bf16_weights()
 
     @property
+    def train_counter(self):
+        """The Keras model's ``_train_counter`` (migt.py:446), which the localisation-weight schedule reads: steps taken since it was last
+        set.  It is kept as a distance from ``iterations``, so it advances with every step; ``finetune`` sets it to 0 while ``iterations``
+        (Adam's bias correction, the dropout seed) carries on."""
+        return self.iterations - self._train_counter_base
+
+    @train_counter.setter
+    def train_counter(self, value):
+        self._train_counter_base = self.iterations - int(value)
+
+    @property
     def loc_weight(self):
         """localization_weight(self._train_counter) (migt.py:446): the schedule at the number of steps taken so far."""
-        return float(self._loc_schedule(self.iterations)) if self.use_loc else 0.0
+        return float(self._loc_schedule(self.train_counter)) if self.use_loc else 0.0
 
     # ------------------------------------------------------------------ parameters
     def _build(self, sd):
@@ -135,6 +163,60 @@ class MIGTTrainer:
 
     def gradients(self):
         return OrderedDict((k, self.g[k].detach().cpu().clone()) for k in self.model.param_shapes().keys())
+
+    # ------------------------------------------------------------------ resume: everything a step reads besides the batch
+    def optimizer_state(self):
+        """Host copies of what ``state_dict()`` leaves out: Adam's moments under the weights' key names and layouts, and the scalars.
+        Every rank of a data-parallel run holds the same state; writing it out is rank 0's business."""
+        names = list(self.model.param_shapes().keys())
+        return dict(m=OrderedDict((k, self.ex.m[k].detach().cpu().clone()) for k in names),
+                    v=OrderedDict((k, self.ex.v[k].detach().cpu().clone()) for k in names),
+                    iterations=self.iterations, train_counter=self.train_counter, schedule_offset=self.schedule_offset,
+                    loss_scale=self.loss_scale, loss_scale_counter=self.loss_scale_counter, seed=self.seed, precision=self.precision)
+
+    def _checked(self, tensors, what, strict):
+        """{name: fp32 host tensor} of ``tensors`` for this trainer's parameters; raises on a wrong shape, and (strict) on a missing or
+        unknown name, before anything on the device is written."""
+        shapes = self.model.param_shapes()
+        missing, unknown = [k for k in shapes if k not in tensors], [k for k in tensors if k not in shapes]
+        if strict and (missing or unknown):
+            raise RuntimeError(f"{what}: missing keys {missing[:8]}, unexpected keys {unknown[:8]}")
+        out = {k: torch.as_tensor(tensors[k]).detach().to("cpu", torch.float32) for k in shapes if k in tensors}
+        bad = [(k, tuple(t.shape), tuple(shapes[k])) for k, t in out.items() if tuple(t.shape) != tuple(shapes[k])]
+        if bad:
+            raise RuntimeError(f"{what}: shape mismatch (name, got, expected) {bad[:8]}")
+        return out
+
+    def load_state_dict(self, state_dict, strict=True):
+        """Weights (the keys of ``state_dict()``) into the fp32 master copy, then what an applied step does to the operand copies."""
+        sd = self._checked(state_dict, "MIGTTrainer.load_state_dict", strict)
+        for k, t in sd.items():
+            self.p[k].copy_(t)
+        self._weights_changed()
+        return self
+
+    def load_optimizer_state(self, state, strict=True):
+        """Inverse of ``optimizer_state()``.  State saved by a trainer of the other precision loads too (the master copy is fp32 either
+        way); the loss scale then starts at this precision's default."""
+        m, v = self._checked(state["m"], "first moments", strict), self._checked(state["v"], "second moments", strict)
+        same_scale = self.bf16 and state.get("precision") == "bf16"
+        scalars = ("iterations", "train_counter", "schedule_offset", "seed", "precision") + (("loss_scale", "loss_scale_counter") if same_scale else ())
+        absent = [k for k in scalars if k not in state]
+        if strict and absent:
+            raise RuntimeError(f"MIGTTrainer.load_optimizer_state: missing {absent}")
+        for views, src in ((self.ex.m, m), (self.ex.v, v)):
+            for k, t in src.items():
+                views[k].copy_(t)
+        self.iterations = int(state.get("iterations", self.iterations))
+        self.train_counter = int(state.get("train_counter", self.iterations))
+        self.schedule_offset = int(state.get("schedule_offset", self.schedule_offset))
+        self.seed = int(state.get("seed", self.seed))
+        if same_scale:
+            self.loss_scale = float(state.get("loss_scale", self.loss_scale))
+            self.loss_scale_counter = int(state.get("loss_scale_counter", self.loss_scale_counter))
+        else:
+            self.loss_scale, self.loss_scale_counter = (self.LOSS_SCALE_INIT if self.bf16 else 1.0), 0
+        return self
 
     # ------------------------------------------------------------------ dense layer (Conv1D: x @ W[in,out] + b[1,out])
     # Dense layers whose sizes fit the tensor-core tiles run forward, data gradient and weight gradient on the exact split-fp16 GEMM
@@ -452,13 +534,7 @@ class MIGTTrainer:
 
     # ------------------------------------------------------------------ schedule + optimizer (models/utils.py:310-564)
     def learning_rate(self, step=None):
-        step = self.iterations if step is None else step
-        init, warm = float(self.cfg.learning_rate), self.warmup_steps
-        if warm and step < warm:
-            return init * (step / float(warm))
-        decay_steps = max(1, int(self.cfg.total_steps) - warm)
-        t = min(max(step - warm, 0), decay_steps) / float(decay_steps)
-        return init * 0.5 * (1.0 + math.cos(math.pi * t))
+        return warmup_cosine(self.iterations if step is None else step, self.init_lr, self.warmup_steps, self.total_steps, self.schedule_offset)
 
     def optimizer_step(self):
         """AdamW on the all-reduced gradients; returns whether the update was applied.
@@ -471,7 +547,6 @@ class MIGTTrainer:
         self.ex.wait()
         lr = self.learning_rate()
         self.iterations += 1
-        self._wsplit = {}
         ls = self.loss_scale
         if self.bf16:
             if not math.isfinite(float(L.sumsq(self.flat_g))):
@@ -496,9 +571,14 @@ class MIGTTrainer:
             L.adamw_keras(self.flat_p[o:o + n], self.flat_g[o:o + n], self.flat_m[o:o + n], self.flat_v[o:o + n], lr=lr, beta1=self.betas[0],
                           beta2=self.betas[1], eps=self.eps, weight_decay=wd if (wd > 0 and self.decay[k]) else 0.0, step=self.iterations,
                           grad_scale=gs, clip_scale=cs)
+        self._weights_changed()
+        return True
+
+    def _weights_changed(self):
+        """flat_p has new values: drop the split-fp16 operand copies and rewrite the bf16 ones."""
+        self._wsplit = {}
         if self.bf16:
             L.dense_weights_bf16(self._w16_table)
-        return True
 
     def train_step(self, batch):
         """(poses [B,T,7], tokens [B,T,h,w]) -> dict(loss, ce_loss, [pose losses], acc, learning_rate) — migt.py:464-505."""
