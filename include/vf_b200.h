@@ -327,9 +327,10 @@ int vf_gather_rows(const float* table, const int64_t* idx, int64_t M, int D, int
 int vf_vq_ema_stats(const float* z, const int64_t* idx, int64_t M, int D, int K,
                     float* counts, float* embed_sum_dk, vf_stream_t s);
 /* Quantize (utils_th.py:75-124, the gradient-trained codebook variant): gradient of beta * mean((q - sg(z))^2) with respect to the [D,K]
- * codebook from the per-code counts / row sums of vf_vq_ema_stats: grad[d,k] = coef * (counts[k] * E[d,k] - embed_sum[d,k]). */
+ * codebook from the per-code counts / row sums of vf_vq_ema_stats: grad[d,k] = coef * (counts[k] * E[d,k] - embed_sum[d,k]), or with
+ * accumulate != 0 grad[d,k] += that (gradient accumulation over several backward passes). */
 int vf_vq_commit_grad(const float* embeddings_dk, const float* counts, const float* embed_sum_dk, int D, int K, float coef,
-                      float* grad_dk, vf_stream_t s);
+                      int accumulate, float* grad_dk, vf_stream_t s);
 /* EMA update + Laplace-smoothed renormalisation (utils_th.py:55-64).  alpha = float32(1 - decay);
  * corr = 1 - decay^counter (post-increment counter), both computed by the host exactly as torch does.
  * Updates cs_hidden[K], dw_hidden[D,K], embeddings[D,K] and the derived Et[K,D], esq[K]. */

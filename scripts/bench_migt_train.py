@@ -1,7 +1,9 @@
 """Full-size transformer training step timing (MIGTConfig defaults: 12 layers, d = 768; B scenes x T views x 64 tokens), the fp32-faithful and
 the bf16 trainer alternated in one process (three timed runs each, after a warm-up), with each trainer's peak allocated memory.  The default
-B = 5, T = 20 is the InteriorNet recipe's batch of 40 scenes over 8 GPUs.  VF_B / VF_T / VF_STEPS change the shape and the steps per run."""
-import os, subprocess, sys
+B = 5, T = 20 is the InteriorNet recipe's batch of 40 scenes over 8 GPUs.  VF_B / VF_T / VF_STEPS change the shape and the steps per run.
+``--accumulate N``: every update accumulates N micro-batches of B scenes (``accumulate_steps``); N = 8 is the InteriorNet update of 8
+replicas on one GPU.  Times and rates are then per update of N x B scenes."""
+import argparse, os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
@@ -11,6 +13,9 @@ from viewformer_b200.config import MIGTConfig
 from viewformer_b200.train_migt import MIGTTrainer
 
 B, T, n = int(os.environ.get("VF_B", "5")), int(os.environ.get("VF_T", "20")), int(os.environ.get("VF_STEPS", "3"))
+ap = argparse.ArgumentParser()
+ap.add_argument("--accumulate", type=int, default=1, help="micro-batches of B scenes per update")
+N = ap.parse_args().accumulate
 cfg = MIGTConfig()
 model = MIGT(cfg, precision="fp32").init_weights(0)
 codes = synth.make_codes(B, T, n_embed=cfg.n_embeddings, seed=1)
@@ -26,7 +31,8 @@ def run(tr, steps):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
-        loss = tr.forward_backward(cams, codes)
+        for _ in range(N):
+            loss = tr.forward_backward(cams, codes)
         tr.optimizer_step()
     e1.record()
     torch.cuda.synchronize()
@@ -35,7 +41,7 @@ def run(tr, steps):
 
 trainers, times, peaks, losses = {}, {}, {}, {}
 for prec in ("fp32", "bf16"):
-    trainers[prec] = MIGTTrainer(model, precision=prec)
+    trainers[prec] = MIGTTrainer(model, precision=prec, accumulate_steps=N)
     times[prec] = []
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
@@ -49,7 +55,7 @@ for _ in range(3):
 for prec in ("fp32", "bf16"):
     t = np.array(times[prec])
     med = float(np.median(t))
-    print(f"[migt train step, full size, {prec}] B={B} T={T}: median {med:.1f} ms/step (runs {', '.join(f'{x:.1f}' for x in t)}; "
-          f"spread {t.max() - t.min():.1f} ms) -> {B * T * 64 / med * 1e3:.0f} tokens/s; step peak {peaks[prec] / 2**30:.2f} GiB above the trainers' state; "
+    print(f"[migt train step, full size, {prec}] {N} x B={B} T={T}: median {med:.1f} ms/update (runs {', '.join(f'{x:.1f}' for x in t)}; "
+          f"spread {t.max() - t.min():.1f} ms) -> {N * B * T * 64 / med * 1e3:.0f} tokens/s; step peak {peaks[prec] / 2**30:.2f} GiB above the trainers' state; "
           f"loss {losses[prec]:.4f}")
 print(f"[bf16 vs fp32] {np.median(times['fp32']) / np.median(times['bf16']):.2f}x")

@@ -646,10 +646,11 @@ def vq_ema_stats(z_rows, idx, k):
     return counts, esum
 
 
-def vq_commit_grad(emb_dk, counts, esum, coef, grad_dk):
+def vq_commit_grad(emb_dk, counts, esum, coef, grad_dk, accumulate=False):
+    """grad_dk = coef (count_k e_k - esum) (``accumulate``: grad_dk += that)."""
     lib = load(True)
     d, k = emb_dk.shape
-    _check(lib.vf_vq_commit_grad(_p(emb_dk), _p(counts), _p(esum), d, k, C.c_float(coef), _p(grad_dk), _stream()))
+    _check(lib.vf_vq_commit_grad(_p(emb_dk), _p(counts), _p(esum), d, k, C.c_float(coef), int(bool(accumulate)), _p(grad_dk), _stream()))
     return grad_dk
 
 

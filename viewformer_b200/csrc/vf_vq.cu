@@ -307,9 +307,12 @@ __global__ void ema_stats_kernel(const float* __restrict__ z, const int64_t* __r
 }
 
 __global__ void commit_grad_kernel(const float* __restrict__ emb, const float* __restrict__ counts, const float* __restrict__ esum, long long n,
-                                   int K, float coef, float* __restrict__ grad) {
+                                   int K, float coef, int accumulate, float* __restrict__ grad) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) grad[i] = coef * (counts[i % K] * emb[i] - esum[i]);
+    if (i < n) {
+        const float g = coef * (counts[i % K] * emb[i] - esum[i]);
+        grad[i] = accumulate ? __fadd_rn(grad[i], g) : g;
+    }
 }
 
 // single block of 1024 threads; thread k owns code k (K <= 1024 handled by striding)
@@ -420,12 +423,13 @@ extern "C" int vf_vq_ema_stats(const float* z, const int64_t* idx, int64_t M, in
 }
 
 // Gradient of the commitment term of Quantize (utils_th.py:113-114, beta mean((q - sg(z))^2)) with respect to the [D,K] codebook:
-// column k collects coef * (count_k e_k - sum of the z rows mapped to k); counts / sums come from vf_vq_ema_stats.
+// column k collects coef * (count_k e_k - sum of the z rows mapped to k); counts / sums come from vf_vq_ema_stats.  accumulate: added to
+// grad (one more backward pass into the same gradient buffer), else written over it.
 extern "C" int vf_vq_commit_grad(const float* embeddings_dk, const float* counts, const float* embed_sum_dk, int D, int K, float coef,
-                                 float* grad_dk, vf_stream_t s) {
+                                 int accumulate, float* grad_dk, vf_stream_t s) {
     VF_CHECK_ARG(embeddings_dk && counts && embed_sum_dk && grad_dk && D > 0 && K > 0, "vf_vq_commit_grad: bad args");
     const long long n = (long long)D * K;
-    commit_grad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, vf_s(s)>>>(embeddings_dk, counts, embed_sum_dk, n, K, coef, grad_dk);
+    commit_grad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, vf_s(s)>>>(embeddings_dk, counts, embed_sum_dk, n, K, coef, accumulate, grad_dk);
     VF_CHECK_LAUNCH("vf_vq_commit_grad");
     return VF_OK;
 }

@@ -38,7 +38,12 @@ class GradExchange:
     (start, end, name of its last parameter) of the flat gradient, closed after the parameter that pushes it past ``bucket_bytes``; the
     last one closes at the end.  Once the backward pass has signalled every gradient of a bucket (``ready``), the bucket is divided by
     the running step's gradient-seed scale and its asynchronous SUM all-reduce starts, so the transfers ride under the rest of the
-    backward pass."""
+    backward pass.
+
+    Gradient accumulation: ``reset(seed_scale, micro_batches=N)`` opens a window of N backward passes that all add into ``flat_g``, which
+    is zeroed only there.  ``next_micro_batch()`` arms each further pass.  In passes 1 .. N-1 a completed bucket is only counted; in pass N
+    it is unscaled and exchanged as above (DDP's ``no_sync``), so a window costs one exchange whatever N is.  ``flush()`` exchanges the
+    buckets of a window that ends early."""
 
     def __init__(self, entries, device, bucket_bytes, group=None):
         self.group = group
@@ -69,27 +74,54 @@ class GradExchange:
     def world(self):
         return dist.get_world_size(self.group) if (dist.is_available() and dist.is_initialized()) else 1
 
-    def reset(self, seed_scale=1.0):
-        """Start a step: zero the gradient, no bucket signalled yet; the backward pass runs on seeds times ``seed_scale`` (a power of two)."""
+    def reset(self, seed_scale=1.0, micro_batches=1):
+        """Open a window of ``micro_batches`` backward passes and arm the first: zero the gradient, no bucket signalled yet.  Every pass of
+        the window runs on seeds times ``seed_scale`` (a power of two), so the one division at the end is exact."""
+        if int(micro_batches) < 1:
+            raise ValueError(f"micro_batches must be >= 1, got {micro_batches}")
         self.flat_g.zero_()
         self.seed_scale = seed_scale
+        self.micro_batches, self.micro = int(micro_batches), 1     # passes in the window; the running pass (1-based)
         self.handles, self._left = [], list(self._bucket_size)
         self.launched.clear()
 
+    def next_micro_batch(self):
+        """Arm the next backward pass of the open window; the previous pass must have signalled every bucket."""
+        self.check_complete()
+        if self.micro >= self.micro_batches:
+            raise RuntimeError(f"the accumulation window of {self.micro_batches} micro-batches is complete")
+        self.micro += 1
+        self._left = list(self._bucket_size)
+
     def ready(self, *names):
-        """The backward pass has finished the gradients of ``names``: unscale and start the all-reduce of every bucket this completes."""
+        """The backward pass has finished the gradients of ``names``.  In the window's last pass: unscale and start the all-reduce of every
+        bucket this completes."""
         for name in names:
             b = self._bucket_of[name]
             self._left[b] -= 1
             if self._left[b] == 0:
-                self.launched.append(b)
-                s, e, _ = self.buckets[b]
-                if self.seed_scale != 1.0:                   # divide the seed scale back out (exact: a power of two)
-                    L.lincomb3(1.0 / self.seed_scale, self.flat_g[s:e], out=self.flat_g[s:e])
-                if self.world() > 1:
-                    self.handles.append(dist.all_reduce(self.flat_g[s:e], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
+                if self.micro == self.micro_batches:
+                    self._exchange(b)
             elif self._left[b] < 0:
                 raise RuntimeError(f"gradient of {name} signalled twice")
+
+    def _exchange(self, b):
+        self.launched.append(b)
+        s, e, _ = self.buckets[b]
+        if self.seed_scale != 1.0:                           # divide the seed scale back out (exact: a power of two)
+            L.lincomb3(1.0 / self.seed_scale, self.flat_g[s:e], out=self.flat_g[s:e])
+        if self.world() > 1:
+            self.handles.append(dist.all_reduce(self.flat_g[s:e], op=dist.ReduceOp.SUM, group=self.group, async_op=True))
+
+    def flush(self):
+        """End the window after the running pass even if it is not the last planned one (an optimizer step on a partial window): unscale
+        and exchange every bucket.  Nothing to do in the window's last pass: its own ``ready`` calls exchange the buckets."""
+        if self.micro == self.micro_batches:
+            return
+        self.check_complete()
+        for b in range(len(self.buckets)):
+            self._exchange(b)
+        self.micro_batches = self.micro
 
     def check_complete(self):
         """End of the backward pass: every bucket must have been signalled."""

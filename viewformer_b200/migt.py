@@ -161,6 +161,10 @@ class MIGT:
         if include_optimizer:
             if getattr(self, "_trainer", None) is None:
                 raise RuntimeError("save_weights(include_optimizer=True) needs a compiled model: call compile() first")
+            tr = self._trainer
+            if 0 < tr.pending < tr.ex.micro_batches:
+                raise RuntimeError(f"save_weights(include_optimizer=True): {tr.pending} of {tr.ex.micro_batches} micro-batches of the "
+                                   "accumulation window are pending; save after the step that closes the window")
             extra, slots = tf_checkpoint.optimizer_entries(self._trainer.optimizer_state())
             tensors.update(extra)
         tf_checkpoint.write_checkpoint(filepath, tensors, slots)
@@ -453,7 +457,8 @@ class MIGT:
         if getattr(self, "_trainer", None) is None:
             self.compile()
         out = self._trainer.train_step(batch)
-        self.load_state_dict(self._trainer.state_dict())
+        if not out["pending"]:                          # inside an accumulation window the weights have not moved
+            self.load_state_dict(self._trainer.state_dict())
         self._train_counter = self._trainer.train_counter
         return out
 

@@ -111,11 +111,21 @@ class _P:
 class VQGANTrainer:
     _seed_scale = 1.0                                   # the gradient-seed scale of the running step (see grad_seed_scale)
 
-    def __init__(self, model, lr=None, betas=(0.5, 0.9), eps=1e-8, bucket_bytes=64 << 20, process_group=None, precision="fp32"):
+    def __init__(self, model, lr=None, betas=(0.5, 0.9), eps=1e-8, bucket_bytes=64 << 20, process_group=None, precision="fp32",
+                 accumulate_grad_batches=1):
         """``precision``: "fp32" (the reference's arithmetic) or "bf16" (single-pass bf16 tensor-core convs, see the module docstring);
-        either way the model is built with precision="fp32" and its fp32 weights are the master copy."""
+        either way the model is built with precision="fp32" and its fp32 weights are the master copy.
+
+        ``accumulate_grad_batches`` = N (Lightning's option of that name, train_codebook_th.py:30,67): ``training_step`` runs forward and
+        backward on its micro-batch with the loss divided by N, adding into one gradient; every N-th call exchanges that gradient once,
+        clips it and runs Adam.  QuantizeEMA moves its codebook in every micro-batch, as the reference's forward does under Lightning.
+        A run option: it is not saved in checkpoints, and a new value takes effect at the next window."""
         if precision not in ("fp32", "bf16"):
             raise ValueError("VQGANTrainer precision must be 'fp32' or 'bf16'")
+        if int(accumulate_grad_batches) < 1:
+            raise ValueError(f"accumulate_grad_batches must be >= 1, got {accumulate_grad_batches}")
+        self.accumulate_grad_batches = int(accumulate_grad_batches)
+        self.pending = 0                                # micro-batches in the gradient since the last optimizer step
         if model.enc_prec.name != "fp32" or model.dec_prec.name != "fp32":
             raise ValueError("VQGANTrainer runs the fp32 path (the reference asserts no mixed precision, vqgan_th.py:326): build the model "
                              "with precision='fp32'")
@@ -419,7 +429,9 @@ class VQGANTrainer:
 
     # ------------------------------------------------------------------ the step
     def forward_backward(self, x_nchw):
-        """x f32 NCHW in [-1,1] -> loss (python float).  Leaves the gradient (summed over ranks once the exchange is waited for) in flat_g."""
+        """x f32 NCHW in [-1,1] -> loss (python float).  Leaves the gradient (summed over ranks once the exchange is waited for) in flat_g.
+        One micro-batch of the accumulation window: the first one (no micro-batch pending, or the previous window complete) opens a new
+        window, the others add their gradient (of the loss divided by the window's length) to the pending one."""
         model, cfg, w = self.model, self.cfg, self.model._w
         was_training = model.training
         model.training = True                                      # QuantizeEMA.forward: EMA statistics + codebook overwrite (utils_th.py:46-64)
@@ -436,9 +448,16 @@ class VQGANTrainer:
         # ---------------- loss (vqgan_th.py:400-411): mean |x - xrec| + codebook_weight * diff
         # the backward pass is linear in its seed, so it runs on seeds times a power of two s (exact in fp32: no CUDA-core result changes)
         # that keeps the split-fp16 operands of the tensor-core convs away from fp16's subnormal range; each gradient bucket is divided
-        # by s when it completes, so flat_g, the all-reduce, clipping and Adam see the unscaled gradient
-        s = self._seed_scale = float(2.0 ** round(math.log2(dec.numel())) if self.grad_seed_scale is None else self.grad_seed_scale)
-        self.ex.reset(s)
+        # by s when it completes, so flat_g, the all-reduce, clipping and Adam see the unscaled gradient.  Under accumulation s is the
+        # window's first micro-batch's, and the seeds are divided by the window's length N (Lightning divides the loss by N)
+        if self.pending in (0, self.ex.micro_batches):
+            s = float(2.0 ** round(math.log2(dec.numel())) if self.grad_seed_scale is None else self.grad_seed_scale)
+            self.ex.reset(s, self.accumulate_grad_batches)
+            self.pending = 0
+        else:
+            self.ex.next_micro_batch()
+        self._seed_scale = self.ex.seed_scale
+        s = self._seed_scale / self.ex.micro_batches
         ddec, l1 = L.l1_grad(x, dec, s / dec.numel())
         rec = l1 / dec.numel()
         loss = rec.to(torch.float32).reshape(()) + float(cfg.codebook_weight) * diff
@@ -449,6 +468,7 @@ class VQGANTrainer:
             dy = bw(dy, *saved)
         model.training = was_training
         self.ex.check_complete()
+        self.pending += 1
         return loss
 
     def _walk_fw(self, stages, h, tape):
@@ -482,7 +502,7 @@ class VQGANTrainer:
 
     def _quant_bw(self, dy, hz, z, quant, idx):
         """Through post_quant_conv, the straight-through estimator and the commitment term (and, for Quantize, the codebook), quant_conv."""
-        model, w, G, s = self.model, self.model._w, self.ex.g, self._seed_scale
+        model, w, G, s = self.model, self.model._w, self.ex.g, self._seed_scale / self.ex.micro_batches
         dq = self._lin_bw("post_quant_conv", w["post_quant_conv"], quant, dy.reshape(-1, dy.shape[-1]))
         cz = s * 2.0 * float(self.cfg.codebook_weight) / z.numel()
         dz = L.lincomb3(1.0, dq, cz, z, -cz, quant)
@@ -491,12 +511,17 @@ class VQGANTrainer:
             # the straight-through output carries no gradient to E (utils_th.py:117)
             emb = self.ex.p["quantize.embeddings"]
             counts, zsum = L.vq_ema_stats(z, idx, emb.shape[1])
-            L.vq_commit_grad(emb, counts, zsum, s * 2.0 * model.beta * float(self.cfg.codebook_weight) / z.numel(), G["quantize.embeddings"])
+            L.vq_commit_grad(emb, counts, zsum, s * 2.0 * model.beta * float(self.cfg.codebook_weight) / z.numel(), G["quantize.embeddings"],
+                             accumulate=True)
             self.ex.ready("quantize.embeddings")
         return self._lin_bw("quant_conv", w["quant_conv"], hz.reshape(-1, hz.shape[-1]), dz).reshape(hz.shape)
 
     def optimizer_step(self):
+        """Clip and Adam on the window's gradient.  Called on a partial window (Lightning's step at the end of an epoch), it steps on the
+        micro-batches accumulated so far."""
+        self.ex.flush()
         self.ex.wait()
+        self.pending = 0
         self.step_count += 1
         gs = 1.0 / self.ex.world()
         clip = float(self.cfg.gradient_clip_val or 0.0)
@@ -521,9 +546,11 @@ class VQGANTrainer:
             self.model._refresh_decode_table()
 
     def training_step(self, batch, batch_idx=0):
-        """vqgan_th.py:413-423 + the optimizer step Lightning runs after it.  Returns the loss of the step (0-d f32 tensor)."""
+        """vqgan_th.py:413-423 + the optimizer step Lightning runs after every ``accumulate_grad_batches``-th call.  Returns the loss of
+        this micro-batch (0-d f32 tensor, not divided by the window's length)."""
         loss = self.forward_backward(batch)
-        self.optimizer_step()
+        if self.pending == self.ex.micro_batches:
+            self.optimizer_step()
         return loss
 
     # ------------------------------------------------------------------ export (reference layouts)
@@ -639,7 +666,11 @@ class VQGANTrainer:
         """A torch pickle in the pytorch-lightning layout the reference's loaders read (utils/torch.py:9-17 takes ``state_dict``; Lightning's
         ``resume_from_checkpoint`` also ``optimizer_states``, ``global_step`` and ``epoch``), with ``config.json`` next to it as the
         reference's checkpoint callback writes it (train/logging_utils_th.py:316-341).  What Lightning has no slot for sits under
-        ``viewformer_b200``.  Under data parallelism call it on rank 0."""
+        ``viewformer_b200``.  Under data parallelism call it on rank 0.  Not in the middle of an accumulation window: the checkpoint has
+        no slot for a pending gradient."""
+        if 0 < self.pending < self.ex.micro_batches:
+            raise RuntimeError(f"save_checkpoint: {self.pending} of {self.ex.micro_batches} micro-batches of the accumulation window are "
+                               "pending; save after the optimizer step that closes the window (or call optimizer_step() first)")
         st = self.optimizer_state()
         ckpt = dict(state_dict=dict(self.export_state_dict()), global_step=self.step_count, epoch=int(epoch),
                     optimizer_states=[adam_state_dict(trainable_names(self.model), st["exp_avg"], st["exp_avg_sq"], self.step_count, self.lr,

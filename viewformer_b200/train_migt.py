@@ -57,9 +57,19 @@ class MIGTTrainer:
     _seed_scale = 1.0                                              # the gradient-seed scale of the running step (see grad_seed_scale)
 
     def __init__(self, model, betas=(0.9, 0.999), eps=1e-8, warmup_steps=2000, bucket_bytes=64 << 20, process_group=None, seed=0,
-                 grad_reduce="sum", precision="fp32", learning_rate=None, total_steps=None):
+                 grad_reduce="sum", precision="fp32", learning_rate=None, total_steps=None, accumulate_steps=1):
         """``learning_rate`` / ``total_steps``: peak rate and horizon of the learning-rate schedule when they differ from the config's (the
-        optimizer a fine-tuning run builds, finetune_transformer.py:81-83); the localisation-weight schedule keeps the config's horizon."""
+        optimizer a fine-tuning run builds, finetune_transformer.py:81-83); the localisation-weight schedule keeps the config's horizon.
+
+        ``accumulate_steps`` = N: ``train_step`` adds the gradient of N micro-batches, each the mean loss of its own scenes, and applies
+        one update per N calls, so every micro-batch plays one more replica of the reference's MirroredStrategy: one GPU with N = 8
+        performs the update of 8 replicas.  ``grad_reduce="mean"`` divides by world size x N.  ``iterations`` (hence the learning rate,
+        the localisation weight, Adam's bias correction and the dropout masks), the loss scale and its good-step counter advance once per
+        window.  A new value takes effect at the next window."""
+        if int(accumulate_steps) < 1:
+            raise ValueError(f"accumulate_steps must be >= 1, got {accumulate_steps}")
+        self.accumulate_steps = int(accumulate_steps)
+        self.pending = 0                                           # micro-batches in the gradient since the last optimizer step
         cfg = model.config
         if cfg.random_pose_multiplier != 1.0:
             raise NotImplementedError("random_pose_multiplier != 1 (pose-scale augmentation, migt.py:350-353) is not supported")
@@ -436,9 +446,13 @@ class MIGTTrainer:
         loss = ce * float(cfg.image_generation_weight)
         self.last = dict(ce_loss=ce, logits=logits.reshape(B, T, Lt, V))
         dhn = [None] * ns
-        self._seed_scale = float(2.0 ** round(math.log2(denom)) if self.grad_seed_scale is None else self.grad_seed_scale)
-        self.ex.reset(self._seed_scale)
-        ls = self.loss_scale * self._seed_scale                                    # gradient seeds carry the loss scale (1 in fp32) and the seed scale
+        if self.pending in (0, self.ex.micro_batches):                            # the first micro-batch opens the accumulation window
+            self.ex.reset(float(2.0 ** round(math.log2(denom)) if self.grad_seed_scale is None else self.grad_seed_scale), self.accumulate_steps)
+            self.pending = 0
+        else:
+            self.ex.next_micro_batch()
+        self._seed_scale = self.ex.seed_scale                                      # the window's: fixed from its first micro-batch
+        ls = self.loss_scale * self._seed_scale                                   # gradient seeds carry the loss scale (1 in fp32) and the seed scale
         dlog = L.cross_entropy_grad(logits, ids.reshape(-1), (view_ok * (float(cfg.image_generation_weight) * ls / denom)).contiguous(),
                                     float(cfg.label_smoothing))
         # tied LM head backward: d hn1 = dlogits wte[:V];  d wte[:V] += dlogits^T hn1
@@ -467,7 +481,8 @@ class MIGTTrainer:
                 e0, e1 = math.exp(-float(w01[0])), math.exp(-float(w01[1]))
                 pls, ols = float(pl.double().sum()), float(ol.double().sum())
                 pose_loss = torch.full_like(pl, float(B * (w01[0] + w01[1]) + e0 * pls + e1 * ols))
-                self.g[wkey].copy_(torch.tensor([lw_now * (B - e0 * pls) * ls, lw_now * (B - e1 * ols) * ls], dtype=torch.float32))
+                dw01 = torch.tensor([lw_now * (B - e0 * pls) * ls, lw_now * (B - e1 * ols) * ls], dtype=torch.float32).to(dev)
+                L.lincomb3(1.0, self.g[wkey], 1.0, dw01, out=self.g[wkey])       # added: the window's earlier micro-batches are in g
                 self.ex.ready(wkey)
                 ps, os_ = e0 * B, e1 * B
             else:
@@ -526,6 +541,7 @@ class MIGTTrainer:
         self._lin_bw(pin, L.gelu_bwd(pe_h, dh_), "pose_embedding.c_fc", need_dx=False)
         self.ex.ready("wpe.embeddings", "wte.weight")
         self.ex.check_complete()
+        self.pending += 1
         self.last["loss_per_scene"] = loss
         return loss.mean()
 
@@ -543,8 +559,13 @@ class MIGTTrainer:
         squares of the flat gradient decides whether all of them are finite.  Non-finite: no update (weights and moments untouched), the
         scale halves (not below 1) and the good-step counter resets, but ``iterations`` still advances, as Keras's do_not_apply_fn does, so
         the learning-rate and localisation schedules move on.  Finite: the update runs on the unscaled gradients (clipping included), and
-        when the counter has reached 1999 the scale doubles (if that is finite) and the counter resets, else the counter counts up."""
+        when the counter has reached 1999 the scale doubles (if that is finite) and the counter resets, else the counter counts up.
+
+        Under accumulation this runs once per window, on the sum of its micro-batches' gradients: one finiteness check, one skip or
+        update.  Called on a partial window, it steps on the micro-batches accumulated so far."""
+        self.ex.flush()
         self.ex.wait()
+        self.pending = 0
         lr = self.learning_rate()
         self.iterations += 1
         ls = self.loss_scale
@@ -561,7 +582,7 @@ class MIGTTrainer:
                 self.loss_scale_counter += 1
         wd = float(self.cfg.weight_decay)
         clip = float(self.cfg.gradient_clip_val or 0.0)
-        gs = (1.0 / self.ex.world() if self.grad_reduce == "mean" else 1.0) / ls
+        gs = (1.0 / (self.ex.world() * self.ex.micro_batches) if self.grad_reduce == "mean" else 1.0) / ls
         for k in self.order:
             cs = 1.0
             if clip > 0:                                                  # tf.clip_by_norm: g * clip / max(|g|, clip), per tensor
@@ -581,11 +602,13 @@ class MIGTTrainer:
             L.dense_weights_bf16(self._w16_table)
 
     def train_step(self, batch):
-        """(poses [B,T,7], tokens [B,T,h,w]) -> dict(loss, ce_loss, [pose losses], acc, learning_rate) — migt.py:464-505."""
+        """(poses [B,T,7], tokens [B,T,h,w]) -> dict(loss, ce_loss, [pose losses], acc, learning_rate, applied, pending) — migt.py:464-505.
+        The metrics are this micro-batch's; ``applied``: an update ran after it (False inside an accumulation window and on a skipped
+        non-finite bf16 window); ``pending``: micro-batches accumulated and not yet stepped on (0 after every optimizer step)."""
         poses, tokens = batch
         loss = self.forward_backward(poses, tokens)
         lr = self.learning_rate()
-        self.optimizer_step()
+        applied = self.optimizer_step() if self.pending == self.ex.micro_batches else False
         out = {k: float(torch.as_tensor(v, dtype=torch.float32).mean()) for k, v in self.last.items() if k.endswith("loss")}
         out["loss"] = float(loss)
         tok = torch.as_tensor(tokens).to(self.device)
@@ -594,6 +617,7 @@ class MIGTTrainer:
         skip = self.cfg.n_loss_skip
         out["acc"] = float((pred[:, skip:] == tok.reshape(tok.shape[0], tok.shape[1], -1)[:, skip:]).float().mean())
         out["learning_rate"] = lr
+        out["applied"], out["pending"] = bool(applied), self.pending
         if self.bf16:
             out["loss_scale"] = self.loss_scale
         return out

@@ -600,15 +600,21 @@ class VQGAN:
         return L.nhwc_to_nchw(L.gather_rows(self._w["q"]["et"], ids.reshape(-1)).reshape(n, hh, ww, -1))
 
     # ------------------------------------------------------------------ training (Lightning surface, vqgan_th.py:413-445)
-    def configure_optimizers(self, resume_from_checkpoint=None):
+    def configure_optimizers(self, resume_from_checkpoint=None, accumulate_grad_batches=None):
         """The trainer object that owns Adam(betas=(0.5, 0.9), lr=config.learning_rate) and the flat parameter / gradient buffers.
         ``resume_from_checkpoint``: a file written by ``VQGANTrainer.save_checkpoint`` (the reference's --resume-from-checkpoint,
-        train/train_codebook_th.py:29,63): weights, EMA buffers, Adam's moments and step count continue from it."""
+        train/train_codebook_th.py:29,63): weights, EMA buffers, Adam's moments and step count continue from it.
+        ``accumulate_grad_batches``: micro-batches per optimizer step (the reference's option of that name, train_codebook_th.py:30,67;
+        see ``VQGANTrainer``); None keeps the trainer's (1 for a new one)."""
         from .train import VQGANTrainer
         if getattr(self, "_trainer", None) is None:
             if self._w is None and resume_from_checkpoint is not None:
                 self.init_weights()                     # the trainer needs device buffers to restore into
-            self._trainer = VQGANTrainer(self, precision=self.train_precision)
+            self._trainer = VQGANTrainer(self, precision=self.train_precision, accumulate_grad_batches=1 if accumulate_grad_batches is None else accumulate_grad_batches)
+        elif accumulate_grad_batches is not None:
+            if int(accumulate_grad_batches) < 1:
+                raise ValueError(f"accumulate_grad_batches must be >= 1, got {accumulate_grad_batches}")
+            self._trainer.accumulate_grad_batches = int(accumulate_grad_batches)
         if resume_from_checkpoint is not None:
             self._trainer.load_checkpoint(resume_from_checkpoint)
         return self._trainer
