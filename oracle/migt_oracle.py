@@ -190,8 +190,10 @@ def pose_head(sd, cfg, h):
 
 
 def forward(sd, cfg, inputs, compute_losses=False, use_localization=True, localization_weight=1.0):
-    """migt.py:338-455 with training=False.  Returns dict(logits, hidden_states, [pose_prediction], loss...)."""
-    poses = inputs["poses"].to(torch.float32)
+    """migt.py:338-455 with training=False.  Returns dict(logits, hidden_states, [pose_prediction], loss...).  Poses are cast to the
+    weights' dtype (the reference's float32; float64 weights give an fp64 reference end to end)."""
+    dt = sd["wte.weight"].dtype
+    poses = inputs["poses"].to(dt)
     ids = inputs["input_ids"]
     orig_shape = list(ids.shape)
     ids = ids.reshape(ids.shape[0], ids.shape[1], -1)
@@ -216,7 +218,7 @@ def forward(sd, cfg, inputs, compute_losses=False, use_localization=True, locali
     if loc_tokens is not None and loc_emb is None:
         loc_emb = wte[loc_tokens.reshape(loc_tokens.shape[0], loc_tokens.shape[1], -1)]
     if out_poses is not None and out_pose_emb is None:
-        out_pose_emb = mlp(sd, "pose_embedding", pose_model_input(cfg, out_poses.to(torch.float32))).unsqueeze(-2)
+        out_pose_emb = mlp(sd, "pose_embedding", pose_model_input(cfg, out_poses.to(dt))).unsqueeze(-2)
     if use_localization and not compute_losses:
         lp = wte[loc_tok].reshape(1, 1, 1, -1).expand(B, loc_seq, 1, wte.shape[1])
         pose_emb = torch.cat([pose_emb, lp], 1)
@@ -248,7 +250,7 @@ def forward(sd, cfg, inputs, compute_losses=False, use_localization=True, locali
     if use_localization:
         pred, xyz, quat = pose_head(sd, cfg, hs[pose_ptr])
         if compute_losses:
-            y = poses.unsqueeze(-2) * torch.tensor([cfg.pose_multiplier] * 3 + [1.0] * 4)
+            y = poses.unsqueeze(-2) * torch.tensor([cfg.pose_multiplier] * 3 + [1.0] * 4, dtype=dt)
             pl = ((y[..., :3] - xyz) ** 2).mean(-1)[:, cfg.n_loss_skip:].mean((1, 2))
             ol = ((y[..., 3:] - quat) ** 2).mean(-1)[:, cfg.n_loss_skip:].mean((1, 2))
             wkey = "pose_loss_weighting_criterion.pos_ori_weights"

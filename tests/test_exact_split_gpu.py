@@ -21,15 +21,14 @@ import os
 import sys
 from collections import defaultdict
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 from oracle import migt_oracle as mo
 from oracle import synth
-from oracle import vqgan_oracle as vo
 from oracle.make_golden import MIGT_TRAIN, SMALL_VQ, vq_images
+from test_faithful_steps_gpu import faithful_report, step_errors, vq_grads64
 from viewformer_b200.config import MIGTConfig, VQGANConfig
 
 pytestmark = pytest.mark.gpu
@@ -516,27 +515,14 @@ def test_split_operand_window(L, monkeypatch, run):
 
 
 # ----------------------------------------------------------------------------- one step against fp64, and the seed scale
-def _vq_grads64(sd, cfg, x, codes):
-    """Gradient of the codebook loss in fp64 autograd through the oracle, with the quantizer's codes fixed to ``codes``."""
-    leaves = {k: v.double().clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    h = vo._conv(leaves, "quant_conv", vo.encoder(leaves, cfg, x.double()))
-    q = vo.embed_code(leaves["quantize.embeddings"].detach(), codes)
-    diff = (q - h).pow(2).mean()
-    dec = vo.decode(leaves, cfg, h + (q - h).detach())
-    vo.compute_loss(cfg, diff, x.double(), dec).backward()
-    return {k: v.grad for k, v in leaves.items() if v.grad is not None}
-
-
-STEP_FLOOR = 1e-7                 # about 2u: tensors whose error is at rounding level on both paths
-
-
 def test_vqgan_step_gradients_vs_fp64(lib, monkeypatch):
     """One codebook training step (small config, 3 images): every exported gradient against fp64 autograd through the oracle with the
     trainer's codes.  Per tensor, the relative error ||g - g64|| / max(||g64||, 1e-4) of the tensor-core trainer is at most twice that of
-    the same trainer under VF_TRAIN_TC=0, plus STEP_FLOOR.  Measured on an H100 (400 W): median 1.8e-6 (tensor cores) vs 2.6e-6 (CUDA
+    the same trainer under VF_TRAIN_TC=0, plus STEP_FLOOR (1e-7).  Measured on an H100 (400 W): median 1.8e-6 (tensor cores) vs 2.6e-6 (CUDA
     cores), worst 1.1e-4 vs 8.3e-5, largest per-tensor ratio 1.35.  At this size the unscaled seeds (1 / 9216) still leave the split
     operands at 2^-12 or above, and the same numbers (largest ratio 1.49) were measured without the seed scale: the window test, not this
-    one, is what catches the trainers leaving the faithful range."""
+    one, is what catches the trainers leaving the faithful range.  At the sizes where conv_wgrad_tc, its upsampled operand and the wider
+    split convs run, and for the transformer: tests/test_faithful_steps_gpu.py."""
     from viewformer_b200 import VQGAN
     from viewformer_b200.train import VQGANTrainer
     cfg = VQGANConfig(**dict(SMALL_VQ, perceptual_weight=0.0))
@@ -552,17 +538,10 @@ def test_vqgan_step_gradients_vs_fp64(lib, monkeypatch):
         codes = tr.last["codes"].cpu().long()
         key = codes.numpy().tobytes()
         if key not in refs:
-            refs[key] = _vq_grads64(sd, cfg, x, codes)
+            refs[key] = vq_grads64(sd, cfg, x, codes)
         ref = refs[key]
-        grads = tr.export_gradients()
-        errs[tc] = {k: float((grads[k].double() - ref[k]).norm()) / max(float(ref[k].norm()), 1e-4) for k in grads}
-    worst = sorted(((errs["1"][k] - 2 * errs["0"][k]) / max(errs["0"][k], 1e-12), k) for k in errs["1"])[-5:]
-    ratio = sorted((errs["1"][k] / max(errs["0"][k], 1e-12), k) for k in errs["1"])
-    print(f"[vqgan step vs fp64] median rel err: tensor cores {np.median(list(errs['1'].values())):.2e}, CUDA cores "
-          f"{np.median(list(errs['0'].values())):.2e}; worst tensor cores {max(errs['1'].values()):.2e}, CUDA cores {max(errs['0'].values()):.2e}")
-    print("[vqgan step vs fp64] largest err ratios tensor/CUDA cores: " + ", ".join(f"{k} {r:.2f} ({errs['1'][k]:.1e} vs {errs['0'][k]:.1e})"
-                                                                                 for r, k in ratio[-6:]))
-    bad = [k for k in errs["1"] if errs["1"][k] > 2 * errs["0"][k] + STEP_FLOOR]
+        errs[tc] = step_errors(tr.export_gradients(), ref)
+    bad = faithful_report("vqgan step vs fp64", errs)
     assert not bad, "tensor-core gradients less accurate than 2x the CUDA-core trainer's: " + ", ".join(
         f"{k} {errs['1'][k]:.2e} vs {errs['0'][k]:.2e}" for k in bad[:8])
 

@@ -27,6 +27,10 @@ Measured on an H100 80GB HBM3 (700 W power limit), worst ratio to the bar per wo
   bf16 transformer step at scripts/bench_migt_train.py's size (B = 5, T = 20, dropout 0.1; 600 items per stream on 132 CTAs): tc_gemm
       bf16 0.90, attn_multiend_train 0.73, attn_multiend_bwd 0.72, migt_embed_bwd 0.33, gelu_bwd 0.32, dense_wgrad_bf16 0.026.
   fp32 trainers, small: simt_gemm 0.076 / 0.23, dense_wgrad_tc 0.22, conv_wgrad 0.026 / 0.18, tc_gemm split 0.051, tc_conv split 0.0029.
+  fp32 codebook step, medium / full size: sumpool2x2 0.94 / 0.98, simt_conv 0.068 / 0.068, conv_wgrad_tc 0.0026 / 0.020, tc_gemm split
+      0.026 / 0.018, conv_wgrad 0.0050 / 0.054, tc_conv split 8.2e-4 / 8.2e-4, conv3x3_small_cout 2.4e-4 / 2.6e-4.
+  fp32 transformer step, full size: layernorm_bwd 0.56, dense_wgrad_tc 0.52, softmax_rows 0.33, tc_gemm split 0.31, conv_wgrad 0.28,
+      simt_gemm 0.27.
 Normalisation, reduction, optimizer and elementwise wrappers (same card; the 14 workloads and tests/test_norm_stats_gpu.py: about 45 s):
   generate / codec / KV cache: groupnorm 0.996 (bf16 outputs: the output rounding itself), layernorm 0.995 (bf16), gn_mean_rstd 0.15 (fused
       sums of a bf16 output) / 0.0096 (statistics pass), split_f16x2 bit-exact.  Largest GroupNorm mean^2 / var: 1.14.
@@ -39,7 +43,7 @@ Normalisation, reduction, optimizer and elementwise wrappers (same card; the 14 
       0.34, pose_loss_grad 0.29, vq_ema_update 0.25, vq_ema_stats 0.20, pose_postprocess 0.12, cameras_prepare 0.089, vq_prepare_codebook
       0.078, row_mean 0.052, cameras_from_relative 0.037, cross_entropy_rows 0.011, l1_grad 0.011; bit-exact: u8_to_unit, unit_to_u8, the
       layout conversions, gather_rows, vq_split3, vq_prepare_codebook_f16, migt_embed, argmax_rows, image_pair_sums, resize_u8 (evaluation).
-  The whole file (19 workloads) runs in about 55 s.  The largest GroupNorm mean^2 / var above comes from synthetic random-weight models.
+  The whole file ran in about 55 s with 19 workloads; the three fp32 medium and full-size steps add 5 s or less each.  The largest GroupNorm mean^2 / var above comes from synthetic random-weight models.
 """
 import os
 import random
@@ -239,6 +243,9 @@ MIGT_BWD = {("layernorm", "float32"), ("layernorm_bwd", "float32"), ("gelu", "fl
             ("migt_embed_bwd", "float32"), ("col_sums", "float32"), ("lincomb3", "float32")}
 VQ_BF16_STEP = {("tc_conv", "bfloat16"), ("tc_conv", "float16"), ("tc_gemm", "bfloat16"), ("conv_wgrad_bf16", "float32"),
                 ("conv_wgrad_tc", "float32"), ("simt_conv_dgrad_s2", "float32"), ("vq_lookup", "float32")} | VQ_BWD | {("split_f16x2", "float32")}
+VQ_FP32_STEP = {("tc_conv", "float16"), ("conv_wgrad_tc", "float32"), ("conv3x3_small_cout", "float32"), ("conv3x3_small_cin", "float32"),
+                ("simt_conv", "float32"), ("simt_conv_dgrad_s2", "float32"), ("conv_wgrad", "float32"), ("simt_gemm", "float32"),
+                ("sumpool2x2", "float32"), ("vq_lookup", "float32"), ("split_f16x2", "float32")} | VQ_BWD
 
 # workload -> (run, the (wrapper, operand dtype) pairs it is known to reach)
 WORKLOADS = {
@@ -269,6 +276,11 @@ WORKLOADS = {
     "migt-step-fp32-small": (lambda mp, L: _migt_step(MIGT_TRAIN, 2, 4, "fp32", 4600),
                              {("tc_gemm", "float16"), ("simt_gemm", "float32"), ("dense_wgrad_tc", "float32"), ("conv_wgrad", "float32")} | MIGT_BWD
                              | {("softmax_bwd_rows", "float32")}),
+    "vq-step-fp32-medium": (lambda mp, L: _vq_step(MEDIUM_VQ, 4, "fp32", 5600), VQ_FP32_STEP),
+    "vq-step-fp32-full": (lambda mp, L: _vq_step(dict(perceptual_weight=0.0), 2, "fp32", 5700), VQ_FP32_STEP),
+    "migt-step-fp32-full": (lambda mp, L: _migt_step(FULL_MIGT_TRAIN, 1, 5, "fp32", 5800),
+                            {("tc_gemm", "float16"), ("simt_gemm", "float32"), ("dense_wgrad_tc", "float32"), ("conv_wgrad", "float32")} | MIGT_BWD
+                            | {("softmax_bwd_rows", "float32")}),
     "vq-train-fp32-small": (lambda mp, L: _vq_step(dict(SMALL_VQ, perceptual_weight=0.0, gradient_clip_val=0.5), 3, "fp32", 4700, full=True),
                            {("adam", "float32"), ("sumsq", "float32"), ("vq_ema_update", "float32"), ("vq_ema_stats", "float32"),
                             ("softmax_rows", "float32")} | VQ_BWD),
