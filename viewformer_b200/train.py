@@ -44,6 +44,7 @@ import torch
 from . import _lib as L
 from .dist import GradExchange
 from .ops import linear
+from .vqgan import tc_conv_shape_ok
 
 
 _REGISTERED = dict(top=("encoder", "decoder", "quantize", "quant_conv", "post_quant_conv"), mid=("block_1", "attn_1", "block_2"),
@@ -108,6 +109,31 @@ class _P:
         self.name, self.tensor, self.setter, self.kind, self.part, self.cin = name, tensor, setter, kind, part, cin
 
 
+def conv_routes(precision, use_tc, k, cin, cout, stride=1, upsample=False, out=False):
+    """Kernel routes (forward, data gradient, weight gradient) of one conv: "bf16" (single-pass bf16 wgmma), "split" (the exact split-fp16
+    tensor-core kernels) or "cuda" (the fp32 CUDA-core kernels).  ``use_tc``: VF_TRAIN_TC is not 0; ``upsample``: the conv runs on the x2
+    map of its input; ``out``: a conv_out, whose backward pass the bf16 step runs on the fp32 step's kernels."""
+    wgrad_split = "split" if use_tc and k == 3 and stride == 1 and cin % 128 == 0 and cout % 128 == 0 else "cuda"
+    if precision == "fp32":
+        split = "split" if use_tc and k == 3 and stride == 1 and cin % 64 == 0 and cout % 64 == 0 else "cuda"
+        return split, split, wgrad_split
+    fw = "bf16" if tc_conv_shape_ok(k, cin, cout) else "cuda"        # stride 2 on the space-to-depth operand, upsample on the x2 map
+    if out:
+        return fw, "split" if fw == "bf16" else "cuda", wgrad_split
+    if fw == "cuda" or stride == 2:
+        return fw, "cuda", "cuda"
+    return fw, "bf16", "bf16" if cin % 128 == 0 and cout % 128 == 0 else "cuda"
+
+
+class _Conv:
+    """One conv of the step: where it sits, its kernel routes (``conv_routes``: ``VQGANTrainer._route_convs``), its split-fp16 weights."""
+
+    def __init__(self, name, cw, stride, upsample, out):
+        self.name, self.cw, self.stride, self.upsample, self.out = name, cw, stride, upsample, out
+        self.fw = self.dgrad = self.wgrad = None
+        self.split = {}                                 # split-fp16 weights per direction, until the next optimizer step
+
+
 class VQGANTrainer:
     _seed_scale = 1.0                                   # the gradient-seed scale of the running step (see grad_seed_scale)
 
@@ -137,12 +163,12 @@ class VQGANTrainer:
         self.betas, self.eps, self.step_count = betas, eps, 0
         self.group = process_group
         self.bucket_bytes = bucket_bytes
+        self.use_tc = os.environ.get("VF_TRAIN_TC", "1") != "0"
+        self.precision, self.bf16 = precision, precision == "bf16"
         self._collect_params()
+        self._route_convs()
         self._flatten()
         self.last = {}
-        self.use_tc = os.environ.get("VF_TRAIN_TC", "1") != "0"
-        self._wsplit = {}
-        self.precision, self.bf16 = precision, precision == "bf16"
         # gradient-seed scale: None = 2^round(log2(numel of the reconstruction)), which brings the loss seeds (1 / numel) to about 1 so that
         # the backward operands sit inside the split-fp16 tensor-core path's faithful range; a number = that fixed power of two (1 = off)
         self.grad_seed_scale = 1.0 if self.bf16 else None
@@ -151,14 +177,14 @@ class VQGANTrainer:
 
     # ------------------------------------------------------------------ parameter registry
     def _collect_params(self):
-        """The trainable tensors in the order of the model's layout: encoder, quantizer block, decoder."""
+        """The trainable tensors in the order of the model's layout: encoder, quantizer block, decoder; a record per conv."""
         w = self.model._w
-        ps, self._convs = [], []
+        ps, self.convs = [], {}
 
-        def conv(name, cw, stride=1):
+        def conv(name, cw, stride=1, upsample=False, out=False):
             if not hasattr(cw, "w_kn"):
                 raise RuntimeError(f"{name}: tensor-core weight layout in an fp32 model")
-            self._convs.append((cw, stride))
+            self.convs[name] = _Conv(name, cw, stride, upsample, out)
             ps.append(_P(name + ".weight", cw.w_kn, lambda t, cw=cw: setattr(cw, "w_kn", t), "conv", cin=cw.cin))
             ps.append(_P(name + ".bias", cw.bias, lambda t, cw=cw: setattr(cw, "bias", t), "vec"))
 
@@ -182,9 +208,9 @@ class VQGANTrainer:
                     lin(n + ".qk", sw["qk"], parts=(n + ".q", n + ".k"))
                     lin(n + ".v", sw["v"]); lin(n + ".proj_out", sw["proj"])
                 elif st.kind == "out":
-                    norm(n + ".norm_out", sw, "norm"); conv(n + ".conv_out", sw["conv"])
+                    norm(n + ".norm_out", sw, "norm"); conv(n + ".conv_out", sw["conv"], out=True)
                 else:
-                    conv(n, sw, st.stride)
+                    conv(n, sw, st.stride, st.upsample)
 
         stages(w["enc"])
         lin("quant_conv", w["quant_conv"])
@@ -194,6 +220,12 @@ class VQGANTrainer:
         lin("post_quant_conv", w["post_quant_conv"])
         stages(w["dec"])
         self.params = ps
+
+    def _route_convs(self):
+        """Each conv's kernel routes under this trainer's precision and VF_TRAIN_TC."""
+        for c in self.convs.values():
+            cw = c.cw
+            c.fw, c.dgrad, c.wgrad = conv_routes(self.precision, self.use_tc, cw.k, cw.cin, cw.cout, c.stride, c.upsample, c.out)
 
     def _flatten(self):
         """Re-home every parameter in the flat buffers of the gradient exchange, in BACKWARD order (decoder.conv_out first)."""
@@ -212,15 +244,19 @@ class VQGANTrainer:
         rewritten from the fp32 master weights in the flat buffer by one launch per step (``_refresh_bf16_weights``)."""
         dev = self.model.device
         self._wb16, entries = {}, []
-        for cw, stride in self._convs:
-            if not self._tc_ok(cw, stride, False):
-                continue
+        for c in [c for c in self.convs.values() if c.fw == "bf16"]:
+            cw = c.cw
             fw = torch.empty((cw.cout, 9 * cw.cin), dtype=torch.bfloat16, device=dev)
-            bw = torch.empty((cw.cin, 9 * cw.cout), dtype=torch.bfloat16, device=dev) if stride == 1 else None
+            bw = torch.empty((cw.cin, 9 * cw.cout), dtype=torch.bfloat16, device=dev) if c.stride == 1 else None
             self._wb16[id(cw)] = (fw, bw)
             entries.append((cw.w_kn, fw, bw))
         self._wb16_table = L.conv_weights_bf16_table(entries, dev)
         self._refresh_bf16_weights()
+
+    @property
+    def _convs(self):
+        """(weights, stride) of every conv, in registration order."""
+        return [(c.cw, c.stride) for c in self.convs.values()]
 
     def _refresh_bf16_weights(self):
         L.conv_weights_bf16(self._wb16_table)
@@ -229,30 +265,23 @@ class VQGANTrainer:
     def _gn_apply(self, x, st, nw, swish, dtype=torch.float32):
         return L.groupnorm(x, nw[0], nw[1], swish=swish, out_dtype=dtype, stats=st)
 
-    def _act(self, x, st, nw, swish, cw):
-        """GroupNorm(+swish) of x as the operand of conv ``cw``: bf16 when the bf16 step runs that conv on the tensor cores, else fp32."""
-        return self._gn_apply(x, st, nw, swish, torch.bfloat16 if self.bf16 and self._tc_ok(cw, 1, False) else torch.float32)
+    def _act(self, x, st, nw, swish, c):
+        """GroupNorm(+swish) of x as the operand of conv ``c``: bf16 when its forward pass runs on bf16 wgmma, else fp32."""
+        return self._gn_apply(x, st, nw, swish, torch.bfloat16 if c.fw == "bf16" else torch.float32)
 
-    # 3x3 stride-1 convolutions whose channel counts fit the tensor-core tiles run on the EXACT split-fp16 tensor-core path (three fp16 MMA
-    # passes, chunked accumulation: fp32-faithful results, DESIGN.md 5.3) in the forward pass and in the data gradient; everything else
-    # (conv_in / conv_out, stride-2 and upsampling convs, 1x1 layers) and every weight gradient stays on the fp32 CUDA-core kernels.
-    def _tc_ok(self, cw, stride, upsample):
-        """3x3 stride-1 convs, incl. the Upsample convs (nearest x2, then a stride-1 conv on the doubled map: vqgan_th.py:29-32).
-        bf16 step: the convs a bf16-built model runs on the tensor cores (_Conv3.tc), stride-2 ones included."""
-        if self.bf16:
-            return cw.k == 3 and cw.cin % 64 == 0 and cw.cout % 16 == 0 and cw.cout >= 64
-        return self.use_tc and cw.k == 3 and stride == 1 and cw.cin % 64 == 0 and cw.cout % 64 == 0
+    @staticmethod
+    def _dgrad_weight(cw, flip=True):
+        """The weights of the conv that computes the data gradient: [tap * Cout, Cin], taps flipped (a stride-2 conv's gather form: not)."""
+        wk = cw.w_kn.reshape(cw.k, cw.k, cw.cin, cw.cout)
+        return (wk.flip(0, 1) if flip else wk).permute(0, 1, 3, 2).reshape(cw.k * cw.k * cw.cout, cw.cin).contiguous()
 
-    def _split_weight(self, key, w_kn, n_out):
-        """[K, n_out] fp32 (K = tap * C + c) -> split-fp16 [n_out, tap * 2C] for L.tc_conv; cached until the next optimizer step."""
-        hit = self._wsplit.get(key)
-        if hit is None:
-            k = w_kn.shape[0]
-            c = k // 9
-            w_nk = w_kn.t().contiguous()                                        # [n_out, 9 * C]
-            hit = L.split_f16x2(w_nk.reshape(n_out * 9, c)).reshape(n_out, 9 * 2 * c)
-            self._wsplit[key] = hit
-        return hit
+    @classmethod
+    def _split_weight(cls, c, direction):
+        """Split-fp16 weights [n_out, tap * 2C] for L.tc_conv, forward ("fw") or data gradient ("bw"); cached until the next optimizer step."""
+        if direction not in c.split:
+            w_nk = (c.cw.w_kn if direction == "fw" else cls._dgrad_weight(c.cw)).t().contiguous()          # [n_out, 9 * C]
+            c.split[direction] = L.split_f16x2(w_nk.reshape(w_nk.shape[0] * 9, -1)).reshape(w_nk.shape[0], -1)
+        return c.split[direction]
 
     @staticmethod
     def _split_act(x):
@@ -265,70 +294,50 @@ class VQGANTrainer:
         hit = getattr(t, "_bf16", None)
         return hit if hit is not None else L.groupnorm(t, None, None, swish=False, out_dtype=torch.bfloat16, normalize=False)
 
-    def _conv_fw(self, cw, a, residual=None, stride=1, upsample=False):
-        if self.bf16 and self._tc_ok(cw, stride, upsample):
-            fw = self._wb16[id(cw)][0]
-            if stride == 2:                                     # space-to-depth operand: a stride-1 tap-table conv (as the bf16 model)
+    def _conv_fw(self, c, a, residual=None):
+        cw = c.cw
+        if c.fw == "bf16":
+            if c.stride == 2:                                   # space-to-depth operand: a stride-1 tap-table conv (as the bf16 model)
                 a16 = L.groupnorm(a, None, None, swish=False, out_dtype=torch.bfloat16, normalize=False, s2d=True)
-                return L.tc_conv(a16, fw, cw.bias, taps=L.TAPS_S2D, coffs=L.s2d_coffs(cw.cin), cin=cw.cin)
-            if upsample or a.dtype != torch.bfloat16:
-                a = L.groupnorm(a, None, None, swish=False, out_dtype=torch.bfloat16, normalize=False, upsample=upsample)
-            return L.tc_conv(a, fw, cw.bias, residual=residual)
-        if self._tc_ok(cw, stride, upsample):
-            a_split = (L.groupnorm(a, None, None, swish=False, out_dtype=torch.float16, normalize=False, upsample=True) if upsample
+                return L.tc_conv(a16, self._wb16[id(cw)][0], cw.bias, taps=L.TAPS_S2D, coffs=L.s2d_coffs(cw.cin), cin=cw.cin)
+            if c.upsample or a.dtype != torch.bfloat16:
+                a = L.groupnorm(a, None, None, swish=False, out_dtype=torch.bfloat16, normalize=False, upsample=c.upsample)
+            return L.tc_conv(a, self._wb16[id(cw)][0], cw.bias, residual=residual)
+        if c.fw == "split":                                     # upsample: the split operand of the materialised x2 map
+            a_split = (L.groupnorm(a, None, None, swish=False, out_dtype=torch.float16, normalize=False, upsample=True) if c.upsample
                        else self._split_act(a))
-            return L.tc_conv(a_split, self._split_weight(("fw", id(cw)), cw.w_kn, cw.cout), cw.bias, residual=residual)
-        return self.model._conv(cw, a, residual=residual, stride=stride, upsample=upsample, stats=False)
+            return L.tc_conv(a_split, self._split_weight(c, "fw"), cw.bias, residual=residual)
+        return self.model._conv(cw, a, residual=residual, stride=c.stride, upsample=c.upsample, stats=False)
 
-    def _conv_bw(self, name, cw, a, dy, stride=1, upsample=False, need_dx=True):
-        """a: the conv's input (NHWC f32); dy: gradient of its output.  Accumulates dW, db; returns dx (or None)."""
-        G = self.ex.g
-        pad = ((1, 1) if stride == 1 else (0, 0)) if cw.k == 3 else (0, 0)
-        if self.use_tc and upsample and L.conv_wgrad_tc_ok(dy, dy, cw.k, stride, False) and cw.cin % 128 == 0:
-            a_up = L.groupnorm(a, None, None, swish=False, out_dtype=torch.float32, normalize=False, upsample=True)
-            L.conv_wgrad_tc(a_up, dy, G[name + ".weight"])
-        elif self.use_tc and L.conv_wgrad_tc_ok(a, dy, cw.k, stride, upsample):
-            L.conv_wgrad_tc(a, dy, G[name + ".weight"])             # exact split-fp16 GEMMs over the pixel axis (K = pixels)
+    def _conv_bw(self, dy, c, x, norm=None, need_dx=True):
+        """x: the conv's fp32 input before ``norm`` = (mean_rstd, (gamma, beta), swish) and the x2 upsample; dy: its output's gradient.
+        Accumulates dW, db; returns dx (or None).  The bf16 weight gradient applies the norm on the way; other routes get a norm pass first."""
+        G, cw = self.ex.g, c.cw
+        gw = G[c.name + ".weight"]
+        if c.wgrad == "bf16":
+            L.conv_wgrad_bf16(x, dy, gw, norm=None if norm is None else (norm[0], norm[1][0], norm[1][1], norm[2]), upsample=c.upsample)
         else:
-            L.conv_wgrad(a, dy, G[name + ".weight"], kh=cw.k, stride=stride, pad=pad, upsample=upsample)
-        L.col_sums(dy.reshape(-1, cw.cout), G[name + ".bias"])
-        self.ex.ready(name + ".bias", name + ".weight")
+            a = x if norm is None else self._gn_apply(x, *norm)
+            if c.wgrad == "split":                              # exact split-fp16 GEMMs over the pixel axis (K = pixels)
+                if c.upsample:
+                    a = L.groupnorm(a, None, None, swish=False, out_dtype=torch.float32, normalize=False, upsample=True)
+                L.conv_wgrad_tc(a, dy, gw)
+            else:
+                L.conv_wgrad(a, dy, gw, kh=cw.k, stride=c.stride, pad=(1, 1) if cw.k == 3 and c.stride == 1 else (0, 0), upsample=c.upsample)
+        L.col_sums(dy.reshape(-1, cw.cout), G[c.name + ".bias"])
+        self.ex.ready(c.name + ".bias", c.name + ".weight")
         if not need_dx:
             return None
-        wk = cw.w_kn.reshape(cw.k, cw.k, cw.cin, cw.cout)
-        if stride == 2:                                         # Downsample: gather form, taps not flipped
-            wd = wk.permute(0, 1, 3, 2).reshape(cw.k * cw.k * cw.cout, cw.cin).contiguous()
-            return L.simt_conv_dgrad_s2(dy, wd, (a.shape[1], a.shape[2]))
-        if self._tc_ok(cw, stride, upsample):
-            key = ("bw", id(cw))
-            if key not in self._wsplit:                         # a data gradient is a conv with flipped taps and swapped channel roles
-                wd = wk.flip(0, 1).permute(0, 1, 3, 2).reshape(cw.k * cw.k * cw.cout, cw.cin).contiguous()
-                self._split_weight(key, wd, cw.cin)
-            dx = L.tc_conv(self._split_act(dy), self._wsplit[key], None)
-            return L.sumpool2x2(dx) if upsample else dx
-        wd = wk.flip(0, 1).permute(0, 1, 3, 2).reshape(cw.k * cw.k * cw.cout, cw.cin).contiguous()      # a data gradient is a conv with flipped taps
-        dx = L.simt_conv(dy, wd, None, kh=cw.k, stride=1, pad=(1, 1) if cw.k == 3 else (0, 0))
-        return L.sumpool2x2(dx) if upsample else dx
-
-    def _conv_bw16(self, name, cw, x, dy, norm=None, stride=1, upsample=False, need_dx=True):
-        """bf16 step.  x: the conv's fp32 input BEFORE ``norm`` = (mean_rstd, (gamma, beta), swish) and before the x2 upsample; dy fp32.
-        Accumulates dW, db; returns dx (or None)."""
-        if stride == 2 or not self._tc_ok(cw, stride, upsample):     # the fp32 step's kernels
-            a = x if norm is None else self._gn_apply(x, norm[0], norm[1], norm[2])
-            return self._conv_bw(name, cw, a, dy, stride=stride, upsample=upsample, need_dx=need_dx)
-        G = self.ex.g
-        gw = G[name + ".weight"]
-        if L.conv_wgrad_bf16_ok(x, dy, cw.k, stride, upsample):
-            L.conv_wgrad_bf16(x, dy, gw, norm=None if norm is None else (norm[0], norm[1][0], norm[1][1], norm[2]), upsample=upsample)
+        if c.dgrad == "bf16":
+            dx = L.tc_conv(self._b16(dy), self._wb16[id(cw)][1], None)
+        elif c.dgrad == "split":                                # a data gradient is a conv with flipped taps and swapped channel roles
+            wd = self._split_weight(c, "bw")
+            dx = L.tc_conv(self._split_act(dy), wd, None)
+        elif c.stride == 2:                                     # Downsample: gather form, taps not flipped
+            return L.simt_conv_dgrad_s2(dy, self._dgrad_weight(cw, flip=False), (x.shape[1], x.shape[2]))
         else:
-            a = x if norm is None else self._gn_apply(x, norm[0], norm[1], norm[2])
-            L.conv_wgrad(a, dy, gw, kh=cw.k, stride=1, pad=(1, 1), upsample=upsample)
-        L.col_sums(dy.reshape(-1, cw.cout), G[name + ".bias"])
-        self.ex.ready(name + ".bias", name + ".weight")
-        if not need_dx:
-            return None
-        dx = L.tc_conv(self._b16(dy), self._wb16[id(cw)][1], None)
-        return L.sumpool2x2(dx) if upsample else dx
+            dx = L.simt_conv(dy, self._dgrad_weight(cw), None, kh=cw.k, stride=1, pad=(1, 1) if cw.k == 3 else (0, 0))
+        return L.sumpool2x2(dx) if c.upsample else dx
 
     def _lin_bw(self, name, ln, x_rows, dy_rows, residual=None):
         """y = x W^T + b.  Accumulates dW [out,in], db; returns dx = dy W (+ residual)."""
@@ -344,31 +353,24 @@ class VQGANTrainer:
     # ------------------------------------------------------------------ blocks
     def _res_fw(self, stage, r, x, tape):
         ex = self.model.exact
+        c1, c2 = self.convs[stage.name + ".conv1"], self.convs[stage.name + ".conv2"]
         st1 = L.gn_mean_rstd(x)
-        h = self._conv_fw(r["c1"], self._act(x, st1, r["n1"], True, r["c1"]))
+        h = self._conv_fw(c1, self._act(x, st1, r["n1"], True, c1))
         st2 = L.gn_mean_rstd(h)
-        a2 = self._act(h, st2, r["n2"], True, r["c2"])
+        a2 = self._act(h, st2, r["n2"], True, c2)
         n, hh, ww, c = x.shape
         res = linear(ex, x.reshape(-1, c), r["sc"], torch.float32).reshape(n, hh, ww, -1) if "sc" in r else x
-        y = self._conv_fw(r["c2"], a2, residual=res)
+        y = self._conv_fw(c2, a2, residual=res)
         tape.append((self._res_bw, stage, r, x, st1, h, st2))
         return y
 
     def _res_bw(self, dy, stage, r, x, st1, h, st2):
         name, G = stage.name, self.ex.g
-        if self.bf16:
-            da2 = self._conv_bw16(name + ".conv2", r["c2"], h, dy, norm=(st2, r["n2"], True))
-        else:
-            a2 = self._gn_apply(h, st2, r["n2"], True)
-            da2 = self._conv_bw(name + ".conv2", r["c2"], a2, dy)
+        da2 = self._conv_bw(dy, self.convs[name + ".conv2"], h, norm=(st2, r["n2"], True))
         dh = L.groupnorm_bwd(h, da2, st2, r["n2"][0], r["n2"][1], G[name + ".norm2.weight"], G[name + ".norm2.bias"], swish=True,
                              out_bf16=self.bf16)
         self.ex.ready(name + ".norm2.bias", name + ".norm2.weight")
-        if self.bf16:
-            da1 = self._conv_bw16(name + ".conv1", r["c1"], x, dh, norm=(st1, r["n1"], True))
-        else:
-            a1 = self._gn_apply(x, st1, r["n1"], True)
-            da1 = self._conv_bw(name + ".conv1", r["c1"], a1, dh)
+        da1 = self._conv_bw(dh, self.convs[name + ".conv1"], x, norm=(st1, r["n1"], True))
         n, hh, ww, c = x.shape
         if "sc" in r:
             dres = self._lin_bw(name + ".nin_shortcut", r["sc"], x.reshape(-1, c), dy.reshape(-1, dy.shape[-1])).reshape(x.shape)
@@ -482,20 +484,17 @@ class VQGANTrainer:
                 ms = L.gn_mean_rstd(h)
                 a = self._gn_apply(h, ms, sw["norm"], True)
                 tape.append((self._out_bw, st, sw, h, ms))
-                h = self._conv_fw(sw["conv"], a)
+                h = self._conv_fw(self.convs[st.name + ".conv_out"], a)
             else:                                                  # the first stage's input is the image: it needs no data gradient
-                tape.append((self._conv_stage_bw, st, sw, h, bool(tape)))
-                h = self._conv_fw(sw, h, stride=st.stride, upsample=st.upsample)
+                c = self.convs[st.name]
+                tape.append((self._conv_bw, c, h, None, bool(tape)))
+                h = self._conv_fw(c, h)
         return h
 
-    def _conv_stage_bw(self, dy, stage, cw, x, need_dx):
-        conv_bw = self._conv_bw16 if self.bf16 else self._conv_bw
-        return conv_bw(stage.name, cw, x, dy, stride=stage.stride, upsample=stage.upsample, need_dx=need_dx)
-
     def _out_bw(self, dy, stage, sw, x, ms):
-        """norm_out + swish + conv_out (conv_out on the fp32 step's kernels in both precisions)."""
+        """norm_out + swish + conv_out (conv_out's backward pass on the fp32 step's kernels in both precisions)."""
         n, G, nw = stage.name, self.ex.g, sw["norm"]
-        da = self._conv_bw(n + ".conv_out", sw["conv"], self._gn_apply(x, ms, nw, True), dy)
+        da = self._conv_bw(dy, self.convs[n + ".conv_out"], x, norm=(ms, nw, True))
         dx = L.groupnorm_bwd(x, da, ms, nw[0], nw[1], G[n + ".norm_out.weight"], G[n + ".norm_out.bias"], swish=True, out_bf16=self.bf16)
         self.ex.ready(n + ".norm_out.bias", n + ".norm_out.weight")
         return dx
@@ -537,7 +536,8 @@ class VQGANTrainer:
 
     def _weights_changed(self):
         """flat_p has new values: everything derived from it is rebuilt."""
-        self._wsplit = {}                               # split-fp16 operand copies of the conv weights are stale now
+        for c in self.convs.values():                   # split-fp16 operand copies of the conv weights are stale now
+            c.split.clear()
         if self.bf16:
             self._refresh_bf16_weights()
         if self.model.quantizer == "commit":

@@ -51,6 +51,22 @@ def warmup_cosine(step, init, warm, total_steps, offset=0):
     return init * 0.5 * (1.0 + math.cos(math.pi * t))
 
 
+def dense_route(precision, use_tc, k, n):
+    """Kernel route of a dense layer x [m, k] W [k, n] (forward, data and weight gradient alike): "bf16" (single-pass bf16 wgmma), "split"
+    (the exact split-fp16 tensor-core GEMM) or "cuda" (fp32 CUDA-core kernels).  ``use_tc``: the bf16 step, or VF_TRAIN_TC is not 0."""
+    if not use_tc or k % 128 or n % 128:
+        return "cuda"
+    return "bf16" if precision == "bf16" else "split"
+
+
+class _Dense:
+    """One dense layer y = x W (+ b): views of W [k, n], b and their gradients (no b: the tied head), its route and split-fp16 copies."""
+
+    def __init__(self, name, w, gw, b, gb, route):
+        self.name, self.w, self.gw, self.b, self.gb, self.route = name, w, gw, b, gb, route
+        self.split = {}                                            # split-fp16 weights per product, until the next optimizer step
+
+
 class MIGTTrainer:
     LOSS_SCALE_INIT = 2.0 ** 15                                    # tf.mixed_precision DynamicLossScale defaults (TF 2.4)
     LOSS_SCALE_GROWTH_STEPS = 2000
@@ -100,12 +116,12 @@ class MIGTTrainer:
         self.schedule_offset = 0                                   # WarmUp.offset (models/utils.py:342-346): the schedule runs on iterations - offset
         self._train_counter_base = 0                               # see train_counter
         self.use_tc = self.bf16 or os.environ.get("VF_TRAIN_TC", "1") != "0"
-        self._wsplit = {}                                          # split-fp16 operand copies of the weights, rebuilt after every step
         self.use_loc = model.use_localization
         from .schedules import parse
         self._loc_schedule = parse(cfg.localization_weight).with_total_steps(int(cfg.total_steps))
         self.dynamic_pose = bool(cfg.use_dynamic_pose_loss) and self.use_loc
         self._build(model.state_dict())
+        self._build_dense()
         if self.bf16:
             self._build_bf16_weights()
 
@@ -144,27 +160,31 @@ class MIGTTrainer:
         # AdamWeightDecay: every variable except the ones whose name contains "bias" (see the module docstring)
         self.decay = {k: ("bias" not in k) for k in order}
 
+    def _build_dense(self):
+        """One record per dense layer, in backward-completion order, with its kernel route; the tied head last."""
+        self.dense = {}
+        for k in self.order:
+            if k.endswith(".weight") and k != "wte.weight" and self.p[k].dim() == 2:
+                name, b = k[:-len(".weight")], k[:-len("weight")] + "bias"
+                route = dense_route(self.precision, self.use_tc, *self.p[k].shape)
+                self.dense[name] = _Dense(name, self.p[k], self.g[k], self.p[b].reshape(-1), self.g[b].reshape(-1), route)
+        # the tied LM head (migt.py:417) is the bias-free layer W = wte[:V] (in V, out d), used transposed: logits are its data-gradient
+        # product on ln_f's output, whose gradient is its forward product on the logits' gradient
+        V = self.cfg.n_embeddings
+        head = self.p["wte.weight"][:V]
+        self.dense["wte"] = _Dense("wte", head, self.g["wte.weight"][:V], None, None, dense_route(self.precision, self.use_tc, *head.shape))
+
     def _build_bf16_weights(self):
-        """bf16 operand copies of every tensor-core dense layer: fw [n, k] (forward, K = k) and bw [k, n] (data gradient, K = n); rewritten
-        from the fp32 master weights by one vf_dense_weights_bf16 launch after every applied step.  The tied head uses wte[:V] as its
-        [k, n] = [V, d] matrix (logits read bw, the data gradient reads fw)."""
+        """bf16 operand copies of every bf16 dense layer's weights: forward [n, k] (K = k) and data gradient [k, n] (K = n); rewritten from
+        the fp32 master weights by one vf_dense_weights_bf16 launch after every applied step."""
         self._w16, entries = {}, []
-        for name in self.order:
-            if not name.endswith(".weight") or name.startswith("wte") or self.p[name].dim() != 2:
-                continue
-            k, n = self.p[name].shape
-            if self._tc_dense_ok(k, n):
-                layer = name[:-len(".weight")]
+        for r in self.dense.values():
+            if r.route == "bf16":
+                k, n = r.w.shape
                 fw = torch.empty((n, k), dtype=torch.bfloat16, device=self.device)
                 bw = torch.empty((k, n), dtype=torch.bfloat16, device=self.device)
-                self._w16[layer] = (fw, bw)
-                entries.append((self.p[name], fw, bw))
-        V, d = self.cfg.n_embeddings, self.cfg.d_model
-        if self._tc_dense_ok(d, V):
-            fw = torch.empty((d, V), dtype=torch.bfloat16, device=self.device)
-            bw = torch.empty((V, d), dtype=torch.bfloat16, device=self.device)
-            self._w16["wte"] = (fw, bw)
-            entries.append((self.p["wte.weight"][:V], fw, bw))
+                self._w16[r.name] = (fw, bw)
+                entries.append((r.w, fw, bw))
         self._w16_table = L.dense_weights_bf16_table(entries, self.device)
         L.dense_weights_bf16(self._w16_table)
 
@@ -231,70 +251,64 @@ class MIGTTrainer:
     # ------------------------------------------------------------------ dense layer (Conv1D: x @ W[in,out] + b[1,out])
     # Dense layers whose sizes fit the tensor-core tiles run forward, data gradient and weight gradient on the exact split-fp16 GEMM
     # (fp32-faithful: three fp16 MMA passes, chunked accumulation — DESIGN.md 5.3); VF_TRAIN_TC=0 keeps everything on the CUDA cores.
-    def _tc_dense_ok(self, k, n):
-        return self.use_tc and k % 128 == 0 and n % 128 == 0
-
-    def _wsplit_get(self, key, make):
-        hit = self._wsplit.get(key)
-        if hit is None:
-            hit = self._wsplit[key] = L.split_f16x2(make())
-        return hit
-
-    def _dense_fw_tc(self, x, W_nk_key, W_nk_make, n, k, bias=None, residual=None):
-        """x [M, k] fp32 @ W^T with W given K-major ([n, k]) -> [M, n] fp32."""
+    def _split_gemm(self, x, r, product, n, k, bias=None, residual=None):
+        """x [M, k] fp32 times layer r's weights on the exact split-fp16 GEMM -> [M, n] fp32: its forward ("fw", x W) or data-gradient
+        ("bw", x W^T) product."""
         out = torch.empty((x.shape[0], n), dtype=torch.float32, device=x.device)
-        L.tc_gemm(L.split_f16x2(x), self._wsplit_get(W_nk_key, W_nk_make), out, M=x.shape[0], N=n, K=k, lda=2 * k, ldb=2 * k, ldc=n,
-                  bias=bias, bias_mode=L.BIAS_N if bias is not None else L.BIAS_NONE, residual=residual, lo_a=k, lo_b=k)
+        xs = L.split_f16x2(x)
+        ws = r.split.get(product)
+        if ws is None:                          # K-major weights: W^T for the forward product, W [k, n] itself for the data gradient
+            ws = r.split[product] = L.split_f16x2(r.w.t().contiguous() if product == "fw" else r.w.contiguous())
+        L.tc_gemm(xs, ws, out, M=x.shape[0], N=n, K=k, lda=2 * k, ldb=2 * k, ldc=n, bias=bias,
+                  bias_mode=L.BIAS_N if bias is not None else L.BIAS_NONE, residual=residual, lo_a=k, lo_b=k)
         return out
 
-    def _lin(self, x, name, act=L.ACT_NONE, residual=None):
-        W, b = self.p[name + ".weight"], self.p[name + ".bias"]
-        k, n = W.shape
-        if self.bf16 and act == L.ACT_NONE and self._tc_dense_ok(k, n):
-            x16 = x if x.dtype == torch.bfloat16 else L.to_bf16(x)
-            out = torch.empty((x.shape[0], n), dtype=torch.float32, device=x.device)
-            L.tc_gemm(x16, self._w16[name][0], out, M=x.shape[0], N=n, K=k, lda=k, ldb=k, ldc=n, bias=b.reshape(-1), bias_mode=L.BIAS_N,
-                      residual=residual)
-            return out
-        if act == L.ACT_NONE and self._tc_dense_ok(k, n):
-            return self._dense_fw_tc(x, ("fw", name), lambda: W.t().contiguous(), n, k, bias=b.reshape(-1), residual=residual)
+    def _lin(self, x, name, residual=None):
+        """The forward product x W (+ b) (+ residual) [m, n] fp32."""
+        r = self.dense[name]
+        k, n = r.w.shape
+        if r.route == "split":
+            return self._split_gemm(x, r, "fw", n, k, bias=r.b, residual=residual)
+        bias_mode = L.BIAS_N if r.b is not None else L.BIAS_NONE
         out = torch.empty((x.shape[0], n), dtype=torch.float32, device=x.device)
-        L.simt_gemm(x, W, out, M=x.shape[0], N=n, K=k, a_strides=(k, 1), b_strides=(n, 1), ldc=n, bias=b.reshape(-1), bias_mode=L.BIAS_N,
-                    act=act, residual=residual)
+        if r.route == "bf16":
+            L.tc_gemm(x if x.dtype == torch.bfloat16 else L.to_bf16(x), self._w16[name][0], out, M=x.shape[0], N=n, K=k, lda=k, ldb=k, ldc=n,
+                      bias=r.b, bias_mode=bias_mode, residual=residual)
+        else:
+            L.simt_gemm(x, r.w, out, M=x.shape[0], N=n, K=k, a_strides=(k, 1), b_strides=(n, 1), ldc=n, bias=r.b, bias_mode=bias_mode,
+                        residual=residual)
         return out
 
-    def _dgrad16(self, dy, name, residual=None, out16=None):
-        """bf16 data gradient dx = dy W^T [m, k] fp32 (or, with out16, written as bf16 only)."""
-        k, n = self.p[name + ".weight"].shape
+    def _dgrad(self, dy, name, residual=None, out16=None):
+        """The data-gradient product dx = dy W^T (+ residual) [m, k] fp32 (bf16 route with ``out16``: written as bf16 only)."""
+        r = self.dense[name]
+        k, n = r.w.shape
         m = dy.shape[0]
-        dx = out16 if out16 is not None else torch.empty((m, k), dtype=torch.float32, device=dy.device)
-        L.tc_gemm(L.to_bf16(dy), self._w16[name][1], dx, M=m, N=k, K=n, lda=n, ldb=n, ldc=k, residual=residual)
+        if r.route == "split":
+            return self._split_gemm(dy, r, "bw", k, n, residual=residual)
+        dx = out16 if out16 is not None and r.route == "bf16" else torch.empty((m, k), dtype=torch.float32, device=dy.device)
+        if r.route == "bf16":
+            L.tc_gemm(L.to_bf16(dy), self._w16[name][1], dx, M=m, N=k, K=n, lda=n, ldb=n, ldc=k, residual=residual)
+        else:
+            L.simt_gemm(dy, r.w, dx, M=m, N=k, K=n, a_strides=(n, 1), b_strides=(1, n), ldc=k, residual=residual)
         return dx
 
     def _lin_bw(self, x, dy, name, *, need_dx=True, residual=None, last=True, out16=None):
-        """Accumulates dW, db of x @ W + b and returns dx = dy W^T (+ residual).  A layer applied to every stream is called once per stream:
-        the weight-gradient kernels accumulate, and readiness is signalled on the ``last`` call.  bf16: ``out16`` receives dx as bf16 only
-        (the attention backward's dO operand)."""
-        W = self.p[name + ".weight"]
-        k, n = W.shape
+        """Accumulates dW (and db) of x W (+ b) and returns dx = dy W^T (+ residual).  A layer applied to every stream is called once per
+        stream: the weight-gradient kernels accumulate, and readiness is signalled on the ``last`` call.  bf16: ``out16`` receives dx as
+        bf16 only (the attention backward's dO operand)."""
+        r = self.dense[name]
+        k, n = r.w.shape
         m = x.shape[0]
-        tc = self._tc_dense_ok(k, n)
-        if tc:
-            (L.dense_wgrad_bf16 if self.bf16 else L.dense_wgrad_tc)(x, dy, self.g[name + ".weight"])
+        if r.route == "cuda":
+            L.conv_wgrad(x.reshape(1, m, 1, k), dy.reshape(1, m, 1, n), r.gw, kh=1, pad=(0, 0), so=(n, 1))
         else:
-            L.conv_wgrad(x.reshape(1, m, 1, k), dy.reshape(1, m, 1, n), self.g[name + ".weight"], kh=1, pad=(0, 0), so=(n, 1))
-        L.col_sums(dy, self.g[name + ".bias"].reshape(-1))
+            (L.dense_wgrad_bf16 if r.route == "bf16" else L.dense_wgrad_tc)(x, dy, r.gw)
+        if r.b is not None:
+            L.col_sums(dy, r.gb)
         if last:
             self.ex.ready(name + ".bias", name + ".weight")
-        if not need_dx:
-            return None
-        if tc and self.bf16:
-            return self._dgrad16(dy, name, residual=residual, out16=out16)
-        if tc:                                  # dx = dy W^T: W [k, n] is already K-major for this product
-            return self._dense_fw_tc(dy, ("bw", name), lambda: W.contiguous(), k, n, residual=residual)
-        dx = torch.empty((m, k), dtype=torch.float32, device=x.device)
-        L.simt_gemm(dy, W, dx, M=m, N=k, K=n, a_strides=(n, 1), b_strides=(1, n), ldc=k, residual=residual)
-        return dx
+        return self._dgrad(dy, name, residual=residual, out16=out16) if need_dx else None
 
     def _ln(self, x, name, dtype=torch.float32):
         return L.layernorm(x, self.p[name + ".gamma"], self.p[name + ".beta"], dtype, eps=LN_EPS)
@@ -371,7 +385,7 @@ class MIGTTrainer:
         training forward per stream.  Returns (outputs bf16 [ns, B*S, d], what the backward pass needs)."""
         d, H = self.cfg.d_model, self.cfg.n_head
         ns, dev = len(a16), a16[0].device
-        w16, bias = self._w16[pre + "attn.c_attn"][0], self.p[pre + "attn.c_attn.bias"].reshape(-1)      # [3d, d]: rows v | q | k
+        w16, bias = self._w16[pre + "attn.c_attn"][0], self.dense[pre + "attn.c_attn"].b                # [3d, d]: rows v | q | k
         qk = torch.empty((B, ns * S, 2 * d), dtype=torch.bfloat16, device=dev)
         vt = torch.empty((B, d, ns * S), dtype=torch.bfloat16, device=dev)
         for s, a in enumerate(a16):
@@ -432,15 +446,7 @@ class MIGTTrainer:
         hn = [self._ln(x, "ln_f") for x in xs]
         denom = float(B * (T - skip) * Lt)
         view_ok = (torch.arange(T, device=dev) >= skip).to(torch.float32).repeat_interleave(Lt).repeat(B)        # [B*S] row mask
-        head_tc = self._tc_dense_ok(d, V)
-        if head_tc and self.bf16:
-            logits = torch.empty((B * S, V), dtype=torch.float32, device=dev)
-            L.tc_gemm(L.to_bf16(hn[1]), self._w16["wte"][1], logits, M=B * S, N=V, K=d, lda=d, ldb=d, ldc=V)
-        elif head_tc:                                                                                              # tied head, first V rows (:417)
-            logits = self._dense_fw_tc(hn[1], ("fw", "wte"), lambda: wte[:V].contiguous(), V, d)
-        else:
-            logits = torch.empty((B * S, V), dtype=torch.float32, device=dev)
-            L.simt_gemm(hn[1], wte, logits, M=B * S, N=V, K=d, a_strides=(d, 1), b_strides=(1, d), ldc=V)
+        logits = self._dgrad(hn[1], "wte")                                                                         # tied head (:417)
         ce_rows = L.cross_entropy_rows(logits, ids.reshape(-1), float(cfg.label_smoothing))
         ce = L.row_mean(ce_rows.reshape(B, S), skip * Lt)
         loss = ce * float(cfg.image_generation_weight)
@@ -455,18 +461,9 @@ class MIGTTrainer:
         ls = self.loss_scale * self._seed_scale                                   # gradient seeds carry the loss scale (1 in fp32) and the seed scale
         dlog = L.cross_entropy_grad(logits, ids.reshape(-1), (view_ok * (float(cfg.image_generation_weight) * ls / denom)).contiguous(),
                                     float(cfg.label_smoothing))
-        # tied LM head backward: d hn1 = dlogits wte[:V];  d wte[:V] += dlogits^T hn1
-        if head_tc and self.bf16:
-            dhn[1] = torch.empty((B * S, d), dtype=torch.float32, device=dev)
-            L.tc_gemm(L.to_bf16(dlog), self._w16["wte"][0], dhn[1], M=B * S, N=d, K=V, lda=V, ldb=V, ldc=d)
-            L.dense_wgrad_bf16(dlog, hn[1], g["wte.weight"][:V])
-        elif head_tc:
-            dhn[1] = self._dense_fw_tc(dlog, ("bw", "wte"), lambda: wte[:V].t().contiguous(), d, V)
-            L.dense_wgrad_tc(dlog, hn[1], g["wte.weight"][:V])
-        else:
-            dhn[1] = torch.empty_like(hn[1])
-            L.simt_gemm(dlog, wte, dhn[1], M=B * S, N=d, K=V, a_strides=(V, 1), b_strides=(d, 1), ldc=d)
-            L.conv_wgrad(dlog.reshape(1, B * S, 1, V), hn[1].reshape(1, B * S, 1, d), g["wte.weight"], kh=1, pad=(0, 0), so=(d, 1))
+        # tied LM head backward: d hn1 = dlogits wte[:V];  d wte[:V] += dlogits^T hn1 (ready with the embeddings)
+        dhn[1] = self._lin(dlog, "wte")
+        self._lin_bw(dlog, hn[1], "wte", need_dx=False, last=False)
         if self.use_loc:
             pc_h = self._lin(hn[2], "pose_classifier.c_fc")
             raw = self._lin(self._gelu(pc_h), "pose_classifier.c_proj")            # [B*S, 7]
@@ -597,7 +594,8 @@ class MIGTTrainer:
 
     def _weights_changed(self):
         """flat_p has new values: drop the split-fp16 operand copies and rewrite the bf16 ones."""
-        self._wsplit = {}
+        for r in self.dense.values():
+            r.split.clear()
         if self.bf16:
             L.dense_weights_bf16(self._w16_table)
 

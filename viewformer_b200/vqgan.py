@@ -82,6 +82,12 @@ def layout(cfg):
     return enc, dec
 
 
+def tc_conv_shape_ok(k, cin, cout, k_align=64):
+    """The conv shapes a tensor-core model runs on the tensor cores: 3x3, Cin a multiple of the K block (``Precision.k_align``
+    channels), Cout a multiple of 16 and at least 64.  The bf16 codebook training step puts the same convs on bf16 wgmma."""
+    return k == 3 and cin % k_align == 0 and cout % 16 == 0 and cout >= 64
+
+
 class _Conv3:
     """3x3 (or 1x1) convolution weights in both kernel layouts."""
 
@@ -90,7 +96,7 @@ class _Conv3:
         self.cout, self.cin, self.k = cout, cin, kh
         w = w.to(device=device, dtype=torch.float32)
         self.bias = b.to(device=device, dtype=torch.float32).contiguous()
-        self.tc = (not exact) and prec.use_tc and kh == 3 and cin % prec.k_align == 0 and cout % 16 == 0 and cout >= 64
+        self.tc = (not exact) and prec.use_tc and tc_conv_shape_ok(kh, cin, cout, prec.k_align)
         self.small_cin = kh == 3 and cin == 3 and cout % 16 == 0 and cout <= 128     # conv_in: dedicated exact kernel
         self.small_cout = kh == 3 and cin == 128 and cout == 3                       # conv_out: dedicated exact kernel
         if self.tc and prec.split:
