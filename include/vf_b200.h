@@ -175,14 +175,12 @@ int vf_tc_gemm_plan(const vf_tc_gemm_t* p, int* plan);
  *   vt  bf16 [B, d, S]   V transposed (row = channel, contiguous over tokens)
  *   out bf16 [B*S, d]    a token of view v attends to all tokens of views <= v; view = token / block
  *   head dim must be 64; S % block == 0.
+ *   first_query: only the query rows >= first_query (rounded down to a 128-row tile) are computed (0: all rows); rows of `out` below the
+ *     first computed tile are left untouched.  With first_query > 0 this is the KV-cache decode step — the context's q|k rows and V^T
+ *     columns stay in `qk` / `vt` from the prefill and the query view's are appended behind them.
+ *   skip_view: the 64 keys of this view are never visited (-1: none; needs block == 64).  Lets the host keep the query view at the start of
+ *     a 128-row tile whatever the number of cached context views.
  * ---------------------------------------------------------------------------------------- */
-int vf_attn_block_causal(const void* qk, const void* vt, int B, int S, int H, int d, int block, void* out, vf_stream_t s);
-/* Same kernel, only the query rows >= first_query (rounded down to a 128-row tile): the KV-cache decode step — the context's q|k rows and
- * V^T columns stay in `qk` / `vt` from the prefill and the query view's are appended behind them. */
-int vf_attn_block_causal_tail(const void* qk_bf16, const void* vt_bf16, int B, int S, int H, int d, int block, int first_query,
-                              void* out_bf16, vf_stream_t s);
-/* KV-cache decode with an unused view slot: as vf_attn_block_causal_tail, but the 64 keys of view `skip_view` are never visited (-1: none).
- * Lets the host keep the query view at the start of a 128-row tile whatever the number of cached context views. */
 int vf_attn_block_causal_decode(const void* qk_bf16, const void* vt_bf16, int B, int S, int H, int d, int block, int first_query,
                                 int skip_view, void* out_bf16, vf_stream_t s);
 /* Branching (multi-end) attention of the 3-stream forward — viewformer/models/branching_attention.py:82-126.  qk [B, n_streams*S, 2d] and
@@ -303,15 +301,6 @@ int vf_ssim_u8_k(const void* a_u8, const void* b_u8, int N, int H, int W, int C,
  * ---------------------------------------------------------------------------------------- */
 int vf_vq_lookup(const float* z, const float* Et, const float* esq, int64_t M, int D, int K,
                  int64_t* idx, float* quant, double* diff_sum, vf_stream_t s);
-/* Tensor-core lookup (same result as vf_vq_lookup):
- *   1. vf_vq_split3: x f32 [rows,D] -> bf16 [rows,3D] = [hi|hi|lo] (codebook=0) or [hi|lo|hi] (codebook=1), hi+lo ~ x to 2^-16
- *   2. vf_tc_gemm: scores[M,K] = -2 * A3 . B3^T + esq   (one bf16 GEMM with K = 3D; |z|^2 is common to all codes)
- *   3. vf_vq_select: per row the approximate minimum; every code within the bf16x3 error bound tol*(|z|^2+|e|^2) of it is
- *      re-scored in fp64 (direct squared differences), so the returned index is the exact-arithmetic nearest neighbour
- *      (ties -> smaller index); also gathers quant and accumulates diff.  n_rescored (nullable) counts rows with > 1 candidate. */
-int vf_vq_split3(const float* x, int64_t rows, int D, int codebook, void* out_bf16, vf_stream_t s);
-int vf_vq_select(const float* scores, const float* z, const float* Et, const float* esq, int64_t M, int D, int K, float tol,
-                 int64_t* idx, float* quant, double* diff_sum, int* n_rescored, vf_stream_t s);
 /* Fused lookup (same result as vf_vq_lookup; viewformer_b200/csrc/vf_vq_fused.cu): one wgmma kernel reads every z row ONCE
  * (fp32 -> fp16 in shared memory), scores it against Eh = fp16(-2 e) [K,D] (vf_vq_prepare_codebook_f16) with wgmma and keeps the
  * two best codes per row straight from the accumulator registers — no score matrix in HBM, 4*D + 8 bytes of traffic per row.  Rows whose two best scores

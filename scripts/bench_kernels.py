@@ -108,16 +108,14 @@ for (Bq, Sq) in ((32, 640), (32, 1280)):
     useful = 4.0 * Bq * H * 64 * 64 * 64 * Tn * (Tn + 1) / 2          # 4*dh*L^2*T(T+1)/2 per (b,h): QK^T + PV, visible blocks only
     rows.append((f"FUSED block-causal attention B{Bq} H12 S{Sq} (useful FLOPs)", ms, useful / ms / 1e9, None))
 
-# VQ lookup: exact fp32 kernel vs tensor-core path
+# VQ lookup: exact fp32 kernel (the fused tensor-core lookup: scripts/bench_vq.py)
 from oracle import synth
 E, _ = synth.make_lookup_inputs(11)
-et, esq = L.vq_prepare_codebook(E.cuda()); et3 = L.vq_split3(et, True)
+et, esq = L.vq_prepare_codebook(E.cuda())
 for Mq in (18432, 1 << 20):
     zq = torch.randn((Mq, 256), device=dev)
     ms = timeit(lambda: L.vq_lookup(zq, et, esq, want_quant=False, want_diff=False), reps=3, warm=1)
     rows.append((f"VQ lookup fp32 CUDA-core  M={Mq}", ms, 2.0 * Mq * 256 * 1024 / ms / 1e9, Mq * 1032 / ms / 1e6))
-    ms = timeit(lambda: L.vq_lookup_tc(zq, et, esq, et3, want_quant=False, want_diff=False), reps=3, warm=1)
-    rows.append((f"VQ lookup tensor-core bf16x3  M={Mq}", ms, 2.0 * Mq * 256 * 1024 / ms / 1e9, Mq * 1032 / ms / 1e6))
 
 print(f"{'kernel':58s} {'ms':>8s} {'TFLOP/s':>9s} {'%peak':>6s} {'GB/s':>8s} {'%hbm':>6s}")
 for name, ms, tf, gbs in rows:

@@ -11,7 +11,6 @@ peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.absp
 E = (torch.rand(256, 1024, device=dev) * 2 - 1) * 3 ** 0.5
 et, esq = L.vq_prepare_codebook(E)
 eh = L.vq_prepare_codebook_f16(et)
-et3 = L.vq_split3(et, True)
 
 
 def timeit(fn, reps=5, warm=2):
@@ -31,10 +30,8 @@ only = sys.argv[1] if len(sys.argv) > 1 else ""
 for M in ([1 << 20] if only == "fused" else [18432, 1 << 17, 1 << 20]):
     z = torch.randn((M, 256), device=dev)
     rows = [("fused wgmma (1 pass, fp16 pairs)", lambda: L.vq_lookup_fused(z, et, esq, eh, emb_dk=E, want_quant=False, want_diff=False))]
-    if only != "fused":
-        rows += [("bf16x3 GEMM + select (round 1)", lambda: L.vq_lookup_tc(z, et, esq, et3, want_quant=False, want_diff=False))]
-        if M <= 1 << 17:
-            rows += [("fp32 CUDA-core", lambda: L.vq_lookup(z, et, esq, want_quant=False, want_diff=False))]
+    if only != "fused" and M <= 1 << 17:
+        rows += [("fp32 CUDA-core", lambda: L.vq_lookup(z, et, esq, want_quant=False, want_diff=False))]
     for name, fn in rows:
         ms = timeit(fn)
         gbs = M * 1032 / ms / 1e6

@@ -1290,14 +1290,6 @@ def check_gather_rows(ba, result, st):
     return bits_equal(result, t[ba["idx"].clamp(0, t.shape[0] - 1)])
 
 
-def check_vq_split3(ba, result, st):
-    """hi = bf16(v), lo = bf16(v - hi), rows [hi | hi | lo] (queries) or [hi | lo | hi] (codebook), bit for bit."""
-    v = ba["x"].float()
-    hi = v.to(torch.bfloat16)
-    lo = (v - hi.float()).to(torch.bfloat16)
-    return bits_equal(result, torch.cat([hi, lo, hi] if ba["codebook"] else [hi, hi, lo], 1))
-
-
 def check_vq_prepare_codebook_f16(ba, result, st):
     """fp16(-2 e) of the codebook rows Et [K, D] (-2 e is exact in fp32), bit for bit."""
     return bits_equal(result, (-2.0 * ba["et"].float()).half())
@@ -1603,7 +1595,6 @@ CHECKERS = {
     "attn_multiend_bwd": (before_attn_bwd, check_attn_multiend_bwd),
     "vq_lookup": (before_lookup, check_vq_lookup),
     "vq_lookup_fused": (before_lookup, check_lookup),
-    "vq_lookup_tc": (before_lookup, check_lookup),
     "gn_mean_rstd": (before_gn_mean_rstd, check_gn_mean_rstd),
     "groupnorm": (before_groupnorm, check_groupnorm),
     "layernorm": (before_layernorm, check_layernorm),
@@ -1627,7 +1618,6 @@ CHECKERS = {
     "nchw_to_nhwc": (before_none, check_nchw_to_nhwc),
     "nhwc_to_nchw": (before_none, check_nhwc_to_nchw),
     "gather_rows": (before_none, check_gather_rows),
-    "vq_split3": (before_none, check_vq_split3),
     "vq_prepare_codebook_f16": (before_none, check_vq_prepare_codebook_f16),
     "vq_prepare_codebook": (before_none, check_vq_prepare_codebook),
     "migt_embed": (before_none, check_migt_embed),

@@ -617,33 +617,6 @@ def test_fused_multiend_attention(L, B, T, H):
         report(f"fused multi-end attention stream {s} B{B} T{T} H{H}", out.float(), w, 2e-2, 2e-2)
 
 
-def test_vq_lookup_tensor_core_bit_exact(L, golden_dir):
-    """bf16x3 tensor-core distance GEMM + exact fp64 re-score == the reference's indices, incl. the adversarial near-ties."""
-    import os
-    from oracle import synth
-    gd = np.load(os.path.join(golden_dir, "vq_lookup.npz"))
-    E, z = synth.make_lookup_inputs(int(gd["seed"]))
-    et, esq = L.vq_prepare_codebook(E.cuda())
-    et3 = L.vq_split3(et, True)
-    hi = et.bfloat16()
-    assert torch.equal(et3[:, :256].cpu(), hi.cpu()) and torch.equal(et3[:, 512:].cpu(), hi.cpu())
-    idx, quant, dsum, nres = L.vq_lookup_tc(z.cuda(), et, esq, et3, count_rescored=True)
-    idx = idx.cpu().numpy()
-    print(f"[vq_lookup_tc] mismatches vs reference: {int((idx != gd['idx']).sum())}/{idx.size}; rows with >1 candidate: {int(nres)}")
-    assert np.array_equal(idx, gd["idx"])
-    e = E.t()[torch.from_numpy(idx)]
-    assert torch.equal(quant.cpu(), z + (e - z))
-    want = float(((e - z).double() ** 2).sum())
-    assert abs(float(dsum) - want) / want < 1e-6
-    idx2, _, _ = L.vq_lookup_tc(z[:77].contiguous().cuda(), et, esq, et3)
-    assert np.array_equal(idx2.cpu().numpy(), gd["idx"][:77])
-    # large random batch: tensor-core result == exact fp32 kernel result
-    zz = torch.randn(40960, 256, generator=g(123)).cuda()
-    a, _, _ = L.vq_lookup_tc(zz, et, esq, et3, want_quant=False, want_diff=False)
-    b, _, _ = L.vq_lookup(zz, et, esq, want_quant=False, want_diff=False)
-    assert torch.equal(a, b)
-
-
 # ----------------------------------------------------------------------------- exact (split-fp16, chunked accumulation) convolutions
 def _split_ref(v):
     """CPU restatement of the VF_F16X2 pair: hi = fp16(v), lo = fp16((v - hi) * 2^11)."""

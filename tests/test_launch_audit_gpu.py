@@ -42,7 +42,7 @@ Normalisation, reduction, optimizer and elementwise wrappers (same card; the 14 
   softmax_rows 0.995 (bf16 output, generate) / 0.18 (fp32, mask modes 0, 1, 2), sumpool2x2 0.975, pose_loss_rows 0.51, vq_commit_grad
       0.34, pose_loss_grad 0.29, vq_ema_update 0.25, vq_ema_stats 0.20, pose_postprocess 0.12, cameras_prepare 0.089, vq_prepare_codebook
       0.078, row_mean 0.052, cameras_from_relative 0.037, cross_entropy_rows 0.011, l1_grad 0.011; bit-exact: u8_to_unit, unit_to_u8, the
-      layout conversions, gather_rows, vq_split3, vq_prepare_codebook_f16, migt_embed, argmax_rows, image_pair_sums, resize_u8 (evaluation).
+      layout conversions, gather_rows, vq_prepare_codebook_f16, migt_embed, argmax_rows, image_pair_sums, resize_u8 (evaluation).
   The whole file ran in about 55 s with 19 workloads; the three fp32 medium and full-size steps add 5 s or less each.  The largest GroupNorm mean^2 / var above comes from synthetic random-weight models.
 """
 import os

@@ -22,8 +22,8 @@ EXPORTS = [
     "vf_simt_gemm", "vf_tc_gemm", "vf_tc_gemm_plan", "vf_vq_lookup", "vf_gather_rows", "vf_vq_ema_stats", "vf_vq_ema_update", "vf_vq_commit_grad",
     "vf_vq_prepare_codebook", "vf_migt_embed", "vf_softmax_rows", "vf_argmax_rows", "vf_pose_postprocess",
     "vf_cameras_prepare", "vf_cameras_from_relative",
-    "vf_conv3x3_small_cin", "vf_conv3x3_small_cout", "vf_groupnorm_finalize", "vf_split_f16x2", "vf_attn_block_causal", "vf_attn_block_causal_tail", "vf_attn_block_causal_decode", "vf_attn_block_multiend",
-    "vf_vq_split3", "vf_vq_select", "vf_cross_entropy_rows", "vf_pose_loss_rows", "vf_row_mean",
+    "vf_conv3x3_small_cin", "vf_conv3x3_small_cout", "vf_groupnorm_finalize", "vf_split_f16x2", "vf_attn_block_causal_decode", "vf_attn_block_multiend",
+    "vf_cross_entropy_rows", "vf_pose_loss_rows", "vf_row_mean",
     "vf_vq_prepare_codebook_f16", "vf_vq_lookup_fused", "vf_resize_u8", "vf_image_pair_sums", "vf_ssim_u8", "vf_ssim_u8_k",
     "vf_conv_wgrad", "vf_pad_transpose_split", "vf_pad_transpose_bf16", "vf_conv_weights_bf16", "vf_sum_splits", "vf_col_sums", "vf_groupnorm_bwd", "vf_softmax_bwd_rows", "vf_l1_grad", "vf_lincomb3", "vf_sumpool2x2", "vf_adam",
     "vf_layernorm_bwd", "vf_gelu_fwd", "vf_gelu_bwd", "vf_migt_embed_bwd", "vf_cross_entropy_grad", "vf_pose_loss_grad", "vf_adamw_keras", "vf_sumsq", "vf_dropout",
@@ -563,34 +563,6 @@ def split_f16x2(x_rows):
     out = torch.empty((rows, 2 * c), dtype=torch.float16, device=x_rows.device)
     _check(lib.vf_split_f16x2(_p(x_rows), C.c_int64(rows), c, _p(out), _stream()))
     return out
-
-
-def vq_split3(x, codebook):
-    """f32 [rows,D] -> bf16 [rows,3D] two-term split ([hi|hi|lo] for queries, [hi|lo|hi] for the codebook)."""
-    lib = load(True)
-    _dev(x, torch.float32)
-    rows, d = x.shape
-    out = torch.empty((rows, 3 * d), dtype=torch.bfloat16, device=x.device)
-    _check(lib.vf_vq_split3(_p(x), C.c_int64(rows), d, int(codebook), _p(out), _stream()))
-    return out
-
-
-def vq_lookup_tc(z_rows, et, esq, et3, want_quant=True, want_diff=True, tol=1e-4, count_rescored=False):
-    """Tensor-core lookup: bf16x3 distance GEMM on the tensor cores + exact fp64 re-score of near-ties.  Same outputs as vq_lookup."""
-    lib = load(True)
-    _dev(z_rows, torch.float32)
-    m, d = z_rows.shape
-    k = et.shape[0]
-    a3 = vq_split3(z_rows, False)
-    scores = torch.empty((m, k), dtype=torch.float32, device=z_rows.device)
-    tc_gemm(a3, et3, scores, M=m, N=k, K=3 * d, lda=3 * d, ldb=3 * d, ldc=k, alpha=-2.0, bias=esq, bias_mode=BIAS_N)
-    idx = torch.empty((m,), dtype=torch.int64, device=z_rows.device)
-    quant = torch.empty((m, d), dtype=torch.float32, device=z_rows.device) if want_quant else None
-    dsum = torch.zeros((1,), dtype=torch.float64, device=z_rows.device) if want_diff else None
-    nres = torch.zeros((1,), dtype=torch.int32, device=z_rows.device) if count_rescored else None
-    _check(lib.vf_vq_select(_p(scores), _p(z_rows), _p(et), _p(esq), C.c_int64(m), d, k, C.c_float(tol), _p(idx), _p(quant), _p(dsum),
-                            _p(nres), _stream()))
-    return (idx, quant, dsum, nres) if count_rescored else (idx, quant, dsum)
 
 
 def vq_prepare_codebook_f16(et):

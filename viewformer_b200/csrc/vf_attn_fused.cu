@@ -297,21 +297,12 @@ struct AttnTrain {           // training-instance options of attn_launch (null: 
 static int attn_launch(const void* qk, const void* vt, int B, int S, int n_streams, int stream, int H, int d, int block, int first_query,
                        int skip_view, void* out, vf_stream_t s, const AttnTrain* train = nullptr);
 
-extern "C" int vf_attn_block_causal(const void* qk, const void* vt, int B, int S, int H, int d, int block, void* out, vf_stream_t s) {
-    return attn_launch(qk, vt, B, S, 1, 0, H, d, block, 0, -1, out, s);
-}
-
-// Only the query rows >= first_query (rounded down to a 128-row tile) are computed: with the context's q|k rows and V^T columns kept from
-// a prefill and the query view appended behind them, this is the KV-cache decode step (BASELINE config 5) — the same fused kernel, no
-// score matrix in HBM.  Rows of `out` below the first computed tile are left untouched.
-extern "C" int vf_attn_block_causal_tail(const void* qk, const void* vt, int B, int S, int H, int d, int block, int first_query, void* out,
-                                         vf_stream_t s) {
-    return attn_launch(qk, vt, B, S, 1, 0, H, d, block, first_query, -1, out, s);
-}
-
-// KV-cache decode with an unused view slot: as vf_attn_block_causal_tail, but the keys of view `skip_view` (64 tokens per view) are never
-// visited.  With an odd number of cached context views the query view would share its 128-row tile with the last context view (half
-// of the tile's softmax work recomputes context rows nobody reads); leaving one slot empty puts the query view at the start of a tile.
+// Single-stream block-causal attention.  Only the query rows >= first_query (rounded down to a 128-row tile) are computed (0: all of
+// them): with the context's q|k rows and V^T columns kept from a prefill and the query view appended behind them, this is the KV-cache
+// decode step (BASELINE config 5) — the same fused kernel, no score matrix in HBM.  Rows of `out` below the first computed tile are left
+// untouched.  The keys of view `skip_view` (64 tokens per view; -1: none) are never visited.  With an odd number of cached context views
+// the query view would share its 128-row tile with the last context view (half of the tile's softmax work recomputes context rows nobody
+// reads); leaving one slot empty puts the query view at the start of a tile.
 extern "C" int vf_attn_block_causal_decode(const void* qk, const void* vt, int B, int S, int H, int d, int block, int first_query, int skip_view,
                                            void* out, vf_stream_t s) {
     VF_CHECK_ARG(skip_view < 0 || block == KT, "vf_attn_block_causal_decode: skipping a view needs 64 tokens per view (block=%d)", block);
@@ -319,7 +310,7 @@ extern "C" int vf_attn_block_causal_decode(const void* qk, const void* vt, int B
 }
 
 // Branching (multi-end) attention, branching_attention.py:82-126: qk [B, n_streams * S, 2d] and V^T [B, d, n_streams * S] hold the streams
-// side by side.  stream = 0: block-causal attention of stream 0 over its own keys (as vf_attn_block_causal, reading the first S rows);
+// side by side.  stream = 0: block-causal attention of stream 0 over its own keys (the first S rows of each batch element);
 // stream = s >= 1: a query of view t of stream s attends to the stream-0 keys of views < t and to the stream-s keys of view t, one joint
 // softmax.  out [B * S, d] receives that stream's attention output.  Streams >= 1 need block == 64 (one view per key tile).
 extern "C" int vf_attn_block_multiend(const void* qk, const void* vt, int B, int S, int n_streams, int stream, int H, int d, int block,

@@ -171,117 +171,6 @@ __global__ void __launch_bounds__(256) vq_lookup_kernel(const float* __restrict_
     }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Tensor-core lookup, step 1: split every fp32 value into two bf16 terms, hi = bf16(x), lo = bf16(x - hi), and lay the
-// row out as [hi | hi | lo] (queries) or [hi | lo | hi] (codebook), so that ONE bf16 GEMM with K = 3D computes
-// hi.hi + hi.lo + lo.hi = x.e - lo.lo  (relative error ~2^-16, fp32 accumulation).
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void split3_kernel(const float* __restrict__ x, int64_t rows, int D, int codebook, __nv_bfloat16* __restrict__ out) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= rows * D) return;
-    const int64_t r = i / D;
-    const int d = (int)(i % D);
-    const float v = x[i];
-    const __nv_bfloat16 hi = __float2bfloat16(v);
-    const __nv_bfloat16 lo = __float2bfloat16(v - __bfloat162float(hi));
-    __nv_bfloat16* o = out + r * 3 * D;
-    o[d] = hi;
-    o[D + d] = codebook ? lo : hi;
-    o[2 * D + d] = codebook ? hi : lo;
-}
-
-// step 3 (one warp per row): the minimum of the approximate scores, then EVERY code whose approximate score lies within the
-// error bound of that minimum is re-scored exactly in fp64 (direct sum of squared differences) and the exact minimum wins,
-// ties to the smaller index (== argmax(-dist) first-index rule, utils_th.py:41).  Error bound of the bf16x3 dot product:
-// |dot3 - z.e| <= 2^-15.5 |z||e|  =>  a gap between two scores is trusted only beyond tol * (|z|^2 + |e|^2), tol = 1e-4.
-__global__ void __launch_bounds__(256) vq_select_kernel(const float* __restrict__ scores, const float* __restrict__ z,
-                                                        const float* __restrict__ Et, const float* __restrict__ esq, int64_t M,
-                                                        int D, int K, float tol, int64_t* __restrict__ idx,
-                                                        float* __restrict__ quant, double* __restrict__ diff_sum,
-                                                        int* __restrict__ n_rescored) {
-    __shared__ double dsum_sh[8];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t row = (int64_t)blockIdx.x * 8 + warp;
-    double ds = 0.0;
-    if (row < M) {
-        const float* sr = scores + row * K;
-        const float* zr = z + row * D;
-        float bd = INFINITY;
-        int bi = 0x7fffffff;
-        for (int c = lane * 4; c < K; c += 128) {
-            const float4 v = __ldg(reinterpret_cast<const float4*>(sr + c));
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-                if (vv[e] < bd) { bd = vv[e]; bi = c + e; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float obd = __shfl_xor_sync(0xffffffffu, bd, o);
-            const int obi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (obd < bd || (obd == bd && obi < bi)) { bd = obd; bi = obi; }
-        }
-        float zz = 0.f;
-        for (int d = lane; d < D; d += 32) zz = fmaf(zr[d], zr[d], zz);
-        zz = warp_sum(zz);
-        const float thr = bd + tol * (zz + __ldg(esq + bi));
-        // exact re-score of every candidate within the bound (almost always exactly one: the approximate winner)
-        double best_d = 0.0;
-        int best = -1, ncand = 0;
-        for (int c0 = 0; c0 < K; c0 += 128) {
-            const int c = c0 + lane * 4;
-            float4 v = make_float4(INFINITY, INFINITY, INFINITY, INFINITY);
-            if (c < K) v = __ldg(reinterpret_cast<const float4*>(sr + c));
-            const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                unsigned m = __ballot_sync(0xffffffffu, vv[e] <= thr);
-                while (m) {
-                    const int src = __ffs(m) - 1;
-                    m &= m - 1;
-                    const int cand = c0 + src * 4 + e;
-                    const float* ec = Et + (int64_t)cand * D;
-                    double dd = 0.0;
-                    for (int d = lane; d < D; d += 32) {
-                        const double t = (double)ec[d] - (double)zr[d];
-                        dd += t * t;
-                    }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) dd += __shfl_xor_sync(0xffffffffu, dd, o);
-                    if (best < 0 || dd < best_d || (dd == best_d && cand < best)) { best_d = dd; best = cand; }
-                    ++ncand;
-                }
-            }
-        }
-        if (lane == 0) {
-            idx[row] = best;
-            if (n_rescored && ncand > 1) atomicAdd(n_rescored, 1);
-        }
-        const float* e = Et + (int64_t)best * D;
-        for (int d = lane * 4; d < D; d += 128) {
-            const float4 ev = __ldg(reinterpret_cast<const float4*>(e + d));
-            const float4 zv = __ldg(reinterpret_cast<const float4*>(zr + d));
-            if (quant)
-                *reinterpret_cast<float4*>(quant + row * D + d) =
-                    make_float4(__fadd_rn(zv.x, __fsub_rn(ev.x, zv.x)), __fadd_rn(zv.y, __fsub_rn(ev.y, zv.y)),
-                                __fadd_rn(zv.z, __fsub_rn(ev.z, zv.z)), __fadd_rn(zv.w, __fsub_rn(ev.w, zv.w)));
-            const float a = ev.x - zv.x, b = ev.y - zv.y, c = ev.z - zv.z, dd = ev.w - zv.w;
-            ds += (double)(a * a) + (double)(b * b) + (double)(c * c) + (double)(dd * dd);
-        }
-    }
-    if (diff_sum) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) ds += __shfl_xor_sync(0xffffffffu, ds, o);
-        if (lane == 0) dsum_sh[warp] = ds;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            double t = 0;
-            for (int w = 0; w < 8; ++w) t += dsum_sh[w];
-            atomicAdd(diff_sum, t);
-        }
-    }
-}
-
 __global__ void gather_rows_kernel(const float* __restrict__ table, const int64_t* __restrict__ idx, int64_t M, int D,
                                    int64_t n_rows, float* __restrict__ out) {
     const int quads = D >> 2;
@@ -380,25 +269,6 @@ extern "C" int vf_vq_lookup(const float* z, const float* Et, const float* esq, i
     const unsigned blocks = (unsigned)((M + LM - 1) / LM);
     vq_lookup_kernel<<<blocks, 256, 0, vf_s(s)>>>(z, Et, esq, M, D, K, idx, quant, diff_sum);
     VF_CHECK_LAUNCH("vf_vq_lookup");
-    return VF_OK;
-}
-
-extern "C" int vf_vq_split3(const float* x, int64_t rows, int D, int codebook, void* out_bf16, vf_stream_t s) {
-    VF_CHECK_ARG(x && out_bf16 && D > 0, "vf_vq_split3: bad args");
-    if (rows == 0) return VF_OK;
-    const int64_t total = rows * D;
-    split3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, vf_s(s)>>>(x, rows, D, codebook, (__nv_bfloat16*)out_bf16);
-    VF_CHECK_LAUNCH("vf_vq_split3");
-    return VF_OK;
-}
-
-extern "C" int vf_vq_select(const float* scores, const float* z, const float* Et, const float* esq, int64_t M, int D, int K, float tol,
-                            int64_t* idx, float* quant, double* diff_sum, int* n_rescored, vf_stream_t s) {
-    if (M == 0) return VF_OK;
-    VF_CHECK_ARG(scores && z && Et && esq && idx, "vf_vq_select: null pointer");
-    VF_CHECK_ARG(D % 4 == 0 && K % 4 == 0, "vf_vq_select: D, K must be multiples of 4");
-    vq_select_kernel<<<(unsigned)((M + 7) / 8), 256, 0, vf_s(s)>>>(scores, z, Et, esq, M, D, K, tol, idx, quant, diff_sum, n_rescored);
-    VF_CHECK_LAUNCH("vf_vq_select");
     return VF_OK;
 }
 

@@ -11,7 +11,7 @@
 //   merge (4 warps)   per row: best code over the 16 sets; if the runner-up lies within the fp16 rounding bound of the best the row
 //                     is queued for the exact pass (PAIR: both candidates known; FULL: a third may hide inside one set)
 // vq_rescue_kernel then settles queued rows in fp64 (direct sum of squared differences, ties to the smaller index — the same rule as
-// vf_vq_lookup / vf_vq_select), so the indices returned equal the fp32 kernels' on every input.
+// vf_vq_lookup), so the indices returned equal the fp32 kernel's on every input.
 //
 // Rounding model (why the tolerance is safe): fp16 operands carry 11 significand bits, |d(z.e)| <= 2^-10 sum|z_i e_i| <= 2^-10 |z||e|;
 // the score -2 z.e + |e|^2 of two codes therefore moves by at most 2^-9 |z| (|e_a| + |e_b|) against each other (worst case, all

@@ -46,7 +46,6 @@ class MIGT:
         self._codebook_model = None
         self._sd = None
         self._w = None
-        self.fused_attention = True     # False: QK^T / softmax / PV as separate kernels (kept for the multi-stream / tf32 paths)
 
     # ------------------------------------------------------------------ plumbing
     @property
@@ -238,10 +237,10 @@ class MIGT:
                     b_bs=(S * d, 0), c_bs=(d * ns * S, 0), c_off=s * S, bias=lw["v"].b, bias_mode=L.BIAS_M)
         if kv_out is not None:
             kv_out.append((qk, vt))                      # context K (k half of qk) and V^T of this layer: the KV cache
-        if ns == 1 and prec.opd == torch.bfloat16 and dh == 64 and self.fused_attention:
+        if ns == 1 and prec.opd == torch.bfloat16 and dh == 64:
             # single-stream forward (the generate() hot path): one fused wgmma kernel, no S x S tensor in HBM
             return [L.attn_block_causal(qk, vt, B, S, H, d, Lt)]
-        if ns > 1 and prec.opd == torch.bfloat16 and dh == 64 and Lt == 64 and self.fused_attention:
+        if ns > 1 and prec.opd == torch.bfloat16 and dh == 64 and Lt == 64:
             # 3-stream forward (multi-context generation, localisation): the same fused kernel with the multi-end key-tile schedule
             return [L.attn_block_multiend(qk, vt, B, S, ns, s, H, d, Lt) for s in range(ns)]
         outs = []
@@ -543,7 +542,7 @@ class MIGT:
         # skipped by the kernel), otherwise half of the decode tile's softmax work would recompute the last context view
         pad = (Tc * Lt) % 128 // Lt if Lt == 64 else 0
         S_tot = (Tc + pad + 1) * Lt
-        if self.prec.opd == torch.bfloat16 and d // H == 64 and ((Tc + pad) * Lt) % 128 == 0 and self.fused_attention:
+        if self.prec.opd == torch.bfloat16 and d // H == 64 and ((Tc + pad) * Lt) % 128 == 0:
             # fused decode: keep every layer's q|k rows and V^T columns in buffers with room for ONE more view, so that a query is
             # "append the view, run the fused block-causal kernel on the last 128-row tile" — no [Nq,H,64,S] score tensor in HBM
             fq, fv = [], []

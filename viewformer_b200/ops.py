@@ -45,10 +45,10 @@ class Linear:
 
 def gemm_nt(prec, A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0), b_bs=(0, 0), c_bs=(0, 0),
             alpha=1.0, bias=None, bias_mode=L.BIAS_NONE, act=L.ACT_NONE, residual=None, a_off=0, b_off=0, c_off=0,
-            causal_block=0, causal_skip_n=False, out2=None, force_simt=False, gn_rows_per_img=0, lo_a=None, lo_b=None):
+            causal_block=0, causal_skip_n=False, gn_rows_per_img=0, lo_a=None, lo_b=None):
     """C[m,n] = act(alpha * sum_k A[m,k]*B[n,k] + bias) + residual  (both operands K-major)."""
     es = A.element_size()
-    tc_ok = (prec.use_tc and not force_simt and A.dtype == B.dtype and A.dtype == prec.opd
+    tc_ok = (prec.use_tc and A.dtype == B.dtype and A.dtype == prec.opd
              and (lda * es) % 16 == 0 and (ldb * es) % 16 == 0 and (K * es) % 16 == 0
              and (a_off * es) % 16 == 0 and (b_off * es) % 16 == 0
              and all((s * es) % 16 == 0 for s in (*a_bs, *b_bs)))
@@ -56,23 +56,21 @@ def gemm_nt(prec, A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0
         return L.tc_gemm(A, B, out, M=M, N=N, K=K, lda=lda, ldb=ldb, ldc=ldc, batch=batch, a_bs=a_bs, b_bs=b_bs,
                          c_bs=c_bs, alpha=alpha, bias=bias, bias_mode=bias_mode, act=act, residual=residual,
                          a_off=a_off, b_off=b_off, c_off=c_off, causal_block=causal_block,
-                         causal_skip_n=causal_skip_n, out2=out2, gn_rows_per_img=gn_rows_per_img, lo_a=lo_a, lo_b=lo_b)
+                         causal_skip_n=causal_skip_n, gn_rows_per_img=gn_rows_per_img, lo_a=lo_a, lo_b=lo_b)
     if A.dtype == torch.float16:
         raise L.LibraryError("split-fp16 (exact) operands have no CUDA-core GEMM: shape not supported by vf_tc_gemm")
     L.simt_gemm(A, B, out, M=M, N=N, K=K, a_strides=(lda, 1), b_strides=(1, ldb), ldc=ldc, batch=batch, a_bs=a_bs,
                 b_bs=b_bs, c_bs=c_bs, alpha=alpha, bias=bias, bias_mode=bias_mode, act=act, residual=residual,
                 a_off=a_off, b_off=b_off, c_off=c_off)
-    if out2 is not None:
-        out2.copy_(out)     # only reachable on the exact path (fp32 -> fp32 alias never requested there)
     return out
 
 
-def linear(prec, x_rows, lin, out_dtype, *, act=L.ACT_NONE, residual=None, out=None, force_simt=False, gn_rows_per_img=0):
+def linear(prec, x_rows, lin, out_dtype, *, act=L.ACT_NONE, residual=None, out=None, gn_rows_per_img=0):
     """x_rows [M, K] (operand dtype) -> [M, N]."""
     M = x_rows.shape[0]
     if out is None:
         out = torch.empty((M, lin.n), dtype=out_dtype, device=x_rows.device)
     gemm_nt(prec, x_rows, lin.w, out, M=M, N=lin.n, K=lin.k, lda=x_rows.shape[1], ldb=lin.ld, ldc=lin.n,
             bias=lin.b, bias_mode=L.BIAS_N if lin.b is not None else L.BIAS_NONE, act=act, residual=residual,
-            force_simt=force_simt, gn_rows_per_img=gn_rows_per_img)
+            gn_rows_per_img=gn_rows_per_img)
     return out

@@ -127,11 +127,10 @@ class VQGAN:
         self.config = load_config(config)
         # ``mixed``: the encoder (whose output feeds the bit-exact codebook argmin) runs in the fp32-faithful ``exact`` arithmetic,
         # the decoder (pixels within a tolerance) on the bf16 tensor-core path.  One precision name otherwise serves both halves.
-        enc_name, dec_name = {"mixed": (os.environ.get("VF_EXACT_ENCODER", "x3"), "bf16")}.get(precision, (precision, precision))
+        enc_name, dec_name = ("x3", "bf16") if precision == "mixed" else (precision, precision)
         self.precision = precision
         self.enc_prec, self.dec_prec = Precision(enc_name), Precision(dec_name)
         self.prec = self.dec_prec                  # quantizer / glue policy
-        self.bf16_edges = True                     # bf16 halves only: conv1 -> norm2 activations travel as bf16 (see _resblock)
         # norm2 + swish fused into conv2's operand path (vf_tc_gemm_t.norm_*, the halo tile is transformed in shared memory):
         # bit-identical to the two-kernel path and tested; the MMA warpgroups do the transform between their MMAs, so it stays
         # opt-in (VF_NORM_ON_LOAD=1) until it is measured faster than conv + vf_groupnorm_apply
@@ -322,7 +321,6 @@ class VQGAN:
         Called at load time and after a gradient step on the codebook (``quantizer="commit"``)."""
         q = self._w["q"]
         q["et"], q["esq"] = L.vq_prepare_codebook(q["emb"])
-        q["et3"] = L.vq_split3(q["et"], True) if self.prec.use_tc else None
         q["eh"] = L.vq_prepare_codebook_f16(q["et"]) if (self.prec.use_tc and L.vq_fused_ok(*q["emb"].shape)) else None
         self._refresh_decode_table()
 
@@ -361,7 +359,7 @@ class VQGAN:
         # GroupNorm statistics taken from the fp32 accumulators in the conv epilogue — 4 B/element less HBM traffic
         n_, h_, w_, _ = x.shape
         c1 = rbw["c1"]
-        edge = torch.bfloat16 if (bf16 and self.bf16_edges and c1.tc and rbw["c2"].tc
+        edge = torch.bfloat16 if (bf16 and c1.tc and rbw["c2"].tc
                                   and L.gn_fusable(c1.cout, 32, n_ * h_ * w_, h_ * w_, c1.cout)) else torch.float32
         h = self._conv(c1, a, out_dtype=edge)
         if h.dtype == torch.bfloat16 and self.norm_on_load and L.conv_norm_fusable(h, rbw["c2"].cout):
@@ -477,12 +475,9 @@ class VQGAN:
     def _quantize(self, z_rows, want_quant=True):
         """QuantizeEMA.forward (utils_th.py:32-68) on rows [M,D]; returns (quant rows | None, diff, idx)."""
         q = self._w["q"]
-        if q["eh"] is not None and os.environ.get("VF_VQ_FUSED", "1") != "0":
+        if q["eh"] is not None:
             # fused wgmma lookup: z read once, scores never leave registers, near-ties settled in fp64: same indices as the fp32 kernel
             idx, quant, dsum = L.vq_lookup_fused(z_rows, q["et"], q["esq"], q["eh"], emb_dk=q["emb"], want_quant=want_quant, want_diff=True)
-        elif q["et3"] is not None and z_rows.shape[1] % 64 == 0:
-            # tensor-core distance GEMM (bf16x3) + exact fp64 re-score of every near-minimal candidate: same indices as the fp32 kernel
-            idx, quant, dsum = L.vq_lookup_tc(z_rows, q["et"], q["esq"], q["et3"], want_quant=want_quant, want_diff=True)
         else:
             idx, quant, dsum = L.vq_lookup(z_rows, q["et"], q["esq"], want_quant=want_quant, want_diff=True)
         if self.training and self.quantizer == "ema":
@@ -504,8 +499,6 @@ class VQGAN:
         corr = float(1.0 - torch.pow(torch.tensor(self.decay), torch.tensor(q["counter"], dtype=torch.int64)))
         alpha = 1 - self.decay
         L.vq_ema_update(counts, esum, alpha, corr, self.eps, q["cs"], q["dw"], q["emb"], q["et"], q["esq"])
-        if q["et3"] is not None:
-            q["et3"] = L.vq_split3(q["et"], True)
         if q["eh"] is not None:
             q["eh"] = L.vq_prepare_codebook_f16(q["et"])
         self._refresh_decode_table()
