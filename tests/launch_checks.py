@@ -1549,9 +1549,11 @@ def check_resize_u8(ba, result, st):
     accepted for a value within that distance of k."""
     x, size = ba["x_u8"], int(ba["size"])
     n, h, w, c = x.shape
-    if h == size and w == size:
+    # resize() hands NHWC to resize_th() unless shape[-2] = W is the size; resize_th() returns NCHW unchanged when shape[-2] = H is the
+    # size, and otherwise grows the height with nearest and shrinks it bilinearly, whatever the width does
+    if size in (w, h):
         return 0.0 if result is x else math.inf
-    method = ba["method"] or ("nearest" if size > w else "bilinear")
+    method = ba["method"] or ("nearest" if size > h else "bilinear")
     xv = x.double() / 255.0
     sh, sw = f32(np.float32(h) / np.float32(size)), f32(np.float32(w) / np.float32(size))
     o = torch.arange(size, device=x.device, dtype=torch.float32)          # source indices and weights in fp32, as the kernel forms them
@@ -1573,6 +1575,76 @@ def check_resize_u8(ba, result, st):
     got = result.double()
     ok = (got == k) | (near_up & (got == k + 1)) | (near_dn & (got == k - 1))
     return 0.0 if bool(ok.all()) else math.inf
+
+
+U64 = 2.0 ** -53
+SSIM_M, SSIM_D = 49 * 49 * 65025, 48 * 49 * 65025      # 49^2 255^2 and 48 49 255^2: the scales of the window sums' moments
+
+
+def box7(t):
+    """Exact 7 x 7 VALID window sums of an integer tensor [N, H, W, C] -> int64 [N, H-6, W-6, C], from a 2-D cumulative sum."""
+    n, h, w, c = t.shape
+    s = torch.zeros(n, h + 1, w + 1, c, dtype=torch.int64, device=t.device)
+    s[:, 1:, 1:] = t.long().cumsum(1).cumsum(2)
+    return s[:, 7:, 7:] - s[:, :-7, 7:] - s[:, 7:, :-7] + s[:, :-7, :-7]
+
+
+def pairwise_sum(x):
+    """Sum over the last dimension by halving: ceil(log2 n) additions per element's chain."""
+    while x.shape[-1] > 1:
+        if x.shape[-1] % 2:
+            x = F.pad(x, (0, 1))
+        x = x[..., 0::2] + x[..., 1::2]
+    return x[..., 0]
+
+
+def ssim64(a, b, k1=0.01, k2=0.03):
+    """SSIM of ``ssim()`` (7 x 7 uniform window, VALID, sample covariance, data range 1) of uint8 images [N, H, W, C] in fp64, from exact
+    integer window moments: with x = 255 X, M = 49^2 255^2 and D = 48 49 255^2, 2 ux uy + C1 = (2 sx sy + C1 M) / M and
+    2 vxy + C2 = (2 (49 sxy - sx sy) + C2 D) / D, and likewise B1, B2; the integers are exact in int64 and the scales cancel in S.
+    C1 = K1^2 and C2 = K2^2 are rounded once in fp64.  Returns (per-window S, the mean per image, T = |A1| |2 vxy| / (B1 B2) per window)."""
+    C1, C2 = float(k1) * float(k1), float(k2) * float(k2)
+    xa, xb = a.long(), b.long()
+    sx, sy, sxx, syy, sxy = box7(xa), box7(xb), box7(xa * xa), box7(xb * xb), box7(xa * xb)
+    n2xy = 2 * (49 * sxy - sx * sy)
+    a1 = (2 * sx * sy).double() + C1 * SSIM_M
+    a2 = n2xy.double() + C2 * SSIM_D
+    b1 = (sx * sx + sy * sy).double() + C1 * SSIM_M
+    b2 = ((49 * sxx - sx * sx) + (49 * syy - sy * sy)).double() + C2 * SSIM_D
+    den = b1 * b2
+    S = (a1 * a2) / den
+    flat = S.reshape(S.shape[0], -1)
+    return S, pairwise_sum(flat) / flat.shape[1], a1.abs() * n2xy.double().abs() / den
+
+
+def ssim_bar(S, T, h, w, c):
+    """The bar of ``check_ssim_u8`` per image (see there) from ssim64's per-window S and T."""
+    total = (h - 6) * (w - 6) * c
+    chunks = min((total + 255) // 256, 64)
+    kc = -(-total // (chunks * 256)) + 5 + 8 + chunks + 1            # kernel: windows per thread, shuffles, warps, chunk atomics, / total
+    kr = math.ceil(math.log2(total)) + 1 if total > 1 else 1           # reference: pairwise sum, / total
+    Sa, Ta = S.abs().reshape(S.shape[0], -1), T.reshape(T.shape[0], -1)
+    return (24 * U64 * (Sa + Ta).sum(1) + (kc + kr) * U64 * Sa.sum(1)) / total
+
+
+def check_ssim_u8(ba, result, st):
+    """Mean SSIM per image against ``ssim64`` (exact int64 window sums, S in fp64).  The kernel also sums each window exactly in integers
+    and forms the numerators 49 sxx - sx^2, 49 sxy - sx sy exactly (|.| < 2^29); S follows in fp64 with the same C1 = K1^2, C2 = K2^2.
+    Per window (u = 2^-53), the kernel: A1 = 2 sx sy / M + C1, B1, B2 one division and one addition of non-negative terms each (2 u
+    relative); A2 = q + C2 with q = 2 nxy / D, which cancels when the covariance is negative: u |q| + u |A2|; the two products and the
+    quotient 3 u: in all 10 u |S| + u T with T = |A1| |q| / (B1 B2).  The reference rounds C1 M, C2 D and its sums (2 u each of A1, B1,
+    B2; u (|q| + 2 |A2|) on A2) and 3 u in S: 11 u |S| + u T.  So each window's S is within 21 u |S| + 2 u T of the exact one; the bar
+    takes 24 u (|S| + T), which covers the second-order terms.  The mean: a per-thread fp64 chain over ceil(total / (chunks 256))
+    windows, 5 shuffles, 8 warp partials, up to 64 chunk atomics (chunks = min(ceil(total / 256), 64)), then / total: a chain of
+    Kc = that sum + 1 roundings of partial sums bounded by sum |S|; the reference's pairwise sum adds ceil(log2 total) + 1.  Bar per
+    image: (24 u sum (|S| + T) + (Kc + Kr) u sum |S|) / total, about 1e-14 at 128 x 128 x 3.  An fp32 E[x^2] - E[x]^2, a dropped row of
+    windows, swapped channels or images, or K1 = 0.01 for 1 is off by 1e-5 or more."""
+    a, b = ba["a_u8"], ba["b_u8"]
+    k1 = 0.01 if ba["k1"] is None else ba["k1"]
+    k2 = 0.03 if ba["k2"] is None else ba["k2"]
+    S, mean, T = ssim64(a, b, k1, k2)
+    _, h, w, c = a.shape
+    return ratio((result.double() - mean).abs(), ssim_bar(S, T, h, w, c))
 
 
 # ----------------------------------------------------------------------------------------------- registry
@@ -1637,6 +1709,7 @@ CHECKERS = {
     "vq_commit_grad": (before_none, check_vq_commit_grad),
     "vq_ema_update": (before_vq_ema_update, check_vq_ema_update),
     "resize_u8": (before_none, check_resize_u8),
+    "ssim_u8": (before_none, check_ssim_u8),
 }
 
 # Launching wrappers without a checker of their own, each with the reason.  test_every_launching_wrapper_has_a_checker allows exactly these.
@@ -1650,8 +1723,6 @@ UNCHECKED = {
                           "bit for bit against torch",
     "conv_weights_bf16": "raw device pointers in its table, as dense_weights_bf16; its copies are the operands of the bf16 tc_conv checks "
                          "and are pinned bit for bit in tests/test_train_bf16_gpu.py",
-    "ssim_u8": "the per-window fp32 bar (cancellation in E[x^2] - E[x]^2) is not derived yet; tests/test_eval_gpu.py compares it with the "
-               "reference metric",
 }
 
 

@@ -1,6 +1,6 @@
 """Every GEMM, convolution, attention, weight-gradient and codebook-lookup launch of the real workloads, and every GroupNorm / LayerNorm
 (forward, statistics, backward), column-sum, softmax-backward, cross-entropy-gradient, embedding-gradient, GELU, lincomb3, Adam, Keras AdamW,
-sumsq, split / bf16 conversion and dropout launch, checked against fp64 on its own operands (tests/launch_checks.py: references and bars).  The kernel tests pin each entry point at a few hand-picked shapes; the workloads
+sumsq, split / bf16 conversion and dropout launch, and the evaluation's resize, pair sums and SSIM, checked against fp64 on its own operands (tests/launch_checks.py: references and bars).  The kernel tests pin each entry point at a few hand-picked shapes; the workloads
 call the same entry points at dozens of others (tile shapes, tails, split-K and tile walks all depend on the shape), which were otherwise
 only held by loose end-to-end bars.
 
@@ -43,6 +43,7 @@ Normalisation, reduction, optimizer and elementwise wrappers (same card; the 14 
       0.34, pose_loss_grad 0.29, vq_ema_update 0.25, vq_ema_stats 0.20, pose_postprocess 0.12, cameras_prepare 0.089, vq_prepare_codebook
       0.078, row_mean 0.052, cameras_from_relative 0.037, cross_entropy_rows 0.011, l1_grad 0.011; bit-exact: u8_to_unit, unit_to_u8, the
       layout conversions, gather_rows, vq_prepare_codebook_f16, migt_embed, argmax_rows, image_pair_sums, resize_u8 (evaluation).
+  ssim_u8 0.014 (evaluation, K1 = 1; exact integer window moments, S in fp64: a bar of about 1e-14 of S).
   The whole file ran in about 55 s with 19 workloads; the three fp32 medium and full-size steps add 5 s or less each.  The largest GroupNorm mean^2 / var above comes from synthetic random-weight models.
 """
 import os
@@ -293,7 +294,7 @@ WORKLOADS = {
                                          ("row_mean", "float32"), ("argmax_rows", "float32"), ("migt_embed", "int32"),
                                          ("pose_postprocess", "float32"), ("layernorm", "float32"), ("gn_mean_rstd", "float32"),
                                          ("groupnorm", "float32")}),
-    "evaluation": (_evaluation, {("resize_u8", "uint8"), ("image_pair_sums", "uint8")}),
+    "evaluation": (_evaluation, {("resize_u8", "uint8"), ("image_pair_sums", "uint8"), ("ssim_u8", "uint8")}),
     "migt-train-fp32-small": (lambda mp, L: _migt_step(dict(MIGT_TRAIN, gradient_clip_val=1.0), 2, 4, "fp32", 4900, full=True),
                               {("adamw_keras", "float32"), ("sumsq", "float32")}),
     "migt-train-bf16-small": (lambda mp, L: _migt_step(dict(SMALL_MIGT_BF16, gradient_clip_val=1.0), 2, 5, "bf16", 5000, full=True),

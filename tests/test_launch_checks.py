@@ -1191,19 +1191,113 @@ def test_quantizer_ema_and_commit():
     assert_pass_and_catch("vq_prepare_codebook", L.vq_prepare_codebook, lambda ba: (et2, sq), lambda ba: (et2, (emb.double()[:-1] ** 2).sum(0).float()), emb)
 
 
-@pytest.mark.parametrize("method", ["nearest", "bilinear"])
-def test_resize_u8(method):
-    """The fp64 restatement accepts torch's uint8 resize of the same image (nearest: F.interpolate; bilinear: the same formula) and rejects
-    the image shifted by one source row."""
-    g = gen(127)
-    h = 48 if method == "bilinear" else 12
-    x = torch.randint(0, 256, (2, h, h, 3), generator=g, dtype=torch.uint8)
-    size = 32
+def _torch_resize(x, size, method):
     v = x.permute(0, 3, 1, 2).float() / 255.0
     if method == "nearest":
         y = F.interpolate(v, size=(size, size), mode="nearest")
     else:
         y = F.interpolate(v, size=(size, size), mode="bilinear", align_corners=False)
-    good = (y.clamp(0, 1) * 255.0).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
-    bad = torch.roll(good, 1, 1)
-    assert_pass_and_catch("resize_u8", L.resize_u8, lambda ba: good, lambda ba: bad, x, size, method)
+    return (y.clamp(0, 1) * 255.0).to(torch.uint8).permute(0, 2, 3, 1).contiguous()
+
+
+@pytest.mark.parametrize("method,hw", [pytest.param("nearest", None, id="nearest"), pytest.param("bilinear", None, id="bilinear")]
+                         + [pytest.param(None, hw, id=f"{hw[0]}x{hw[1]}") for hw in ((96, 160), (160, 96), (128, 200), (200, 128), (480, 640))])
+def test_resize_u8(method, hw):
+    """The fp64 restatement accepts torch's uint8 resize of the same image (nearest: F.interpolate; bilinear: the same formula) and rejects
+    the image shifted by one source row.  Non-square frames to 128 under the default rule: the method follows the height (96 x 160 grows
+    with nearest, 160 x 96 shrinks bilinearly), and a width-keyed choice is rejected; 128 x 200 and 200 x 128 must come back as the input
+    itself, and a resized copy is rejected."""
+    g = gen(127)
+    if hw is None:
+        h = 48 if method == "bilinear" else 12
+        x = torch.randint(0, 256, (2, h, h, 3), generator=g, dtype=torch.uint8)
+        size = 32
+        good = _torch_resize(x, size, method)
+        assert_pass_and_catch("resize_u8", L.resize_u8, lambda ba: good, lambda ba: torch.roll(good, 1, 1), x, size, method)
+        return
+    h, w = hw
+    x = torch.randint(0, 256, (2, h, w, 3), generator=g, dtype=torch.uint8)
+    size = 128
+    by_w = _torch_resize(x, size, "nearest" if size > w else "bilinear")
+    if size in (h, w):
+        assert_pass_and_catch("resize_u8", L.resize_u8, lambda ba: ba["x_u8"], lambda ba: by_w, x, size)
+        return
+    good = _torch_resize(x, size, "nearest" if size > h else "bilinear")
+    bad = torch.roll(good, 1, 1) if (size > h) == (size > w) else by_w
+    assert_pass_and_catch("resize_u8", L.resize_u8, lambda ba: good, lambda ba: bad, x, size)
+
+
+# ----------------------------------------------------------------------------------------------- SSIM
+def _ssim_ld(a, b, k1=0.01, k2=0.03):
+    """ssim() (metrics.py:17-73) in numpy long double, in the reference's own order: 1/49 box means of X = x / 255, X^2, XY, then
+    49/48 (E[XY] - E[X] E[Y]).  Long double carries 64 significant bits, so a flat window's cancellation costs ~1e-17 of S."""
+    assert np.finfo(np.longdouble).nmant >= 63
+    from numpy.lib.stride_tricks import sliding_window_view
+    X, Y = a.numpy().astype(np.longdouble) / 255, b.numpy().astype(np.longdouble) / 255
+    box = lambda t: sliding_window_view(t, (7, 7), axis=(1, 2)).sum((-2, -1)) / 49
+    ux, uy, uxx, uyy, uxy = box(X), box(Y), box(X * X), box(Y * Y), box(X * Y)
+    cn = np.longdouble(49) / 48
+    vx, vy, vxy = cn * (uxx - ux * ux), cn * (uyy - uy * uy), cn * (uxy - ux * uy)
+    C1, C2 = np.longdouble(float(k1) * float(k1)), np.longdouble(float(k2) * float(k2))        # fp64 K^2, as the kernel takes it
+    S = (2 * ux * uy + C1) * (2 * vxy + C2) / ((ux * ux + uy * uy + C1) * (vx + vy + C2))
+    return torch.from_numpy(S.reshape(S.shape[0], -1).mean(1).astype(np.float64))
+
+
+def _ssim_f32(a, b, k1=0.01, k2=0.03):
+    """The parent kernel's arithmetic in torch fp32: exact window sums, then means, E[x^2] - E[x]^2 and S one fp32 operation at a time."""
+    sx, sy, sxx, syy, sxy = (lc.box7(t).float() for t in (a, b, a.long() * a.long(), b.long() * b.long(), a.long() * b.long()))
+    d1, d2, cn = 49.0 * 255.0, 49.0 * 65025.0, torch.tensor(49.0 / 48.0, dtype=torch.float32)
+    ux, uy, uxx, uyy, uxy = sx / d1, sy / d1, sxx / d2, syy / d2, sxy / d2
+    vx, vy, vxy = cn * (uxx - ux * ux), cn * (uyy - uy * uy), cn * (uxy - ux * uy)
+    C1, C2 = lc.f32(lc.f32(k1) * lc.f32(k1)), lc.f32(lc.f32(k2) * lc.f32(k2))
+    S = ((2.0 * ux * uy + C1) * (2.0 * vxy + C2)) / ((ux * ux + uy * uy + C1) * (vx + vy + C2))
+    return S.double().reshape(S.shape[0], -1).mean(1)
+
+
+def test_ssim_u8_flat_level_pairs_and_fp32_moments():
+    """Flat images at level pairs 1 to 3 apart: the variances are exactly 0 and C2 dominates B2, so the fp32 E[x^2] - E[x]^2 of the
+    parent kernel leaves ~1e-4 in S (199 / 196, 224 / 223 are the worst) in every window alike.  The long-double restatement passes
+    (K1 = 0.01 and the Evaluator's K1 = 1), the fp32 one is caught."""
+    pairs = [(199, 196), (224, 223), (100, 101), (37, 40), (255, 254), (1, 0), (128, 128)]
+    a = torch.tensor([p[0] for p in pairs], dtype=torch.uint8)[:, None, None, None].expand(-1, 9, 11, 1).contiguous()
+    b = torch.tensor([p[1] for p in pairs], dtype=torch.uint8)[:, None, None, None].expand(-1, 9, 11, 1).contiguous()
+    for k1 in (0.01, 1.0):
+        good, bad = _ssim_ld(a, b, k1), _ssim_f32(a, b, k1)
+        print(f"[ssim flat K1={k1}] fp32 moments off by {float((bad - good).abs().max()):.3g}")
+        assert_pass_and_catch("ssim_u8", L.ssim_u8, lambda ba: good, lambda ba: bad, a, b, k1=k1)
+
+
+def test_ssim_u8_windows_channels_images_constants():
+    """Noisy synthetic pairs 13 x 29 x 3: the long-double restatement passes; dropping the last row or the last column of windows,
+    pairing a's channel 0 with b's channel 1, swapping the two images' results, or using K1 = 0.01 where 1 was asked are caught."""
+    from oracle import synth
+    g = gen(131)
+    a = synth.make_images_uint8(1, 2, size=32, seed=7)[0][:, :13, :29].contiguous()
+    b = (a.int() + torch.randint(-30, 31, a.shape, generator=g)).clamp(0, 255).to(torch.uint8)
+    good = _ssim_ld(a, b)
+    mutants = {"last window row": _ssim_ld(a[:, :-1], b[:, :-1]), "last window column": _ssim_ld(a[:, :, :-1], b[:, :, :-1]),
+               "channels": _ssim_ld(a, b[..., [1, 0, 2]]), "images": good[[1, 0]]}
+    for name, bad in mutants.items():
+        print(f"[ssim {name}]", end=" ")
+        assert_pass_and_catch("ssim_u8", L.ssim_u8, lambda ba: good, lambda ba: bad, a, b)
+    assert_pass_and_catch("ssim_u8", L.ssim_u8, lambda ba: _ssim_ld(a, b, 1.0), lambda ba: good, a, b, k1=1.0)
+    assert_pass_and_catch("ssim_u8", L.ssim_u8, lambda ba: _ssim_ld(a, b, 0.01, 0.1), lambda ba: good, a, b, k2=0.1)
+
+
+def test_ssim_u8_rejects_mismatched_images_before_any_launch(monkeypatch):
+    """a and b of different shapes (a smaller b would be read past its end by the kernel): a ValueError before the library is called."""
+    calls = []
+
+    class Lib:
+        def __getattr__(self, name):
+            return lambda *args: calls.append(name) or 0
+    monkeypatch.setattr(L, "load", lambda require_device=False: Lib())
+    a = torch.zeros(2, 16, 16, 3, dtype=torch.uint8)
+    for b in (torch.zeros(2, 8, 16, 3, dtype=torch.uint8), torch.zeros(2, 16, 15, 3, dtype=torch.uint8), torch.zeros(1, 16, 16, 3, dtype=torch.uint8),
+              torch.zeros(2, 16, 16, 1, dtype=torch.uint8), a[0]):
+        for k1 in (None, 1.0):
+            with pytest.raises(ValueError, match="one shape"):
+                L.ssim_u8(a, b, k1=k1)
+            with pytest.raises(ValueError, match="one shape"):
+                L.ssim_u8(b, a, k1=k1)
+    assert not calls

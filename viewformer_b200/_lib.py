@@ -209,15 +209,17 @@ def nhwc_to_nchw(x):
 
 
 def resize_u8(x_u8, size, method=None):
-    """data/_common.py:19-44 (resize_th) for uint8 NHWC images [N,H,W,C] -> [N,size,size,C]: bilinear (align_corners=False) when
-    shrinking, nearest when growing (or the explicit ``method``)."""
+    """data/_common.py:19-62 (resize, then resize_th) for uint8 NHWC images [N,H,W,C] -> [N,size,size,C]: bilinear (align_corners=False)
+    when the height shrinks, nearest when it grows (or the explicit ``method``).  The input comes back unchanged when W == size (resize()
+    tests shape[-2] of NHWC) or H == size (resize_th() tests shape[-2] of NCHW), so a non-square frame with one side already at ``size``
+    stays non-square, as in the reference."""
     lib = load(True)
     _dev(x_u8, torch.uint8)
     n, h, w, c = x_u8.shape
-    if w == size and h == size:
+    if w == size or h == size:
         return x_u8
     if method is None:
-        method = "nearest" if size > w else "bilinear"
+        method = "nearest" if size > h else "bilinear"
     assert method in ("nearest", "bilinear")
     out = torch.empty((n, size, size, c), dtype=torch.uint8, device=x_u8.device)
     _check(lib.vf_resize_u8(_p(x_u8), n, h, w, c, size, size, int(method == "bilinear"), _p(out), _stream()))
@@ -240,6 +242,8 @@ def ssim_u8(a_u8, b_u8, k1=None, k2=None):
     """utils/metrics.py:17-73 on uint8 NHWC images -> float64 [N] mean SSIM per image.  ``k1`` / ``k2``: the K1 / K2 of ``ssim()``
     (defaults 0.01 / 0.03); the reference's SSIMMetric passes K1 = 1 (metrics.py:183)."""
     lib = load(True)
+    if a_u8.dim() != 4 or a_u8.shape != b_u8.shape:
+        raise ValueError(f"ssim_u8: a and b must be uint8 [N,H,W,C] images of one shape, got {tuple(a_u8.shape)} and {tuple(b_u8.shape)}")
     _dev(a_u8, torch.uint8)
     _dev(b_u8, torch.uint8)
     n, h, w, c = a_u8.shape

@@ -75,33 +75,37 @@ __global__ void __launch_bounds__(256) pair_sums_kernel(const uint8_t* __restric
     }
 }
 
-// grid (chunks, N): every thread strides over the (H-6)(W-6)C window positions of one image; integer window sums are exact
+// grid (chunks, N): every thread strides over the (H-6)(W-6)C window positions of one image and adds its windows' S to out[n]; the integer
+// window sums are exact, and so are the variance and covariance numerators formed from them, so S is evaluated in fp64 from exact
+// integers.  In the reference's E[x^2] - E[x]^2 in fp32, one ulp of E[x^2] is a relative error of ~1e-4 in S wherever the window is flat
+// (the variances vanish and C2 dominates B2), and every window of a flat region carries it with the same sign.
 __global__ void __launch_bounds__(256) ssim_u8_kernel(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b, int H, int W, int C,
-                                                      float C1, float C2, double* __restrict__ out) {
+                                                      double C1, double C2, double* __restrict__ out) {
     __shared__ double sh[8];
     const int OH = H - 6, OW = W - 6;
     const long long total = (long long)OH * OW * C;
     const uint8_t* pa = a + (long long)blockIdx.y * H * W * C;
     const uint8_t* pb = b + (long long)blockIdx.y * H * W * C;
-    const float cov_norm = 49.f / 48.f;                   // C1 = (K1 R)^2, C2 = (K2 R)^2 with data range R = 1 come from the caller
+    // With X = x / 255 and window sums s = sum x, sxx = sum x^2 (49 pixels): ux uy = sx sy / M, and the sample (co)variance
+    // 49/48 (E[XY] - E[X] E[Y]) = (49 sxy - sx sy) / D.  C1 = (K1 R)^2, C2 = (K2 R)^2 with data range R = 1 come from the caller.
+    const double M = 49.0 * 49.0 * 65025.0, D = 48.0 * 49.0 * 65025.0;
     double acc = 0.0;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
         const int c = (int)(i % C);
         const long long r = i / C;
         const int ox = (int)(r % OW), oy = (int)(r / OW);
-        unsigned sx = 0, sy = 0, sxx = 0, syy = 0, sxy = 0;
+        int sx = 0, sy = 0, sxx = 0, syy = 0, sxy = 0;
         for (int dy = 0; dy < 7; ++dy)
             for (int dx = 0; dx < 7; ++dx) {
                 const long long o = ((long long)(oy + dy) * W + ox + dx) * C + c;
-                const unsigned xv = pa[o], yv = pb[o];
+                const int xv = pa[o], yv = pb[o];
                 sx += xv; sy += yv; sxx += xv * xv; syy += yv * yv; sxy += xv * yv;
             }
-        // window means of X = x/255 etc. (the reference filters with 1/49 weights in fp32; the integer sums here are exact)
-        const float ux = (float)sx / (49.f * 255.f), uy = (float)sy / (49.f * 255.f);
-        const float uxx = (float)sxx / (49.f * 65025.f), uyy = (float)syy / (49.f * 65025.f), uxy = (float)sxy / (49.f * 65025.f);
-        const float vx = cov_norm * (uxx - ux * ux), vy = cov_norm * (uyy - uy * uy), vxy = cov_norm * (uxy - ux * uy);
-        const float A1 = 2.f * ux * uy + C1, A2 = 2.f * vxy + C2, B1 = ux * ux + uy * uy + C1, B2 = vx + vy + C2;
-        acc += (double)((A1 * A2) / (B1 * B2));
+        // every product and numerator below is an integer of magnitude < 2^29: exact in int and in fp64
+        const int nx = 49 * sxx - sx * sx, ny = 49 * syy - sy * sy, nxy = 49 * sxy - sx * sy;
+        const double A1 = (double)(2 * sx * sy) / M + C1, B1 = (double)(sx * sx + sy * sy) / M + C1;
+        const double A2 = (double)(2 * nxy) / D + C2, B2 = (double)(nx + ny) / D + C2;
+        acc += (A1 * A2) / (B1 * B2);
     }
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
@@ -109,8 +113,14 @@ __global__ void __launch_bounds__(256) ssim_u8_kernel(const uint8_t* __restrict_
     if (threadIdx.x == 0) {
         double t = 0;
         for (int w = 0; w < 8; ++w) t += sh[w];
-        atomicAdd(out + blockIdx.y, t / (double)total);
+        atomicAdd(out + blockIdx.y, t);
     }
+}
+
+// the mean over the window positions, once the sum of every chunk is in: identical images give exactly 1
+__global__ void ssim_mean_kernel(double* __restrict__ out, int N, double total) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n < N) out[n] /= total;
 }
 
 }  // namespace
@@ -144,10 +154,11 @@ extern "C" int vf_ssim_u8_k(const void* a, const void* b, int N, int H, int W, i
     const long long total = (long long)(H - 6) * (W - 6) * C;
     int chunks = (int)((total + 255) / 256);
     if (chunks > 64) chunks = 64;
-    const float k1 = (float)K1, k2 = (float)K2;
     ssim_u8_kernel<<<dim3(chunks, N), 256, 0, vf_s(s)>>>(reinterpret_cast<const uint8_t*>(a), reinterpret_cast<const uint8_t*>(b), H, W, C,
-                                                         k1 * k1, k2 * k2, out);
+                                                         K1 * K1, K2 * K2, out);
     VF_CHECK_LAUNCH("vf_ssim_u8");
+    ssim_mean_kernel<<<(N + 255) / 256, 256, 0, vf_s(s)>>>(out, N, (double)total);
+    VF_CHECK_LAUNCH("vf_ssim_u8 (mean)");
     return VF_OK;
 }
 
