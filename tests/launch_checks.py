@@ -303,7 +303,7 @@ def check_tc_gemm(ba, result, st):
             res = view(st["res"], c_off, (M, N), (ldc, 1))[rows].double()
         ref, bar = _epilogue(acc, s, K, ba, bv, res, got_t.dtype == torch.bfloat16)
         got = view(got_t, c_off, (M, N), (ldc, 1))[rows].double()
-        worst = max(worst, ratio(((got - ref).abs() * keep), bar))
+        worst = max(worst, ratio(torch.where(keep, (got - ref).abs(), 0.0), bar))      # skipped tiles hold any bits, NaN included
         if f32 is not None and b16 is not None:
             worst = max(worst, bits_equal(view(b16, c_off, (M, N), (ldc, 1))[rows], view(f32, c_off, (M, N), (ldc, 1))[rows].to(torch.bfloat16)))
     gn = getattr(result, "_gn_sums", None)

@@ -105,6 +105,31 @@ def test_tc_gemm_c_off_window_batched_gelu_out2():
     assert run("tc_gemm", L.tc_gemm, bad_out2, A, B, out, **kw) == math.inf
 
 
+def test_tc_gemm_shared_operand_stride_zero():
+    """The shared-scene KV query's QK^T (MIGT._query_block): every query batch entry reads the one cached scene through a stride-0 batch
+    (b_bs[0] = 0) at b_off = d, head h at column h dh; the output rows have S_ctx + 64 columns, of which this GEMM writes the first S_ctx.
+    Mutant: query i reads the keys of scene i (the per-scene offset of an unshared cache where the batch stride is 0)."""
+    Nq, H, dh, S_ctx = 3, 2, 64, 128
+    d, ld = H * dh, S_ctx + 64
+    q = torch.randn(Nq * 64, 2 * d, generator=gen(15)).bfloat16()
+    kc = (torch.randn(Nq, S_ctx, 2 * d, generator=gen(16)) / 8).bfloat16()       # Nq scenes in storage, the call reads scene 0
+    out = torch.zeros(Nq, H, 64, ld)
+    kw = dict(M=64, N=S_ctx, K=dh, lda=2 * d, ldb=2 * d, ldc=ld, batch=(Nq, H), a_bs=(64 * 2 * d, dh), b_bs=(0, dh),
+              c_bs=(H * 64 * ld, 64 * ld), b_off=d)
+
+    def write(scene_of):
+        def w(ba):
+            out.zero_()
+            for i in range(Nq):
+                for h in range(H):
+                    qi = q[i * 64:(i + 1) * 64, h * dh:(h + 1) * dh]
+                    ks = kc[scene_of(i), :, d + h * dh:d + (h + 1) * dh]
+                    out[i, h, :, :S_ctx] = _gemm_ref(qi, ks).float()
+            return out
+        return w
+    assert_pass_and_catch("tc_gemm", L.tc_gemm, write(lambda i: 0), write(lambda i: i), q, kc, out, **kw)
+
+
 def test_tc_gemm_operand_readings():
     """TF32 truncation, split-fp16 pairs at lo_a / lo_b, k_offsets and the causal k-limit are read as the kernel reads them."""
     M, N, K = 96, 64, 64
@@ -129,15 +154,16 @@ def test_tc_gemm_operand_readings():
     kw = dict(M=M, N=N, K=K, lda=2 * la, ldb=2 * K, ldc=N, batch=(2, 1), c_bs=(M * N, 0), lo_a=la, lo_b=K, k_offsets=[0, 8])
     assert_pass_and_catch("tc_gemm", L.tc_gemm, lambda ba: outs.copy_(ref), lambda ba: outs.copy_(torch.stack([ref[0], ref[0]])),
                           Aop, Bop, outs, **kw)
-    # causal QK^T: only visible columns are compared
+    # causal QK^T: only visible columns are compared; the skipped tiles of a torch.empty buffer hold any bits, NaN and inf included
     S, blk = 256, 64
     q, k = torch.randn(S, 64, generator=gen(11)).bfloat16(), torch.randn(S, 64, generator=gen(12)).bfloat16()
     sc = torch.empty(S, S)
     full = (q.double() @ k.double().t()).float()
     vis = (torch.arange(S)[None, :] // blk) <= (torch.arange(S)[:, None] // blk)
+    junk = torch.tensor([1e30, math.nan, math.inf, -math.inf]).repeat(S * S // 4).reshape(S, S)
 
     def hidden_garbage(ba):
-        return sc.copy_(torch.where(vis, full, torch.full_like(full, 1e30)))
+        return sc.copy_(torch.where(vis, full, junk))
 
     def visible_garbage(ba):
         hidden_garbage(ba)
@@ -1098,6 +1124,19 @@ def test_softmax_rows_masks(fault):
     else:
         kw.update(mask_mode=1, row0=blk, cols=2 * S)
         good, bad = _masked_softmax(sc, S, 1, blk, row0=blk), _masked_softmax(sc, S, 1, blk)
+    assert_pass_and_catch("softmax_rows", L.softmax_rows, lambda ba: P.copy_(good), lambda ba: P.copy_(bad), sc, P, **kw)
+
+
+def test_softmax_rows_all_keys_bf16():
+    """The shared-scene KV query's softmax (MIGT._query_block): mask mode 0 over S_ctx + 64 columns, 64 rows per batch entry, bf16
+    probabilities.  Mutant: the last column (the query view's last own key) masked out."""
+    rows, cols = 2 * 2 * 64, 3 * 64 + 64
+    sc = torch.randn(rows, cols, generator=gen(125)) * 3
+    P = torch.empty(rows, cols, dtype=torch.bfloat16)
+    good = torch.softmax(sc.double(), 1).to(torch.bfloat16)
+    bad = torch.softmax(sc.double()[:, :-1], 1)
+    bad = torch.cat([bad, torch.zeros(rows, 1, dtype=torch.float64)], 1).to(torch.bfloat16)
+    kw = dict(rows_total=rows, rows_per_batch=64, cols=cols, ld_in=cols, ld_out=cols)
     assert_pass_and_catch("softmax_rows", L.softmax_rows, lambda ba: P.copy_(good), lambda ba: P.copy_(bad), sc, P, **kw)
 
 
