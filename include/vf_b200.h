@@ -44,6 +44,8 @@ int vf_device_check(void);
 /* out[r, :] = in[r*in_row_stride : +row_len] * (1/255) * 2 - 1 for r < rows (rows=1: flat array; rows=B with
  * in_row_stride = T*H*W*3 selects the first views of every scene without a gather copy) */
 int vf_u8_to_unit_f32(const uint8_t* in, float* out, int64_t rows, int64_t row_len, int64_t in_row_stride, vf_stream_t s);
+/* the same strided read of f32 images in [0, 1]: out = in * 2 - 1 (convert_image_dtype is the identity for float32 input) */
+int vf_f01_to_unit_f32(const float* in, float* out, int64_t rows, int64_t row_len, int64_t in_row_stride, vf_stream_t s);
 int vf_unit_f32_to_u8(const float* in, uint8_t* out, int64_t n, vf_stream_t s);      /* clip[-1,1]/2+.5 -> trunc(x*255.5) */
 int vf_nchw_to_nhwc_f32(const float* in, float* out, int N, int C, int H, int W, vf_stream_t s);
 int vf_nhwc_to_nchw_f32(const float* in, float* out, int N, int C, int H, int W, vf_stream_t s);
@@ -73,8 +75,9 @@ int vf_groupnorm_apply(const void* x, int x_dtype, const float* mean_rstd, const
                        int N, int H, int W, int C, int groups, float eps, int normalize, int swish,
                        int layout, void* y, int y_dtype, vf_stream_t s);
 
-/* Exact fp32 3x3 stride-1 pad-1 convolutions for the two tiny-channel layers (vqgan_th.py:159-163 conv_in 3->128,
- * :285-289 conv_out 128->3).  NHWC; weights [9*Cin, Cout] fp32 (k = tap*Cin + c). */
+/* Exact fp32 3x3 stride-1 pad-1 convolutions for the two tiny-channel layers (vqgan_th.py:159-163 conv_in C->128,
+ * :285-289 conv_out 128->C), C = 3 (RGB) or 4 (RGB + mask); other counts are rejected.  NHWC; weights [9*Cin, Cout] fp32
+ * (k = tap*Cin + c). */
 int vf_conv3x3_small_cin(const float* x, const float* w_kn, const float* bias, int N, int H, int W, int Cin, int Cout,
                          float* y, double* gn_sums /* optional [N][32][2]: GroupNorm(32) sums of y, Cout = 128 only */,
                          vf_stream_t s);
@@ -283,12 +286,14 @@ int vf_dense_weights_bf16(const vf_dense_weights_bf16_t* table, int n, vf_stream
  * Evaluation-side kernels (SURVEY.md §8 f2 / f3)
  *   vf_resize_u8: data/_common.py:19-44 (resize_th) on uint8 NHWC images: bilinear (align_corners = False) when `bilinear`, else
  *     torch 'nearest'; result = uint8(clamp(interp(x / 255), 0, 1) * 255).
+ *   vf_resize_f32: the same on f32 NHWC images in [0, 1]: result = clamp(interp(x), 0, 1), not quantised.
  *   vf_image_pair_sums: out[2n] = sum |a - b|, out[2n+1] = sum (a - b)^2 over image n (exact integers) -> MSE / MAE / RMSE / PSNR.
  *   vf_ssim_u8: utils/metrics.py:17-73 (7x7 uniform window, VALID, sample covariance, data range 1); out[n] = mean SSIM of image n.
  *   vf_ssim_u8_k: the same with explicit K1 / K2 — utils/metrics.py:176-184 (SSIMMetric, the one the evaluators use) calls
  *     ssim(gt, images, 1), i.e. K1 = 1, so C1 = 1 instead of 1e-4.
  * ---------------------------------------------------------------------------------------- */
 int vf_resize_u8(const void* x_u8, int N, int H, int W, int C, int OH, int OW, int bilinear, void* y_u8, vf_stream_t s);
+int vf_resize_f32(const float* x, int N, int H, int W, int C, int OH, int OW, int bilinear, float* y, vf_stream_t s);
 int vf_image_pair_sums(const void* a_u8, const void* b_u8, int N, int64_t per_image, uint64_t* out, vf_stream_t s);
 int vf_ssim_u8(const void* a_u8, const void* b_u8, int N, int H, int W, int C, double* out, vf_stream_t s);
 int vf_ssim_u8_k(const void* a_u8, const void* b_u8, int N, int H, int W, int C, double K1, double K2, double* out, vf_stream_t s);

@@ -43,7 +43,9 @@ const char* vf_model_last_error(void);
  * precision: "mixed" (codebook default: bit-exact codes, bf16 decoder), "bf16", "tf32", "fp32".  device: CUDA ordinal. */
 int vf_vq_create(const char* config_json, const char* checkpoint_dir, const char* precision, int device, int64_t seed, vf_handle_t* out);
 int vf_vq_info(vf_handle_t h, int* image_size, int* tokens_per_side, int* n_embed, int* in_channels);
-/* images: [n,S,S,C] uint8 / [n,C,S,S] f32 in [-1,1] / [n,S,S,C] f32 per `layout`; codes: int64 [n,s,s] */
+/* images: [n,S,S,C] uint8 / [n,C,S,S] f32 in [-1,1] / [n,S,S,C] f32 per `layout`; codes: int64 [n,s,s].  C is the codebook's
+ * in_channels (vf_vq_info: 3 for RGB, 4 for RGB + mask) for vf_vq_encode, its out_ch (equal in every released codebook) for
+ * vf_vq_decode_code. */
 int vf_vq_encode(vf_handle_t h, const void* images, int layout, int n, int64_t* codes, vf_cuda_stream_t stream);
 int vf_vq_decode_code(vf_handle_t h, const int64_t* codes, int n, void* images, int layout, vf_cuda_stream_t stream);
 
@@ -59,7 +61,7 @@ int vf_migt_prefill_context(vf_handle_t h, const int32_t* context_ids, const flo
 /* query_poses f32 [Nq,7]; Nq = B of the cache (one query per scene) or any Nq when the cache holds one scene; codes int64 [Nq,s,s] */
 int vf_migt_query(vf_handle_t h, vf_handle_t cache, const float* query_poses, int Nq, int64_t* codes, vf_cuda_stream_t stream);
 
-/* images uint8 [B,T,S,S,3], cameras f32 [B,T,7] (world poses: xyz + wxyz quaternion) -> generated_images uint8 [B,S,S,3],
+/* images uint8 [B,T,S,S,in_channels], cameras f32 [B,T,7] (world poses: xyz + wxyz quaternion) -> generated_images uint8 [B,S,S,out_ch],
  * generated_cameras f32 [B,7] (NULL to skip; written only by localising models) */
 int vf_generate(vf_handle_t transformer, vf_handle_t codebook, const uint8_t* images, const float* cameras, int B, int T,
                 uint8_t* generated_images, float* generated_cameras, vf_cuda_stream_t stream);

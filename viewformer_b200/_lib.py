@@ -17,14 +17,14 @@ ACT_NONE, ACT_GELU = 0, 1
 BIAS_NONE, BIAS_N, BIAS_M = 0, 1, 2
 
 EXPORTS = [
-    "vf_last_error", "vf_version", "vf_sizeof_simt_gemm", "vf_sizeof_tc_gemm", "vf_device_check", "vf_u8_to_unit_f32", "vf_unit_f32_to_u8",
+    "vf_last_error", "vf_version", "vf_sizeof_simt_gemm", "vf_sizeof_tc_gemm", "vf_device_check", "vf_u8_to_unit_f32", "vf_f01_to_unit_f32", "vf_unit_f32_to_u8",
     "vf_nchw_to_nhwc_f32", "vf_nhwc_to_nchw_f32", "vf_groupnorm_stats", "vf_groupnorm_apply", "vf_layernorm",
     "vf_simt_gemm", "vf_tc_gemm", "vf_tc_gemm_plan", "vf_vq_lookup", "vf_gather_rows", "vf_vq_ema_stats", "vf_vq_ema_update", "vf_vq_commit_grad",
     "vf_vq_prepare_codebook", "vf_migt_embed", "vf_softmax_rows", "vf_argmax_rows", "vf_pose_postprocess",
     "vf_cameras_prepare", "vf_cameras_from_relative",
     "vf_conv3x3_small_cin", "vf_conv3x3_small_cout", "vf_groupnorm_finalize", "vf_split_f16x2", "vf_attn_block_causal_decode", "vf_attn_block_multiend",
     "vf_cross_entropy_rows", "vf_pose_loss_rows", "vf_row_mean",
-    "vf_vq_prepare_codebook_f16", "vf_vq_lookup_fused", "vf_resize_u8", "vf_image_pair_sums", "vf_ssim_u8", "vf_ssim_u8_k",
+    "vf_vq_prepare_codebook_f16", "vf_vq_lookup_fused", "vf_resize_u8", "vf_resize_f32", "vf_image_pair_sums", "vf_ssim_u8", "vf_ssim_u8_k",
     "vf_conv_wgrad", "vf_pad_transpose_split", "vf_pad_transpose_bf16", "vf_conv_weights_bf16", "vf_sum_splits", "vf_col_sums", "vf_groupnorm_bwd", "vf_softmax_bwd_rows", "vf_l1_grad", "vf_lincomb3", "vf_sumpool2x2", "vf_adam",
     "vf_layernorm_bwd", "vf_gelu_fwd", "vf_gelu_bwd", "vf_migt_embed_bwd", "vf_cross_entropy_grad", "vf_pose_loss_grad", "vf_adamw_keras", "vf_sumsq", "vf_dropout",
     "vf_attn_multiend_train", "vf_attn_multiend_bwd", "vf_to_bf16", "vf_dense_weights_bf16",
@@ -431,7 +431,7 @@ def s2d_coffs(c):
 
 
 def conv3x3_small_cin(x, w_kn, bias, gn_groups=0):
-    """exact fp32 conv_in (Cin=3): x f32 [N,H,W,3], w_kn [27, Cout].  ``gn_groups=32`` (Cout = 128) also accumulates the
+    """exact fp32 conv_in (Cin = 3 or 4): x f32 [N,H,W,Cin], w_kn [9 Cin, Cout].  ``gn_groups=32`` (Cout = 128) also accumulates the
     GroupNorm statistics of the output and attaches them as ``_gn_sums`` (consumed by ``groupnorm``)."""
     lib = load(True)
     _dev(x, torch.float32)
@@ -448,7 +448,7 @@ def conv3x3_small_cin(x, w_kn, bias, gn_groups=0):
 
 
 def conv3x3_small_cout(x, w_kn, bias):
-    """exact fp32-accumulate conv_out (128 -> 3): x f32|bf16 [N,H,W,128], w_kn [1152, 3]."""
+    """exact fp32-accumulate conv_out (128 -> Cout, Cout = 3 or 4): x f32|bf16 [N,H,W,128], w_kn [1152, Cout]."""
     lib = load(True)
     _dev(x)
     n, h, w, cin = x.shape

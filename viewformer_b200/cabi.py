@@ -83,8 +83,8 @@ def vq_info(h):
 
 
 def vq_encode(h, images_ptr, layout, n, codes_ptr, stream):
-    """images: layout 0 = uint8 NHWC [n,S,S,3] (evaluate_transformer.py:105-110), 1 = f32 NCHW in [-1,1] (generate_codes.py:21-26),
-    2 = f32 NHWC.  codes: int64 [n,s,s] (vqgan_th.py:379-383 ``[-1]``)."""
+    """images with C = the model's in_channels: layout 0 = uint8 NHWC [n,S,S,C] (evaluate_transformer.py:105-110), 1 = f32 NCHW in
+    [-1,1] (generate_codes.py:21-26), 2 = f32 NHWC.  codes: int64 [n,s,s] (vqgan_th.py:379-383 ``[-1]``)."""
     m = _models[h]
     S, s, _, C = vq_info(h)
     with torch.cuda.device(m.device), _stream(m, stream):
@@ -101,9 +101,11 @@ def vq_encode(h, images_ptr, layout, n, codes_ptr, stream):
 
 
 def vq_decode_code(h, codes_ptr, n, images_ptr, layout, stream):
-    """codes int64 [n,s,s] -> images in the given layout (vqgan_th.py:390-393; layout 0 applies evaluate_transformer.py:127-129)."""
+    """codes int64 [n,s,s] -> images with C = the model's out_ch in the given layout (vqgan_th.py:390-393; layout 0 applies
+    evaluate_transformer.py:127-129)."""
     m = _models[h]
-    S, s, _, C = vq_info(h)
+    S, s, _, _ = vq_info(h)
+    C = int(m.config.out_ch)
     with torch.cuda.device(m.device), _stream(m, stream):
         codes = _wrap(codes_ptr, (n, s, s), "i64", m.device)
         if layout == 0:
@@ -168,14 +170,15 @@ def migt_query(h, cache_h, poses_ptr, Nq, codes_ptr, stream):
 
 
 def generate(h_migt, h_vq, images_ptr, cameras_ptr, B, T, out_images_ptr, out_cameras_ptr, stream):
-    """generate_batch_predictions (evaluate_transformer.py:97-146): images uint8 [B,T,S,S,3], cameras f32 [B,T,7] ->
-    generated_images uint8 [B,S,S,3] (+ generated_cameras f32 [B,7] if the pointer is non-null and the model localises)."""
+    """generate_batch_predictions (evaluate_transformer.py:97-146): images uint8 [B,T,S,S,in_channels], cameras f32 [B,T,7] ->
+    generated_images uint8 [B,S,S,out_ch] (+ generated_cameras f32 [B,7] if the pointer is non-null and the model localises)."""
     tr, vq = _models[h_migt], _models[h_vq]
     S, _, _, C = vq_info(h_vq)
+    C_out = int(vq.config.out_ch)
     from .generate import generate_batch_predictions
     with torch.cuda.device(vq.device), _stream(vq, stream):
         out = generate_batch_predictions(tr, vq, _wrap(images_ptr, (B, T, S, S, C), "u8", vq.device), _wrap(cameras_ptr, (B, T, 7), "f32", vq.device))
-        _wrap(out_images_ptr, (B, S, S, C), "u8", vq.device).copy_(torch.as_tensor(out["generated_images"]).to(vq.device))
+        _wrap(out_images_ptr, (B, S, S, C_out), "u8", vq.device).copy_(torch.as_tensor(out["generated_images"]).to(vq.device))
         if out_cameras_ptr:
             _wrap(out_cameras_ptr, (B, 7), "f32", vq.device).copy_(torch.as_tensor(out["generated_cameras"], dtype=torch.float32).to(vq.device))
     return 0

@@ -1,7 +1,7 @@
 // Exact fp32 3x3 convolutions for the two layers whose channel counts are too small for a tensor-core tile:
-//   conv_in   3 -> 128 @128x128  (viewformer/models/vqgan_th.py:159-163): output-write bound
-//   conv_out  128 -> 3 @128x128  (vqgan_th.py:285-289): input-read bound
-// Both are stride-1, pad-1, NHWC.
+//   conv_in   C -> 128 @128x128  (viewformer/models/vqgan_th.py:159-163): output-write bound
+//   conv_out  128 -> C @128x128  (vqgan_th.py:285-289): input-read bound
+// C = 3 (RGB) or 4 (RGB + mask: the CO3Dv2 codebooks, data/loaders/co3dv2.py:149-153).  Both are stride-1, pad-1, NHWC.
 #include "vf_common.cuh"
 
 namespace {
@@ -66,20 +66,23 @@ __global__ void __launch_bounds__(256) conv3x3_small_cin_kernel(const float* __r
 }
 
 // ------------------------------------------------------------------------------------------------
-// Cin = 3, Cout = 128 (conv_in of the released models).  Block = 8 warps over a ROWS x 64-pixel tile:
-//   * the (ROWS+2) x 66 x 3 input patch is staged once in shared memory (zero padded), so every input read in the main loop
-//     is a warp-uniform LDS.128 broadcast;
-//   * lane l owns output channels 4l..4l+3 (exactly one GroupNorm(32) group) and keeps its 27 x 4 weights in registers;
+// Cin = CIN (3 or 4), Cout = 128 (conv_in of the released models).  Block = 8 warps over a ROWS x 64-pixel tile:
+//   * the (ROWS+2) x 66 x CIN input patch is staged once in shared memory (zero padded to 4 floats per pixel), so every input read in
+//     the main loop is a warp-uniform LDS.128 broadcast;
+//   * lane l owns output channels 4l..4l+3 (exactly one GroupNorm(32) group) and keeps its 9 CIN x 4 weights in registers;
 //   * every store is one coalesced 512-byte pixel row;
 //   * the GroupNorm statistics of the OUTPUT (sum, sum of squares per (image, group)) are accumulated on the fly —
 //     one fp64 RED per (block, group, statistic) — which removes the separate 2.4 GB statistics pass of the encoder.
-// FFMA-bound: 27 * 128 FMA per pixel.
+// FFMA-bound: 9 CIN * 128 FMA per pixel.  The FMA order is (dy, dx, channel) for every CIN.
 // ------------------------------------------------------------------------------------------------
 constexpr int CI_ROWS = 4, CI_W = 64;
-__global__ void __launch_bounds__(256) conv3x3_cin3_cout128_kernel(const float* __restrict__ x, const float* __restrict__ w_kn,
-                                                                   const float* __restrict__ bias, int N, int H, int W,
-                                                                   float* __restrict__ y, double* __restrict__ gn_sums) {
-    // patch[r][c][k]: r = 0..ROWS+1 input rows, c = 0..CI_W+1 input columns, k = 0..2 channels, padded to 4 floats per pixel
+template <int CIN>
+__global__ void __launch_bounds__(256) conv3x3_cin_cout128_kernel(const float* __restrict__ x, const float* __restrict__ w_kn,
+                                                                  const float* __restrict__ bias, int N, int H, int W,
+                                                                  float* __restrict__ y, double* __restrict__ gn_sums) {
+    static_assert(CIN == 3 || CIN == 4, "conv_in: 3 or 4 input channels");
+    constexpr int KR = 3 * CIN;                          // inputs per filter row: 3 columns x CIN channels
+    // patch[r][c][k]: r = 0..ROWS+1 input rows, c = 0..CI_W+1 input columns, k = 0..CIN-1 channels, padded to 4 floats per pixel
     __shared__ __align__(16) float patch[(CI_ROWS + 2) * (CI_W + 2) * 4];
     __shared__ float red[8][32][2];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -89,14 +92,15 @@ __global__ void __launch_bounds__(256) conv3x3_cin3_cout128_kernel(const float* 
         const int iy = y0 + r - 1, ix = x0 + c - 1;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
-            const float* px = x + (((int64_t)n * H + iy) * W + ix) * 3;
+            const float* px = x + (((int64_t)n * H + iy) * W + ix) * CIN;
             v.x = __ldg(px); v.y = __ldg(px + 1); v.z = __ldg(px + 2);
+            if (CIN == 4) v.w = __ldg(px + 3);
         }
         *reinterpret_cast<float4*>(&patch[i * 4]) = v;
     }
-    float4 wr[27];
+    float4 wr[3 * KR];
 #pragma unroll
-    for (int k = 0; k < 27; ++k) wr[k] = __ldg(reinterpret_cast<const float4*>(w_kn + k * 128) + lane);
+    for (int k = 0; k < 3 * KR; ++k) wr[k] = __ldg(reinterpret_cast<const float4*>(w_kn + k * 128) + lane);
     const float4 b4 = bias ? __ldg(reinterpret_cast<const float4*>(bias) + lane) : make_float4(0.f, 0.f, 0.f, 0.f);
     __syncthreads();
     float gs = 0.f, gq = 0.f;
@@ -112,27 +116,37 @@ __global__ void __launch_bounds__(256) conv3x3_cin3_cout128_kernel(const float* 
 #pragma unroll
             for (int dy = 0; dy < 3; ++dy) {
                 const float4* row = reinterpret_cast<const float4*>(&patch[((r + dy) * (CI_W + 2) + c) * 4]);
-                const float4 p0 = row[0], p1 = row[1], p2 = row[2], p3 = row[3];      // input columns c-1 .. c+2 (tile-relative + 1)
-                const float in0[9] = {p0.x, p0.y, p0.z, p1.x, p1.y, p1.z, p2.x, p2.y, p2.z};
-                const float in1[9] = {p1.x, p1.y, p1.z, p2.x, p2.y, p2.z, p3.x, p3.y, p3.z};
+                const float4 p[4] = {row[0], row[1], row[2], row[3]};      // input columns c-1 .. c+2 (tile-relative + 1)
+                float in0[KR], in1[KR];
 #pragma unroll
-                for (int k = 0; k < 9; ++k) {
-                    const float4 w4 = wr[dy * 9 + k];
+                for (int dx = 0; dx < 3; ++dx) {
+                    const float q0[4] = {p[dx].x, p[dx].y, p[dx].z, p[dx].w};
+                    const float q1[4] = {p[dx + 1].x, p[dx + 1].y, p[dx + 1].z, p[dx + 1].w};
+#pragma unroll
+                    for (int ch = 0; ch < CIN; ++ch) {
+                        in0[dx * CIN + ch] = q0[ch];
+                        in1[dx * CIN + ch] = q1[ch];
+                    }
+                }
+#pragma unroll
+                for (int k = 0; k < KR; ++k) {
+                    const float4 w4 = wr[dy * KR + k];
                     a0.x = fmaf(in0[k], w4.x, a0.x); a0.y = fmaf(in0[k], w4.y, a0.y); a0.z = fmaf(in0[k], w4.z, a0.z); a0.w = fmaf(in0[k], w4.w, a0.w);
                     a1.x = fmaf(in1[k], w4.x, a1.x); a1.y = fmaf(in1[k], w4.y, a1.y); a1.z = fmaf(in1[k], w4.z, a1.z); a1.w = fmaf(in1[k], w4.w, a1.w);
                 }
             }
             const int xx = x0 + c;
             float* o = y + (((int64_t)n * H + yy) * W + xx) * 128 + lane * 4;
+            // sums of squares contracted explicitly, so that every CIN instance rounds them alike
             if (xx < W) {
                 *reinterpret_cast<float4*>(o) = a0;
                 gs += (a0.x + a0.y) + (a0.z + a0.w);
-                gq += (a0.x * a0.x + a0.y * a0.y) + (a0.z * a0.z + a0.w * a0.w);
+                gq += fmaf(a0.x, a0.x, a0.y * a0.y) + fmaf(a0.z, a0.z, a0.w * a0.w);
             }
             if (xx + 1 < W) {
                 *reinterpret_cast<float4*>(o + 128) = a1;
                 gs += (a1.x + a1.y) + (a1.z + a1.w);
-                gq += (a1.x * a1.x + a1.y * a1.y) + (a1.z * a1.z + a1.w * a1.w);
+                gq += fmaf(a1.x, a1.x, a1.y * a1.y) + fmaf(a1.z, a1.z, a1.w * a1.w);
             }
         }
     }
@@ -150,6 +164,7 @@ __global__ void __launch_bounds__(256) conv3x3_cin3_cout128_kernel(const float* 
     }
 }
 
+
 // ------------------------------------------------------------------------------------------------
 // Small Cout (<= 4), Cin == 128: one warp walks a run of pixels along x; lane l owns input channels 4l..4l+3 and keeps
 // its 9 x 4 x COUT weights in registers; per pixel 9 coalesced 512-byte loads, COUT warp reductions.
@@ -163,21 +178,22 @@ template <> __device__ __forceinline__ float4 ld4<__nv_bfloat16>(const __nv_bflo
     return make_float4(fa.x, fa.y, fb.x, fb.y);
 }
 
-// COUT = 3, Cin = 128 (conv_out of the released models): a warp walks a 32-pixel run of one row four pixels at a time.
+// COUT = 3 or 4, Cin = 128 (conv_out of the released models): a warp walks a 32-pixel run of one row four pixels at a time.
 // Lane l owns input channels 4l..4l+3; the 3 x 6 input float4 of the 4-pixel window are all requested before the first FMA;
-// weights sit in shared memory as [tap][out][128] (conflict-free LDS.128); the 12 partial sums (4 pixels x 3 outputs) are
-// folded across the warp with one butterfly that halves the value count every step (16 shuffles instead of 60) and land as
-// 12 consecutive floats of the output row.
-template <typename InT>
-__global__ void __launch_bounds__(256) conv3x3_cout3_kernel(const InT* __restrict__ x, const float* __restrict__ w_kn,
-                                                            const float* __restrict__ bias, int N, int H, int W,
-                                                            float* __restrict__ y) {
+// weights sit in shared memory as [tap][out][128] (conflict-free LDS.128); the 4 COUT partial sums (4 pixels x COUT outputs, in
+// 16 slots) are folded across the warp with one butterfly that halves the value count every step (16 shuffles instead of 60) and
+// land as 4 COUT consecutive floats of the output row.
+template <int COUT, typename InT>
+__global__ void __launch_bounds__(256) conv3x3_cout_kernel(const InT* __restrict__ x, const float* __restrict__ w_kn,
+                                                           const float* __restrict__ bias, int N, int H, int W,
+                                                           float* __restrict__ y) {
+    static_assert(COUT == 3 || COUT == 4, "conv_out: 3 or 4 output channels");
     constexpr int CIN = 128;
-    __shared__ __align__(16) float ws[27 * CIN];          // [(tap * 3 + o)][c]
-    for (int i = threadIdx.x; i < 27 * CIN; i += 256) {
+    __shared__ __align__(16) float ws[9 * COUT * CIN];    // [(tap * COUT + o)][c]
+    for (int i = threadIdx.x; i < 9 * COUT * CIN; i += 256) {
         const int to = i / CIN, c = i - to * CIN;
-        const int t = to / 3, o = to - t * 3;
-        ws[i] = __ldg(w_kn + (int64_t)(t * CIN + c) * 3 + o);
+        const int t = to / COUT, o = to - t * COUT;
+        ws[i] = __ldg(w_kn + (int64_t)(t * CIN + c) * COUT + o);
     }
     __syncthreads();
     const int lane = threadIdx.x & 31;
@@ -187,7 +203,7 @@ __global__ void __launch_bounds__(256) conv3x3_cout3_kernel(const InT* __restric
     const int row = warp_global / runs_per_row;           // n*H + y
     if (row >= N * H) return;
     const int yy = row % H, n = row / H;
-    const float b_lane = bias ? __ldg(bias + ((lane >> 1) % 3)) : 0.f;      // lanes 2i, 2i+1 end up with value i = px*3 + o
+    const float b_lane = bias ? __ldg(bias + ((lane >> 1) % COUT)) : 0.f;   // lanes 2i, 2i+1 end up with value i = px*COUT + o
     const int x0 = run * 32, x1 = min(W, x0 + 32);
     for (int xx = x0; xx < x1; xx += 4) {
         float4 in[3][6];                                  // rows yy-1..yy+1, columns xx-1..xx+4
@@ -213,14 +229,14 @@ __global__ void __launch_bounds__(256) conv3x3_cout3_kernel(const InT* __restric
 #pragma unroll
             for (int dx = 0; dx < 3; ++dx)
 #pragma unroll
-                for (int o = 0; o < 3; ++o) {
-                    const float4 w4 = *reinterpret_cast<const float4*>(&ws[((dy * 3 + dx) * 3 + o) * CIN + lane * 4]);
+                for (int o = 0; o < COUT; ++o) {
+                    const float4 w4 = *reinterpret_cast<const float4*>(&ws[((dy * 3 + dx) * COUT + o) * CIN + lane * 4]);
 #pragma unroll
                     for (int px = 0; px < 4; ++px) {
                         const float4 a = in[dy][px + dx];
-                        float t = v[px * 3 + o];
+                        float t = v[px * COUT + o];
                         t = fmaf(a.x, w4.x, t); t = fmaf(a.y, w4.y, t); t = fmaf(a.z, w4.z, t); t = fmaf(a.w, w4.w, t);
-                        v[px * 3 + o] = t;
+                        v[px * COUT + o] = t;
                     }
                 }
         // butterfly: after the step with offset `off` a lane keeps the half of the values selected by its bit `off`
@@ -235,9 +251,9 @@ __global__ void __launch_bounds__(256) conv3x3_cout3_kernel(const InT* __restric
             }
         }
         v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
-        const int idx = lane >> 1;                        // = px * 3 + o
-        if ((lane & 1) == 0 && idx < 12 && xx + idx / 3 < x1)
-            y[(((int64_t)n * H + yy) * W + xx) * 3 + idx] = v[0] + b_lane;
+        const int idx = lane >> 1;                        // = px * COUT + o
+        if ((lane & 1) == 0 && idx < 4 * COUT && xx + idx / COUT < x1)
+            y[(((int64_t)n * H + yy) * W + xx) * COUT + idx] = v[0] + b_lane;
     }
 }
 
@@ -246,7 +262,8 @@ __global__ void __launch_bounds__(256) conv3x3_cout3_kernel(const InT* __restric
 extern "C" int vf_conv3x3_small_cin(const float* x, const float* w_kn, const float* bias, int N, int H, int W, int Cin, int Cout,
                                     float* y, double* gn_sums, vf_stream_t s) {
     VF_CHECK_ARG(x && w_kn && y, "vf_conv3x3_small_cin: null pointer");
-    VF_CHECK_ARG(Cin == 3 && Cout % 16 == 0 && Cout <= 128, "vf_conv3x3_small_cin: supports Cin=3, Cout%%16==0, Cout<=128 (got %d->%d)", Cin, Cout);
+    VF_CHECK_ARG((Cin == 3 || Cin == 4) && Cout % 16 == 0 && Cout <= 128,
+                 "vf_conv3x3_small_cin: supports Cin = 3 or 4, Cout%%16==0, Cout<=128 (got %d->%d)", Cin, Cout);
     VF_CHECK_ARG(!gn_sums || Cout == 128, "vf_conv3x3_small_cin: fused GroupNorm(32) statistics need Cout = 128");
     if (N == 0) return VF_OK;
     VF_CHECK_ARG(H <= 65535 * CI_ROWS && N <= 65535, "vf_conv3x3_small_cin: grid too large");
@@ -256,13 +273,19 @@ extern "C" int vf_conv3x3_small_cin(const float* x, const float* w_kn, const flo
             if (e != cudaSuccess) { vf_set_error("vf_conv3x3_small_cin: memset: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
         }
         dim3 grid((W + CI_W - 1) / CI_W, (H + CI_ROWS - 1) / CI_ROWS, N);
-        conv3x3_cin3_cout128_kernel<<<grid, 256, 0, vf_s(s)>>>(x, w_kn, bias, N, H, W, y, gn_sums);
+        if (Cin == 3)
+            conv3x3_cin_cout128_kernel<3><<<grid, 256, 0, vf_s(s)>>>(x, w_kn, bias, N, H, W, y, gn_sums);
+        else
+            conv3x3_cin_cout128_kernel<4><<<grid, 256, 0, vf_s(s)>>>(x, w_kn, bias, N, H, W, y, gn_sums);
         VF_CHECK_LAUNCH("vf_conv3x3_small_cin");
         return VF_OK;
     }
     dim3 grid((W + 63) / 64, H, N);
     VF_CHECK_ARG(H <= 65535, "vf_conv3x3_small_cin: grid too large");
-    conv3x3_small_cin_kernel<3><<<grid, 32 * (Cout / 16), sizeof(float) * 27 * Cout, vf_s(s)>>>(x, w_kn, bias, N, H, W, Cout, y);
+    if (Cin == 3)
+        conv3x3_small_cin_kernel<3><<<grid, 32 * (Cout / 16), sizeof(float) * 27 * Cout, vf_s(s)>>>(x, w_kn, bias, N, H, W, Cout, y);
+    else
+        conv3x3_small_cin_kernel<4><<<grid, 32 * (Cout / 16), sizeof(float) * 36 * Cout, vf_s(s)>>>(x, w_kn, bias, N, H, W, Cout, y);
     VF_CHECK_LAUNCH("vf_conv3x3_small_cin");
     return VF_OK;
 }
@@ -270,15 +293,20 @@ extern "C" int vf_conv3x3_small_cin(const float* x, const float* w_kn, const flo
 extern "C" int vf_conv3x3_small_cout(const void* x, int x_dtype, const float* w_kn, const float* bias, int N, int H, int W, int Cin,
                                      int Cout, float* y, vf_stream_t s) {
     VF_CHECK_ARG(x && w_kn && y, "vf_conv3x3_small_cout: null pointer");
-    VF_CHECK_ARG(Cin == 128 && Cout == 3, "vf_conv3x3_small_cout: supports 128->3 (got %d->%d)", Cin, Cout);
+    VF_CHECK_ARG(Cin == 128 && (Cout == 3 || Cout == 4), "vf_conv3x3_small_cout: supports 128->3 and 128->4 (got %d->%d)", Cin, Cout);
+    VF_CHECK_ARG(x_dtype == VF_F32 || x_dtype == VF_BF16, "vf_conv3x3_small_cout: x must be fp32 or bf16");
     if (N == 0) return VF_OK;
     const long long warps = (long long)N * H * ((W + 31) / 32);
     VF_CHECK_ARG(warps < (1ll << 31), "vf_conv3x3_small_cout: too many pixels");
     const unsigned blocks = (unsigned)((warps + 7) / 8);
-    if (x_dtype == VF_F32)
-        conv3x3_cout3_kernel<float><<<blocks, 256, 0, vf_s(s)>>>((const float*)x, w_kn, bias, N, H, W, y);
+    if (Cout == 3 && x_dtype == VF_F32)
+        conv3x3_cout_kernel<3, float><<<blocks, 256, 0, vf_s(s)>>>((const float*)x, w_kn, bias, N, H, W, y);
+    else if (Cout == 3)
+        conv3x3_cout_kernel<3, __nv_bfloat16><<<blocks, 256, 0, vf_s(s)>>>((const __nv_bfloat16*)x, w_kn, bias, N, H, W, y);
+    else if (x_dtype == VF_F32)
+        conv3x3_cout_kernel<4, float><<<blocks, 256, 0, vf_s(s)>>>((const float*)x, w_kn, bias, N, H, W, y);
     else
-        conv3x3_cout3_kernel<__nv_bfloat16><<<blocks, 256, 0, vf_s(s)>>>((const __nv_bfloat16*)x, w_kn, bias, N, H, W, y);
+        conv3x3_cout_kernel<4, __nv_bfloat16><<<blocks, 256, 0, vf_s(s)>>>((const __nv_bfloat16*)x, w_kn, bias, N, H, W, y);
     VF_CHECK_LAUNCH("vf_conv3x3_small_cout");
     return VF_OK;
 }

@@ -1,10 +1,12 @@
 // Evaluation-side kernels around the hot path (SURVEY.md §8 f2 / f3): the dataset resize rule and the image metrics.
 //   vf_resize_u8        viewformer/data/_common.py:19-44 (resize_th): uint8 -> float /255 -> torch.nn.functional.interpolate
 //                       (bilinear align_corners=False when shrinking, nearest when growing) -> clamp -> * 255 -> uint8 (truncation)
+//   vf_resize_f32       the same interpolation of f32 images in [0, 1] (the float images resize_th takes), clamped to [0, 1], not quantised
 //   vf_image_pair_sums  per-image sum |a-b| and sum (a-b)^2 over uint8 images: MSE / MAE / RMSE / PSNR follow exactly on the host
 //                       (viewformer/utils/metrics.py:173-205, tf.image.psnr)
 //   vf_ssim_u8[_k]      viewformer/utils/metrics.py:17-73: 7x7 uniform window, VALID, sample covariance, K1 = 0.01, K2 = 0.03 (or the caller's),
 //                       data range 1, mean over (H-6) x (W-6) x C
+#include <type_traits>
 #include "vf_common.cuh"
 
 namespace {
@@ -15,8 +17,9 @@ __device__ __forceinline__ float src_index(float scale, int dst) {
     return s < 0.f ? 0.f : s;
 }
 
-__global__ void resize_u8_kernel(const uint8_t* __restrict__ x, int N, int H, int W, int C, int OH, int OW, int bilinear,
-                                 uint8_t* __restrict__ y) {
+// T = uint8_t: pixels read as x / 255 and written as trunc(255 v); T = float: read and written as they are
+template <typename T>
+__global__ void resize_kernel(const T* __restrict__ x, int N, int H, int W, int C, int OH, int OW, int bilinear, T* __restrict__ y) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long total = (long long)N * OH * OW * C;
     if (i >= total) return;
@@ -26,8 +29,12 @@ __global__ void resize_u8_kernel(const uint8_t* __restrict__ x, int N, int H, in
     r /= OW;
     const int oy = (int)(r % OH);
     const int n = (int)(r / OH);
-    const uint8_t* img = x + (long long)n * H * W * C;
-    auto px = [&](int yy, int xx) { return __fdiv_rn((float)img[((long long)yy * W + xx) * C + c], 255.f); };
+    const T* img = x + (long long)n * H * W * C;
+    auto px = [&](int yy, int xx) {
+        const T p = img[((long long)yy * W + xx) * C + c];
+        if constexpr (std::is_same<T, float>::value) return p;
+        else return __fdiv_rn((float)p, 255.f);
+    };
     float v;
     if (!bilinear) {
         // torch 'nearest': src = min(floor(dst * scale), in - 1), scale = (float)in / out
@@ -49,7 +56,8 @@ __global__ void resize_u8_kernel(const uint8_t* __restrict__ x, int N, int H, in
         v = __fadd_rn(__fmul_rn(ly0, top), __fmul_rn(ly1, bot));
     }
     v = fminf(fmaxf(v, 0.f), 1.f);
-    y[i] = (uint8_t)(__fmul_rn(v, 255.f));          // .to(torch.uint8): truncation toward zero
+    if constexpr (std::is_same<T, float>::value) y[i] = v;
+    else y[i] = (uint8_t)(__fmul_rn(v, 255.f));     // .to(torch.uint8): truncation toward zero
 }
 
 // one block per image: exact integer sums
@@ -129,9 +137,18 @@ extern "C" int vf_resize_u8(const void* x, int N, int H, int W, int C, int OH, i
     VF_CHECK_ARG(x && y && N >= 0 && H > 0 && W > 0 && C > 0 && OH > 0 && OW > 0, "vf_resize_u8: bad args");
     const long long total = (long long)N * OH * OW * C;
     if (total == 0) return VF_OK;
-    resize_u8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, vf_s(s)>>>(reinterpret_cast<const uint8_t*>(x), N, H, W, C, OH, OW, bilinear,
-                                                                            reinterpret_cast<uint8_t*>(y));
+    resize_kernel<uint8_t><<<(unsigned)((total + 255) / 256), 256, 0, vf_s(s)>>>(reinterpret_cast<const uint8_t*>(x), N, H, W, C, OH, OW,
+                                                                                bilinear, reinterpret_cast<uint8_t*>(y));
     VF_CHECK_LAUNCH("vf_resize_u8");
+    return VF_OK;
+}
+
+extern "C" int vf_resize_f32(const float* x, int N, int H, int W, int C, int OH, int OW, int bilinear, float* y, vf_stream_t s) {
+    VF_CHECK_ARG(x && y && N >= 0 && H > 0 && W > 0 && C > 0 && OH > 0 && OW > 0, "vf_resize_f32: bad args");
+    const long long total = (long long)N * OH * OW * C;
+    if (total == 0) return VF_OK;
+    resize_kernel<float><<<(unsigned)((total + 255) / 256), 256, 0, vf_s(s)>>>(x, N, H, W, C, OH, OW, bilinear, y);
+    VF_CHECK_LAUNCH("vf_resize_f32");
     return VF_OK;
 }
 

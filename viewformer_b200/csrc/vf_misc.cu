@@ -54,6 +54,13 @@ __global__ void u8_to_unit_kernel(const uint8_t* __restrict__ in, float* __restr
     }
 }
 
+// f32 images in [0, 1] -> x * 2 - 1 (convert_image_dtype is the identity for float32 input), op by op
+__global__ void f01_to_unit_kernel(const float* __restrict__ in, float* __restrict__ out, int64_t n, int64_t in_row_stride) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    out[(int64_t)blockIdx.y * n + i] = __fsub_rn(__fmul_rn(__ldg(in + (int64_t)blockIdx.y * in_row_stride + i), 2.0f), 1.0f);
+}
+
 __global__ void unit_to_u8_kernel(const float* __restrict__ in, uint8_t* __restrict__ out, int64_t n) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -302,6 +309,14 @@ extern "C" int vf_u8_to_unit_f32(const uint8_t* in, float* out, int64_t rows, in
     dim3 grid(nblk(row_len, 1024), (unsigned)rows);
     u8_to_unit_kernel<<<grid, 256, 0, vf_s(s)>>>(in, out, row_len, in_row_stride);
     VF_CHECK_LAUNCH("vf_u8_to_unit_f32");
+    return VF_OK;
+}
+extern "C" int vf_f01_to_unit_f32(const float* in, float* out, int64_t rows, int64_t row_len, int64_t in_row_stride, vf_stream_t s) {
+    VF_CHECK_ARG(in && out && rows >= 0 && row_len >= 0 && rows <= 65535, "vf_f01_to_unit_f32: bad args");
+    if (rows == 0 || row_len == 0) return VF_OK;
+    dim3 grid(nblk(row_len, 256), (unsigned)rows);
+    f01_to_unit_kernel<<<grid, 256, 0, vf_s(s)>>>(in, out, row_len, in_row_stride);
+    VF_CHECK_LAUNCH("vf_f01_to_unit_f32");
     return VF_OK;
 }
 extern "C" int vf_unit_f32_to_u8(const float* in, uint8_t* out, int64_t n, vf_stream_t s) {

@@ -112,9 +112,15 @@ def decode_example(buf):
 
 
 def decode_frames(frame_bytes):
-    """bytes_list of encoded images -> uint8 [T,H,W,3] (PIL; the reference uses tf.io.decode_image)."""
+    """bytes_list of encoded images -> uint8 [T,H,W,C] with the channels that are stored, as tf.io.decode_image returns them (PIL):
+    C = 4 for the RGBA PNG frames of 4-channel datasets (data/tfrecord_dataset.py:318-321, CO3Dv2's masked RGB + mask), C = 3 for
+    everything else (RGB JPEG; other modes are converted to RGB)."""
     from PIL import Image
-    return np.stack([np.asarray(Image.open(io.BytesIO(b)).convert("RGB")) for b in frame_bytes])
+
+    def decode(b):
+        im = Image.open(io.BytesIO(b))
+        return np.asarray(im if im.mode == "RGBA" else im.convert("RGB"))
+    return np.stack([decode(b) for b in frame_bytes])
 
 
 # ----------------------------------------------------------------------------------------------- generate-codes
@@ -126,6 +132,7 @@ class LatentCodeTransformer:
     def __init__(self, model, batch_size=None, device=None):
         self.model = model if device is None else model.to(device)
         self.image_size = model.config.image_size
+        self.in_channels = getattr(model.config, "in_channels", 3)      # a config without the field is an RGB codebook's
         self.batch_size = batch_size if batch_size is not None else model.config.batch_size
         self.dataset_info = None
 
@@ -165,6 +172,9 @@ class LatentCodeTransformer:
             frames = np.asarray(scene["frames"])
             if frames.dtype != np.uint8:
                 raise TypeError("LatentCodeTransformer takes uint8 frames (NHWC)")
+            if frames.ndim != 4 or frames.shape[-1] != self.in_channels:
+                raise ValueError(f"LatentCodeTransformer: the codebook takes {self.in_channels}-channel frames, got frames of shape "
+                                 f"{frames.shape}")
             pending.append((np.asarray(scene["cameras"], dtype=np.float32), len(frames)))
             frames_buf.append(frames)
             flush()

@@ -9,7 +9,8 @@
 import torch
 
 from . import _lib as L
-from .generate import reduce_cameras
+from .generate import reduce_cameras, resize_images
+from .vqgan import image_tensor
 
 
 def transformer_predict(cameras, codes, *, transformer_model):
@@ -46,17 +47,18 @@ def run_with_batchsize(fn, batch_size, *args, **kwargs):
 
 
 def encode_images(frames, *, codebook_model):
-    """uint8 frames [..., H, W, 3] -> codes int64 [..., h, w]; frames are resized with the dataset rule (data/_common.py:19-44)."""
-    frames = torch.as_tensor(frames)
+    """frames [..., H, W, C], uint8 or float32 in [0, 1] -> codes int64 [..., h, w]; frames are resized with the dataset rule
+    (data/_common.py:19-44).  Any other dtype raises TypeError."""
+    frames = image_tensor(frames, "encode_images")
     lead = frames.shape[:-3]
     x = frames.reshape((-1,) + tuple(frames.shape[-3:])).to(codebook_model.device).contiguous()
-    x = L.resize_u8(x, codebook_model.config.image_size)
-    codes = codebook_model.encode_u8(x)
+    x = resize_images(x, codebook_model.config.image_size)
+    codes = codebook_model.encode_images(x)
     return codes.reshape(tuple(lead) + tuple(codes.shape[-2:]))
 
 
 def decode_code(codes, *, codebook_model):
-    """codes [..., h, w] -> uint8 images [..., H, W, 3] (clip, /2 + 0.5, saturate-cast; evaluate_transformer.py:127-129)."""
+    """codes [..., h, w] -> uint8 images [..., H, W, out_ch] (clip, /2 + 0.5, saturate-cast; evaluate_transformer.py:127-129)."""
     codes = torch.as_tensor(codes)
     lead = codes.shape[:-2]
     img = codebook_model.decode_code_u8(codes.reshape((-1,) + tuple(codes.shape[-2:])))

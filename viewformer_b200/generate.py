@@ -9,6 +9,13 @@ torch on whatever device the cameras live on; all image / token work runs in lib
 import torch
 
 from . import _lib as L
+from . import float_images
+from .vqgan import image_tensor
+
+
+def resize_images(x, size):
+    """The dataset resize rule (data/_common.py:19-62) on uint8 images or on float32 images in [0, 1], which stay float32."""
+    return L.resize_u8(x, size) if x.dtype == torch.uint8 else float_images.resize_f32(x, size)
 
 
 # --------------------------------------------------------------------------- quaternion helpers (utils/geometry_tf.py:6-13,44-91)
@@ -69,9 +76,12 @@ def normalize_cameras(cameras):
 
 # --------------------------------------------------------------------------- generate
 def generate_batch_predictions(transformer_model, codebook_model, images, cameras, *, encode_target=None):
-    """images uint8 [B,T,H,W,3] (host or device), cameras f32 [B,T,7] ->
-    dict(ground_truth_images [B,H,W,3] u8, generated_images [B,H,W,3] u8, ground_truth_cameras [B,7],
+    """images [B,T,H,W,C] (host or device), cameras f32 [B,T,7] ->
+    dict(ground_truth_images [B,H,W,C] (the input's), generated_images [B,S,S,out_ch] u8, ground_truth_cameras [B,7],
          generated_cameras [B,7]) — evaluate_transformer.py:97-146.
+
+    ``images``: uint8, or float32 in [0, 1] as evaluate_co3dv2_challenge.py:72-77 passes them (``convert_image_dtype`` keeps float32
+    as it is, then ``x * 2 - 1``); C is the codebook's ``in_channels``.  Any other dtype raises TypeError: nothing is cast.
 
     ``encode_target``: the reference encodes all T views and, when the model localises, runs a second
     forward on the true codes of the target view (:134-136).  Default: encode the target only when that
@@ -82,7 +92,7 @@ def generate_batch_predictions(transformer_model, codebook_model, images, camera
         with torch.cuda.device(_dev):            # kernels launch on the current device's stream: make the models' device current
             return generate_batch_predictions(transformer_model, codebook_model, images, cameras, encode_target=encode_target)
     dev = transformer_model.device
-    images = torch.as_tensor(images)
+    images = image_tensor(images, "generate_batch_predictions")
     cameras = torch.as_tensor(cameras)
     if cameras.dtype != torch.float32:
         cameras = cameras.to(torch.float32)
@@ -101,9 +111,9 @@ def generate_batch_predictions(transformer_model, codebook_model, images, camera
     if not img_dev.is_contiguous():
         img_dev = img_dev.contiguous()
     if images.shape[2] != size or images.shape[3] != size:        # resize_tf (evaluate_transformer.py:104, data/_common.py:19-62)
-        img_dev = L.resize_u8(img_dev[:, :n_enc].reshape((-1,) + tuple(img_dev.shape[2:])).contiguous(), size)
+        img_dev = resize_images(img_dev[:, :n_enc].reshape((-1,) + tuple(img_dev.shape[2:])).contiguous(), size)
         img_dev = img_dev.reshape((B, n_enc) + tuple(img_dev.shape[1:]))
-    codes = codebook_model.encode_u8(img_dev, first_views=n_enc).reshape(B, n_enc, side, side)
+    codes = codebook_model.encode_images(img_dev, first_views=n_enc).reshape(B, n_enc, side, side)
 
     gen_codes = transformer_model.generate_codes(codes[:, : T - 1], cams_dev)
     gen_images = codebook_model.decode_code_u8(gen_codes)
@@ -126,7 +136,8 @@ class GraphedPredictions:
     or from device tensors), outputs live in static device tensors that the next call overwrites.
 
     Only the non-localising configuration is graph-safe: camera localisation ends in a host-side quaternion mean
-    (``reduce_cameras``), which a capture cannot contain."""
+    (``reduce_cameras``), which a capture cannot contain.  Images are uint8 only (the static buffer's dtype), [scenes, views, S, S,
+    in_channels]; float images go through ``generate_batch_predictions``."""
 
     def __init__(self, transformer_model, codebook_model, scenes, views, warmup=2):
         if transformer_model.use_localization:
@@ -134,7 +145,7 @@ class GraphedPredictions:
         dev = transformer_model.device
         size = codebook_model.config.image_size
         self.device = dev
-        self.images = torch.zeros((scenes, views, size, size, 3), dtype=torch.uint8, device=dev)
+        self.images = torch.zeros((scenes, views, size, size, codebook_model.config.in_channels), dtype=torch.uint8, device=dev)
         self.cameras = torch.zeros((scenes, views, 7), dtype=torch.float32, device=dev)
         self.cameras[..., 3] = 1.0                                   # identity quaternions for the warm-up passes
         side = torch.cuda.Stream(device=dev)
@@ -151,7 +162,7 @@ class GraphedPredictions:
         self.launches_per_replay = L.launch_count() - n0             # libvf_b200 kernel-launching calls recorded in the graph
 
     def __call__(self, images, cameras):
-        self.images.copy_(torch.as_tensor(images), non_blocking=True)
+        self.images.copy_(image_tensor(images, "GraphedPredictions", (torch.uint8,)), non_blocking=True)
         self.cameras.copy_(torch.as_tensor(cameras), non_blocking=True)
         self.graph.replay()
         return self.outputs
@@ -160,13 +171,14 @@ class GraphedPredictions:
 def generate_batch_predictions_multictx(transformer_model, codebook_model, images, cameras):
     """Multi-context variant — viewformer/evaluate/evaluate_transformer_multictx.py:37-95: one 3-stream forward yields,
     for every context size i, the query view rendered from context views 0..i-1 (stream 1) and the query localised
-    against them (stream 2).  Returns generated_images [B,T,H,W,3] u8 and generated_cameras [B,T,7]."""
+    against them (stream 2).  Returns generated_images [B,T,S,S,out_ch] u8 and generated_cameras [B,T,7].  ``images``: uint8 or
+    float32 in [0, 1], as ``generate_batch_predictions`` takes them."""
     _dev = getattr(codebook_model, "device", None)
     if _dev is not None and _dev.type == "cuda" and _dev.index is not None and _dev.index != torch.cuda.current_device():
         with torch.cuda.device(_dev):            # kernels launch on the current device's stream: make the models' device current
             return generate_batch_predictions_multictx(transformer_model, codebook_model, images, cameras)
     dev = transformer_model.device
-    images = torch.as_tensor(images)
+    images = image_tensor(images, "generate_batch_predictions_multictx")
     cameras = torch.as_tensor(cameras)
     if cameras.dtype != torch.float32:
         cameras = cameras.to(torch.float32)
@@ -176,7 +188,7 @@ def generate_batch_predictions_multictx(transformer_model, codebook_model, image
     B, T = images.shape[:2]
     side = transformer_model.token_image_size
     img_dev = images.to(device=dev, non_blocking=True) if images.device != dev else images
-    codes = codebook_model.encode_u8(img_dev.contiguous(), first_views=T).reshape(B, T, side, side)
+    codes = codebook_model.encode_images(img_dev.contiguous(), first_views=T).reshape(B, T, side, side)
     mask = torch.full_like(codes[:, :1], transformer_model.mask_token)
     input_ids = torch.cat([codes[:, :-1], mask], 1)                                    # :61-62
     context_cameras = torch.cat([cams[:, :-1], torch.zeros_like(cams[:, :1])], 1)      # :63

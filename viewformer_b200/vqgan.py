@@ -22,6 +22,7 @@ import os
 import torch
 
 from . import _lib as L
+from . import float_images
 from .config import VQGANConfig, load_config
 from .ops import Precision, Linear, gemm_nt, linear
 
@@ -88,6 +89,15 @@ def tc_conv_shape_ok(k, cin, cout, k_align=64):
     return k == 3 and cin % k_align == 0 and cout % 16 == 0 and cout >= 64
 
 
+def image_tensor(images, what, dtypes=(torch.uint8, torch.float32)):
+    """``images`` as a tensor of one of ``dtypes`` (uint8, or float32 in [0, 1]); anything else raises TypeError instead of being cast."""
+    t = torch.as_tensor(images)
+    if t.dtype not in dtypes:
+        raise TypeError(f"{what}: images must be {' or '.join(str(d).replace('torch.', '') for d in dtypes)}"
+                        f"{' (float32 in [0, 1])' if torch.float32 in dtypes else ''}, got {t.dtype}; they are not cast")
+    return t
+
+
 class _Conv3:
     """3x3 (or 1x1) convolution weights in both kernel layouts."""
 
@@ -97,8 +107,8 @@ class _Conv3:
         w = w.to(device=device, dtype=torch.float32)
         self.bias = b.to(device=device, dtype=torch.float32).contiguous()
         self.tc = (not exact) and prec.use_tc and tc_conv_shape_ok(kh, cin, cout, prec.k_align)
-        self.small_cin = kh == 3 and cin == 3 and cout % 16 == 0 and cout <= 128     # conv_in: dedicated exact kernel
-        self.small_cout = kh == 3 and cin == 128 and cout == 3                       # conv_out: dedicated exact kernel
+        self.small_cin = kh == 3 and cin in (3, 4) and cout % 16 == 0 and cout <= 128     # conv_in: dedicated exact kernel (RGB, RGBA)
+        self.small_cout = kh == 3 and cin == 128 and cout in (3, 4)                       # conv_out: dedicated exact kernel
         if self.tc and prec.split:
             # exact mode: per tap [hi(Cin) | lo(Cin)] fp16 halves of the fp32 weights
             self.w_nk = L.split_f16x2(w.permute(0, 2, 3, 1).reshape(cout * kh * kw, cin).contiguous()).reshape(cout, kh * kw * 2 * cin)
@@ -464,11 +474,11 @@ class VQGAN:
         return h
 
     def _encoder(self, x):
-        """Encoder.forward (vqgan_th.py:203-225); x f32 [N,H,W,3] -> f32 [N,h,w,z_channels]."""
+        """Encoder.forward (vqgan_th.py:203-225); x f32 [N,H,W,in_channels] -> f32 [N,h,w,z_channels]."""
         return self._walk(self._w["enc"], x, self.enc_prec)
 
     def _decoder(self, z):
-        """Decoder.forward (vqgan_th.py:291-318); z f32 [N,h,w,z_channels] (post_quant_conv applied) -> f32 [N,H,W,3]."""
+        """Decoder.forward (vqgan_th.py:291-318); z f32 [N,h,w,z_channels] (post_quant_conv applied) -> f32 [N,H,W,out_ch]."""
         return self._walk(self._w["dec"], z, self.dec_prec)
 
     # ------------------------------------------------------------------ quantizer
@@ -537,9 +547,20 @@ class VQGAN:
     @L.on_model_device
     def encode_u8(self, images_u8_nhwc, first_views=None):
         """uint8 NHWC images -> codes int64 [N,h,w] (evaluate_transformer.py:105-110 in one device pass).
-        With ``first_views=n`` the input is [B,T,H,W,3] and views 0..n-1 of every scene are encoded ([B*n,h,w])."""
+        With ``first_views=n`` the input is [B,T,H,W,C] and views 0..n-1 of every scene are encoded ([B*n,h,w]).
+        Any other dtype raises TypeError: a float image in [0, 1] cast to uint8 would become 0 / 1 bytes."""
+        return self.encode_images(image_tensor(images_u8_nhwc, "encode_u8", (torch.uint8,)), first_views)
+
+    @L.on_model_device
+    def encode_images(self, images_nhwc, first_views=None):
+        """``encode_u8`` for uint8 images or float32 images in [0, 1], the two inputs of the reference's
+        ``tf.image.convert_image_dtype(images, tf.float32) * 2 - 1`` (the identity for float32): codes int64 [N,h,w]."""
+        images = image_tensor(images_nhwc, "encode_images")
+        if images.shape[-1] != self.config.in_channels:
+            raise ValueError(f"encode_images: the codebook takes {self.config.in_channels}-channel images, got shape {tuple(images.shape)}")
         self._need_weights()
-        x = L.u8_to_unit(self._in(images_u8_nhwc, torch.uint8), first_views)
+        x = self._in(images, images.dtype)
+        x = L.u8_to_unit(x, first_views) if x.dtype == torch.uint8 else float_images.f01_to_unit(x, first_views)
         zr, hh, ww = self.encode_rows(x)
         _, _, idx = self._quantize(zr, want_quant=False)
         return idx.reshape(x.shape[0], hh, ww)
