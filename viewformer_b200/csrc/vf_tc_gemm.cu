@@ -6,7 +6,9 @@
 //   shared-memory staging tile -> alpha, bias, GELU, residual, GroupNorm statistics, f32/bf16 stores.
 //
 // Warp roles (384 threads): warps 0..7 = MMA + epilogue (warpgroup g owns tile rows [64g, 64g+64)), warps 8..11 = TMA producer
-// warpgroup (one elected thread issues the loads; the warpgroup hands its registers to the MMA warpgroups).
+// warpgroup (one elected thread issues the loads; the warpgroup hands its registers to the MMA warpgroups).  Exact mode moves the
+// epilogue's stores onto warps 9..11 of the producer warpgroup: the MMA warps write the staging tile, hand it over through an
+// mbarrier pair and go straight on to the next tile's MMAs while those warps add bias and residual, store and fold the GroupNorm sums.
 // A CTA walks 128 x BLOCK_N output tiles; the producer runs ahead across tiles, so the next tile's operands stream in while the
 // epilogue of this one runs.  GEMM operands are K-major; the convolution reads its A operand straight from the NHWC activation
 // tensor with a 4-D tensor map: for every filter tap the box [TN images x TH rows x TW cols x 64 channels] shifted by (dy,dx)
@@ -126,8 +128,15 @@ constexpr int MAX_STAGES = 8;
 template <int kBlockN, int kStages, bool kExact>
 __host__ __device__ constexpr int tc_smem_bytes() {
     return operand_bytes(kStages, A_STAGE_BYTES + kBlockN * ROW_BYTES, kBlockN * ROW_BYTES, kExact) +
-           NUM_EPI_WARPS * 32 * (kBlockN / 2 + 4) * 4 /*epilogue staging*/ + 1024 /*align slack*/ + 8 * (2 * MAX_STAGES + 8) /*barriers*/;
+           NUM_EPI_WARPS * 32 * (kBlockN / 2 + 4) * 4 /*epilogue staging*/ + 1024 /*align slack*/ +
+           8 * (2 * MAX_STAGES + 2 * halo_buffers(kExact) + 2) /*barriers: ring, halo tiles, staging handover (exact)*/;
 }
+
+// Exact mode's staging handover: MMA warps arrive on stg_full once the tile's chunk sums are in the staging tile, the epilogue warps
+// (9..11 of the producer warpgroup) on stg_empty once they have stored it.  Every thread of either side arrives.
+constexpr int NUM_STORE_WARPS = 3;
+static_assert(NUM_EPI_WARPS + 1 + NUM_STORE_WARPS == NUM_THREADS / 32, "warp roles");
+constexpr int STORE_RES_VECS = 4;              // residual float4 loads in flight per lane of an epilogue warp (fits 80 registers)
 
 // L2 prefetch of the residual rows a conv tile's epilogue will read: one bulk prefetch per (image, output row) of the tile, spanning
 // its valid pixels from channel n0 on (the columns between the tile's channel slices ride along).
@@ -184,6 +193,136 @@ __device__ __forceinline__ void normalise_halo(const TcParams& p, uint8_t* tile,
     }
 }
 
+// Exact mode's epilogue, run by warps 9..11: one 32-row x HALF_N slice of the staging tile, the slice the MMA+epilogue warp
+// `quarter + 4 col_half` stores on the bf16 / TF32 path, with that path's lane mapping, bias -> residual -> store order and GroupNorm
+// shuffle tree (so outputs and fp32 GroupNorm partials are the same bits).  The residual comes from L2 (the producer prefetched it),
+// STORE_RES_VECS vectors at a time.
+template <int kBlockN>
+__device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& ti, const float* stg, int quarter, int col_half, int lane) {
+    constexpr int HALF_N = kBlockN / 2;
+    constexpr int STG_LD = HALF_N + 4;
+    // row bookkeeping: lane l stores tile row 32*quarter + l
+    const int row = quarter * 32 + lane;
+    long long my_off;
+    int my_ok, gm;
+    if (p.conv) {
+        const int lx = row % p.TW;
+        const int q = row / p.TW;
+        const int ly = q % p.TH;
+        const int ln = q / p.TH;
+        const int img = ti.img0 + ln, oy = ti.oy0 + ly, ox = ti.ox0 + lx;
+        my_ok = (img < p.Nimg) && (oy < p.OH) && (ox < p.OW);
+        gm = (img * p.OH + oy) * p.OW + ox;
+        my_off = (long long)gm * p.ldc;
+    } else {
+        gm = ti.m0 + row;
+        my_ok = gm < p.M;
+        my_off = (long long)ti.b1 * p.c_sb1 + (long long)ti.b2 * p.c_sb2 + (long long)gm * p.ldc;
+    }
+    const float bias_m = (p.bias_mode == VF_BIAS_M && my_ok) ? __ldg(p.bias + gm) : 0.f;
+
+    constexpr int VPR = HALF_N / 4;                // float4 vectors per half row
+    constexpr int RPI = 32 / VPR;                  // rows per iteration
+    constexpr int ITERS = 32 / RPI;
+    constexpr int RB = STORE_RES_VECS;
+    static_assert(ITERS % RB == 0, "residual batches");
+    const int r_sub = lane / VPR;
+    const int c_ln = (lane % VPR) * 4;
+    const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
+    const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
+    if (fast) {
+        float4 resv[RB];
+        float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
+        float gs = 0.f, gq = 0.f;
+#pragma unroll 1
+        for (int i0 = 0; i0 < ITERS; i0 += RB) {
+            if (p.residual) {
+#pragma unroll
+                for (int k = 0; k < RB; ++k) {
+                    const int rr = (i0 + k) * RPI + r_sub;
+                    const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
+                    const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
+                    // out-of-range rows read row 0 and are never stored (unconditional: the loads stay independent)
+                    resv[k] = __ldg(reinterpret_cast<const float4*>(p.residual + (ok ? off_row + n_ln : (long long)n_ln)));
+                }
+            }
+#pragma unroll
+            for (int k = 0; k < RB; ++k) {
+                const int i = i0 + k;
+                const int rr = i * RPI + r_sub;
+                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
+                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
+                const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
+                float4 v = *reinterpret_cast<const float4*>(stg + rr * STG_LD + c_ln);
+                if (p.bias_mode == VF_BIAS_N) { v.x += bias4.x; v.y += bias4.y; v.z += bias4.z; v.w += bias4.w; }
+                else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
+                if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
+                if (p.residual) {
+                    const float4 r = resv[k];
+                    v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
+                }
+                if (ok) {
+                    gs += (v.x + v.y) + (v.z + v.w);
+                    // the recorded GroupNorm partials (tests/golden/exact_conv_bits.json) are this rounding; written out, so that which
+                    // product the compiler would fuse into the add cannot change it
+                    gq += __fmaf_rn(v.y, v.y, __fmul_rn(v.x, v.x)) + __fmaf_rn(v.w, v.w, __fmul_rn(v.z, v.z));
+                    const long long off = off_row + n_ln;
+                    if (p.C_f32) *reinterpret_cast<float4*>(p.C_f32 + off) = v;
+                    if (p.C_bf16) {
+                        __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
+                        uint2 u;
+                        u.x = *reinterpret_cast<uint32_t*>(&lo);
+                        u.y = *reinterpret_cast<uint32_t*>(&hi);
+                        *reinterpret_cast<uint2*>(p.C_bf16 + off) = u;
+                    }
+                }
+            }
+        }
+        if (p.gn_sums) {
+            // the 32 rows of a slice lie in one image; lanes with equal column vector (different r_sub) and the cpg/4 neighbouring
+            // lanes of a group are folded with shuffles, then one fp64 RED per (image, group)
+            const unsigned okmask = __ballot_sync(0xffffffffu, my_ok);
+#pragma unroll
+            for (int o = VPR; o < 32; o <<= 1) {
+                gs += __shfl_xor_sync(0xffffffffu, gs, o);
+                gq += __shfl_xor_sync(0xffffffffu, gq, o);
+            }
+            const int lpg = p.gn_cpg >> 2;
+            for (int o = 1; o < lpg; o <<= 1) {
+                gs += __shfl_xor_sync(0xffffffffu, gs, o);
+                gq += __shfl_xor_sync(0xffffffffu, gq, o);
+            }
+            const int gm_first = __shfl_sync(0xffffffffu, gm, okmask ? (__ffs(okmask) - 1) : 0);
+            if (okmask && r_sub == 0 && (lane % lpg) == 0) {
+                const long long slot = ((long long)(gm_first / p.gn_rows_per_img) * p.gn_groups + n_ln / p.gn_cpg) * 2;
+                atomicAdd(p.gn_sums + slot, (double)gs);
+                atomicAdd(p.gn_sums + slot + 1, (double)gq);
+            }
+        }
+    } else {
+        // generic path (N tails, unaligned leading dimensions): scalar, same arithmetic order
+#pragma unroll 1
+        for (int rr = 0; rr < 32; ++rr) {
+            const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
+            const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
+            const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
+            if (!ok) continue;
+            for (int c = lane; c < HALF_N; c += 32) {
+                const int n = ti.n0 + col_half * HALF_N + c;
+                if (n >= p.Ncols) continue;
+                float x = stg[rr * STG_LD + c];
+                x += (p.bias_mode == VF_BIAS_N) ? __ldg(p.bias + n) : bm;
+                if (p.act == VF_ACT_GELU_ERF) x = vf_gelu_erf(x);
+                const long long off = off_row + n;
+                if (p.residual) x += __ldg(p.residual + off);
+                if (p.C_f32) p.C_f32[off] = x;
+                if (p.C_bf16) p.C_bf16[off] = __float2bfloat16(x);
+            }
+        }
+    }
+}
+
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x, +gridDim.x, ...
 template <int kBlockN, int kStages, WgKind kKind>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_constant__ TcParams p) {
@@ -206,6 +345,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     constexpr int NHB = halo_buffers(kExact);
     uint64_t* a_full_bar = empty_bar + MAX_STAGES;      // [NHB]  halo mode: A halo tiles
     uint64_t* a_empty_bar = a_full_bar + NHB;           // [NHB]
+    uint64_t* stg_full = a_empty_bar + NHB;             // exact mode: staging tile written (MMA warps -> epilogue warps)
+    uint64_t* stg_empty = stg_full + 1;                 //             staging tile stored  (epilogue warps -> MMA warps)
     constexpr int NG = kStages;                         // ring depth (normal mode)
     // halo mode carves the same operand region differently: NHB halo buffers, then a ring of B-only slots
     constexpr int NGH = halo_slots(kExact);
@@ -225,13 +366,35 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             mbar_init(&a_full_bar[a], 1);
             mbar_init(&a_empty_bar[a], NUM_MMA_THREADS);
         }
+        if constexpr (kExact) {
+            mbar_init(stg_full, NUM_MMA_THREADS);
+            mbar_init(stg_empty, 32 * NUM_STORE_WARPS);
+        }
         mbar_fence_init();
     }
     __syncthreads();
 
     if (warp >= NUM_EPI_WARPS) {
-        // ===================== TMA producer =====================
-        setmaxnreg_dec<40>();
+        // ===================== TMA producer (warp 8), exact mode's epilogue (warps 9..11) =====================
+        setmaxnreg_dec<kExact ? 80 : 40>();           // 208 x 256 + 80 x 128 <= 64K (exact), 232 x 256 + 40 x 128 (bf16 / TF32)
+        if constexpr (kExact) {
+            if (warp > NUM_EPI_WARPS) {
+                // every role walks the same tiles; epilogue warp e stores staging slices e, e + 3, e + 6
+                const int e = warp - NUM_EPI_WARPS - 1;
+                uint32_t spar = 0;
+                for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+                    const TileInfo ti = decode_tile(p, t, kBlockN);
+                    if (ti.skip) continue;
+                    mbar_wait(stg_full, spar, "vf_tc_gemm epilogue");      // spans one K loop: well under a millisecond
+#pragma unroll 1
+                    for (int s = e; s < NUM_EPI_WARPS; s += NUM_STORE_WARPS)
+                        store_slice<kBlockN>(p, ti, staging + s * (32 * STG_LD), s & 3, s >> 2, lane);
+                    mbar_arrive(stg_empty);
+                    spar ^= 1;
+                }
+                return;
+            }
+        }
         if (warp == NUM_EPI_WARPS && elect_one()) {
             int stage = 0;
             uint32_t phase = 0;
@@ -287,54 +450,82 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                     }
                     continue;
                 }
-                if (kExact && p.conv && p.residual && p.vec_ok && ti.n0 + kBlockN <= p.Ncols) prefetch_residual_l2(p, ti, kBlockN);
-                for (int kb = 0; kb < ti.nkb; ++kb) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1, "vf_tc_gemm producer");
-                    mbar_expect_tx(&full_bar[stage], (uint32_t)STAGE_BYTES);
-                    uint8_t* sa = smem + stage * STAGE_BYTES;
-                    uint8_t* sb = sa + A_STAGE_BYTES;
-                    int kcoord_b = kb * p.bk_elems;
-                    if (p.conv) {
-                        int kbr = kb, a_half = 0;
-                        if (p.exact) {       // product pass j: 0 = (lo_x, hi_w), 1 = (hi_x, lo_w), 2 = (hi_x, hi_w)
-                            const int j = kb / p.exact_kpp;
-                            kbr = kb - j * p.exact_kpp;
-                            a_half = (j == 0) ? p.exact_clog : 0;
-                            const int tap_ = kbr / p.cin_blocks, cb_ = kbr - tap_ * p.cin_blocks;
-                            kcoord_b = ((tap_ * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb_) * p.bk_elems;
+                if constexpr (kExact) {
+                    // tap-box convs and GEMMs: product pass j (0 = (lo_x, hi_w), 1 = (hi_x, lo_w), 2 = (hi_x, hi_w)), k-block kbr of
+                    // the pass, for a conv its tap and channel block cb.  Walked by counters: the ring is 4 k-blocks deep, so the one
+                    // producer thread's latency per k-block (divisions, dependent constant loads) would show in the MMA rate.
+                    if (p.conv && p.residual && p.vec_ok && ti.n0 + kBlockN <= p.Ncols) prefetch_residual_l2(p, ti, kBlockN);
+                    int j = 0, kbr = 0, tap = 0, cb = 0;
+                    for (int kb = 0; kb < ti.nkb; ++kb) {
+                        mbar_wait(&empty_bar[stage], phase ^ 1, "vf_tc_gemm producer");
+                        mbar_expect_tx(&full_bar[stage], (uint32_t)STAGE_BYTES);
+                        uint8_t* sa = smem + stage * STAGE_BYTES;
+                        uint8_t* sb = sa + A_STAGE_BYTES;
+                        if (p.conv) {
+                            tma_load_4d(sa, &p.tmA, &full_bar[stage], (j == 0 ? p.exact_clog : 0) + p.tap_coff[tap] + cb * p.bk_elems,
+                                        ti.ox0 + p.tap_dx[tap], ti.oy0 + p.tap_dy[tap], ti.img0);
+                            tma_load_4d(sb, &p.tmB, &full_bar[stage], ((tap * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb) * p.bk_elems,
+                                        ti.n0, 0, 0);
+                        } else {
+                            const int kcoord_a = (j == 0 ? p.exact_clog : 0) + kbr * p.bk_elems + (p.gemm_koff ? p.tap_coff[ti.b1] : 0);
+                            tma_load_4d(sa, &p.tmA, &full_bar[stage], kcoord_a, ti.m0, ti.b2 * p.a_bm2, ti.b1 * p.a_bm1);
+                            tma_load_4d(sb, &p.tmB, &full_bar[stage], (j == 1 ? p.exact_lo_b : 0) + kbr * p.bk_elems, ti.n0,
+                                        ti.b2 * p.b_bm2, ti.b1 * p.b_bm1);
                         }
-                        const int tap = kbr / p.cin_blocks;
-                        const int cb = kbr - tap * p.cin_blocks;
-                        tma_load_4d(sa, &p.tmA, &full_bar[stage], a_half + p.tap_coff[tap] + cb * p.bk_elems, ti.ox0 + p.tap_dx[tap],
-                                    ti.oy0 + p.tap_dy[tap], ti.img0);
-                    } else {
-                        int kcoord_a = kb * p.bk_elems;
-                        if (p.exact) {       // same three passes for a plain GEMM: A rows [hi(K) .. | lo(K) ..], B rows likewise
-                            const int j = kb / p.exact_kpp, kbr = kb - j * p.exact_kpp;
-                            kcoord_a = (j == 0 ? p.exact_clog : 0) + kbr * p.bk_elems;
-                            kcoord_b = (j == 1 ? p.exact_lo_b : 0) + kbr * p.bk_elems;
-                        }
-                        if (p.gemm_koff) kcoord_a += p.tap_coff[ti.b1];
-                        tma_load_4d(sa, &p.tmA, &full_bar[stage], kcoord_a, ti.m0, ti.b2 * p.a_bm2, ti.b1 * p.a_bm1);
+                        if (++kbr == p.exact_kpp) { kbr = tap = cb = 0; ++j; }
+                        else if (++cb == p.cin_blocks) { cb = 0; ++tap; }
+                        if (++stage == NG) { stage = 0; phase ^= 1; }
                     }
-                    tma_load_4d(sb, &p.tmB, &full_bar[stage], kcoord_b, ti.n0, ti.b2 * p.b_bm2, ti.b1 * p.b_bm1);
-                    if (++stage == NG) { stage = 0; phase ^= 1; }
+                } else {
+                    for (int kb = 0; kb < ti.nkb; ++kb) {
+                        mbar_wait(&empty_bar[stage], phase ^ 1, "vf_tc_gemm producer");
+                        mbar_expect_tx(&full_bar[stage], (uint32_t)STAGE_BYTES);
+                        uint8_t* sa = smem + stage * STAGE_BYTES;
+                        uint8_t* sb = sa + A_STAGE_BYTES;
+                        int kcoord_b = kb * p.bk_elems;
+                        if (p.conv) {
+                            int kbr = kb, a_half = 0;
+                            if (p.exact) {       // product pass j: 0 = (lo_x, hi_w), 1 = (hi_x, lo_w), 2 = (hi_x, hi_w)
+                                const int j = kb / p.exact_kpp;
+                                kbr = kb - j * p.exact_kpp;
+                                a_half = (j == 0) ? p.exact_clog : 0;
+                                const int tap_ = kbr / p.cin_blocks, cb_ = kbr - tap_ * p.cin_blocks;
+                                kcoord_b = ((tap_ * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb_) * p.bk_elems;
+                            }
+                            const int tap = kbr / p.cin_blocks;
+                            const int cb = kbr - tap * p.cin_blocks;
+                            tma_load_4d(sa, &p.tmA, &full_bar[stage], a_half + p.tap_coff[tap] + cb * p.bk_elems, ti.ox0 + p.tap_dx[tap],
+                                        ti.oy0 + p.tap_dy[tap], ti.img0);
+                        } else {
+                            int kcoord_a = kb * p.bk_elems;
+                            if (p.exact) {       // same three passes for a plain GEMM: A rows [hi(K) .. | lo(K) ..], B rows likewise
+                                const int j = kb / p.exact_kpp, kbr = kb - j * p.exact_kpp;
+                                kcoord_a = (j == 0 ? p.exact_clog : 0) + kbr * p.bk_elems;
+                                kcoord_b = (j == 1 ? p.exact_lo_b : 0) + kbr * p.bk_elems;
+                            }
+                            if (p.gemm_koff) kcoord_a += p.tap_coff[ti.b1];
+                            tma_load_4d(sa, &p.tmA, &full_bar[stage], kcoord_a, ti.m0, ti.b2 * p.a_bm2, ti.b1 * p.a_bm1);
+                        }
+                        tma_load_4d(sb, &p.tmB, &full_bar[stage], kcoord_b, ti.n0, ti.b2 * p.b_bm2, ti.b1 * p.b_bm1);
+                        if (++stage == NG) { stage = 0; phase ^= 1; }
+                    }
                 }
             }
         }
         return;
     }
 
-    // ===================== MMA + epilogue (warps 0..7) =====================
-    setmaxnreg_inc<232>();
+    // ===================== MMA + epilogue (warps 0..7; exact mode: MMA and staging only) =====================
+    setmaxnreg_inc<kExact ? 208 : 232>();       // exact: the chunk sums, no epilogue state
     const int wg = warp >> 2;                          // MMA: warpgroup wg computes tile rows [64 wg, 64 wg + 64)
     const int quarter = warp & 3;                      // epilogue: this warp stores tile rows [32 quarter, +32) ...
     const int col_half = warp >> 2;                    // ... of column half col_half
     float* stg = staging + warp * (32 * STG_LD);       // the epilogue's staging tile of this warp [32][STG_LD]
     int stage = 0, ab = 0;
-    uint32_t phase = 0, aphase = 0, tpar = 0;
+    uint32_t phase = 0, aphase = 0, tpar = 0, spar = 0;
 
-    // fragment -> staging: element (r, c) of the 128 x kBlockN tile goes to the staging tile of the epilogue warp that stores it.
+    // fragment -> staging: element (r, c) of the 128 x kBlockN tile goes to the staging slice of the warp that stores it (slice
+    // quarter + 4 col_half: MMA+epilogue warp of that number, or in exact mode the epilogue warp that takes it).
     // Exact halo mode with 16 x 8-pixel tiles: MMA row group g of warpgroup wg is image row g, columns [8 wg, 8 wg + 8), stored as
     // tile row 16 g + 8 wg + i, so that every epilogue warp sums the same pixels as on the tap-box path (same GroupNorm partials).
     const bool col_split = kExact && p.halo && p.TW == 16;
@@ -454,8 +645,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             reg_fence(acc);
             retire_prev();
         };
-        // exact mode: the chunk sums take the registers the row bookkeeping, bias and residual would hold during the loop
-        if constexpr (kExact) k_loop();
+        if constexpr (kExact) {
+            // hand the chunk sums over to the epilogue warps and go straight on to the next tile
+            k_loop();
+            mbar_wait(stg_empty, spar ^ 1, "vf_tc_gemm mma(staging)");    // the epilogue warps have stored the previous tile
+            to_staging(csum, 1.0f);
+            mbar_arrive(stg_full);
+            spar ^= 1;
+            continue;
+        }
 
         // row bookkeeping: lane l stores tile row 32*quarter + l
         const int row = quarter * 32 + lane;
@@ -485,9 +683,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
         const int c_ln = (lane % VPR) * 4;             // column inside this warp's half
         const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
         // fast path: full-width tile, 16-byte aligned rows -> vector I/O and the whole residual tile prefetched into
-        // registers BEFORE the main loop, so its DRAM latency hides behind this tile's MMAs.  Exact mode keeps the chunk sums in
-        // those registers and loads the residual tile in the epilogue loop, half a tile at a time (a whole tile would spill), from
-        // L2: the producer prefetched it there while the K loop ran.
+        // registers BEFORE the main loop, so its DRAM latency hides behind this tile's MMAs.
         const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
         auto residual_at = [&](int i) {
             const int rr = i * RPI + r_sub;
@@ -498,22 +694,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             const long long o = ok ? off_row + n_ln : (long long)n_ln;
             return __ldg(reinterpret_cast<const float4*>(p.residual + o));
         };
-        constexpr int RB = kExact ? ITERS / 2 : ITERS;
-        float4 resv[RB];
+        float4 resv[ITERS];
         auto load_residual = [&](int i0) {
             if (fast && p.residual) {
 #pragma unroll
-                for (int i = 0; i < RB; ++i) resv[i] = residual_at(i0 + i);
+                for (int i = 0; i < ITERS; ++i) resv[i] = residual_at(i0 + i);
             }
         };
-        if constexpr (!kExact) load_residual(0);
+        load_residual(0);
         float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (fast && p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
 
-        if constexpr (!kExact) k_loop();
+        k_loop();
         named_sync(1, NUM_MMA_THREADS);                           // the previous tile's epilogue is done with the staging tile
-        if constexpr (kExact) to_staging(csum, 1.0f);
-        else to_staging(acc, p.alpha);
+        to_staging(acc, p.alpha);
         named_sync(1, NUM_MMA_THREADS);                           // staging tile complete
 
         // ---- phase 2: lanes span the columns of a tile row -> fully coalesced stores; bias / activation / residual here
@@ -521,7 +715,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             float gs = 0.f, gq = 0.f;                 // fused GroupNorm statistics of this lane's 4 channels
 #pragma unroll
             for (int i = 0; i < ITERS; ++i) {
-                if (kExact && i % RB == 0) load_residual(i);
                 const int rr = i * RPI + r_sub;
                 const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
                 const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
@@ -531,7 +724,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                 else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
                 if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
                 if (p.residual) {
-                    const float4 r = resv[i % RB];
+                    const float4 r = resv[i];
                     v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
                 }
                 if (ok) {
