@@ -359,6 +359,17 @@ int vf_pose_postprocess(const float* raw, int64_t rows, float pose_multiplier, f
 int vf_cameras_prepare(const float* cams, int B, int T, int relative, float* out, float* transform, vf_stream_t s);
 /* inverse map (evaluate_transformer.py:81-87): out[b,i] = transform[b] o cams[b,i];  cams [B,n,7], transform [B,7] */
 int vf_cameras_from_relative(const float* cams, const float* transform, int B, int n, float* out, vf_stream_t s);
+/* nearest cameras of 7-Scenes localisation: for each of Q query cameras [Q,7] (xyz | wxyz), the k database cameras of least distance,
+ * ascending, ties to the lower database index (a stable sort: tf.argsort at evaluate/evaluate_sevenscenes.py:189, tf.argmin at
+ * evaluate_sevenscenes_baseline.py:93).  Distances in fp32 with x1 = the database camera, x2 = the query:
+ *   mode 0: 0.3 |xyz1 - xyz2| + 2 asin |vec(n(q1) n(q2)*)|   (evaluate_sevenscenes.py:36-45, n = l2 normalisation, eps 1e-12)
+ *   mode 1: |xyz1 - xyz2|;  mode 2: 2 asin |vec(n(q1) n(q2)*)|  (evaluate_sevenscenes_baseline.py:43-51)
+ * The argument of asin is clamped to 1: for a pose 180 degrees from the query it can round above 1, where the reference's distance is
+ * NaN and its argsort order undefined; here it is pi.
+ * db [N,7] shared by all queries when db_stride == 0, else query q reads db + q * db_stride (floats, >= 7 N).
+ * 1 <= k <= 64, k <= N.  idx_out int32 [Q,k], dist_out f32 [Q,k]. */
+int vf_camera_knn(const float* db, int64_t N, int64_t db_stride, const float* queries, int Q, int mode, int k, int32_t* idx_out,
+                  float* dist_out, vf_stream_t s);
 /* evaluation losses of MIGT.call(compute_losses=True) — models/migt.py:417-448, 165-177 */
 int vf_cross_entropy_rows(const float* logits, const int32_t* labels, int64_t rows, int cols, float smoothing, float* out,
                           vf_stream_t s);                       /* sparse softmax CE per row (fp32) */

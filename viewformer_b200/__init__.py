@@ -16,6 +16,10 @@ def __getattr__(name):   # lazy: importing the package must not require the buil
     if name in ("generate_batch_predictions", "generate_batch_predictions_multictx", "GraphedPredictions"):
         from . import generate
         return getattr(generate, name)
+    if name in ("generate_other_viewpoints", "compute_camera_distances", "SceneLookup", "generate_batch_predictions_using_generated_images",
+                "generate_batch_predictions_using_pose_refinement", "generate_batch_predictions_baseline", "BaselineEvaluator"):
+        from . import sevenscenes
+        return getattr(sevenscenes, name)
     if name in ("transformer_predict", "run_with_batchsize", "encode_images", "decode_code", "generate_codebook_predictions"):
         from . import evaluate
         return getattr(evaluate, name)
@@ -31,7 +35,8 @@ def __getattr__(name):   # lazy: importing the package must not require the buil
     if name in ("LatentCodeTransformer", "write_token_dataset", "load_token_dataset", "read_tfrecords", "TFRecordWriter", "process_batch"):
         from . import data
         return getattr(data, name)
-    if name in ("compat", "schedules", "tf_checkpoint", "cabi", "metrics", "data", "evaluate", "generate", "registry", "train", "train_migt"):
+    if name in ("compat", "schedules", "tf_checkpoint", "cabi", "metrics", "data", "evaluate", "generate", "registry", "train", "train_migt",
+                "sevenscenes"):
         import importlib
         return importlib.import_module("." + name, __name__)
     raise AttributeError(name)

@@ -21,7 +21,7 @@ EXPORTS = [
     "vf_nchw_to_nhwc_f32", "vf_nhwc_to_nchw_f32", "vf_groupnorm_stats", "vf_groupnorm_apply", "vf_layernorm",
     "vf_simt_gemm", "vf_tc_gemm", "vf_tc_gemm_plan", "vf_vq_lookup", "vf_gather_rows", "vf_vq_ema_stats", "vf_vq_ema_update", "vf_vq_commit_grad",
     "vf_vq_prepare_codebook", "vf_migt_embed", "vf_softmax_rows", "vf_argmax_rows", "vf_pose_postprocess",
-    "vf_cameras_prepare", "vf_cameras_from_relative",
+    "vf_cameras_prepare", "vf_cameras_from_relative", "vf_camera_knn",
     "vf_conv3x3_small_cin", "vf_conv3x3_small_cout", "vf_groupnorm_finalize", "vf_split_f16x2", "vf_attn_block_causal_decode", "vf_attn_block_multiend",
     "vf_cross_entropy_rows", "vf_pose_loss_rows", "vf_row_mean",
     "vf_vq_prepare_codebook_f16", "vf_vq_lookup_fused", "vf_resize_u8", "vf_resize_f32", "vf_image_pair_sums", "vf_ssim_u8", "vf_ssim_u8_k",

@@ -242,6 +242,77 @@ __global__ void cameras_from_relative_kernel(const float* __restrict__ cams, con
     o[3] = q.w; o[4] = q.x; o[5] = q.y; o[6] = q.z;
 }
 
+// nearest cameras (evaluate_sevenscenes.py:36-45, 187-189; evaluate_sevenscenes_baseline.py:43-51, 93): one CTA per query.  Each
+// database camera becomes a 64-bit key (order-preserving bits of its fp32 distance | its index), so keys are unique and ascending key
+// order is ascending distance with ties to the lower index; k rounds of a block-wide min over the keys above the last one picked.
+// The first KNN_CACHE keys are kept in shared memory; a larger database recomputes the rest each round.
+constexpr int KNN_THREADS = 256;
+constexpr int KNN_CACHE = 8192;                    // 64 KB of keys: a 7-Scenes training split (1 000 - 7 000 frames) fits whole
+
+__device__ __forceinline__ Quat qnormalize(Quat q) {   // l2_normalize(axis=-1, epsilon=1e-12), geometry_tf.py:44-45
+    const float r = rsqrtf(fmaxf(((q.w * q.w + q.x * q.x) + q.y * q.y) + q.z * q.z, 1e-12f));
+    return Quat{q.w * r, q.x * r, q.y * r, q.z * r};
+}
+
+__device__ __forceinline__ unsigned long long knn_key(const float* __restrict__ c, float px, float py, float pz, Quat qconj, int mode,
+                                                      uint32_t i) {
+    float d = 0.f;
+    if (mode != 2) {
+        const float dx = c[0] - px, dy = c[1] - py, dz = c[2] - pz;
+        d = sqrtf((dx * dx + dy * dy) + dz * dz);
+        if (mode == 0) d = __fmul_rn(d, 0.3f);     // pos * 0.3, rounded before the sum as the reference rounds it
+    }
+    if (mode != 1) {
+        const Quat r = qmul(qnormalize(Quat{c[3], c[4], c[5], c[6]}), qconj);
+        d = __fadd_rn(d, 2.f * asinf(fminf(sqrtf((r.x * r.x + r.y * r.y) + r.z * r.z), 1.f)));
+    }
+    uint32_t u = __float_as_uint(d);
+    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    return ((unsigned long long)u << 32) | i;
+}
+
+__global__ void __launch_bounds__(KNN_THREADS) camera_knn_kernel(const float* __restrict__ db, int64_t N, int64_t db_stride,
+                                                                 const float* __restrict__ queries, int mode, int k, int ncache,
+                                                                 int32_t* __restrict__ idx_out, float* __restrict__ dist_out) {
+    extern __shared__ unsigned long long keys[];
+    __shared__ unsigned long long warp_min[KNN_THREADS / 32];
+    __shared__ unsigned long long picked;
+    const int64_t qi = blockIdx.x;
+    const float* q = queries + qi * 7;
+    const float* base = db + qi * db_stride;
+    const float px = q[0], py = q[1], pz = q[2];
+    const Quat qn = qnormalize(Quat{q[3], q[4], q[5], q[6]});
+    const Quat qconj = {qn.w, -qn.x, -qn.y, -qn.z};
+    for (int i = threadIdx.x; i < ncache; i += KNN_THREADS) keys[i] = knn_key(base + (int64_t)i * 7, px, py, pz, qconj, mode, (uint32_t)i);
+    __syncthreads();
+    unsigned long long lo = 0;                     // keys are unique: round r takes the least key >= (round r-1's key) + 1
+    for (int r = 0; r < k; ++r) {
+        unsigned long long best = ~0ull;
+        for (int64_t i = threadIdx.x; i < N; i += KNN_THREADS) {
+            const unsigned long long key = i < ncache ? keys[i] : knn_key(base + i * 7, px, py, pz, qconj, mode, (uint32_t)i);
+            if (key >= lo && key < best) best = key;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+            best = other < best ? other : best;
+        }
+        if ((threadIdx.x & 31) == 0) warp_min[threadIdx.x >> 5] = best;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned long long b = warp_min[0];
+            for (int w = 1; w < KNN_THREADS / 32; ++w) b = warp_min[w] < b ? warp_min[w] : b;
+            uint32_t u = (uint32_t)(b >> 32);
+            u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+            idx_out[qi * k + r] = (int32_t)(uint32_t)b;
+            dist_out[qi * k + r] = __uint_as_float(u);
+            picked = b;
+        }
+        __syncthreads();
+        lo = picked + 1;
+    }
+}
+
 // sparse softmax cross-entropy per row (tf.nn.sparse_softmax_cross_entropy_with_logits, models/migt.py:99-104,419-423);
 // label smoothing s: loss = (1-s) * nll + s * (lse - mean(logits)).  One warp per row.
 __global__ void __launch_bounds__(256) ce_rows_kernel(const float* __restrict__ logits, const int32_t* __restrict__ labels,
@@ -392,6 +463,27 @@ extern "C" int vf_cameras_from_relative(const float* cams, const float* transfor
     if (B == 0) return VF_OK;
     cameras_from_relative_kernel<<<(B * n + 127) / 128, 128, 0, vf_s(s)>>>(cams, transform, B, n, out);
     VF_CHECK_LAUNCH("vf_cameras_from_relative");
+    return VF_OK;
+}
+extern "C" int vf_camera_knn(const float* db, int64_t N, int64_t db_stride, const float* queries, int Q, int mode, int k, int32_t* idx_out,
+                             float* dist_out, vf_stream_t s) {
+    VF_CHECK_ARG(db && queries && idx_out && dist_out, "vf_camera_knn: null");
+    VF_CHECK_ARG(Q >= 0 && N >= 1 && N < (1ll << 31) && db_stride >= 0, "vf_camera_knn: bad sizes (N %lld, Q %d)", (long long)N, Q);
+    VF_CHECK_ARG(mode >= 0 && mode <= 2, "vf_camera_knn: mode %d (0 combined, 1 position, 2 orientation)", mode);
+    VF_CHECK_ARG(k >= 1 && k <= 64 && k <= N, "vf_camera_knn: k %d outside [1, min(64, N = %lld)]", k, (long long)N);
+    VF_CHECK_ARG(db_stride == 0 || db_stride >= N * 7, "vf_camera_knn: db_stride %lld overlaps the %lld cameras of a query",
+                 (long long)db_stride, (long long)N);
+    if (Q == 0) return VF_OK;
+    static vf_per_device_flag flag;
+    bool& configured = flag.current();
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(camera_knn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, KNN_CACHE * 8);
+        if (e != cudaSuccess) { vf_set_error("vf_camera_knn: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return VF_ERR_CUDA; }
+        configured = true;
+    }
+    const int ncache = (int)(N < KNN_CACHE ? N : KNN_CACHE);
+    camera_knn_kernel<<<(unsigned)Q, KNN_THREADS, (size_t)ncache * 8, vf_s(s)>>>(db, N, db_stride, queries, mode, k, ncache, idx_out, dist_out);
+    VF_CHECK_LAUNCH("vf_camera_knn");
     return VF_OK;
 }
 extern "C" int vf_cross_entropy_rows(const float* logits, const int32_t* labels, int64_t rows, int cols, float smoothing, float* out,

@@ -75,6 +75,13 @@ def normalize_cameras(cameras):
 
 
 # --------------------------------------------------------------------------- generate
+def localize_last_view(transformer_model, codes, cams):
+    """The localisation forward of evaluate_transformer.py:134-136 and evaluate_sevenscenes.py:103-104,143-144: codes [B,T,h,w] of all
+    T views, prepared cameras [B,T,7] of which the first T-1 are given -> the last view's camera [B,1,7] in the model's pose frame."""
+    out = transformer_model(dict(input_ids=codes, poses=cams[:, :-1].contiguous()))
+    return reduce_cameras(out["pose_prediction"][:, -1:], -2)
+
+
 def generate_batch_predictions(transformer_model, codebook_model, images, cameras, *, encode_target=None):
     """images [B,T,H,W,C] (host or device), cameras f32 [B,T,7] ->
     dict(ground_truth_images [B,H,W,C] (the input's), generated_images [B,S,S,out_ch] u8, ground_truth_cameras [B,7],
@@ -119,8 +126,7 @@ def generate_batch_predictions(transformer_model, codebook_model, images, camera
     gen_images = codebook_model.decode_code_u8(gen_codes)
 
     if use_loc:
-        out = transformer_model(dict(input_ids=codes, poses=cams_dev[:, :-1].contiguous()))
-        gen_cam = reduce_cameras(out["pose_prediction"][:, -1:], -2)
+        gen_cam = localize_last_view(transformer_model, codes, cams_dev)
     else:
         gen_cam = cams_dev[:, :1]
     if relative:
