@@ -404,6 +404,8 @@ def test_gemm_walk_by_row_blocks(L):
     out = torch.empty((M, N), device="cuda")
     k = dict(M=M, N=N, K=K, lda=K, ldb=K, ldc=N, bias=_mat(N, 852), bias_mode=L.BIAS_N)
     _gemm_plan(L, "bf16 gemm row blocks", (A, B, out), k, 2)
+    with pytest.raises(L.LibraryError, match="row strides"):     # the plan validates a parameter block as the launch does
+        L.tc_gemm(A, B, out, plan=True, **dict(k, lda=K + 1))
     before, check = lc.CHECKERS["tc_gemm"]
     ba = lc.bind(L.tc_gemm, A, B, out, **k)
     st = before(ba, random.Random(0))

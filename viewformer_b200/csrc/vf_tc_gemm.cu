@@ -9,6 +9,7 @@
 // warpgroup (one elected thread issues the loads; the warpgroup hands its registers to the MMA warpgroups).  Exact mode moves the
 // epilogue's stores onto warps 9..11 of the producer warpgroup: the MMA warps write the staging tile, hand it over through an
 // mbarrier pair and go straight on to the next tile's MMAs while those warps add bias and residual, store and fold the GroupNorm sums.
+// Both roles run the same epilogue function, store_slice.  vf_tc_gemm_plan and vf_tc_gemm share one validation and tiling, tc_setup.
 // A CTA walks 128 x BLOCK_N output tiles; the producer runs ahead across tiles, so the next tile's operands stream in while the
 // epilogue of this one runs.  GEMM operands are K-major; the convolution reads its A operand straight from the NHWC activation
 // tensor with a 4-D tensor map: for every filter tap the box [TN images x TH rows x TW cols x 64 channels] shifted by (dy,dx)
@@ -56,7 +57,6 @@ struct TcParams {
                                // 0 = one shifted TMA box per tap
     double* gn_sums;           // optional fused GroupNorm statistics of the OUTPUT: [images][groups][2] (sum, sum of squares)
     int gn_groups, gn_cpg, gn_rows_per_img;
-    int exact;                 // split-fp16 operands (VF_F16X2), three product passes, chunked accumulation (see EXACT_LO_SCALE)
     int exact_kc;              // k-blocks per accumulation chunk (divides ntaps * cin_blocks)
     int exact_clog;            // logical channels of the split activation tensor (= Ctot / 2): the lo half starts there
     int exact_kpp;             // k-blocks per product pass = ntaps * cin_blocks (conv) or K / 64 (gemm)
@@ -193,79 +193,99 @@ __device__ __forceinline__ void normalise_halo(const TcParams& p, uint8_t* tile,
     }
 }
 
-// Exact mode's epilogue, run by warps 9..11: one 32-row x HALF_N slice of the staging tile, the slice the MMA+epilogue warp
-// `quarter + 4 col_half` stores on the bf16 / TF32 path, with that path's lane mapping, bias -> residual -> store order and GroupNorm
-// shuffle tree (so outputs and fp32 GroupNorm partials are the same bits).  The residual comes from L2 (the producer prefetched it),
-// STORE_RES_VECS vectors at a time.
+// ---- epilogue: one 32-row x HALF_N slice of the staging tile -> bias, GELU, residual, f32 / bf16 stores, GroupNorm statistics ----
+// Slice s = quarter + 4 col_half holds tile rows [32 quarter, +32) and columns [HALF_N col_half, +HALF_N).  In the bf16 / TF32
+// instances MMA warp s stores slice s; in exact mode epilogue warp e (9..11) stores slices e, e + 3, e + 6.  Both run store_slice, so
+// exact mode keeps the lanes' rows and columns, the arithmetic order and the GroupNorm shuffle tree of the other instances.
+// Vector path geometry: VPR float4 vectors span a slice row, a warp covers RPI rows per iteration, ITERS iterations.
 template <int kBlockN>
-__device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& ti, const float* stg, int quarter, int col_half, int lane) {
-    constexpr int HALF_N = kBlockN / 2;
-    constexpr int STG_LD = HALF_N + 4;
-    // row bookkeeping: lane l stores tile row 32*quarter + l
+struct EpiGeom {
+    static constexpr int HALF_N = kBlockN / 2, STG_LD = HALF_N + 4, VPR = HALF_N / 4, RPI = 32 / VPR, ITERS = 32 / RPI;
+};
+
+// Row bookkeeping: lane l owns tile row 32 quarter + l; the other lanes of the warp read it with shuffles.
+struct EpiLane {
+    long long off;      // the row's element offset in C and in the residual
+    int ok, gm;         // the row lies inside the output; its global row (GEMM) or pixel (conv)
+    float bias_m;       // VF_BIAS_M: the row's bias
+};
+
+__device__ __forceinline__ EpiLane epi_lane(const TcParams& p, const TileInfo& ti, int quarter, int lane) {
     const int row = quarter * 32 + lane;
-    long long my_off;
-    int my_ok, gm;
+    long long off;
+    int ok, gm;
     if (p.conv) {
         const int lx = row % p.TW;
         const int q = row / p.TW;
         const int ly = q % p.TH;
         const int ln = q / p.TH;
         const int img = ti.img0 + ln, oy = ti.oy0 + ly, ox = ti.ox0 + lx;
-        my_ok = (img < p.Nimg) && (oy < p.OH) && (ox < p.OW);
+        ok = (img < p.Nimg) && (oy < p.OH) && (ox < p.OW);
         gm = (img * p.OH + oy) * p.OW + ox;
-        my_off = (long long)gm * p.ldc;
+        off = (long long)gm * p.ldc;
     } else {
         gm = ti.m0 + row;
-        my_ok = gm < p.M;
-        my_off = (long long)ti.b1 * p.c_sb1 + (long long)ti.b2 * p.c_sb2 + (long long)gm * p.ldc;
+        ok = gm < p.M;
+        off = (long long)ti.b1 * p.c_sb1 + (long long)ti.b2 * p.c_sb2 + (long long)gm * p.ldc;
     }
-    const float bias_m = (p.bias_mode == VF_BIAS_M && my_ok) ? __ldg(p.bias + gm) : 0.f;
+    const float bias_m = (p.bias_mode == VF_BIAS_M && ok) ? __ldg(p.bias + gm) : 0.f;
+    return {off, ok, gm, bias_m};
+}
 
-    constexpr int VPR = HALF_N / 4;                // float4 vectors per half row
-    constexpr int RPI = 32 / VPR;                  // rows per iteration
-    constexpr int ITERS = 32 / RPI;
-    constexpr int RB = STORE_RES_VECS;
-    static_assert(ITERS % RB == 0, "residual batches");
-    const int r_sub = lane / VPR;
-    const int c_ln = (lane % VPR) * 4;
-    const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
-    const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
+// The vector path's residual float4 of slice row rr at column n_ln.  Unconditional (out-of-range rows read row 0 and are never
+// stored): a predicated load would make the compiler funnel a batch of loads through one temporary and serialise their latencies.
+__device__ __forceinline__ float4 residual_vec(const TcParams& p, const EpiLane& el, int rr, int n_ln) {
+    const int ok = __shfl_sync(0xffffffffu, el.ok, rr);
+    const long long off_row = __shfl_sync(0xffffffffu, el.off, rr);
+    return __ldg(reinterpret_cast<const float4*>(p.residual + (ok ? off_row + n_ln : (long long)n_ln)));
+}
+
+// stg: the slice, [32][STG_LD].  fast: the vector path (full-width tile, 16-byte aligned rows), whose VF_BIAS_N bias (bias4) and
+// residual (resv) each role loads on its own schedule.  The bf16 / TF32 MMA warps pass all three in, the residual as all ITERS vectors
+// loaded into registers before their K loop, so the DRAM latency hides under the tile's MMAs.  Exact mode's epilogue warps have 80
+// registers: they pass nothing, and store_slice computes them here, the residual from L2 (the producer prefetched it) STORE_RES_VECS
+// vectors at a time.
+template <int kBlockN, bool kExact>
+__device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& ti, const EpiLane& el, const float* stg, int col_half,
+                                            int lane, bool fast, float4 bias4, const float4* resv) {
+    using G = EpiGeom<kBlockN>;
+    constexpr int RB = kExact ? STORE_RES_VECS : G::ITERS;     // residual vectors per batch
+    static_assert(G::ITERS % RB == 0, "residual batches");
+    const int r_sub = lane / G::VPR;
+    const int c_ln = (lane % G::VPR) * 4;         // column inside the slice
+    const int n_ln = ti.n0 + col_half * G::HALF_N + c_ln;
+    if constexpr (kExact) fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
     if (fast) {
-        float4 resv[RB];
-        float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
-        float gs = 0.f, gq = 0.f;
+        if constexpr (kExact) {
+            bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
+        }
+        float gs = 0.f, gq = 0.f;                 // fused GroupNorm statistics of this lane's 4 channels
 #pragma unroll 1
-        for (int i0 = 0; i0 < ITERS; i0 += RB) {
-            if (p.residual) {
+        for (int i0 = 0; i0 < G::ITERS; i0 += RB) {
+            float4 resb[RB];
+            if (kExact && p.residual) {
 #pragma unroll
-                for (int k = 0; k < RB; ++k) {
-                    const int rr = (i0 + k) * RPI + r_sub;
-                    const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                    const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                    // out-of-range rows read row 0 and are never stored (unconditional: the loads stay independent)
-                    resv[k] = __ldg(reinterpret_cast<const float4*>(p.residual + (ok ? off_row + n_ln : (long long)n_ln)));
-                }
+                for (int k = 0; k < RB; ++k) resb[k] = residual_vec(p, el, (i0 + k) * G::RPI + r_sub, n_ln);
             }
 #pragma unroll
             for (int k = 0; k < RB; ++k) {
-                const int i = i0 + k;
-                const int rr = i * RPI + r_sub;
-                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
-                float4 v = *reinterpret_cast<const float4*>(stg + rr * STG_LD + c_ln);
+                const int rr = (i0 + k) * G::RPI + r_sub;
+                const int ok = __shfl_sync(0xffffffffu, el.ok, rr);
+                const long long off_row = __shfl_sync(0xffffffffu, el.off, rr);
+                const float bm = __shfl_sync(0xffffffffu, el.bias_m, rr);
+                float4 v = *reinterpret_cast<const float4*>(stg + rr * G::STG_LD + c_ln);
                 if (p.bias_mode == VF_BIAS_N) { v.x += bias4.x; v.y += bias4.y; v.z += bias4.z; v.w += bias4.w; }
                 else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
                 if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
                 if (p.residual) {
-                    const float4 r = resv[k];
+                    const float4 r = kExact ? resb[k] : resv[i0 + k];
                     v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
                 }
                 if (ok) {
                     gs += (v.x + v.y) + (v.z + v.w);
-                    // the recorded GroupNorm partials (tests/golden/exact_conv_bits.json) are this rounding; written out, so that which
-                    // product the compiler would fuse into the add cannot change it
+                    // the GroupNorm partials (recorded for exact mode in tests/golden/exact_conv_bits.json) are this rounding; written
+                    // out, so that which product the compiler would fuse into the add cannot change it
                     gq += __fmaf_rn(v.y, v.y, __fmul_rn(v.x, v.x)) + __fmaf_rn(v.w, v.w, __fmul_rn(v.z, v.z));
                     const long long off = off_row + n_ln;
                     if (p.C_f32) *reinterpret_cast<float4*>(p.C_f32 + off) = v;
@@ -282,9 +302,9 @@ __device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& t
         if (p.gn_sums) {
             // the 32 rows of a slice lie in one image; lanes with equal column vector (different r_sub) and the cpg/4 neighbouring
             // lanes of a group are folded with shuffles, then one fp64 RED per (image, group)
-            const unsigned okmask = __ballot_sync(0xffffffffu, my_ok);
+            const unsigned okmask = __ballot_sync(0xffffffffu, el.ok);
 #pragma unroll
-            for (int o = VPR; o < 32; o <<= 1) {
+            for (int o = G::VPR; o < 32; o <<= 1) {
                 gs += __shfl_xor_sync(0xffffffffu, gs, o);
                 gq += __shfl_xor_sync(0xffffffffu, gq, o);
             }
@@ -293,7 +313,7 @@ __device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& t
                 gs += __shfl_xor_sync(0xffffffffu, gs, o);
                 gq += __shfl_xor_sync(0xffffffffu, gq, o);
             }
-            const int gm_first = __shfl_sync(0xffffffffu, gm, okmask ? (__ffs(okmask) - 1) : 0);
+            const int gm_first = __shfl_sync(0xffffffffu, el.gm, okmask ? (__ffs(okmask) - 1) : 0);
             if (okmask && r_sub == 0 && (lane % lpg) == 0) {
                 const long long slot = ((long long)(gm_first / p.gn_rows_per_img) * p.gn_groups + n_ln / p.gn_cpg) * 2;
                 atomicAdd(p.gn_sums + slot, (double)gs);
@@ -304,14 +324,14 @@ __device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& t
         // generic path (N tails, unaligned leading dimensions): scalar, same arithmetic order
 #pragma unroll 1
         for (int rr = 0; rr < 32; ++rr) {
-            const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-            const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-            const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
+            const int ok = __shfl_sync(0xffffffffu, el.ok, rr);
+            const long long off_row = __shfl_sync(0xffffffffu, el.off, rr);
+            const float bm = __shfl_sync(0xffffffffu, el.bias_m, rr);
             if (!ok) continue;
-            for (int c = lane; c < HALF_N; c += 32) {
-                const int n = ti.n0 + col_half * HALF_N + c;
+            for (int c = lane; c < G::HALF_N; c += 32) {
+                const int n = ti.n0 + col_half * G::HALF_N + c;
                 if (n >= p.Ncols) continue;
-                float x = stg[rr * STG_LD + c];
+                float x = stg[rr * G::STG_LD + c];
                 x += (p.bias_mode == VF_BIAS_N) ? __ldg(p.bias + n) : bm;
                 if (p.act == VF_ACT_GELU_ERF) x = vf_gelu_erf(x);
                 const long long off = off_row + n;
@@ -333,7 +353,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
     constexpr int STG_LD = HALF_N + 4;         // staging row stride (floats): +4 keeps 128-bit row reads conflict-free
     constexpr int STG_BYTES = NUM_EPI_WARPS * 32 * STG_LD * 4;
     constexpr int NACC = kBlockN / 2;          // accumulator registers per thread (64 rows x kBlockN per warpgroup)
-    constexpr bool kExact = kKind == F16;      // fp16 operands are always split-fp16 pairs (TcParams::exact)
+    constexpr bool kExact = kKind == F16;      // fp16 operands are always split-fp16 pairs (VF_F16X2)
 
     extern __shared__ uint8_t smem_raw[];
     // 1024B alignment required by the 128B swizzle atoms
@@ -388,7 +408,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                     mbar_wait(stg_full, spar, "vf_tc_gemm epilogue");      // spans one K loop: well under a millisecond
 #pragma unroll 1
                     for (int s = e; s < NUM_EPI_WARPS; s += NUM_STORE_WARPS)
-                        store_slice<kBlockN>(p, ti, staging + s * (32 * STG_LD), s & 3, s >> 2, lane);
+                        store_slice<kBlockN, true>(p, ti, epi_lane(p, ti, s & 3, lane), staging + s * (32 * STG_LD), s >> 2, lane,
+                                                   false, float4(), nullptr);
                     mbar_arrive(stg_empty);
                     spar ^= 1;
                 }
@@ -482,31 +503,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
                         mbar_expect_tx(&full_bar[stage], (uint32_t)STAGE_BYTES);
                         uint8_t* sa = smem + stage * STAGE_BYTES;
                         uint8_t* sb = sa + A_STAGE_BYTES;
-                        int kcoord_b = kb * p.bk_elems;
                         if (p.conv) {
-                            int kbr = kb, a_half = 0;
-                            if (p.exact) {       // product pass j: 0 = (lo_x, hi_w), 1 = (hi_x, lo_w), 2 = (hi_x, hi_w)
-                                const int j = kb / p.exact_kpp;
-                                kbr = kb - j * p.exact_kpp;
-                                a_half = (j == 0) ? p.exact_clog : 0;
-                                const int tap_ = kbr / p.cin_blocks, cb_ = kbr - tap_ * p.cin_blocks;
-                                kcoord_b = ((tap_ * 2 + (j == 1 ? 1 : 0)) * p.cin_blocks + cb_) * p.bk_elems;
-                            }
-                            const int tap = kbr / p.cin_blocks;
-                            const int cb = kbr - tap * p.cin_blocks;
-                            tma_load_4d(sa, &p.tmA, &full_bar[stage], a_half + p.tap_coff[tap] + cb * p.bk_elems, ti.ox0 + p.tap_dx[tap],
+                            const int tap = kb / p.cin_blocks;
+                            const int cb = kb - tap * p.cin_blocks;
+                            tma_load_4d(sa, &p.tmA, &full_bar[stage], p.tap_coff[tap] + cb * p.bk_elems, ti.ox0 + p.tap_dx[tap],
                                         ti.oy0 + p.tap_dy[tap], ti.img0);
                         } else {
                             int kcoord_a = kb * p.bk_elems;
-                            if (p.exact) {       // same three passes for a plain GEMM: A rows [hi(K) .. | lo(K) ..], B rows likewise
-                                const int j = kb / p.exact_kpp, kbr = kb - j * p.exact_kpp;
-                                kcoord_a = (j == 0 ? p.exact_clog : 0) + kbr * p.bk_elems;
-                                kcoord_b = (j == 1 ? p.exact_lo_b : 0) + kbr * p.bk_elems;
-                            }
                             if (p.gemm_koff) kcoord_a += p.tap_coff[ti.b1];
                             tma_load_4d(sa, &p.tmA, &full_bar[stage], kcoord_a, ti.m0, ti.b2 * p.a_bm2, ti.b1 * p.a_bm1);
                         }
-                        tma_load_4d(sb, &p.tmB, &full_bar[stage], kcoord_b, ti.n0, ti.b2 * p.b_bm2, ti.b1 * p.b_bm1);
+                        tma_load_4d(sb, &p.tmB, &full_bar[stage], kb * p.bk_elems, ti.n0, ti.b2 * p.b_bm2, ti.b1 * p.b_bm1);
                         if (++stage == NG) { stage = 0; phase ^= 1; }
                     }
                 }
@@ -556,7 +563,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             // ---- phase 1: K loop.  One wgmma group (4 MMA steps of one k-block) stays in flight: once the group of k-block kb is
             // issued, wait for kb-1's and hand its ring slot back to the producer.
             const int nkb = (p.halo && !kExact) ? 9 * p.cin_blocks : ti.nkb;
-            const int nsmall = p.exact ? 2 * p.exact_kpp / p.exact_kc : 0;     // exact mode: cross-term chunks come first
+            const int nsmall = kExact ? 2 * p.exact_kpp / p.exact_kc : 0;      // exact mode: cross-term chunks come first
             int prev_stage = -1, prev_halo = -1, in_chunk = 0, ck = 0, tap = 0, j = 0, cb = 0;
             bool fresh = true;
             uint32_t a_base = 0;
@@ -655,53 +662,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
             continue;
         }
 
-        // row bookkeeping: lane l stores tile row 32*quarter + l
-        const int row = quarter * 32 + lane;
-        long long my_off;
-        int my_ok, gm;
-        if (p.conv) {
-            const int lx = row % p.TW;
-            const int q = row / p.TW;
-            const int ly = q % p.TH;
-            const int ln = q / p.TH;
-            const int img = ti.img0 + ln, oy = ti.oy0 + ly, ox = ti.ox0 + lx;
-            my_ok = (img < p.Nimg) && (oy < p.OH) && (ox < p.OW);
-            gm = (img * p.OH + oy) * p.OW + ox;
-            my_off = (long long)gm * p.ldc;
-        } else {
-            gm = ti.m0 + row;
-            my_ok = gm < p.M;
-            my_off = (long long)ti.b1 * p.c_sb1 + (long long)ti.b2 * p.c_sb2 + (long long)gm * p.ldc;
-        }
-        const float bias_m = (p.bias_mode == VF_BIAS_M && my_ok) ? __ldg(p.bias + gm) : 0.f;
-
-        // phase-2 geometry: VPR float4 vectors span one tile row; a warp covers RPI rows per iteration
-        constexpr int VPR = HALF_N / 4;                // 16 (BLOCK_N=128) or 8 (BLOCK_N=64) vectors per half row
-        constexpr int RPI = 32 / VPR;                  // 2 or 4 rows per iteration
-        constexpr int ITERS = 32 / RPI;
-        const int r_sub = lane / VPR;
-        const int c_ln = (lane % VPR) * 4;             // column inside this warp's half
-        const int n_ln = ti.n0 + col_half * HALF_N + c_ln;
-        // fast path: full-width tile, 16-byte aligned rows -> vector I/O and the whole residual tile prefetched into
-        // registers BEFORE the main loop, so its DRAM latency hides behind this tile's MMAs.
+        // vector path: the bias and the whole residual of this warp's slice go into registers BEFORE the K loop, so their DRAM latency
+        // hides behind this tile's MMAs
+        using G = EpiGeom<kBlockN>;
+        const EpiLane el = epi_lane(p, ti, quarter, lane);
+        const int n_ln = ti.n0 + col_half * HALF_N + (lane % G::VPR) * 4;
         const bool fast = p.vec_ok && (ti.n0 + kBlockN <= p.Ncols);
-        auto residual_at = [&](int i) {
-            const int rr = i * RPI + r_sub;
-            const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-            const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-            // unconditional load (out-of-range rows read row 0 and are never stored): a predicated load would make
-            // the compiler funnel all 32 loads through one temporary and serialise their DRAM latencies
-            const long long o = ok ? off_row + n_ln : (long long)n_ln;
-            return __ldg(reinterpret_cast<const float4*>(p.residual + o));
-        };
-        float4 resv[ITERS];
-        auto load_residual = [&](int i0) {
-            if (fast && p.residual) {
+        float4 resv[G::ITERS];
+        if (fast && p.residual) {
 #pragma unroll
-                for (int i = 0; i < ITERS; ++i) resv[i] = residual_at(i0 + i);
-            }
-        };
-        load_residual(0);
+            for (int i = 0; i < G::ITERS; ++i) resv[i] = residual_vec(p, el, i * G::RPI + lane / G::VPR, n_ln);
+        }
         float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (fast && p.bias_mode == VF_BIAS_N) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + n_ln));
 
@@ -709,80 +680,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tc_gemm_kernel(const __grid_co
         named_sync(1, NUM_MMA_THREADS);                           // the previous tile's epilogue is done with the staging tile
         to_staging(acc, p.alpha);
         named_sync(1, NUM_MMA_THREADS);                           // staging tile complete
-
-        // ---- phase 2: lanes span the columns of a tile row -> fully coalesced stores; bias / activation / residual here
-        if (fast) {
-            float gs = 0.f, gq = 0.f;                 // fused GroupNorm statistics of this lane's 4 channels
-#pragma unroll
-            for (int i = 0; i < ITERS; ++i) {
-                const int rr = i * RPI + r_sub;
-                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
-                float4 v = *reinterpret_cast<const float4*>(stg + rr * STG_LD + c_ln);
-                if (p.bias_mode == VF_BIAS_N) { v.x += bias4.x; v.y += bias4.y; v.z += bias4.z; v.w += bias4.w; }
-                else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
-                if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
-                if (p.residual) {
-                    const float4 r = resv[i];
-                    v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
-                }
-                if (ok) {
-                    gs += (v.x + v.y) + (v.z + v.w);
-                    gq += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
-                    const long long off = off_row + n_ln;
-                    if (p.C_f32) *reinterpret_cast<float4*>(p.C_f32 + off) = v;
-                    if (p.C_bf16) {
-                        __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-                        uint2 u;
-                        u.x = *reinterpret_cast<uint32_t*>(&lo);
-                        u.y = *reinterpret_cast<uint32_t*>(&hi);
-                        *reinterpret_cast<uint2*>(p.C_bf16 + off) = u;
-                    }
-                }
-            }
-            if (p.gn_sums) {
-                // the 32 rows of a warp lie in one image; lanes with equal column vector (different r_sub) and the
-                // cpg/4 neighbouring lanes of a group are folded with shuffles, then one fp64 RED per (image, group)
-                const unsigned okmask = __ballot_sync(0xffffffffu, my_ok);
-#pragma unroll
-                for (int o = VPR; o < 32; o <<= 1) {
-                    gs += __shfl_xor_sync(0xffffffffu, gs, o);
-                    gq += __shfl_xor_sync(0xffffffffu, gq, o);
-                }
-                const int lpg = p.gn_cpg >> 2;
-                for (int o = 1; o < lpg; o <<= 1) {
-                    gs += __shfl_xor_sync(0xffffffffu, gs, o);
-                    gq += __shfl_xor_sync(0xffffffffu, gq, o);
-                }
-                const int gm_first = __shfl_sync(0xffffffffu, gm, okmask ? (__ffs(okmask) - 1) : 0);
-                if (okmask && r_sub == 0 && (lane % lpg) == 0) {
-                    const long long slot = ((long long)(gm_first / p.gn_rows_per_img) * p.gn_groups + n_ln / p.gn_cpg) * 2;
-                    atomicAdd(p.gn_sums + slot, (double)gs);
-                    atomicAdd(p.gn_sums + slot + 1, (double)gq);
-                }
-            }
-        } else {
-            // generic path (N tails, unaligned leading dimensions): scalar, same arithmetic order
-#pragma unroll 1
-            for (int rr = 0; rr < 32; ++rr) {
-                const int ok = __shfl_sync(0xffffffffu, my_ok, rr);
-                const long long off_row = __shfl_sync(0xffffffffu, my_off, rr);
-                const float bm = __shfl_sync(0xffffffffu, bias_m, rr);
-                if (!ok) continue;
-                for (int c = lane; c < HALF_N; c += 32) {
-                    const int n = ti.n0 + col_half * HALF_N + c;
-                    if (n >= p.Ncols) continue;
-                    float x = stg[rr * STG_LD + c];
-                    x += (p.bias_mode == VF_BIAS_N) ? __ldg(p.bias + n) : bm;
-                    if (p.act == VF_ACT_GELU_ERF) x = vf_gelu_erf(x);
-                    const long long off = off_row + n;
-                    if (p.residual) x += __ldg(p.residual + off);
-                    if (p.C_f32) p.C_f32[off] = x;
-                    if (p.C_bf16) p.C_bf16[off] = __float2bfloat16(x);
-                }
-            }
-        }
+        store_slice<kBlockN, false>(p, ti, el, stg, col_half, lane, fast, bias4, resv);
     }
 }
 
@@ -861,33 +759,11 @@ int persistent_ctas() {
     return num_sms;
 }
 
-}  // namespace
-
-extern "C" int vf_tc_gemm_plan(const vf_tc_gemm_t* q, int* plan) {
-    VF_CHECK_ARG(q && plan, "vf_tc_gemm_plan: null argument");
-    const bool exact = q->ab_dtype == VF_F16X2;
-    const int bk = ROW_BYTES / (q->ab_dtype == VF_F32 ? 4 : 2);
-    const int block_n = (q->Ncols > 64) ? 128 : 64;
-    int TW = 0, TH = 0, TN = 0, halo = 0;
-    long long tiles_m;
-    if (q->conv) {
-        VF_CHECK_ARG(q->ntaps >= 1 && q->ntaps <= 9 && q->OW > 0 && q->OH > 0 && q->N > 0, "vf_tc_gemm_plan: conv shape");
-        halo = conv_tiling(q, exact, bk, &TW, &TH, &TN) ? 1 : 0;
-        tiles_m = (long long)((q->OW + TW - 1) / TW) * ((q->OH + TH - 1) / TH) * ((q->N + TN - 1) / TN);
-    } else {
-        VF_CHECK_ARG(q->M > 0 && q->batch1 > 0 && q->batch2 > 0, "vf_tc_gemm_plan: gemm shape");
-        tiles_m = (long long)((q->M + BLOCK_M - 1) / BLOCK_M) * q->batch1 * q->batch2;
-    }
-    const long long total = tiles_m * ((q->Ncols + block_n - 1) / block_n);
-    VF_CHECK_ARG(total > 0 && total < (1ll << 31), "vf_tc_gemm_plan: tile count out of range");
-    const int ctas = persistent_ctas();
-    const int vals[8] = {block_n, TW, TH, TN, halo, exact ? 1 : 0, (int)total, (int)(total < ctas ? total : ctas)};
-    for (int i = 0; i < 8; ++i) plan[i] = vals[i];
-    return VF_OK;
-}
-
-extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
-    VF_CHECK_ARG(q && q->A && q->B, "vf_tc_gemm: null operand");
+// Validates a parameter block and fills the kernel parameters that decide the tile walk: shapes, tiling, tile counts, the epilogue
+// and normalise-on-load options, block_n and the persistent CTA count.  vf_tc_gemm_plan reports from it and vf_tc_gemm launches it,
+// so the plan is the launch's tiling; vf_tc_gemm adds the tensor maps, vec_ok and the GroupNorm sums.
+int tc_setup(const vf_tc_gemm_t* q, TcParams& prm, int& block_n, int& ctas) {
+    VF_CHECK_ARG(q->A && q->B, "vf_tc_gemm: null operand");
     VF_CHECK_ARG(q->C_f32 || q->C_bf16, "vf_tc_gemm: no output");
     VF_CHECK_ARG(q->ab_dtype == VF_BF16 || q->ab_dtype == VF_F32 || q->ab_dtype == VF_F16X2, "vf_tc_gemm: bad dtype");
     const bool exact = q->ab_dtype == VF_F16X2;
@@ -901,12 +777,9 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     }
     VF_CHECK_ARG(q->bias_mode == VF_BIAS_NONE || q->bias, "vf_tc_gemm: bias pointer missing");
     VF_CHECK_ARG(!q->norm_mean_rstd || q->conv, "vf_tc_gemm: fused input GroupNorm is a convolution option");
-    const bool tf32 = q->ab_dtype == VF_F32;
-    const int tm_dtype = tf32 ? VF_F32 : VF_BF16;        // tensor-map element type (fp16 and bf16 move identically)
-    const int es = tf32 ? 4 : 2;
+    const int es = q->ab_dtype == VF_F32 ? 4 : 2;
     const int bk = ROW_BYTES / es;                       // K elements per block: 64 bf16 / 32 tf32
 
-    TcParams prm;
     memset(&prm, 0, sizeof(prm));
     prm.conv = q->conv;
     prm.Ncols = q->Ncols;
@@ -923,12 +796,10 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     prm.causal_skip_n = q->causal_skip_n;
 
     // N tile: 128 when the problem is wide enough, else 64 (fewer wasted MMA columns and accumulator registers)
-    const int block_n = (q->Ncols > 64) ? 128 : 64;
-    const int b_box_rows = block_n;
+    block_n = (q->Ncols > 64) ? 128 : 64;
     dim3 grid;
-    int rc;
     if (q->conv) {
-        VF_CHECK_ARG(q->ntaps >= 1 && q->ntaps <= 9, "vf_tc_gemm: ntaps");
+        VF_CHECK_ARG(q->ntaps >= 1 && q->ntaps <= 9 && q->OW > 0 && q->OH > 0 && q->N > 0, "vf_tc_gemm: conv shape");
         VF_CHECK_ARG(q->Cin % bk == 0 && q->Ctot % (16 / es) == 0, "vf_tc_gemm: conv Cin=%d must be a multiple of %d", q->Cin, bk);
         VF_CHECK_ARG(q->causal_block == 0, "vf_tc_gemm: causal with conv");
         int TW, TH, TN;
@@ -954,7 +825,6 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         prm.cin_blocks = q->Cin / bk;
         prm.num_k_blocks = q->ntaps * prm.cin_blocks;
         if (exact) {
-            prm.exact = 1;
             prm.exact_kpp = prm.num_k_blocks;
             prm.exact_clog = q->Ctot / 2;
             prm.exact_kc = (prm.num_k_blocks % 3 == 0) ? 3 : 1;      // k-blocks (= 4 MMA steps each) per accumulation chunk
@@ -963,15 +833,6 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         prm.M = q->N * q->OH * q->OW;
         prm.batch2 = 1;
         for (int t = 0; t < q->ntaps; ++t) { prm.tap_dy[t] = q->tap_dy[t]; prm.tap_dx[t] = q->tap_dx[t]; prm.tap_coff[t] = q->tap_coff[t]; }
-        const uint64_t dimsA[4] = {(uint64_t)q->Ctot, (uint64_t)q->W, (uint64_t)q->H, (uint64_t)q->N};
-        const uint64_t strA[3] = {(uint64_t)q->Ctot * es, (uint64_t)q->W * q->Ctot * es, (uint64_t)q->H * q->W * q->Ctot * es};
-        const uint32_t boxA[4] = {(uint32_t)bk, (uint32_t)(halo ? TW + 2 : TW), (uint32_t)(halo ? TH + 2 : TH), (uint32_t)TN};
-        if ((rc = make_tmap(&prm.tmA, tm_dtype, q->A, dimsA, strA, boxA)) != VF_OK) return rc;
-        const uint64_t Ktot = (uint64_t)q->ntaps * q->Cin * (exact ? 2 : 1);
-        const uint64_t dimsB[4] = {Ktot, (uint64_t)q->Ncols, 1, 1};
-        const uint64_t strB[3] = {Ktot * es, Ktot * es * q->Ncols, Ktot * es * q->Ncols};
-        const uint32_t boxB[4] = {(uint32_t)bk, (uint32_t)b_box_rows, 1, 1};
-        if ((rc = make_tmap(&prm.tmB, tm_dtype, q->B, dimsB, strB, boxB)) != VF_OK) return rc;
         const int ntiles_img = (q->N + TN - 1) / TN;
         grid = dim3(prm.tiles_x * prm.tiles_y * ntiles_img, (q->Ncols + block_n - 1) / block_n, 1);
     } else {
@@ -979,11 +840,11 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         VF_CHECK_ARG((q->lda * es) % 16 == 0 && (q->ldb * es) % 16 == 0, "vf_tc_gemm: row strides must be 16-byte multiples");
         VF_CHECK_ARG((q->a_sb1 * es) % 16 == 0 && (q->a_sb2 * es) % 16 == 0 && (q->b_sb1 * es) % 16 == 0 && (q->b_sb2 * es) % 16 == 0,
                      "vf_tc_gemm: batch strides must be 16-byte multiples");
+        VF_CHECK_ARG(q->causal_block == 0 || (q->causal_block % bk == 0 || bk % q->causal_block == 0), "vf_tc_gemm: causal block");
         prm.M = q->M;
         prm.batch2 = q->batch2;
         prm.num_k_blocks = (q->K + bk - 1) / bk;
         if (exact) {
-            prm.exact = 1;
             prm.exact_kpp = prm.num_k_blocks;
             prm.exact_clog = (int)q->exact_lo_a;
             prm.exact_lo_b = (int)q->exact_lo_b;
@@ -993,14 +854,12 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         prm.c_sb1 = q->c_sb1; prm.c_sb2 = q->c_sb2;
         // ntaps > 0 in gemm mode: batch1 index b reads A shifted by tap_coff[b] >= 0 elements along K (one operand, several shifted
         // views — the weight gradient of a 3x3 convolution over a transposed, zero-padded activation: vf_conv_wgrad_tc)
-        long long max_koff = 0;
         if (q->ntaps > 0) {
             VF_CHECK_ARG(q->ntaps == q->batch1 && q->ntaps <= 9, "vf_tc_gemm: gemm K offsets need ntaps == batch1 <= 9");
             prm.gemm_koff = 1;
             for (int t = 0; t < q->ntaps; ++t) {
                 VF_CHECK_ARG(q->tap_coff[t] >= 0 && q->tap_coff[t] % 8 == 0, "vf_tc_gemm: K offsets must be non-negative multiples of 8 (16-byte TMA box starts)");
                 prm.tap_coff[t] = q->tap_coff[t];
-                if (q->tap_coff[t] > max_koff) max_koff = q->tap_coff[t];
             }
         }
         // an operand with batch stride 0 is shared by every batch: its tensor map gets a size-1 batch dim and the
@@ -1009,6 +868,55 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         prm.a_bm2 = (q->batch2 > 1 && q->a_sb2 != 0) ? 1 : 0;
         prm.b_bm1 = (q->batch1 > 1 && q->b_sb1 != 0) ? 1 : 0;
         prm.b_bm2 = (q->batch2 > 1 && q->b_sb2 != 0) ? 1 : 0;
+        grid = dim3((q->M + BLOCK_M - 1) / BLOCK_M, (q->Ncols + block_n - 1) / block_n, q->batch1 * q->batch2);
+    }
+    // persistent launch: `grid` is the tile space (m tiles, n tiles, batches); one CTA per SM walks it, n fastest
+    prm.tiles_m = (int)grid.x;
+    prm.tiles_n = (int)grid.y;
+    const long long total = (long long)prm.tiles_m * grid.y * grid.z;
+    VF_CHECK_ARG(total > 0 && total < (1ll << 31), "vf_tc_gemm: tile count out of range");
+    prm.total_tiles = (int)total;
+    const int num_sms = persistent_ctas();
+    ctas = (int)(total < num_sms ? total : num_sms);
+    return VF_OK;
+}
+
+}  // namespace
+
+extern "C" int vf_tc_gemm_plan(const vf_tc_gemm_t* q, int* plan) {
+    VF_CHECK_ARG(q && plan, "vf_tc_gemm_plan: null argument");
+    TcParams prm;
+    int block_n, ctas, rc;
+    if ((rc = tc_setup(q, prm, block_n, ctas)) != VF_OK) return rc;
+    const int vals[8] = {block_n, prm.TW, prm.TH, prm.TN, prm.halo, q->ab_dtype == VF_F16X2 ? 1 : 0, prm.total_tiles, ctas};
+    for (int i = 0; i < 8; ++i) plan[i] = vals[i];
+    return VF_OK;
+}
+
+extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
+    VF_CHECK_ARG(q, "vf_tc_gemm: null argument");
+    TcParams prm;
+    int block_n, ctas, rc;
+    if ((rc = tc_setup(q, prm, block_n, ctas)) != VF_OK) return rc;
+    const bool exact = q->ab_dtype == VF_F16X2;
+    const bool tf32 = q->ab_dtype == VF_F32;
+    const int tm_dtype = tf32 ? VF_F32 : VF_BF16;        // tensor-map element type (fp16 and bf16 move identically)
+    const int es = tf32 ? 4 : 2;
+    const int bk = prm.bk_elems;
+    if (q->conv) {
+        const bool halo = prm.halo;
+        const uint64_t dimsA[4] = {(uint64_t)q->Ctot, (uint64_t)q->W, (uint64_t)q->H, (uint64_t)q->N};
+        const uint64_t strA[3] = {(uint64_t)q->Ctot * es, (uint64_t)q->W * q->Ctot * es, (uint64_t)q->H * q->W * q->Ctot * es};
+        const uint32_t boxA[4] = {(uint32_t)bk, (uint32_t)(halo ? prm.TW + 2 : prm.TW), (uint32_t)(halo ? prm.TH + 2 : prm.TH), (uint32_t)prm.TN};
+        if ((rc = make_tmap(&prm.tmA, tm_dtype, q->A, dimsA, strA, boxA)) != VF_OK) return rc;
+        const uint64_t Ktot = (uint64_t)q->ntaps * q->Cin * (exact ? 2 : 1);
+        const uint64_t dimsB[4] = {Ktot, (uint64_t)q->Ncols, 1, 1};
+        const uint64_t strB[3] = {Ktot * es, Ktot * es * q->Ncols, Ktot * es * q->Ncols};
+        const uint32_t boxB[4] = {(uint32_t)bk, (uint32_t)block_n, 1, 1};
+        if ((rc = make_tmap(&prm.tmB, tm_dtype, q->B, dimsB, strB, boxB)) != VF_OK) return rc;
+    } else {
+        long long max_koff = 0;
+        for (int t = 0; t < q->ntaps; ++t) max_koff = q->tap_coff[t] > max_koff ? q->tap_coff[t] : max_koff;
         const uint64_t fbA = (uint64_t)q->lda * es * (uint64_t)q->M, fbB = (uint64_t)q->ldb * es * (uint64_t)q->Ncols;
         const uint64_t dimsA[4] = {(uint64_t)((exact ? q->exact_lo_a + q->K : q->K) + max_koff), (uint64_t)q->M, prm.a_bm2 ? (uint64_t)q->batch2 : 1, prm.a_bm1 ? (uint64_t)q->batch1 : 1};
         const uint64_t strA[3] = {(uint64_t)q->lda * es, prm.a_bm2 ? (uint64_t)q->a_sb2 * es : fbA, prm.a_bm1 ? (uint64_t)q->a_sb1 * es : fbA};
@@ -1016,19 +924,9 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
         if ((rc = make_tmap(&prm.tmA, tm_dtype, q->A, dimsA, strA, boxA)) != VF_OK) return rc;
         const uint64_t dimsB[4] = {(uint64_t)(exact ? q->exact_lo_b + q->K : q->K), (uint64_t)q->Ncols, prm.b_bm2 ? (uint64_t)q->batch2 : 1, prm.b_bm1 ? (uint64_t)q->batch1 : 1};
         const uint64_t strB[3] = {(uint64_t)q->ldb * es, prm.b_bm2 ? (uint64_t)q->b_sb2 * es : fbB, prm.b_bm1 ? (uint64_t)q->b_sb1 * es : fbB};
-        const uint32_t boxB[4] = {(uint32_t)bk, (uint32_t)b_box_rows, 1, 1};
+        const uint32_t boxB[4] = {(uint32_t)bk, (uint32_t)block_n, 1, 1};
         if ((rc = make_tmap(&prm.tmB, tm_dtype, q->B, dimsB, strB, boxB)) != VF_OK) return rc;
-        VF_CHECK_ARG(q->causal_block == 0 || (q->causal_block % bk == 0 || bk % q->causal_block == 0), "vf_tc_gemm: causal block");
-        grid = dim3((q->M + BLOCK_M - 1) / BLOCK_M, (q->Ncols + block_n - 1) / block_n, q->batch1 * q->batch2);
     }
-    // persistent launch: `grid` so far is the tile space (m tiles, n tiles, batches); one CTA per SM walks it, n fastest
-    prm.tiles_m = (int)grid.x;
-    prm.tiles_n = (int)grid.y;
-    const long long total = (long long)prm.tiles_m * grid.y * grid.z;
-    VF_CHECK_ARG(total > 0 && total < (1ll << 31), "vf_tc_gemm: tile count out of range");
-    prm.total_tiles = (int)total;
-    const int num_sms = persistent_ctas();
-    const dim3 pgrid((unsigned)(total < num_sms ? total : num_sms), 1, 1);      // persistent CTAs
     {
         auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
         auto a8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };
@@ -1053,6 +951,7 @@ extern "C" int vf_tc_gemm(const vf_tc_gemm_t* q, vf_stream_t s) {
     }
     cudaStream_t st = vf_s(s);
     const WgKind kind = tf32 ? TF32 : (exact ? F16 : BF16);
+    const dim3 pgrid((unsigned)ctas, 1, 1);
     if (block_n == 128) return launch_kind<128, 4>(prm, kind, pgrid, st);
     return launch_kind<64, 6>(prm, kind, pgrid, st);
 }
