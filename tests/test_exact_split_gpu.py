@@ -142,7 +142,7 @@ def test_pad_transpose_split_bits(L, n, h, w, c, mode):
     fill = 1234.0
     out = torch.full((copies * c, 2, lrow), fill, dtype=torch.float16, device="cuda")
     lib = L.load(True)
-    L._check(lib.vf_pad_transpose_split(L._p(x.cuda()), n, h, w, c, pitch, copies, L.C.c_int64(margin), L.C.c_int64(lrow), L._p(out), L._stream()))
+    L._check(lib.vf_pad_transpose_split(x.cuda(), n, h, w, c, pitch, copies, margin, lrow, out, L._stream()))
     torch.cuda.synchronize()
     want = pad_transpose_ref(x, pitch, copies, margin, lrow, fill)
     assert torch.equal(bits(out), bits(want))

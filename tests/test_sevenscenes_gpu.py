@@ -86,11 +86,11 @@ def test_camera_knn_rejects_bad_arguments(L):
         with pytest.raises(L.LibraryError, match="k"):
             camera_knn(db, qs, k)
     with pytest.raises(L.LibraryError, match="mode"):
-        L._check(L.load().vf_camera_knn(L._p(db), L.C.c_int64(10), L.C.c_int64(0), L._p(qs), 2, 3, 1, L._p(torch.empty(2, dtype=torch.int32,
-                 device="cuda")), L._p(torch.empty(2, device="cuda")), L._stream()))
+        L._check(L.load().vf_camera_knn(db, 10, 0, qs, 2, 3, 1, torch.empty(2, dtype=torch.int32, device="cuda"), torch.empty(2, device="cuda"),
+                                        L._stream()))
     with pytest.raises(L.LibraryError, match="db_stride"):
-        L._check(L.load().vf_camera_knn(L._p(db), L.C.c_int64(10), L.C.c_int64(35), L._p(qs), 2, 0, 1, L._p(torch.empty(2, dtype=torch.int32,
-                 device="cuda")), L._p(torch.empty(2, device="cuda")), L._stream()))
+        L._check(L.load().vf_camera_knn(db, 10, 35, qs, 2, 0, 1, torch.empty(2, dtype=torch.int32, device="cuda"), torch.empty(2, device="cuda"),
+                                        L._stream()))
     with pytest.raises(ValueError):
         camera_knn(torch.zeros(3, 10, 7, device="cuda"), qs, 1)
 

@@ -36,8 +36,7 @@ def _gn_apply_bf16(x, mr, gamma, beta, swish):
     from viewformer_b200 import _lib as L
     n, h, w, c = x.shape
     y = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    L._check(L.load(True).vf_groupnorm_apply(L._p(x), L.F32, L._p(mr), L._p(gamma), L._p(beta), n, h, w, c, 32, L.C.c_float(1e-6), 1, int(swish),
-                                             0, L._p(y), L.BF16, L._stream()))
+    L._check(L.load(True).vf_groupnorm_apply(x, L.F32, mr, gamma, beta, n, h, w, c, 32, 1e-6, 1, int(swish), 0, y, L.BF16, L._stream()))
     return y
 
 

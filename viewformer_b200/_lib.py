@@ -1,8 +1,8 @@
 """ctypes binding of libvf_b200.so (include/vf_b200.h) + thin tensor-level helpers.
 
-torch is used here only as the device-memory / stream plumbing: every helper passes raw
-``data_ptr()`` values and the current CUDA stream handle across the C-ABI.  There is no CPU or
-PyTorch fallback: if the shared library is missing or the device is not sm_90, calls raise.
+torch is used here only as the device-memory / stream plumbing.  ``PROTOTYPES`` declares every entry point's parameter types, so a
+call site passes tensors, plain Python numbers and the current CUDA stream handle, and ctypes converts them as the header says.
+There is no CPU or PyTorch fallback: if the shared library is missing or the device is not sm_90, calls raise.
 """
 import ctypes as C
 import os
@@ -16,21 +16,29 @@ F32, BF16, F16X2 = 0, 1, 2     # F16X2: an fp32 value as two fp16 (hi | lo*2^11)
 ACT_NONE, ACT_GELU = 0, 1
 BIAS_NONE, BIAS_N, BIAS_M = 0, 1, 2
 
-EXPORTS = [
-    "vf_last_error", "vf_version", "vf_sizeof_simt_gemm", "vf_sizeof_tc_gemm", "vf_device_check", "vf_u8_to_unit_f32", "vf_f01_to_unit_f32", "vf_unit_f32_to_u8",
-    "vf_nchw_to_nhwc_f32", "vf_nhwc_to_nchw_f32", "vf_groupnorm_stats", "vf_groupnorm_apply", "vf_layernorm",
-    "vf_simt_gemm", "vf_tc_gemm", "vf_tc_gemm_plan", "vf_vq_lookup", "vf_gather_rows", "vf_vq_ema_stats", "vf_vq_ema_update", "vf_vq_commit_grad",
-    "vf_vq_prepare_codebook", "vf_migt_embed", "vf_softmax_rows", "vf_argmax_rows", "vf_pose_postprocess",
-    "vf_cameras_prepare", "vf_cameras_from_relative", "vf_camera_knn",
-    "vf_conv3x3_small_cin", "vf_conv3x3_small_cout", "vf_groupnorm_finalize", "vf_split_f16x2", "vf_attn_block_causal_decode", "vf_attn_block_multiend",
-    "vf_cross_entropy_rows", "vf_pose_loss_rows", "vf_row_mean",
-    "vf_vq_prepare_codebook_f16", "vf_vq_lookup_fused", "vf_resize_u8", "vf_resize_f32", "vf_image_pair_sums", "vf_ssim_u8", "vf_ssim_u8_k",
-    "vf_conv_wgrad", "vf_pad_transpose_split", "vf_pad_transpose_bf16", "vf_conv_weights_bf16", "vf_sum_splits", "vf_col_sums", "vf_groupnorm_bwd", "vf_softmax_bwd_rows", "vf_l1_grad", "vf_lincomb3", "vf_sumpool2x2", "vf_adam",
-    "vf_layernorm_bwd", "vf_gelu_fwd", "vf_gelu_bwd", "vf_migt_embed_bwd", "vf_cross_entropy_grad", "vf_pose_loss_grad", "vf_adamw_keras", "vf_sumsq", "vf_dropout",
-    "vf_attn_multiend_train", "vf_attn_multiend_bwd", "vf_to_bf16", "vf_dense_weights_bf16",
-]
+
+class LibraryError(RuntimeError):
+    pass
 
 
+class DevPtr(C.c_void_p):
+    """Argument type of a device pointer: a CUDA tensor passes its data_ptr(), an int its own value, None NULL; an explicit c_void_p is
+    taken as it is.  A CPU tensor raises here instead of faulting on the device.  The address goes through c_void_p's own conversion,
+    which keeps the full pointer width (a bare int returned from here would be passed as a C int) and costs less than a c_void_p object."""
+
+    @classmethod
+    def from_param(cls, obj):
+        if isinstance(obj, torch.Tensor):
+            if not obj.is_cuda:
+                raise LibraryError(f"a device pointer argument got a {obj.device} tensor")
+            obj = obj.data_ptr()
+        return C.c_void_p.from_param(obj)            # an int, None or a c_void_p; anything else is a TypeError
+
+
+_p = DevPtr.from_param      # explicit conversion for raw callers that still wrap their pointers themselves
+
+
+# Host-side mirrors of the parameter structs of include/vf_b200.h (tests/test_abi.py compares them field by field).
 class SimtGemm(C.Structure):
     _fields_ = [
         ("A", C.c_void_p), ("a_dtype", C.c_int), ("conv", C.c_int),
@@ -67,27 +75,72 @@ class TcGemm(C.Structure):
     ]
 
 
+class ConvWeightsBf16(C.Structure):            # a row of vf_conv_weights_bf16's device table
+    _fields_ = [("w_kn", C.c_void_p), ("fw_bf16", C.c_void_p), ("bw_bf16", C.c_void_p), ("cin", C.c_int64), ("cout", C.c_int64)]
+
+
+class DenseWeightsBf16(C.Structure):           # a row of vf_dense_weights_bf16's device table
+    _fields_ = [("w_kn", C.c_void_p), ("fw_bf16", C.c_void_p), ("bw_bf16", C.c_void_p), ("k", C.c_int64), ("n", C.c_int64)]
+
+
+def _prototypes():
+    """The parameter types of every function include/vf_b200.h declares, in order (tests/test_abi.py holds this table to the header).
+    p: a device pointer, the two weight tables included; s: vf_stream_t.  The parameter blocks and the plan array are host memory."""
+    i, i64, u64, f32, f64, p, s = C.c_int, C.c_int64, C.c_uint64, C.c_float, C.c_double, DevPtr, C.c_void_p
+    return {
+        "vf_last_error": [], "vf_version": [], "vf_sizeof_simt_gemm": [], "vf_sizeof_tc_gemm": [], "vf_device_check": [],
+        "vf_u8_to_unit_f32": [p, p, i64, i64, i64, s], "vf_f01_to_unit_f32": [p, p, i64, i64, i64, s], "vf_unit_f32_to_u8": [p, p, i64, s],
+        "vf_nchw_to_nhwc_f32": [p, p, i, i, i, i, s], "vf_nhwc_to_nchw_f32": [p, p, i, i, i, i, s], "vf_split_f16x2": [p, i64, i, p, s],
+        "vf_groupnorm_stats": [p, i, i, i, i, f32, p, p, s], "vf_groupnorm_finalize": [p, i, f64, f32, p, s],
+        "vf_groupnorm_apply": [p, i, p, p, p, i, i, i, i, i, f32, i, i, i, p, i, s], "vf_conv3x3_small_cin": [p, p, p, i, i, i, i, i, p, p, s],
+        "vf_conv3x3_small_cout": [p, i, p, p, i, i, i, i, i, p, s], "vf_layernorm": [p, p, p, i64, i, f32, p, i, s],
+        "vf_simt_gemm": [C.POINTER(SimtGemm), s], "vf_tc_gemm": [C.POINTER(TcGemm), s], "vf_tc_gemm_plan": [C.POINTER(TcGemm), C.POINTER(C.c_int)],
+        "vf_attn_block_causal_decode": [p, p, i, i, i, i, i, i, i, p, s], "vf_attn_block_multiend": [p, p, i, i, i, i, i, i, i, p, s],
+        "vf_attn_multiend_train": [p, p, i, i, i, i, i, i, i, f32, u64, p, p, p, s],
+        "vf_attn_multiend_bwd": [p, p, p, p, p, i, i, i, i, i, i, f32, u64, p, s],
+        "vf_conv_wgrad": [p, p, i, i, i, i, i, i, i, i, i, i, i, i, i, i64, i64, p, s], "vf_col_sums": [p, i64, i, p, s],
+        "vf_groupnorm_bwd": [p, p, p, p, p, i, i, i, i, i, p, p, p, p, p, p, s], "vf_softmax_bwd_rows": [p, p, i64, i, p, s],
+        "vf_l1_grad": [p, p, i64, f32, p, p, s], "vf_lincomb3": [f32, p, f32, p, f32, p, i64, p, s],
+        "vf_pad_transpose_split": [p, i, i, i, i, i, i, i64, i64, p, s], "vf_sum_splits": [p, i, i, i64, i, p, s],
+        "vf_pad_transpose_bf16": [p, i, i, i, i, i, i, i, i64, i64, p, p, p, i, i, p, s], "vf_conv_weights_bf16": [p, i, s],
+        "vf_sumpool2x2": [p, i, i, i, i, p, s], "vf_adam": [p, p, p, p, i64, f32, f32, f32, f32, i, f32, s],
+        "vf_layernorm_bwd": [p, p, p, p, i64, i, f32, p, p, p, s], "vf_gelu_fwd": [p, i64, p, s], "vf_gelu_bwd": [p, p, i64, p, s],
+        "vf_migt_embed_bwd": [p, p, i, i64, i, i, p, p, p, s], "vf_cross_entropy_grad": [p, p, p, i64, i, f32, p, s],
+        "vf_pose_loss_grad": [p, p, p, i64, i, f32, f32, f32, p, s], "vf_adamw_keras": [p, p, p, p, i64, f32, f32, f32, f32, f32, i, f32, f32, s],
+        "vf_sumsq": [p, i64, p, s], "vf_dropout": [p, i64, f32, u64, p, s], "vf_to_bf16": [p, i64, f32, u64, p, p, s],
+        "vf_dense_weights_bf16": [p, i, s], "vf_resize_u8": [p, i, i, i, i, i, i, i, p, s], "vf_resize_f32": [p, i, i, i, i, i, i, i, p, s],
+        "vf_image_pair_sums": [p, p, i, i64, p, s], "vf_ssim_u8": [p, p, i, i, i, i, p, s], "vf_ssim_u8_k": [p, p, i, i, i, i, f64, f64, p, s],
+        "vf_vq_lookup": [p, p, p, i64, i, i, p, p, p, s], "vf_vq_prepare_codebook_f16": [p, i, i, p, s],
+        "vf_vq_lookup_fused": [p, p, p, p, p, i64, i, i, f32, p, p, p, p, p, s], "vf_gather_rows": [p, p, i64, i, i64, p, s],
+        "vf_vq_ema_stats": [p, p, i64, i, i, p, p, s], "vf_vq_commit_grad": [p, p, p, i, i, f32, i, p, s],
+        "vf_vq_ema_update": [p, p, i, i, f32, f32, f32, p, p, p, p, p, s], "vf_vq_prepare_codebook": [p, i, i, p, p, s],
+        "vf_migt_embed": [p, i, p, p, p, i64, i, i, p, s], "vf_softmax_rows": [p, i64, i, i, i64, i, i, i, p, i, i64, s],
+        "vf_argmax_rows": [p, i64, i, i64, p, s], "vf_pose_postprocess": [p, i64, f32, p, s], "vf_cameras_prepare": [p, i, i, i, p, p, s],
+        "vf_cameras_from_relative": [p, p, i, i, p, s], "vf_camera_knn": [p, i64, i64, p, i, i, i, p, p, s],
+        "vf_cross_entropy_rows": [p, p, i64, i, f32, p, s], "vf_pose_loss_rows": [p, p, i64, i, f32, p, p, s], "vf_row_mean": [p, i64, i, i, p, s],
+    }
+
+
+PROTOTYPES = _prototypes()          # every entry point returns int, except vf_last_error (const char*)
+EXPORTS = tuple(PROTOTYPES)
+
 _lib = None
 _device_ok = []
 
 
-class LibraryError(RuntimeError):
-    pass
-
-
 def load(require_device=False):
-    """dlopen the in-tree library.  Fails loudly — there is no fallback path."""
+    """dlopen the in-tree library and declare every entry point's types.  Fails loudly — there is no fallback path."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise LibraryError(f"{LIB_PATH} not found — run `python -m viewformer_b200.build` (no CPU/PyTorch fallback exists)")
         lib = C.CDLL(LIB_PATH)
-        lib.vf_last_error.restype = C.c_char_p
-        for name in EXPORTS:
+        for name, argtypes in PROTOTYPES.items():
             if not hasattr(lib, name):
                 raise LibraryError(f"{LIB_PATH} does not export {name}")
-            if name != "vf_last_error":
-                getattr(lib, name).restype = C.c_int
+            fn = getattr(lib, name)
+            fn.argtypes = argtypes
+            fn.restype = C.c_char_p if name == "vf_last_error" else C.c_int
         if lib.vf_sizeof_simt_gemm() != C.sizeof(SimtGemm) or lib.vf_sizeof_tc_gemm() != C.sizeof(TcGemm):
             raise LibraryError("parameter struct layout mismatch between _lib.py and include/vf_b200.h")
         _lib = lib
@@ -122,7 +175,11 @@ def _check(rc):
 
 
 def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _seed64(seed):                  # a dropout seed as the uint64 the kernels hash: negative and wide seeds wrap here, explicitly
+    return int(seed) & ((1 << 64) - 1)
 
 
 def on_model_device(fn):
@@ -139,10 +196,6 @@ def on_model_device(fn):
         with torch.cuda.device(dev):
             return fn(self, *a, **k)
     return wrap
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 def _dt(t):
@@ -173,12 +226,12 @@ def u8_to_unit(x_u8, first_views=None):
     _dev(x_u8, torch.uint8)
     if first_views is None:
         out = torch.empty(x_u8.shape, dtype=torch.float32, device=x_u8.device)
-        _check(lib.vf_u8_to_unit_f32(_p(x_u8), _p(out), C.c_int64(1), C.c_int64(x_u8.numel()), C.c_int64(0), _stream()))
+        _check(lib.vf_u8_to_unit_f32(x_u8, out, 1, x_u8.numel(), 0, _stream()))
         return out
     b, t = x_u8.shape[:2]
     per_view = x_u8[0, 0].numel()
     out = torch.empty((b * first_views,) + tuple(x_u8.shape[2:]), dtype=torch.float32, device=x_u8.device)
-    _check(lib.vf_u8_to_unit_f32(_p(x_u8), _p(out), C.c_int64(b), C.c_int64(first_views * per_view), C.c_int64(t * per_view), _stream()))
+    _check(lib.vf_u8_to_unit_f32(x_u8, out, b, first_views * per_view, t * per_view, _stream()))
     return out
 
 
@@ -186,7 +239,7 @@ def unit_to_u8(x):
     lib = load(True)
     _dev(x, torch.float32)
     out = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
-    _check(lib.vf_unit_f32_to_u8(_p(x), _p(out), C.c_int64(x.numel()), _stream()))
+    _check(lib.vf_unit_f32_to_u8(x, out, x.numel(), _stream()))
     return out
 
 
@@ -195,7 +248,7 @@ def nchw_to_nhwc(x):
     _dev(x, torch.float32)
     n, c, h, w = x.shape
     out = torch.empty((n, h, w, c), dtype=torch.float32, device=x.device)
-    _check(lib.vf_nchw_to_nhwc_f32(_p(x), _p(out), n, c, h, w, _stream()))
+    _check(lib.vf_nchw_to_nhwc_f32(x, out, n, c, h, w, _stream()))
     return out
 
 
@@ -204,7 +257,7 @@ def nhwc_to_nchw(x):
     _dev(x, torch.float32)
     n, h, w, c = x.shape
     out = torch.empty((n, c, h, w), dtype=torch.float32, device=x.device)
-    _check(lib.vf_nhwc_to_nchw_f32(_p(x), _p(out), n, c, h, w, _stream()))
+    _check(lib.vf_nhwc_to_nchw_f32(x, out, n, c, h, w, _stream()))
     return out
 
 
@@ -222,7 +275,7 @@ def resize_u8(x_u8, size, method=None):
         method = "nearest" if size > h else "bilinear"
     assert method in ("nearest", "bilinear")
     out = torch.empty((n, size, size, c), dtype=torch.uint8, device=x_u8.device)
-    _check(lib.vf_resize_u8(_p(x_u8), n, h, w, c, size, size, int(method == "bilinear"), _p(out), _stream()))
+    _check(lib.vf_resize_u8(x_u8, n, h, w, c, size, size, int(method == "bilinear"), out, _stream()))
     return out
 
 
@@ -234,7 +287,7 @@ def image_pair_sums(a_u8, b_u8):
     assert a_u8.shape == b_u8.shape
     n = a_u8.shape[0]
     out = torch.empty((n, 2), dtype=torch.int64, device=a_u8.device)
-    _check(lib.vf_image_pair_sums(_p(a_u8), _p(b_u8), n, C.c_int64(a_u8[0].numel() if n else 1), _p(out), _stream()))
+    _check(lib.vf_image_pair_sums(a_u8, b_u8, n, a_u8[0].numel() if n else 1, out, _stream()))
     return out
 
 
@@ -249,10 +302,9 @@ def ssim_u8(a_u8, b_u8, k1=None, k2=None):
     n, h, w, c = a_u8.shape
     out = torch.empty((n,), dtype=torch.float64, device=a_u8.device)
     if k1 is None and k2 is None:
-        _check(lib.vf_ssim_u8(_p(a_u8), _p(b_u8), n, h, w, c, _p(out), _stream()))
+        _check(lib.vf_ssim_u8(a_u8, b_u8, n, h, w, c, out, _stream()))
     else:
-        _check(lib.vf_ssim_u8_k(_p(a_u8), _p(b_u8), n, h, w, c, C.c_double(0.01 if k1 is None else float(k1)),
-                                C.c_double(0.03 if k2 is None else float(k2)), _p(out), _stream()))
+        _check(lib.vf_ssim_u8_k(a_u8, b_u8, n, h, w, c, 0.01 if k1 is None else float(k1), 0.03 if k2 is None else float(k2), out, _stream()))
     return out
 
 
@@ -270,8 +322,8 @@ def groupnorm(x, gamma, beta, *, swish, out_dtype, eps=1e-6, groups=32, upsample
     if out_dtype == torch.float16:          # split-fp16 pair [hi | lo] (exact tensor-core operand): twice the channels
         oshape = oshape[:3] + (2 * oshape[3],)
     y = torch.empty(oshape, dtype=out_dtype, device=x.device)
-    _check(lib.vf_groupnorm_apply(_p(x), _dt(x), _p(stats), _p(gamma), _p(beta), n, h, w, c, groups, C.c_float(eps),
-                                  int(normalize), int(swish), 1 if upsample else (2 if s2d else 0), _p(y), _dt(y), _stream()))
+    _check(lib.vf_groupnorm_apply(x, _dt(x), stats, gamma, beta, n, h, w, c, groups, eps,
+                                  int(normalize), int(swish), 1 if upsample else (2 if s2d else 0), y, _dt(y), _stream()))
     return y
 
 
@@ -281,15 +333,25 @@ def layernorm(x, gamma, beta, out_dtype, eps=1e-5):
     d = x.shape[-1]
     rows = x.numel() // d
     y = torch.empty(x.shape, dtype=out_dtype, device=x.device)
-    _check(lib.vf_layernorm(_p(x), _p(gamma), _p(beta), C.c_int64(rows), d, C.c_float(eps), _p(y), _dt(y), _stream()))
+    _check(lib.vf_layernorm(x, gamma, beta, rows, d, eps, y, _dt(y), _stream()))
     return y
 
 
 # ----------------------------------------------------------------------------------------------- GEMM / conv
-def _outs(out):
-    f32 = out if (out is not None and out.dtype == torch.float32) else None
-    b16 = out if (out is not None and out.dtype == torch.bfloat16) else None
-    return f32, b16
+def _epilogue(p, out, ldc, *, c_bs=(0, 0), out2=None, alpha=1.0, bias=None, bias_mode=BIAS_N, act=ACT_NONE, residual=None, c_off=0):
+    """The epilogue fields vf_simt_gemm_t and vf_tc_gemm_t share: C = act(alpha*acc + bias) + residual, written to ``out`` and ``out2``
+    (one f32, one bf16) from element ``c_off`` on, with row stride ``ldc`` and batch strides ``c_bs``; the residual is f32 and indexed as C."""
+    p.alpha, p.act, p.ldc = alpha, act, ldc
+    p.c_sb1, p.c_sb2 = c_bs
+    p.bias, p.bias_mode = (bias.data_ptr(), bias_mode) if bias is not None else (None, BIAS_NONE)
+    p.residual = residual.data_ptr() + c_off * 4 if residual is not None else None
+    for o in (o for o in (out, out2) if o is not None):
+        if o.dtype == torch.float32:
+            p.C_f32 = o.data_ptr() + c_off * 4
+        elif o.dtype == torch.bfloat16:
+            p.C_bf16 = o.data_ptr() + c_off * 2
+        else:
+            raise TypeError(f"GEMM output must be float32 or bfloat16, got {o.dtype}")
 
 
 def simt_conv(x, w_kn, bias, *, kh, stride=1, pad=(1, 1), upsample=False, residual=None, out_dtype=torch.float32, out=None):
@@ -305,22 +367,11 @@ def simt_conv(x, w_kn, bias, *, kh, stride=1, pad=(1, 1), upsample=False, residu
         oh, ow = vh // 2, vw // 2
     if out is None:
         out = torch.empty((n, oh, ow, cout), dtype=out_dtype, device=x.device)
-    p = SimtGemm()
-    p.A, p.a_dtype, p.conv = x.data_ptr(), _dt(x), 1
-    p.N, p.H, p.W, p.Cin = n, h, w, cin
-    p.OH, p.OW, p.KH, p.KW, p.stride = oh, ow, kh, kh, stride
-    p.pad_t, p.pad_l, p.upsample2x = pad[0], pad[1], int(upsample)
-    p.B, p.b_dtype, p.b_sk, p.b_sn = w_kn.data_ptr(), _dt(w_kn), cout, 1
-    p.M, p.Ncols, p.K, p.batch1, p.batch2 = n * oh * ow, cout, kh * kh * cin, 1, 1
-    p.alpha = 1.0
-    p.bias, p.bias_mode = (bias.data_ptr(), BIAS_N) if bias is not None else (None, BIAS_NONE)
-    p.act = ACT_NONE
-    p.residual = residual.data_ptr() if residual is not None else None
-    f32, b16 = _outs(out)
-    p.C_f32 = f32.data_ptr() if f32 is not None else None
-    p.C_bf16 = b16.data_ptr() if b16 is not None else None
-    p.ldc = cout
-    _check(lib.vf_simt_gemm(C.byref(p), _stream()))
+    p = SimtGemm(A=x.data_ptr(), a_dtype=_dt(x), conv=1, N=n, H=h, W=w, Cin=cin, OH=oh, OW=ow, KH=kh, KW=kh, stride=stride,
+                 pad_t=pad[0], pad_l=pad[1], upsample2x=int(upsample), B=w_kn.data_ptr(), b_dtype=_dt(w_kn), b_sk=cout, b_sn=1,
+                 M=n * oh * ow, Ncols=cout, K=kh * kh * cin, batch1=1, batch2=1)
+    _epilogue(p, out, cout, bias=bias, residual=residual)
+    _check(lib.vf_simt_gemm(p, _stream()))
     return out
 
 
@@ -329,24 +380,14 @@ def simt_gemm(A, B, out, *, M, N, K, a_strides, b_strides, ldc, batch=(1, 1), a_
     """Dense strided fp32 GEMM: C[m,n] = act(alpha*sum_k A(m,k) B(k,n) + bias) + residual.
     a_strides = (stride_m, stride_k), b_strides = (stride_k, stride_n) in elements; *_off element offsets."""
     lib = load(True)
-    p = SimtGemm()
-    p.A, p.a_dtype, p.conv = A.data_ptr() + a_off * A.element_size(), _dt(A), 0
+    p = SimtGemm(A=A.data_ptr() + a_off * A.element_size(), a_dtype=_dt(A), conv=0, B=B.data_ptr() + b_off * B.element_size(), b_dtype=_dt(B),
+                 M=M, Ncols=N, K=K, batch1=batch[0], batch2=batch[1])
     p.a_sm, p.a_sk = a_strides
-    p.B, p.b_dtype = B.data_ptr() + b_off * B.element_size(), _dt(B)
     p.b_sk, p.b_sn = b_strides
-    p.M, p.Ncols, p.K, p.batch1, p.batch2 = M, N, K, batch[0], batch[1]
     p.a_sb1, p.a_sb2 = a_bs
     p.b_sb1, p.b_sb2 = b_bs
-    p.c_sb1, p.c_sb2 = c_bs
-    p.alpha = alpha
-    p.bias, p.bias_mode = (bias.data_ptr(), bias_mode) if bias is not None else (None, BIAS_NONE)
-    p.act = act
-    p.residual = (residual.data_ptr() + c_off * 4) if residual is not None else None
-    f32, b16 = _outs(out)
-    p.C_f32 = (f32.data_ptr() + c_off * 4) if f32 is not None else None
-    p.C_bf16 = (b16.data_ptr() + c_off * 2) if b16 is not None else None
-    p.ldc = ldc
-    _check(lib.vf_simt_gemm(C.byref(p), _stream()))
+    _epilogue(p, out, ldc, c_bs=c_bs, alpha=alpha, bias=bias, bias_mode=bias_mode, act=act, residual=residual, c_off=c_off)
+    _check(lib.vf_simt_gemm(p, _stream()))
     return out
 
 
@@ -356,10 +397,17 @@ _PLAN_KEYS = ("block_n", "TW", "TH", "TN", "halo", "exact", "tiles", "ctas")
 def _plan(p):
     """vf_tc_gemm_plan: the tiling vf_tc_gemm would launch for parameter block p, as a dict of _PLAN_KEYS (nothing is launched)."""
     plan = (C.c_int * len(_PLAN_KEYS))()
-    rc = load(True).vf_tc_gemm_plan(C.byref(p), plan)
+    rc = load(True).vf_tc_gemm_plan(p, plan)
     if rc != 0:
         raise LibraryError(f"libvf_b200 error {rc}: {_lib.vf_last_error().decode()}")
     return dict(zip(_PLAN_KEYS, plan))
+
+
+def _fuse_gn_sums(p, out, images, groups, rows_per_img=0):
+    """Point p's epilogue (vf_tc_gemm_t.gn_sums) at fresh fp64 GroupNorm sums [images, groups, 2] of ``out``, kept as ``out._gn_sums``."""
+    sums = torch.empty((images, groups, 2), dtype=torch.float64, device=out.device)
+    p.gn_sums, p.gn_groups, p.gn_rows_per_img = sums.data_ptr(), groups, rows_per_img
+    out._gn_sums = (sums, groups)
 
 
 def tc_gemm(A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0), b_bs=(0, 0), c_bs=(0, 0), alpha=1.0,
@@ -371,44 +419,24 @@ def tc_gemm(A, B, out, *, M, N, K, lda, ldb, ldc, batch=(1, 1), a_bs=(0, 0), b_b
     ``plan=True`` launches nothing and returns the tiling this call would take (see _plan)."""
     lib = load(True)
     assert A.dtype == B.dtype
-    p = TcGemm()
+    p = TcGemm(conv=0, ab_dtype=_dt(A), A=A.data_ptr() + a_off * A.element_size(), B=B.data_ptr() + b_off * B.element_size(),
+               M=M, Ncols=N, K=K, batch1=batch[0], batch2=batch[1], lda=lda, ldb=ldb)
     if A.dtype == torch.float16:
         p.exact_lo_a, p.exact_lo_b = (K if lo_a is None else lo_a), (K if lo_b is None else lo_b)
-    p.conv, p.ab_dtype = 0, _dt(A)
-    p.A = A.data_ptr() + a_off * A.element_size()
-    p.B = B.data_ptr() + b_off * B.element_size()
-    p.M, p.Ncols, p.K, p.batch1, p.batch2 = M, N, K, batch[0], batch[1]
-    p.lda, p.ldb = lda, ldb
     p.a_sb1, p.a_sb2 = a_bs
     p.b_sb1, p.b_sb2 = b_bs
-    p.c_sb1, p.c_sb2 = c_bs
     p.causal_block, p.causal_skip_n = causal_block, int(causal_skip_n)
     if k_offsets is not None:            # batch1 index b reads A shifted by k_offsets[b] elements along K (vf_tc_gemm_t.ntaps in gemm mode)
         assert len(k_offsets) == batch[0] <= 9
         p.ntaps = len(k_offsets)
         for i, o in enumerate(k_offsets):
             p.tap_coff[i] = int(o)
-    p.alpha = alpha
-    p.bias, p.bias_mode = (bias.data_ptr(), bias_mode) if bias is not None else (None, BIAS_NONE)
-    p.act = act
-    p.residual = (residual.data_ptr() + c_off * 4) if residual is not None else None
-    for o in (out, out2):
-        if o is None:
-            continue
-        if o.dtype == torch.float32:
-            p.C_f32 = o.data_ptr() + c_off * 4
-        else:
-            p.C_bf16 = o.data_ptr() + c_off * 2
-    p.ldc = ldc
+    _epilogue(p, out, ldc, c_bs=c_bs, out2=out2, alpha=alpha, bias=bias, bias_mode=bias_mode, act=act, residual=residual, c_off=c_off)
     if plan:
         return _plan(p)
-    sums = None
     if gn_rows_per_img and batch == (1, 1) and gn_fusable(N, gn_groups, M, gn_rows_per_img, ldc):
-        sums = torch.empty((M // gn_rows_per_img, gn_groups, 2), dtype=torch.float64, device=out.device)
-        p.gn_sums, p.gn_groups, p.gn_rows_per_img = sums.data_ptr(), gn_groups, gn_rows_per_img
-    _check(lib.vf_tc_gemm(C.byref(p), _stream()))
-    if sums is not None:
-        out._gn_sums = (sums, gn_groups)
+        _fuse_gn_sums(p, out, M // gn_rows_per_img, gn_groups, gn_rows_per_img)
+    _check(lib.vf_tc_gemm(p, _stream()))
     return out
 
 
@@ -441,7 +469,7 @@ def conv3x3_small_cin(x, w_kn, bias, gn_groups=0):
     sums = None
     if gn_groups == 32 and cout == 128:
         sums = torch.empty((n, 32, 2), dtype=torch.float64, device=x.device)
-    _check(lib.vf_conv3x3_small_cin(_p(x), _p(w_kn), _p(bias), n, h, w, cin, cout, _p(y), _p(sums), _stream()))
+    _check(lib.vf_conv3x3_small_cin(x, w_kn, bias, n, h, w, cin, cout, y, sums, _stream()))
     if sums is not None:
         y._gn_sums = (sums, 32)
     return y
@@ -454,7 +482,7 @@ def conv3x3_small_cout(x, w_kn, bias):
     n, h, w, cin = x.shape
     cout = w_kn.shape[1]
     y = torch.empty((n, h, w, cout), dtype=torch.float32, device=x.device)
-    _check(lib.vf_conv3x3_small_cout(_p(x), _dt(x), _p(w_kn), _p(bias), n, h, w, cin, cout, _p(y), _stream()))
+    _check(lib.vf_conv3x3_small_cout(x, _dt(x), w_kn, bias, n, h, w, cin, cout, y, _stream()))
     return y
 
 
@@ -472,13 +500,12 @@ def gn_mean_rstd(x, groups=32, eps=1e-6):
     stats = torch.empty((n, groups, 2), dtype=torch.float32, device=x.device)
     fused = getattr(x, "_gn_sums", None)
     if fused is not None and fused[1] == groups:
-        _check(lib.vf_groupnorm_finalize(_p(fused[0]), n * groups, C.c_double(float(h * w * (c // groups))), C.c_float(eps),
-                                         _p(stats), _stream()))
+        _check(lib.vf_groupnorm_finalize(fused[0], n * groups, float(h * w * (c // groups)), eps, stats, _stream()))
     else:
         if x.dtype != torch.float32:
             raise LibraryError("gn_mean_rstd: a bf16 input needs fused statistics from its producer")
         sums = torch.empty((n, groups, 2), dtype=torch.float64, device=x.device)
-        _check(lib.vf_groupnorm_stats(_p(x), n, h * w, c, groups, C.c_float(eps), _p(sums), _p(stats), _stream()))
+        _check(lib.vf_groupnorm_stats(x, n, h * w, c, groups, eps, sums, stats, _stream()))
     return stats
 
 
@@ -497,41 +524,23 @@ def tc_conv(x, w_nk, bias, *, taps=TAPS_3x3, coffs=None, cin=None, out_hw=None, 
     oh, ow = (h, w) if out_hw is None else out_hw
     if out is None:
         out = torch.empty((n, oh, ow, cout), dtype=out_dtype, device=x.device)
-    p = TcGemm()
-    p.conv, p.ab_dtype = 1, _dt(x)
     assert w_nk.dtype == x.dtype and w_nk.shape[1] == len(taps) * cin * split
-    p.A, p.B = x.data_ptr(), w_nk.data_ptr()
-    p.Ncols = cout
-    p.N, p.H, p.W, p.Ctot, p.Cin, p.OH, p.OW, p.ntaps = n, h, w, ctot, cin, oh, ow, len(taps)
+    p = TcGemm(conv=1, ab_dtype=_dt(x), A=x.data_ptr(), B=w_nk.data_ptr(), Ncols=cout, N=n, H=h, W=w, Ctot=ctot, Cin=cin, OH=oh, OW=ow,
+               ntaps=len(taps))
     for i, (dy, dx) in enumerate(taps):
         p.tap_dy[i], p.tap_dx[i] = dy, dx
         p.tap_coff[i] = 0 if coffs is None else coffs[i]
-    p.alpha = 1.0
-    p.bias, p.bias_mode = (bias.data_ptr(), BIAS_N) if bias is not None else (None, BIAS_NONE)
-    p.act = ACT_NONE
-    p.residual = residual.data_ptr() if residual is not None else None
-    for o in (out, out2):
-        if o is None:
-            continue
-        if o.dtype == torch.float32:
-            p.C_f32 = o.data_ptr()
-        else:
-            p.C_bf16 = o.data_ptr()
-    p.ldc = cout
+    _epilogue(p, out, cout, out2=out2, bias=bias, residual=residual)
     if plan:
         return _plan(p)
-    sums = None
     if gn_groups and gn_fusable(cout, gn_groups, n * oh * ow, oh * ow, cout):
-        sums = torch.empty((n, gn_groups, 2), dtype=torch.float64, device=out.device)
-        p.gn_sums, p.gn_groups = sums.data_ptr(), gn_groups
+        _fuse_gn_sums(p, out, n, gn_groups)
     if norm is not None:
         mr, gamma, beta, ngroups, swish = norm
         _dev(mr, torch.float32); _dev(gamma, torch.float32); _dev(beta, torch.float32)
         p.norm_mean_rstd, p.norm_gamma, p.norm_beta = mr.data_ptr(), gamma.data_ptr(), beta.data_ptr()
         p.norm_groups, p.norm_swish = ngroups, int(swish)      # 0 none, 1 = ex2/rcp fp32 (as vf_groupnorm_apply), 2 = packed bf16 tanh
-    _check(lib.vf_tc_gemm(C.byref(p), _stream()))
-    if sums is not None:
-        out._gn_sums = (sums, gn_groups)
+    _check(lib.vf_tc_gemm(p, _stream()))
     return out
 
 
@@ -542,7 +551,7 @@ def vq_prepare_codebook(emb_dk):
     d, k = emb_dk.shape
     et = torch.empty((k, d), dtype=torch.float32, device=emb_dk.device)
     esq = torch.empty((k,), dtype=torch.float32, device=emb_dk.device)
-    _check(lib.vf_vq_prepare_codebook(_p(emb_dk), d, k, _p(et), _p(esq), _stream()))
+    _check(lib.vf_vq_prepare_codebook(emb_dk, d, k, et, esq, _stream()))
     return et, esq
 
 
@@ -555,7 +564,7 @@ def vq_lookup(z_rows, et, esq, want_quant=True, want_diff=True):
     idx = torch.empty((m,), dtype=torch.int64, device=z_rows.device)
     quant = torch.empty((m, d), dtype=torch.float32, device=z_rows.device) if want_quant else None
     dsum = torch.zeros((1,), dtype=torch.float64, device=z_rows.device) if want_diff else None
-    _check(lib.vf_vq_lookup(_p(z_rows), _p(et), _p(esq), C.c_int64(m), d, k, _p(idx), _p(quant), _p(dsum), _stream()))
+    _check(lib.vf_vq_lookup(z_rows, et, esq, m, d, k, idx, quant, dsum, _stream()))
     return idx, quant, dsum
 
 
@@ -565,7 +574,7 @@ def split_f16x2(x_rows):
     _dev(x_rows, torch.float32)
     rows, c = x_rows.shape
     out = torch.empty((rows, 2 * c), dtype=torch.float16, device=x_rows.device)
-    _check(lib.vf_split_f16x2(_p(x_rows), C.c_int64(rows), c, _p(out), _stream()))
+    _check(lib.vf_split_f16x2(x_rows, rows, c, out, _stream()))
     return out
 
 
@@ -575,7 +584,7 @@ def vq_prepare_codebook_f16(et):
     _dev(et, torch.float32)
     k, d = et.shape
     eh = torch.empty((k, d), dtype=torch.float16, device=et.device)
-    _check(lib.vf_vq_prepare_codebook_f16(_p(et), k, d, _p(eh), _stream()))
+    _check(lib.vf_vq_prepare_codebook_f16(et, k, d, eh, _stream()))
     return eh
 
 
@@ -597,8 +606,7 @@ def vq_lookup_fused(z_rows, et, esq, eh, emb_dk=None, want_quant=True, want_diff
     counter = torch.empty((2,), dtype=torch.int32, device=z_rows.device)
     quant = torch.empty((m, d), dtype=torch.float32, device=z_rows.device) if want_quant else None
     dsum = torch.zeros((1,), dtype=torch.float64, device=z_rows.device) if want_diff else None
-    _check(lib.vf_vq_lookup_fused(_p(z_rows), _p(eh), _p(et), _p(emb_dk), _p(esq), C.c_int64(m), d, k, C.c_float(tol_factor), _p(idx), _p(work),
-                                  _p(counter), _p(quant), _p(dsum), _stream()))
+    _check(lib.vf_vq_lookup_fused(z_rows, eh, et, emb_dk, esq, m, d, k, tol_factor, idx, work, counter, quant, dsum, _stream()))
     return (idx, quant, dsum, counter) if return_counts else (idx, quant, dsum)
 
 
@@ -609,7 +617,7 @@ def gather_rows(table, idx):
     m = idx.numel()
     d = table.shape[1]
     out = torch.empty((m, d), dtype=torch.float32, device=table.device)
-    _check(lib.vf_gather_rows(_p(table), _p(idx), C.c_int64(m), d, C.c_int64(table.shape[0]), _p(out), _stream()))
+    _check(lib.vf_gather_rows(table, idx, m, d, table.shape[0], out, _stream()))
     return out
 
 
@@ -618,7 +626,7 @@ def vq_ema_stats(z_rows, idx, k):
     m, d = z_rows.shape
     counts = torch.zeros((k,), dtype=torch.float32, device=z_rows.device)
     esum = torch.zeros((d, k), dtype=torch.float32, device=z_rows.device)
-    _check(lib.vf_vq_ema_stats(_p(z_rows), _p(idx), C.c_int64(m), d, k, _p(counts), _p(esum), _stream()))
+    _check(lib.vf_vq_ema_stats(z_rows, idx, m, d, k, counts, esum, _stream()))
     return counts, esum
 
 
@@ -626,15 +634,14 @@ def vq_commit_grad(emb_dk, counts, esum, coef, grad_dk, accumulate=False):
     """grad_dk = coef (count_k e_k - esum) (``accumulate``: grad_dk += that)."""
     lib = load(True)
     d, k = emb_dk.shape
-    _check(lib.vf_vq_commit_grad(_p(emb_dk), _p(counts), _p(esum), d, k, C.c_float(coef), int(bool(accumulate)), _p(grad_dk), _stream()))
+    _check(lib.vf_vq_commit_grad(emb_dk, counts, esum, d, k, coef, int(bool(accumulate)), grad_dk, _stream()))
     return grad_dk
 
 
 def vq_ema_update(counts, esum, alpha, corr, eps, cs_hidden, dw_hidden, emb_dk, et, esq):
     lib = load(True)
     d, k = emb_dk.shape
-    _check(lib.vf_vq_ema_update(_p(counts), _p(esum), d, k, C.c_float(alpha), C.c_float(corr), C.c_float(eps),
-                                _p(cs_hidden), _p(dw_hidden), _p(emb_dk), _p(et), _p(esq), _stream()))
+    _check(lib.vf_vq_ema_update(counts, esum, d, k, alpha, corr, eps, cs_hidden, dw_hidden, emb_dk, et, esq, _stream()))
 
 
 # ----------------------------------------------------------------------------------------------- transformer glue
@@ -642,8 +649,7 @@ def migt_embed(ids_i32, fixed_token, wte, wpe, pose_rows, BT, L):
     lib = load(True)
     d = wte.shape[1]
     out = torch.empty((BT * L, d), dtype=torch.float32, device=wte.device)
-    _check(lib.vf_migt_embed(_p(ids_i32), int(fixed_token), _p(wte), _p(wpe), _p(pose_rows), C.c_int64(BT), L, d, _p(out),
-                             _stream()))
+    _check(lib.vf_migt_embed(ids_i32, int(fixed_token), wte, wpe, pose_rows, BT, L, d, out, _stream()))
     return out
 
 
@@ -656,7 +662,7 @@ def attn_block_causal(qk, vt, B, S, H, d, block, first_query=0, out=None, skip_v
     _dev(vt, torch.bfloat16)
     if out is None:
         out = torch.empty((B * S, d), dtype=torch.bfloat16, device=qk.device)
-    _check(lib.vf_attn_block_causal_decode(_p(qk), _p(vt), B, S, H, d, block, int(first_query), int(skip_view), _p(out), _stream()))
+    _check(lib.vf_attn_block_causal_decode(qk, vt, B, S, H, d, block, int(first_query), int(skip_view), out, _stream()))
     return out
 
 
@@ -668,7 +674,7 @@ def attn_block_multiend(qk, vt, B, S, n_streams, stream, H, d, block, out=None):
     _dev(vt, torch.bfloat16)
     if out is None:
         out = torch.empty((B * S, d), dtype=torch.bfloat16, device=qk.device)
-    _check(lib.vf_attn_block_multiend(_p(qk), _p(vt), B, S, n_streams, stream, H, d, block, _p(out), _stream()))
+    _check(lib.vf_attn_block_multiend(qk, vt, B, S, n_streams, stream, H, d, block, out, _stream()))
     return out
 
 
@@ -684,8 +690,7 @@ def attn_multiend_train(qk, vt, B, S, n_streams, stream, H, d, block, *, rate=0.
     for t in (lse, out_f32):
         if t is not None:
             _dev(t, torch.float32)
-    _check(lib.vf_attn_multiend_train(_p(qk), _p(vt), B, S, n_streams, stream, H, d, block, C.c_float(rate),
-                                      C.c_uint64(int(seed) & ((1 << 64) - 1)), _p(lse), _p(out_f32), _p(out), _stream()))
+    _check(lib.vf_attn_multiend_train(qk, vt, B, S, n_streams, stream, H, d, block, rate, _seed64(seed), lse, out_f32, out, _stream()))
     return out
 
 
@@ -697,8 +702,7 @@ def attn_multiend_bwd(qk, vt, dout, out_f32, lse, B, S, n_streams, H, d, block, 
         _dev(t, dt)
     if dvqk is None:
         dvqk = torch.zeros((n_streams, B * S, 3 * d), dtype=torch.float32, device=qk.device)
-    _check(lib.vf_attn_multiend_bwd(_p(qk), _p(vt), _p(dout), _p(out_f32), _p(lse), B, S, n_streams, H, d, block, C.c_float(rate),
-                                    C.c_uint64(int(seed) & ((1 << 64) - 1)), _p(dvqk), _stream()))
+    _check(lib.vf_attn_multiend_bwd(qk, vt, dout, out_f32, lse, B, S, n_streams, H, d, block, rate, _seed64(seed), dvqk, _stream()))
     return dvqk
 
 
@@ -708,8 +712,14 @@ def to_bf16(x, rate=0.0, seed=0, out_f32=False):
     _dev(x, torch.float32)
     y16 = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     y = torch.empty_like(x) if out_f32 else None
-    _check(lib.vf_to_bf16(_p(x), C.c_int64(x.numel()), C.c_float(rate), C.c_uint64(int(seed) & ((1 << 64) - 1)), _p(y), _p(y16), _stream()))
+    _check(lib.vf_to_bf16(x, x.numel(), rate, _seed64(seed), y, y16, _stream()))
     return (y, y16) if out_f32 else y16
+
+
+def _device_table(struct, rows, device):
+    """Host struct rows -> the bytes of the device array a one-launch kernel walks, as int64 [n, sizeof(struct) / 8]."""
+    words = memoryview(bytearray((struct * len(rows))(*rows))).cast("q").tolist()
+    return torch.tensor(words, dtype=torch.int64).reshape(-1, C.sizeof(struct) // 8).to(device)
 
 
 def dense_weights_bf16_table(entries, device):
@@ -721,20 +731,19 @@ def dense_weights_bf16_table(entries, device):
         k, n = w_kn.shape
         assert fw is None or (fw.dtype == torch.bfloat16 and fw.is_contiguous() and tuple(fw.shape) == (n, k))
         assert bw is None or (bw.dtype == torch.bfloat16 and bw.is_contiguous() and tuple(bw.shape) == (k, n))
-        rows.append([w_kn.data_ptr(), fw.data_ptr() if fw is not None else 0, bw.data_ptr() if bw is not None else 0, k, n])
-    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 5).to(device)
+        rows.append(DenseWeightsBf16(w_kn.data_ptr(), fw.data_ptr() if fw is not None else None, bw.data_ptr() if bw is not None else None, k, n))
+    return _device_table(DenseWeightsBf16, rows, device)
 
 
 def dense_weights_bf16(table):
     """Rewrite every dense layer's bf16 operand copies listed in ``table`` (dense_weights_bf16_table) from its fp32 master weights: one launch."""
     lib = load(True)
-    _check(lib.vf_dense_weights_bf16(_p(table), table.shape[0], _stream()))
+    _check(lib.vf_dense_weights_bf16(table, table.shape[0], _stream()))
 
 
 def softmax_rows(scores, P, *, rows_total, rows_per_batch, cols, ld_in, ld_out, mask_mode=0, block=0, row0=0):
     lib = load(True)
-    _check(lib.vf_softmax_rows(_p(scores), C.c_int64(rows_total), rows_per_batch, cols, C.c_int64(ld_in), mask_mode, block,
-                               row0, _p(P), _dt(P), C.c_int64(ld_out), _stream()))
+    _check(lib.vf_softmax_rows(scores, rows_total, rows_per_batch, cols, ld_in, mask_mode, block, row0, P, _dt(P), ld_out, _stream()))
     return P
 
 
@@ -743,7 +752,7 @@ def argmax_rows(x_rows):
     _dev(x_rows, torch.float32)
     rows, cols = x_rows.shape
     out = torch.empty((rows,), dtype=torch.int64, device=x_rows.device)
-    _check(lib.vf_argmax_rows(_p(x_rows), C.c_int64(rows), cols, C.c_int64(cols), _p(out), _stream()))
+    _check(lib.vf_argmax_rows(x_rows, rows, cols, cols, out, _stream()))
     return out
 
 
@@ -751,7 +760,7 @@ def pose_postprocess(raw_rows, mult):
     lib = load(True)
     _dev(raw_rows, torch.float32)
     out = torch.empty_like(raw_rows)
-    _check(lib.vf_pose_postprocess(_p(raw_rows), C.c_int64(raw_rows.shape[0]), C.c_float(mult), _p(out), _stream()))
+    _check(lib.vf_pose_postprocess(raw_rows, raw_rows.shape[0], mult, out, _stream()))
     return out
 
 
@@ -762,7 +771,7 @@ def cameras_prepare(cams, relative):
     b, t, _ = cams.shape
     out = torch.empty_like(cams)
     tr = torch.empty((b, 7), dtype=torch.float32, device=cams.device)
-    _check(lib.vf_cameras_prepare(_p(cams), b, t, int(relative), _p(out), _p(tr), _stream()))
+    _check(lib.vf_cameras_prepare(cams, b, t, int(relative), out, tr, _stream()))
     return out, tr
 
 
@@ -771,7 +780,7 @@ def cameras_from_relative(cams, transform):
     _dev(cams, torch.float32)
     b, n, _ = cams.shape
     out = torch.empty_like(cams)
-    _check(lib.vf_cameras_from_relative(_p(cams), _p(transform), b, n, _p(out), _stream()))
+    _check(lib.vf_cameras_from_relative(cams, transform, b, n, out, _stream()))
     return out
 
 
@@ -781,7 +790,7 @@ def cross_entropy_rows(logits_rows, labels_i32, smoothing=0.0):
     _dev(labels_i32, torch.int32)
     rows, cols = logits_rows.shape
     out = torch.empty((rows,), dtype=torch.float32, device=logits_rows.device)
-    _check(lib.vf_cross_entropy_rows(_p(logits_rows), _p(labels_i32), C.c_int64(rows), cols, C.c_float(smoothing), _p(out), _stream()))
+    _check(lib.vf_cross_entropy_rows(logits_rows, labels_i32, rows, cols, smoothing, out, _stream()))
     return out
 
 
@@ -790,7 +799,7 @@ def pose_loss_rows(raw_rows, poses_bt7, tokens_per_view, mult):
     rows = raw_rows.shape[0]
     pos = torch.empty((rows,), dtype=torch.float32, device=raw_rows.device)
     ori = torch.empty((rows,), dtype=torch.float32, device=raw_rows.device)
-    _check(lib.vf_pose_loss_rows(_p(raw_rows), _p(poses_bt7), C.c_int64(rows), tokens_per_view, C.c_float(mult), _p(pos), _p(ori), _stream()))
+    _check(lib.vf_pose_loss_rows(raw_rows, poses_bt7, rows, tokens_per_view, mult, pos, ori, _stream()))
     return pos, ori
 
 
@@ -800,7 +809,7 @@ def row_mean(x_rows, start=0):
     _dev(x_rows, torch.float32)
     rows, n = x_rows.shape
     out = torch.empty((rows,), dtype=torch.float32, device=x_rows.device)
-    _check(lib.vf_row_mean(_p(x_rows), C.c_int64(rows), n, start, _p(out), _stream()))
+    _check(lib.vf_row_mean(x_rows, rows, n, start, out, _stream()))
     return out
 
 
@@ -814,16 +823,10 @@ def simt_conv_dgrad_s2(dy, w_dgrad_kn, in_hw):
     h, w = in_hw
     cin = w_dgrad_kn.shape[1]
     out = torch.empty((n, h, w, cin), dtype=torch.float32, device=dy.device)
-    p = SimtGemm()
-    p.A, p.a_dtype, p.conv = dy.data_ptr(), F32, 2
-    p.N, p.H, p.W, p.Cin = n, oh, ow, cout
-    p.OH, p.OW, p.KH, p.KW, p.stride = h, w, 3, 3, 1
-    p.pad_t, p.pad_l, p.upsample2x = 0, 0, 0
-    p.B, p.b_dtype, p.b_sk, p.b_sn = w_dgrad_kn.data_ptr(), F32, cin, 1
-    p.M, p.Ncols, p.K, p.batch1, p.batch2 = n * h * w, cin, 9 * cout, 1, 1
-    p.alpha, p.act, p.bias_mode = 1.0, ACT_NONE, BIAS_NONE
-    p.C_f32, p.ldc = out.data_ptr(), cin
-    _check(lib.vf_simt_gemm(C.byref(p), _stream()))
+    p = SimtGemm(A=dy.data_ptr(), a_dtype=F32, conv=2, N=n, H=oh, W=ow, Cin=cout, OH=h, OW=w, KH=3, KW=3, stride=1,
+                 B=w_dgrad_kn.data_ptr(), b_dtype=F32, b_sk=cin, b_sn=1, M=n * h * w, Ncols=cin, K=9 * cout, batch1=1, batch2=1)
+    _epilogue(p, out, cin)
+    _check(lib.vf_simt_gemm(p, _stream()))
     return out
 
 
@@ -834,8 +837,7 @@ def conv_wgrad(x, dy, dw, *, kh, stride=1, pad=(1, 1), upsample=False, so=None):
     n, h, w, cin = x.shape
     _, oh, ow, cout = dy.shape
     so_k, so_n = (cout, 1) if so is None else so
-    _check(lib.vf_conv_wgrad(_p(x), _p(dy), n, h, w, cin, oh, ow, cout, kh, kh, stride, pad[0], pad[1], int(upsample), C.c_int64(so_k),
-                             C.c_int64(so_n), _p(dw), _stream()))
+    _check(lib.vf_conv_wgrad(x, dy, n, h, w, cin, oh, ow, cout, kh, kh, stride, pad[0], pad[1], int(upsample), so_k, so_n, dw, _stream()))
     return dw
 
 
@@ -920,7 +922,7 @@ def _wgrad_tc(x, dy, dw, *, bf16, conv, norm=None, upsample=False, accumulate=Tr
     ld = 1 if bf16 else 2
     tc_gemm(at, bt, partial, M=M, N=cout, K=kc, lda=ld * la, ldb=ld * lb, ldc=cout, batch=(blocks, splits), a_bs=(0, kc), b_bs=(0, kc),
             c_bs=(splits * M * cout if conv else 0, M * cout), lo_a=la, lo_b=lb, k_offsets=[margin - pitch, margin, margin + pitch] if conv else None)
-    _check(lib.vf_sum_splits(_p(partial), blocks, splits, C.c_int64(M * cout), int(accumulate), _p(dw), _stream()))
+    _check(lib.vf_sum_splits(partial, blocks, splits, M * cout, int(accumulate), dw, _stream()))
     return dw
 
 
@@ -932,7 +934,7 @@ def pad_transpose_split(x, out, *, pitch, copies, margin, norm=None, upsample=Fa
     lib = load(True)
     _dev(x, torch.float32); _dev(out, torch.float16)
     n, h, w, c = x.shape
-    _check(lib.vf_pad_transpose_split(_p(x), n, h, w, c, pitch, copies, C.c_int64(margin), C.c_int64(out.shape[-1]), _p(out), _stream()))
+    _check(lib.vf_pad_transpose_split(x, n, h, w, c, pitch, copies, margin, out.shape[-1], out, _stream()))
     return out
 
 
@@ -945,8 +947,8 @@ def pad_transpose_bf16(x, out, *, pitch, copies, margin, norm=None, upsample=Fal
     n, h, w, c = x.shape
     mr, gamma, beta, swish = norm if norm is not None else (None, None, None, False)
     groups = mr.shape[1] if mr is not None else 0
-    _check(lib.vf_pad_transpose_bf16(_p(x), n, h, w, c, int(upsample), pitch, copies, C.c_int64(margin), C.c_int64(out.shape[-1]), _p(mr), _p(gamma),
-                                     _p(beta), groups, int(swish), _p(out), _stream()))
+    _check(lib.vf_pad_transpose_bf16(x, n, h, w, c, int(upsample), pitch, copies, margin, out.shape[-1], mr, gamma,
+                                     beta, groups, int(swish), out, _stream()))
     return out
 
 
@@ -958,20 +960,20 @@ def conv_weights_bf16_table(entries, device):
         _dev(w_kn, torch.float32); _dev(fw, torch.bfloat16)
         k, cout = w_kn.shape
         assert k % 9 == 0 and fw.shape == (cout, k) and (bw is None or (bw.dtype == torch.bfloat16 and bw.shape == (k // 9, 9 * cout)))
-        rows.append([w_kn.data_ptr(), fw.data_ptr(), bw.data_ptr() if bw is not None else 0, k // 9, cout])
-    return torch.tensor(rows, dtype=torch.int64).reshape(-1, 5).to(device)
+        rows.append(ConvWeightsBf16(w_kn.data_ptr(), fw.data_ptr(), bw.data_ptr() if bw is not None else None, k // 9, cout))
+    return _device_table(ConvWeightsBf16, rows, device)
 
 
 def conv_weights_bf16(table):
     """Rewrite every conv's bf16 operand copies listed in ``table`` (conv_weights_bf16_table) from its fp32 master weights: one launch."""
     lib = load(True)
-    _check(lib.vf_conv_weights_bf16(_p(table), table.shape[0], _stream()))
+    _check(lib.vf_conv_weights_bf16(table, table.shape[0], _stream()))
 
 
 def col_sums(x_rows, out):
     lib = load(True)
     _dev(x_rows, torch.float32)
-    _check(lib.vf_col_sums(_p(x_rows), C.c_int64(x_rows.numel() // x_rows.shape[-1]), x_rows.shape[-1], _p(out), _stream()))
+    _check(lib.vf_col_sums(x_rows, x_rows.numel() // x_rows.shape[-1], x_rows.shape[-1], out, _stream()))
     return out
 
 
@@ -983,8 +985,7 @@ def groupnorm_bwd(x, dout, mean_rstd, gamma, beta, dgamma, dbeta, *, swish, grou
     dx = torch.empty_like(x)
     dx16 = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if out_bf16 else None
     gs = torch.empty((n, groups, 2), dtype=torch.float64, device=x.device)
-    _check(lib.vf_groupnorm_bwd(_p(x), _p(dout), _p(mean_rstd), _p(gamma), _p(beta), n, h * w, c, groups, int(swish), _p(add), _p(gs),
-                                _p(dgamma), _p(dbeta), _p(dx), _p(dx16), _stream()))
+    _check(lib.vf_groupnorm_bwd(x, dout, mean_rstd, gamma, beta, n, h * w, c, groups, int(swish), add, gs, dgamma, dbeta, dx, dx16, _stream()))
     if dx16 is not None:
         dx._bf16 = dx16
     return dx
@@ -993,7 +994,7 @@ def groupnorm_bwd(x, dout, mean_rstd, gamma, beta, dgamma, dbeta, *, swish, grou
 def softmax_bwd_rows(P, dP):
     lib = load(True)
     dS = torch.empty_like(P)
-    _check(lib.vf_softmax_bwd_rows(_p(P), _p(dP), C.c_int64(P.numel() // P.shape[-1]), P.shape[-1], _p(dS), _stream()))
+    _check(lib.vf_softmax_bwd_rows(P, dP, P.numel() // P.shape[-1], P.shape[-1], dS, _stream()))
     return dS
 
 
@@ -1002,7 +1003,7 @@ def l1_grad(x, y, scale):
     lib = load(True)
     dy = torch.empty_like(y)
     ls = torch.zeros((1,), dtype=torch.float64, device=y.device)
-    _check(lib.vf_l1_grad(_p(x), _p(y), C.c_int64(y.numel()), C.c_float(scale), _p(dy), _p(ls), _stream()))
+    _check(lib.vf_l1_grad(x, y, y.numel(), scale, dy, ls, _stream()))
     return dy, ls
 
 
@@ -1010,7 +1011,7 @@ def lincomb3(a, x, b=0.0, y=None, c=0.0, z=None, out=None):
     lib = load(True)
     if out is None:
         out = torch.empty_like(x)
-    _check(lib.vf_lincomb3(C.c_float(a), _p(x), C.c_float(b), _p(y), C.c_float(c), _p(z), C.c_int64(x.numel()), _p(out), _stream()))
+    _check(lib.vf_lincomb3(a, x, b, y, c, z, x.numel(), out, _stream()))
     return out
 
 
@@ -1018,74 +1019,71 @@ def sumpool2x2(x):
     lib = load(True)
     n, h2, w2, c = x.shape
     y = torch.empty((n, h2 // 2, w2 // 2, c), dtype=torch.float32, device=x.device)
-    _check(lib.vf_sumpool2x2(_p(x), n, h2 // 2, w2 // 2, c, _p(y), _stream()))
+    _check(lib.vf_sumpool2x2(x, n, h2 // 2, w2 // 2, c, y, _stream()))
     return y
 
 
 def adam(p, g, m, v, *, lr, beta1, beta2, eps, step, grad_scale=1.0):
     lib = load(True)
-    _check(lib.vf_adam(_p(p), _p(g), _p(m), _p(v), C.c_int64(p.numel()), C.c_float(lr), C.c_float(beta1), C.c_float(beta2), C.c_float(eps),
-                       int(step), C.c_float(grad_scale), _stream()))
+    _check(lib.vf_adam(p, g, m, v, p.numel(), lr, beta1, beta2, eps, int(step), grad_scale, _stream()))
 
 
 def layernorm_bwd(x, dy, gamma, dgamma, dbeta, eps=1e-5, add=None):
     lib = load(True)
     d = x.shape[-1]
     dx = torch.empty_like(x)
-    _check(lib.vf_layernorm_bwd(_p(x), _p(dy), _p(gamma), _p(add), C.c_int64(x.numel() // d), d, C.c_float(eps), _p(dgamma), _p(dbeta), _p(dx), _stream()))
+    _check(lib.vf_layernorm_bwd(x, dy, gamma, add, x.numel() // d, d, eps, dgamma, dbeta, dx, _stream()))
     return dx
 
 
 def gelu(x):
     lib = load(True)
     y = torch.empty_like(x)
-    _check(lib.vf_gelu_fwd(_p(x), C.c_int64(x.numel()), _p(y), _stream()))
+    _check(lib.vf_gelu_fwd(x, x.numel(), y, _stream()))
     return y
 
 
 def gelu_bwd(pre, dy):
     lib = load(True)
     out = torch.empty_like(pre)
-    _check(lib.vf_gelu_bwd(_p(pre), _p(dy), C.c_int64(pre.numel()), _p(out), _stream()))
+    _check(lib.vf_gelu_bwd(pre, dy, pre.numel(), out, _stream()))
     return out
 
 
 def migt_embed_bwd(dh, ids_i32, fixed_token, BT, L, dwte, dwpe, dpose):
     lib = load(True)
-    _check(lib.vf_migt_embed_bwd(_p(dh), _p(ids_i32), int(fixed_token), C.c_int64(BT), L, dh.shape[-1], _p(dwte), _p(dwpe), _p(dpose), _stream()))
+    _check(lib.vf_migt_embed_bwd(dh, ids_i32, int(fixed_token), BT, L, dh.shape[-1], dwte, dwpe, dpose, _stream()))
 
 
 def cross_entropy_grad(logits_rows, labels_i32, row_weight, smoothing=0.0):
     lib = load(True)
     rows, cols = logits_rows.shape
     out = torch.empty_like(logits_rows)
-    _check(lib.vf_cross_entropy_grad(_p(logits_rows), _p(labels_i32), _p(row_weight), C.c_int64(rows), cols, C.c_float(smoothing), _p(out), _stream()))
+    _check(lib.vf_cross_entropy_grad(logits_rows, labels_i32, row_weight, rows, cols, smoothing, out, _stream()))
     return out
 
 
 def pose_loss_grad(raw_rows, poses_bt7, row_weight, tokens_per_view, mult, pos_scale=1.0, ori_scale=1.0):
     lib = load(True)
     out = torch.empty_like(raw_rows)
-    _check(lib.vf_pose_loss_grad(_p(raw_rows), _p(poses_bt7), _p(row_weight), C.c_int64(raw_rows.shape[0]), tokens_per_view, C.c_float(mult),
-                                 C.c_float(pos_scale), C.c_float(ori_scale), _p(out), _stream()))
+    _check(lib.vf_pose_loss_grad(raw_rows, poses_bt7, row_weight, raw_rows.shape[0], tokens_per_view, mult, pos_scale, ori_scale, out, _stream()))
     return out
 
 
 def adamw_keras(p, g, m, v, *, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0, clip_scale=1.0):
     lib = load(True)
-    _check(lib.vf_adamw_keras(_p(p), _p(g), _p(m), _p(v), C.c_int64(p.numel()), C.c_float(lr), C.c_float(beta1), C.c_float(beta2), C.c_float(eps),
-                              C.c_float(weight_decay), int(step), C.c_float(grad_scale), C.c_float(clip_scale), _stream()))
+    _check(lib.vf_adamw_keras(p, g, m, v, p.numel(), lr, beta1, beta2, eps, weight_decay, int(step), grad_scale, clip_scale, _stream()))
 
 
 def sumsq(x):
     lib = load(True)
     out = torch.zeros((1,), dtype=torch.float64, device=x.device)
-    _check(lib.vf_sumsq(_p(x), C.c_int64(x.numel()), _p(out), _stream()))
+    _check(lib.vf_sumsq(x, x.numel(), out, _stream()))
     return out
 
 
 def dropout(x, rate, seed):
     lib = load(True)
     y = torch.empty_like(x)
-    _check(lib.vf_dropout(_p(x), C.c_int64(x.numel()), C.c_float(rate), C.c_uint64(int(seed) & ((1 << 64) - 1)), _p(y), _stream()))
+    _check(lib.vf_dropout(x, x.numel(), rate, _seed64(seed), y, _stream()))
     return y

@@ -3,8 +3,6 @@ scans a scene's camera database with the reference's distances (evaluate_sevensc
 in a stable order.  Like every launching wrapper it is checked against fp64 on its own operands in the tests
 (tests/launch_checks_cameras.py).
 """
-import ctypes as C
-
 import torch
 
 from . import _lib as L
@@ -25,6 +23,5 @@ def camera_knn(db, queries, k, mode="combined"):
     n, stride = db.shape[-2], (db.shape[1] * 7 if db.dim() == 3 else 0)
     idx = torch.empty((q, max(int(k), 0)), dtype=torch.int32, device=queries.device)
     dist = torch.empty((q, max(int(k), 0)), dtype=torch.float32, device=queries.device)
-    L._check(lib.vf_camera_knn(L._p(db), C.c_int64(n), C.c_int64(stride), L._p(queries), q, DISTANCE_MODES[mode], int(k), L._p(idx),
-                               L._p(dist), L._stream()))
+    L._check(lib.vf_camera_knn(db, n, stride, queries, q, DISTANCE_MODES[mode], int(k), idx, dist, L._stream()))
     return idx, dist

@@ -3,8 +3,6 @@ encoder takes, and the dataset resize rule in float.  Thin wrappers of ``vf_f01_
 the float counterparts of ``_lib.u8_to_unit`` / ``_lib.resize_u8``; like every launching wrapper they are checked against fp64 on their
 own operands (tests/launch_checks_float.py) in the tests and in a launch audit of the four-channel workloads.
 """
-import ctypes as C
-
 import torch
 
 from . import _lib as L
@@ -17,12 +15,12 @@ def f01_to_unit(x, first_views=None):
     L._dev(x, torch.float32)
     if first_views is None:
         out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
-        L._check(lib.vf_f01_to_unit_f32(L._p(x), L._p(out), C.c_int64(1), C.c_int64(x.numel()), C.c_int64(0), L._stream()))
+        L._check(lib.vf_f01_to_unit_f32(x, out, 1, x.numel(), 0, L._stream()))
         return out
     b, t = x.shape[:2]
     per_view = x[0, 0].numel()
     out = torch.empty((b * first_views,) + tuple(x.shape[2:]), dtype=torch.float32, device=x.device)
-    L._check(lib.vf_f01_to_unit_f32(L._p(x), L._p(out), C.c_int64(b), C.c_int64(first_views * per_view), C.c_int64(t * per_view), L._stream()))
+    L._check(lib.vf_f01_to_unit_f32(x, out, b, first_views * per_view, t * per_view, L._stream()))
     return out
 
 
@@ -39,5 +37,5 @@ def resize_f32(x, size, method=None):
         method = "nearest" if size > h else "bilinear"
     assert method in ("nearest", "bilinear")
     out = torch.empty((n, size, size, c), dtype=torch.float32, device=x.device)
-    L._check(lib.vf_resize_f32(L._p(x), n, h, w, c, size, size, int(method == "bilinear"), L._p(out), L._stream()))
+    L._check(lib.vf_resize_f32(x, n, h, w, c, size, size, int(method == "bilinear"), out, L._stream()))
     return out
