@@ -2,8 +2,9 @@
 the bf16 trainer alternated in one process (three timed runs each, after a warm-up), with each trainer's peak allocated memory.  The default
 B = 5, T = 20 is the InteriorNet recipe's batch of 40 scenes over 8 GPUs.  VF_B / VF_T / VF_STEPS change the shape and the steps per run.
 ``--accumulate N``: every update accumulates N micro-batches of B scenes (``accumulate_steps``); N = 8 is the InteriorNet update of 8
-replicas on one GPU.  Times and rates are then per update of N x B scenes."""
-import argparse, os, subprocess, sys
+replicas on one GPU.  Times and rates are then per update of N x B scenes.  ``--random-pose-multiplier C``: alternate the bf16 trainer
+without the pose-scale augmentation and with random_pose_multiplier C instead of the two precisions (the augmentation's cost)."""
+import argparse, dataclasses, os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
@@ -15,9 +16,17 @@ from viewformer_b200.train_migt import MIGTTrainer
 B, T, n = int(os.environ.get("VF_B", "5")), int(os.environ.get("VF_T", "20")), int(os.environ.get("VF_STEPS", "3"))
 ap = argparse.ArgumentParser()
 ap.add_argument("--accumulate", type=int, default=1, help="micro-batches of B scenes per update")
-N = ap.parse_args().accumulate
+ap.add_argument("--random-pose-multiplier", type=float, default=None, help="compare bf16 at c = 1 and at this c")
+args = ap.parse_args()
+N = args.accumulate
 cfg = MIGTConfig()
 model = MIGT(cfg, precision="fp32").init_weights(0)
+if args.random_pose_multiplier is None:
+    arms = {"fp32": ("fp32", model), "bf16": ("bf16", model)}
+else:
+    c = args.random_pose_multiplier
+    scaled = MIGT(dataclasses.replace(cfg, random_pose_multiplier=c), precision="fp32").load_state_dict(model.state_dict())
+    arms = {"bf16 c=1": ("bf16", model), f"bf16 c={c:g}": ("bf16", scaled)}
 codes = synth.make_codes(B, T, n_embed=cfg.n_embeddings, seed=1)
 cams = mo.normalize_cameras(mo.to_relative_cameras(synth.make_cameras(B, T, seed=2))[0])
 try:
@@ -40,8 +49,8 @@ def run(tr, steps):
 
 
 trainers, times, peaks, losses = {}, {}, {}, {}
-for prec in ("fp32", "bf16"):
-    trainers[prec] = MIGTTrainer(model, precision=prec, accumulate_steps=N)
+for prec, (precision, m) in arms.items():
+    trainers[prec] = MIGTTrainer(m, precision=precision, accumulate_steps=N)
     times[prec] = []
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
@@ -49,13 +58,14 @@ for prec in ("fp32", "bf16"):
     run(trainers[prec], 2)                                     # warm-up: module loads, operand buffers
     peaks[prec] = torch.cuda.max_memory_allocated() - base
 for _ in range(3):
-    for prec in ("fp32", "bf16"):
+    for prec in arms:
         ms, losses[prec] = run(trainers[prec], n)
         times[prec].append(ms)
-for prec in ("fp32", "bf16"):
+for prec in arms:
     t = np.array(times[prec])
     med = float(np.median(t))
     print(f"[migt train step, full size, {prec}] {N} x B={B} T={T}: median {med:.1f} ms/update (runs {', '.join(f'{x:.1f}' for x in t)}; "
           f"spread {t.max() - t.min():.1f} ms) -> {N * B * T * 64 / med * 1e3:.0f} tokens/s; step peak {peaks[prec] / 2**30:.2f} GiB above the trainers' state; "
           f"loss {losses[prec]:.4f}")
-print(f"[bf16 vs fp32] {np.median(times['fp32']) / np.median(times['bf16']):.2f}x")
+a, b = arms
+print(f"[{b} vs {a}] {np.median(times[a]) / np.median(times[b]):.2f}x")

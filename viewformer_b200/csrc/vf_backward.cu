@@ -10,6 +10,7 @@
 //   vf_sumpool2x2          backward of the nearest x2 upsampling
 //   vf_adam                torch.optim.Adam step (betas (0.5, 0.9) at the call site) over a flat parameter / gradient buffer
 #include "vf_common.cuh"
+#include "../../include/vf_b200_pose.h"
 #include <cuda_fp16.h>
 
 namespace {
@@ -376,16 +377,20 @@ __global__ void __launch_bounds__(256) ce_grad_kernel(const float* __restrict__ 
     }
 }
 
-// d/draw of sum_rows w[row] * (pos_loss + ori_loss) (pose_loss_kernel in vf_misc.cu): pos = mean_3 (y m - r)^2, ori = mean_4 (y - r)^2
+// d/draw of sum_rows w[row] * (pos_loss + ori_loss) (pose_loss_kernel in vf_misc.cu): pos = mean_3 (y m - r/c)^2, ori = mean_4 (y - r)^2,
+// c = scene_mult[view / views_per_scene] or 1 (null): the position gradient carries the factor 1/c of r/c
 __global__ void pose_loss_grad_kernel(const float* __restrict__ raw, const float* __restrict__ poses, const float* __restrict__ w, long long rows,
-                                      int tokens_per_view, float mult, float pos_scale, float ori_scale, float* __restrict__ draw) {
+                                      int tokens_per_view, float mult, int views_per_scene, const float* __restrict__ scene_mult, float pos_scale,
+                                      float ori_scale, float* __restrict__ draw) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= rows) return;
     const float* r = raw + i * 7;
-    const float* y = poses + (i / tokens_per_view) * 7;
+    const long long view = i / tokens_per_view;
+    const float* y = poses + view * 7;
+    const float c = scene_mult ? scene_mult[view / views_per_scene] : 1.0f;      // x / 1 == x: the unscaled path keeps its bits
     const float wp = w[i] * pos_scale, wo = w[i] * ori_scale;
 #pragma unroll
-    for (int j = 0; j < 3; ++j) draw[i * 7 + j] = wp * (-2.0f / 3.0f) * (y[j] * mult - r[j]);
+    for (int j = 0; j < 3; ++j) draw[i * 7 + j] = wp * (-2.0f / 3.0f) * (y[j] * mult - r[j] / c) / c;
 #pragma unroll
     for (int j = 3; j < 7; ++j) draw[i * 7 + j] = wo * (-2.0f / 4.0f) * (y[j] - r[j]);
 }
@@ -819,8 +824,19 @@ extern "C" int vf_pose_loss_grad(const float* raw, const float* poses, const flo
                                  float pose_multiplier, float pos_scale, float ori_scale, float* draw, vf_stream_t s) {
     VF_CHECK_ARG(raw && poses && row_weight && draw && tokens_per_view > 0, "vf_pose_loss_grad: bad args");
     if (rows == 0) return VF_OK;
-    pose_loss_grad_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, vf_s(s)>>>(raw, poses, row_weight, rows, tokens_per_view, pose_multiplier, pos_scale, ori_scale, draw);
+    pose_loss_grad_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, vf_s(s)>>>(raw, poses, row_weight, rows, tokens_per_view, pose_multiplier, 1,
+                                                                              nullptr, pos_scale, ori_scale, draw);
     VF_CHECK_LAUNCH("vf_pose_loss_grad");
+    return VF_OK;
+}
+extern "C" int vf_pose_loss_grad_scaled(const float* raw, const float* poses, const float* row_weight, int64_t rows, int tokens_per_view,
+                                        float pose_multiplier, int views_per_scene, const float* scene_mult, float pos_scale, float ori_scale,
+                                        float* draw, vf_stream_t s) {
+    VF_CHECK_ARG(raw && poses && row_weight && draw && tokens_per_view > 0 && views_per_scene > 0, "vf_pose_loss_grad_scaled: bad args");
+    if (rows == 0) return VF_OK;
+    pose_loss_grad_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, vf_s(s)>>>(raw, poses, row_weight, rows, tokens_per_view, pose_multiplier,
+                                                                              views_per_scene, scene_mult, pos_scale, ori_scale, draw);
+    VF_CHECK_LAUNCH("vf_pose_loss_grad_scaled");
     return VF_OK;
 }
 extern "C" int vf_adamw_keras(float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,

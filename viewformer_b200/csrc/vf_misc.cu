@@ -1,6 +1,7 @@
 // Small HBM-bound kernels: pixel conversion, layout permutes, transformer glue
 // (embedding sum, row softmax with block-causal masks, argmax, pose post-processing), casts, loss sums.
 #include "vf_common.cuh"
+#include "../../include/vf_b200_pose.h"
 #include <stdarg.h>
 
 // ------------------------------------------------------------------------------------------ errors
@@ -335,21 +336,40 @@ __global__ void __launch_bounds__(256) ce_rows_kernel(const float* __restrict__ 
     }
 }
 
-// pose regression losses per token (models/migt.py:165-171): raw [rows,7] MLP output, target pose of the token's view
-// (poses [BT,7], tokens_per_view consecutive rows share a view) scaled by [m,m,m,1,1,1,1]; pos = mean_3 (y-xyz)^2, ori = mean_4 (y-q)^2
+// pose regression losses per token (models/migt.py:158-171): raw [rows,7] MLP output, target pose of the token's view
+// (poses [BT,7], tokens_per_view consecutive rows share a view) scaled by [m,m,m,1,1,1,1]; pos = mean_3 (y-xyz/c)^2, ori = mean_4 (y-q)^2
+// with c = scene_mult[view / views_per_scene] (the training-time pose scale of the view's scene), or 1 when scene_mult is null
 __global__ void pose_loss_kernel(const float* __restrict__ raw, const float* __restrict__ poses, int64_t rows, int tokens_per_view,
-                                 float mult, float* __restrict__ pos_out, float* __restrict__ ori_out) {
+                                 float mult, int views_per_scene, const float* __restrict__ scene_mult, float* __restrict__ pos_out,
+                                 float* __restrict__ ori_out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= rows) return;
     const float* r = raw + i * 7;
-    const float* y = poses + (i / tokens_per_view) * 7;
+    const int64_t view = i / tokens_per_view;
+    const float* y = poses + view * 7;
+    const float c = scene_mult ? scene_mult[view / views_per_scene] : 1.0f;      // x / 1 == x: the unscaled path keeps its bits
     float p = 0.f, o = 0.f;
 #pragma unroll
-    for (int j = 0; j < 3; ++j) { const float d = y[j] * mult - r[j]; p += d * d; }
+    for (int j = 0; j < 3; ++j) { const float d = y[j] * mult - r[j] / c; p += d * d; }
 #pragma unroll
     for (int j = 3; j < 7; ++j) { const float d = y[j] - r[j]; o += d * d; }
     pos_out[i] = p / 3.0f;
     ori_out[i] = o / 4.0f;
+}
+
+// get_model_input (models/migt.py:139-145): out [rows,7] = [(xyz * mult) * c | quaternion] of poses [rows,7], rounded after each product
+// as the reference does, c = scene_mult[row / views_per_scene] (omitted when scene_mult is null)
+__global__ void pose_model_input_kernel(const float* __restrict__ poses, int64_t rows, int views_per_scene, float mult,
+                                        const float* __restrict__ scene_mult, float* __restrict__ out) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rows * 7) return;
+    const int64_t row = i / 7;
+    float v = poses[i];
+    if (i - row * 7 < 3) {
+        v = v * mult;
+        if (scene_mult) v = v * scene_mult[row / views_per_scene];
+    }
+    out[i] = v;
 }
 
 // out[b] = mean(x[b, start:n])  — one block per b
@@ -498,8 +518,25 @@ extern "C" int vf_pose_loss_rows(const float* raw, const float* poses, int64_t r
                                  float* pos_out, float* ori_out, vf_stream_t s) {
     VF_CHECK_ARG(raw && poses && pos_out && ori_out && tokens_per_view > 0, "vf_pose_loss_rows: bad args");
     if (rows == 0) return VF_OK;
-    pose_loss_kernel<<<nblk(rows, 256), 256, 0, vf_s(s)>>>(raw, poses, rows, tokens_per_view, pose_multiplier, pos_out, ori_out);
+    pose_loss_kernel<<<nblk(rows, 256), 256, 0, vf_s(s)>>>(raw, poses, rows, tokens_per_view, pose_multiplier, 1, nullptr, pos_out, ori_out);
     VF_CHECK_LAUNCH("vf_pose_loss_rows");
+    return VF_OK;
+}
+extern "C" int vf_pose_loss_rows_scaled(const float* raw, const float* poses, int64_t rows, int tokens_per_view, float pose_multiplier,
+                                        int views_per_scene, const float* scene_mult, float* pos_out, float* ori_out, vf_stream_t s) {
+    VF_CHECK_ARG(raw && poses && pos_out && ori_out && tokens_per_view > 0 && views_per_scene > 0, "vf_pose_loss_rows_scaled: bad args");
+    if (rows == 0) return VF_OK;
+    pose_loss_kernel<<<nblk(rows, 256), 256, 0, vf_s(s)>>>(raw, poses, rows, tokens_per_view, pose_multiplier, views_per_scene, scene_mult,
+                                                          pos_out, ori_out);
+    VF_CHECK_LAUNCH("vf_pose_loss_rows_scaled");
+    return VF_OK;
+}
+extern "C" int vf_pose_model_input(const float* poses, int64_t rows, int views_per_scene, float pose_multiplier, const float* scene_mult,
+                                   float* out, vf_stream_t s) {
+    VF_CHECK_ARG(poses && out && rows >= 0 && views_per_scene > 0, "vf_pose_model_input: bad args");
+    if (rows == 0) return VF_OK;
+    pose_model_input_kernel<<<nblk(rows * 7, 256), 256, 0, vf_s(s)>>>(poses, rows, views_per_scene, pose_multiplier, scene_mult, out);
+    VF_CHECK_LAUNCH("vf_pose_model_input");
     return VF_OK;
 }
 extern "C" int vf_row_mean(const float* x, int64_t rows, int n, int start, float* out, vf_stream_t s) {

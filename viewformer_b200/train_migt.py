@@ -33,8 +33,10 @@ import os
 from collections import OrderedDict
 
 import torch
+import torch.distributed as dist
 
 from . import _lib as L
+from . import pose_scale as PS
 from .dist import GradExchange
 
 LN_EPS = 1e-5
@@ -87,8 +89,8 @@ class MIGTTrainer:
         self.accumulate_steps = int(accumulate_steps)
         self.pending = 0                                           # micro-batches in the gradient since the last optimizer step
         cfg = model.config
-        if cfg.random_pose_multiplier != 1.0:
-            raise NotImplementedError("random_pose_multiplier != 1 (pose-scale augmentation, migt.py:350-353) is not supported")
+        if not (math.isfinite(cfg.random_pose_multiplier) and cfg.random_pose_multiplier > 0):
+            raise ValueError(f"random_pose_multiplier must be a positive number, got {cfg.random_pose_multiplier}")
         if precision not in ("fp32", "bf16"):
             raise ValueError(f"precision must be 'fp32' or 'bf16', got {precision!r}")
         self.precision, self.bf16 = precision, precision == "bf16"
@@ -402,7 +404,21 @@ class MIGTTrainer:
         return o16, (qk, vt, o32, lse)
 
     # ------------------------------------------------------------------ the step
-    def forward_backward(self, poses, tokens):
+    def _pose_scale(self, B, pose_scale_u):
+        """(u, r) of this micro-batch's pose-scale augmentation, fp32 [B] on the host: r = c ** u (migt.py:349-354).  u: the hashed draw
+        (pose_scale.pose_scale_exponents), or ``pose_scale_u`` when given.  Each scene of each micro-batch of each rank draws its own u, as each
+        MirroredStrategy replica runs its own tf.random.uniform (DESIGN.md section 6)."""
+        if pose_scale_u is None:
+            rank = dist.get_rank(self.group) if (dist.is_available() and dist.is_initialized()) else 0
+            micro = 0 if self.pending in (0, self.ex.micro_batches) else self.pending
+            u = PS.pose_scale_exponents(self.seed, self.iterations, rank, micro, B)
+        else:
+            u = torch.as_tensor(pose_scale_u, dtype=torch.float32).reshape(B).clone()
+        return u, torch.pow(torch.tensor(float(self.cfg.random_pose_multiplier), dtype=torch.float32), u)
+
+    def forward_backward(self, poses, tokens, pose_scale_u=None):
+        """One micro-batch's loss and gradient.  ``pose_scale_u`` [B]: the exponents of the pose-scale augmentation in place of the hashed
+        draw (random_pose_multiplier != 1 only)."""
         cfg, dev, p, g = self.cfg, self.device, self.p, self.g
         tokens = torch.as_tensor(tokens)
         B, T = tokens.shape[:2]
@@ -410,8 +426,18 @@ class MIGTTrainer:
         S, skip = T * Lt, cfg.n_loss_skip
         ids = tokens.reshape(B, T, Lt).to(device=dev, dtype=torch.int32).contiguous()
         poses = torch.as_tensor(poses, dtype=torch.float32).to(dev).reshape(B * T, 7).contiguous()
-        mult = torch.tensor([cfg.pose_multiplier] * 3 + [1.0] * 4, dtype=torch.float32, device=dev)
-        pin = (poses * mult).contiguous()                                           # get_model_input (migt.py:139-145)
+        # get_model_input (migt.py:139-145); with random_pose_multiplier c != 1 scene b's xyz is also scaled by r_b = c ** u_b and its
+        # predicted xyz divided by r_b before the position loss (:158-160)
+        if cfg.random_pose_multiplier != 1.0:
+            pose_u, pose_r = self._pose_scale(B, pose_scale_u)
+            scene_mult = pose_r.to(dev)
+            pin = PS.pose_model_input(poses, float(cfg.pose_multiplier), T, scene_mult)
+        else:
+            if pose_scale_u is not None:
+                raise ValueError("pose_scale_u is given but random_pose_multiplier is 1: there is no pose-scale augmentation to draw")
+            scene_mult = None
+            mult = torch.tensor([cfg.pose_multiplier] * 3 + [1.0] * 4, dtype=torch.float32, device=dev)
+            pin = (poses * mult).contiguous()
         # ---------------- embeddings: three streams (migt.py:354-405)
         pe_h = self._lin(pin, "pose_embedding.c_fc")
         pe = self._lin(self._gelu(pe_h), "pose_embedding.c_proj")                # [B*T, d]
@@ -451,6 +477,8 @@ class MIGTTrainer:
         ce = L.row_mean(ce_rows.reshape(B, S), skip * Lt)
         loss = ce * float(cfg.image_generation_weight)
         self.last = dict(ce_loss=ce, logits=logits.reshape(B, T, Lt, V))
+        if scene_mult is not None:
+            self.last.update(pose_scale_u=pose_u, pose_scale=pose_r)
         dhn = [None] * ns
         if self.pending in (0, self.ex.micro_batches):                            # the first micro-batch opens the accumulation window
             self.ex.reset(float(2.0 ** round(math.log2(denom)) if self.grad_seed_scale is None else self.grad_seed_scale), self.accumulate_steps)
@@ -467,7 +495,10 @@ class MIGTTrainer:
         if self.use_loc:
             pc_h = self._lin(hn[2], "pose_classifier.c_fc")
             raw = self._lin(self._gelu(pc_h), "pose_classifier.c_proj")            # [B*S, 7]
-            pl_rows, ol_rows = L.pose_loss_rows(raw, poses, Lt, float(cfg.pose_multiplier))
+            if scene_mult is None:
+                pl_rows, ol_rows = L.pose_loss_rows(raw, poses, Lt, float(cfg.pose_multiplier))
+            else:
+                pl_rows, ol_rows = PS.pose_loss_rows_scaled(raw, poses, Lt, float(cfg.pose_multiplier), T, scene_mult)
             pl, ol = L.row_mean(pl_rows.reshape(B, S), skip * Lt), L.row_mean(ol_rows.reshape(B, S), skip * Lt)
             lw_now = self.loc_weight
             if self.dynamic_pose:
@@ -486,7 +517,11 @@ class MIGTTrainer:
                 pose_loss, ps, os_ = pl + ol, 1.0, 1.0
             loss = loss + pose_loss * lw_now
             self.last.update(pose_pos_loss=pl, pose_ori_loss=ol, pose_loss=pose_loss)
-            draw = L.pose_loss_grad(raw, poses, (view_ok * (lw_now * ls / denom)).contiguous(), Lt, float(cfg.pose_multiplier), ps, os_)
+            row_w = (view_ok * (lw_now * ls / denom)).contiguous()
+            if scene_mult is None:
+                draw = L.pose_loss_grad(raw, poses, row_w, Lt, float(cfg.pose_multiplier), ps, os_)
+            else:
+                draw = PS.pose_loss_grad_scaled(raw, poses, row_w, Lt, float(cfg.pose_multiplier), T, scene_mult, ps, os_)
             dg_ = self._lin_bw(self._gelu(pc_h), draw, "pose_classifier.c_proj")
             dhn[2] = self._lin_bw(hn[2], L.gelu_bwd(pc_h, dg_), "pose_classifier.c_fc")
         else:
@@ -599,12 +634,13 @@ class MIGTTrainer:
         if self.bf16:
             L.dense_weights_bf16(self._w16_table)
 
-    def train_step(self, batch):
+    def train_step(self, batch, pose_scale_u=None):
         """(poses [B,T,7], tokens [B,T,h,w]) -> dict(loss, ce_loss, [pose losses], acc, learning_rate, applied, pending) — migt.py:464-505.
         The metrics are this micro-batch's; ``applied``: an update ran after it (False inside an accumulation window and on a skipped
-        non-finite bf16 window); ``pending``: micro-batches accumulated and not yet stepped on (0 after every optimizer step)."""
+        non-finite bf16 window); ``pending``: micro-batches accumulated and not yet stepped on (0 after every optimizer step).
+        ``pose_scale_u``: see forward_backward."""
         poses, tokens = batch
-        loss = self.forward_backward(poses, tokens)
+        loss = self.forward_backward(poses, tokens, pose_scale_u=pose_scale_u)
         lr = self.learning_rate()
         applied = self.optimizer_step() if self.pending == self.ex.micro_batches else False
         out = {k: float(torch.as_tensor(v, dtype=torch.float32).mean()) for k, v in self.last.items() if k.endswith("loss")}
