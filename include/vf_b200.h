@@ -303,13 +303,19 @@ int vf_ssim_u8_k(const void* a_u8, const void* b_u8, int N, int H, int W, int C,
  * replaces: models/utils_th.py:34-44 (distance, argmax(-dist), gather), :66 (diff), :70-72 (embed_code)
  *   z [M,D] f32 rows; codebook given TRANSPOSED as Et [K,D] (built once at weight load) with esq[K]=|e|^2.
  *   idx int64 [M]; quant (nullable) f32 [M,D]; diff_sum (nullable) double[1], += sum((e-z)^2).
+ *   Index rule of both lookups: the nearest code, equal distances to the smaller index; a NaN distance counts as +inf.  So a row
+ *   with a NaN or +-inf element (all its distances NaN or +inf) gets code 0, as argmax(-dist) gives for NaN in the reference, and a
+ *   NaN code is never chosen over a finite one; quant and diff_sum follow from that index (NaN / inf for such rows).
  * ---------------------------------------------------------------------------------------- */
 int vf_vq_lookup(const float* z, const float* Et, const float* esq, int64_t M, int D, int K,
                  int64_t* idx, float* quant, double* diff_sum, vf_stream_t s);
 /* Fused lookup (same result as vf_vq_lookup; viewformer_b200/csrc/vf_vq_fused.cu): one wgmma kernel reads every z row ONCE
  * (fp32 -> fp16 in shared memory), scores it against Eh = fp16(-2 e) [K,D] (vf_vq_prepare_codebook_f16) with wgmma and keeps the
  * two best codes per row straight from the accumulator registers — no score matrix in HBM, 4*D + 8 bytes of traffic per row.  Rows whose two best scores
- * lie within the fp16 rounding bound (tol_factor x worst case; 0.25 recommended) are settled exactly in fp64 by a second kernel.
+ * lie within the fp16 rounding bound are settled exactly in fp64 by a second kernel.  tol_factor scales the bound's relative part:
+ * 1.0 is the proven worst case (fp16 subnormals and accumulation included), under which every row whose fp64 gap exceeds the bound
+ * gets the fp64 nearest code; below 1.0, rows whose fp16 roundings align can be misranked.  Rows outside the fp16 / fixed-point
+ * range and codebooks with a code beyond it (or a NaN code) are decided by the exact pass.
  *   D % 64 == 0, D <= 256, K % 256 == 0, K <= 1024, M < 2^31.  worklist: int4[M] scratch; counter: int[2] scratch, on return
  *   counter[0] = rows settled between two candidates, counter[1] = rows settled over all codes.  quant / diff_sum nullable. */
 int vf_vq_prepare_codebook_f16(const float* Et, int K, int D, void* Eh_f16, vf_stream_t s);

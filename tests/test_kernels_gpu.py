@@ -731,9 +731,9 @@ def test_vq_lookup_fused_bit_exact(L, golden_dir):
     b, _, _ = L.vq_lookup(zz, et, esq, want_quant=False, want_diff=False)
     print(f"[vq_lookup_fused] 40960 random rows: mismatches {int((a != b).sum())}; settled exactly: pair {int(cnt[0])}, all-codes {int(cnt[1])}")
     assert torch.equal(a, b)
-    # worst-case tolerance (tol_factor = 1): same indices, more rows take the exact pass
-    a1, _, _, cnt1 = L.vq_lookup_fused(zz, et, esq, eh, want_quant=False, want_diff=False, tol_factor=1.0, return_counts=True)
-    assert torch.equal(a1, b) and int(cnt1.sum()) >= int(cnt.sum())
+    # a quarter of the worst-case tolerance (the default, tol_factor = 1): same indices on random rows, fewer rows take the exact pass
+    a1, _, _, cnt1 = L.vq_lookup_fused(zz, et, esq, eh, want_quant=False, want_diff=False, tol_factor=0.25, return_counts=True)
+    assert torch.equal(a1, b) and int(cnt1.sum()) <= int(cnt.sum())
     # rows beyond fp16 range / non-finite rows go to the exact pass instead of producing garbage
     zbig = zz[:300].clone()
     zbig[5] *= 1e5

@@ -592,9 +592,11 @@ def vq_fused_ok(d, k):
     return d % 64 == 0 and d <= 256 and k % 256 == 0 and k <= 1024
 
 
-def vq_lookup_fused(z_rows, et, esq, eh, emb_dk=None, want_quant=True, want_diff=True, tol_factor=0.25, return_counts=False):
+def vq_lookup_fused(z_rows, et, esq, eh, emb_dk=None, want_quant=True, want_diff=True, tol_factor=1.0, return_counts=False):
     """Fused wgmma lookup (vf_vq_fused.cu): z read once, top-2 from the accumulator registers, exact fp64 settlement of near-ties.  Same outputs as
-    vq_lookup; ``return_counts`` adds the int32[2] tensor (rows settled between two candidates, rows settled over all codes)."""
+    vq_lookup; ``return_counts`` adds the int32[2] tensor (rows settled between two candidates, rows settled over all codes).  ``tol_factor``
+    scales the fp16 rounding bound that sends a row to the exact pass: 1.0 is the proven worst case, smaller values can misrank rows whose
+    roundings align."""
     lib = load(True)
     _dev(z_rows, torch.float32)
     m, d = z_rows.shape

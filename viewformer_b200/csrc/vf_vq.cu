@@ -8,6 +8,9 @@ constexpr int LM = 64, LN = 64, LK = 16, LPAD = 4;
 
 // One CTA = 64 z rows against the whole codebook.  64x64x16 register-tiled fp32 dot products, running
 // (min dist, first index) per row; distance evaluated in the reference's order (|z|^2 - 2 z.e) + |e|^2.
+// Non-finite distances: NaN counts as +inf and equal distances go to the smaller index, so a row with a NaN or +-inf element
+// (every distance NaN or +inf) returns code 0, as the reference's argmax(-dist) does for NaN, and a NaN code is never chosen
+// over a finite one.
 __global__ void __launch_bounds__(256) vq_lookup_kernel(const float* __restrict__ z, const float* __restrict__ Et,
                                                         const float* __restrict__ esq, int64_t M, int D, int K,
                                                         int64_t* __restrict__ idx, float* __restrict__ quant,
@@ -82,7 +85,8 @@ __global__ void __launch_bounds__(256) vq_lookup_kernel(const float* __restrict_
             for (int j = 0; j < 4; ++j) {
                 const int c = c0 + tx * 4 + j;
                 if (c < K) {
-                    const float dist = __fadd_rn(__fsub_rn(zi, 2.0f * acc[i][j]), __ldg(esq + c));
+                    // NaN reads as +inf, and +inf distances tie: a row with a NaN or +-inf element gets code 0
+                    const float dist = fminf(__fadd_rn(__fsub_rn(zi, 2.0f * acc[i][j]), __ldg(esq + c)), INFINITY);
                     if (dist < bd[i] || (dist == bd[i] && c < bi[i])) { sd[i] = bd[i]; si[i] = bi[i]; bd[i] = dist; bi[i] = c; }
                     else if (dist < sd[i] || (dist == sd[i] && c < si[i])) { sd[i] = dist; si[i] = c; }
                 }

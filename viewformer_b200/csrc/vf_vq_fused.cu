@@ -11,12 +11,17 @@
 //   merge (4 warps)   per row: best code over the 16 sets; if the runner-up lies within the fp16 rounding bound of the best the row
 //                     is queued for the exact pass (PAIR: both candidates known; FULL: a third may hide inside one set)
 // vq_rescue_kernel then settles queued rows in fp64 (direct sum of squared differences, ties to the smaller index — the same rule as
-// vf_vq_lookup), so the indices returned equal the fp32 kernel's on every input.
+// vf_vq_lookup), so with tol_factor = 1 the index returned is the fp64 nearest code on every row whose fp64 gap to the runner-up
+// exceeds the fp16 rounding bound below, and the fp32 kernel's index wherever the fp32 kernel itself is decisive.  Non-finite rows
+// (a NaN or +-inf element) are settled over all codes with NaN read as +inf, so they return code 0, as vf_vq_lookup does.
 //
-// Rounding model (why the tolerance is safe): fp16 operands carry 11 significand bits, |d(z.e)| <= 2^-10 sum|z_i e_i| <= 2^-10 |z||e|;
-// the score -2 z.e + |e|^2 of two codes therefore moves by at most 2^-9 |z| (|e_a| + |e_b|) against each other (worst case, all
-// roundings aligned; rms is ~40x smaller).  `tol_factor` scales that bound (1.0 = worst case; default 0.25 = ~10 sigma); index
-// packing (6 mantissa bits) and the truncating tensor-core accumulation add 2^-16 |s| which is always included unscaled.
+// Rounding model (why the tolerance is safe): an fp16 operand x carries an error of at most max(2^-11 |x|, 2^-25) (relative in
+// the normal range, absolute among the subnormals below 2^-14).  The relative part gives |d(z.e)| <= 2^-10 sum|z_i e_i| <=
+// 2^-10 |z||e|, so the score -2 z.e + |e|^2 of two codes moves by at most 2^-9 |z| (|e_a| + |e_b|) against each other; this is
+// reached when all roundings align (tests/test_vq_lookup_edges_host.py builds such rows), while random roundings move it ~40x
+// less.  `tol_factor` scales that bound: 1.0 (the default of viewformer_b200._lib) is the proven worst case, smaller factors are
+// a statistical bet that aligned rows do not occur.  Always included unscaled: the subnormal part, 2^-23 sqrt(D) (|z| + |e_a| +
+// |e_b|) + D 2^-48; index packing (6 mantissa bits) and the truncating tensor-core accumulation, 2^-16 |s| + 4 G.
 #include "vf_wgmma.cuh"
 #include <cuda_fp16.h>
 
@@ -94,13 +99,16 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
     __syncthreads();
     {
         float mx = 0.f;
-        for (int i = threadIdx.x; i < p.K; i += THREADS) mx = fmaxf(mx, __ldg(p.esq + i));
+        for (int i = threadIdx.x; i < p.K; i += THREADS) {
+            const float v = __ldg(p.esq + i);
+            mx = fmaxf(mx, v == v ? v : INFINITY);              // fmaxf drops NaN: a NaN code must fail codebook_ok below
+        }
         mx = warp_max(mx);
         if ((threadIdx.x & 31) == 0) atomicMax(&esqmax_bits, __float_as_int(mx));      // non-negative floats order like their bit patterns
     }
     __syncthreads();
     const float esqmax = fmaxf(__int_as_float(esqmax_bits), 1e-30f);
-    const bool codebook_ok = esqmax < 1.0e9f;                    // every -2 e_i representable in fp16 (|e_i| <= |e| < 31623); NaN fails too
+    const bool codebook_ok = esqmax < 1.0e9f;                    // every -2 e_i representable in fp16 (|e_i| <= |e| < 31623); NaN / inf fail
     const int kexp = ((__float_as_int(17.2f * esqmax) >> 23) & 255) - 127 + 2;          // 2^(kexp - 1) > 17.2 max|e|^2
     const int c_bits = ((kexp + 127) << 23) | 0x400000;          // C = 1.5 * 2^kexp
     const float c_off = __int_as_float(c_bits);
@@ -266,6 +274,7 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
                 }
                     // key -> (value, code, set): value = ((key - key0) >> 8) * G, code = n*256 + g*64 + idx6, set = n*4 + g
                     const float vscale = g_step * 0.00390625f;            // G / 256
+                    const float sub_k = 1.1920929e-7f * sqrtf((float)p.D), sub_0 = (float)p.D * 3.5527137e-15f;    // 2^-23 sqrt(D), D 2^-48
                     float bv = __int_as_float(0x7f800000);
                     int bc = 0x7fffffff, bset = -1;
 #pragma unroll
@@ -292,8 +301,10 @@ __global__ void __launch_bounds__(THREADS, 1) vq_lookup_fused_kernel(const __gri
                         const int c = n * TN + g * 64 + (int)(k & 63u);
                         if (c == bc) { inside |= 1u << i; continue; }
                         // truncating tensor-core accumulation (2^-16 relative, generous) + the fixed-point step of both scores
-                        const float slack = 1.52587891e-5f * (fabsf(v) + fabsf(bv)) + 4.0f * g_step;
-                        const float tol = p.tol_factor * 0.001953125f * znorm * (eb + sqrtf(__ldg(p.esq + c))) + slack;
+                        // + fp16 subnormal operands (absolute rounding 2^-25, see the rounding model above)
+                        const float ec = sqrtf(__ldg(p.esq + c));
+                        const float slack = 1.52587891e-5f * (fabsf(v) + fabsf(bv)) + 4.0f * g_step + sub_k * (znorm + eb + ec) + sub_0;
+                        const float tol = p.tol_factor * 0.001953125f * znorm * (eb + ec) + slack;
                         if (v - bv <= tol) { ++within; inside |= 1u << i; oc = c; oset = n * 4 + g; }
                     }
                     p.idx[gr] = (long long)bc;
@@ -424,7 +435,7 @@ __global__ void __launch_bounds__(256) vq_rescue_kernel(const float* __restrict_
         }
         __syncthreads();
         const int nc = ncand;
-        double bd = 1e300;
+        double bd = INFINITY;
         int bi = 0x7fffffff;
         auto score64 = [&](int c) {
             const float* ec = Et + (long long)c * D;
@@ -435,6 +446,7 @@ __global__ void __launch_bounds__(256) vq_rescue_kernel(const float* __restrict_
             }
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) dd += __shfl_xor_sync(0xffffffffu, dd, o);
+            dd = fmin(dd, (double)INFINITY);                  // NaN reads as +inf; +inf ties go to the smaller index (vf_vq_lookup's rule)
             if (dd < bd || (dd == bd && c < bi)) { bd = dd; bi = c; }
         };
         if (nc <= MAXCAND) {
