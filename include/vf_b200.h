@@ -24,7 +24,7 @@ typedef void* vf_stream_t; /* cudaStream_t */
 
 enum { VF_F32 = 0, VF_BF16 = 1, VF_F16X2 = 2 /* fp32 value as two fp16: [.., hi(C) | lo(C)], lo = fp16((v - hi) * 2^11); fp32-faithful for
                                                    tensors with amax in [2^-10, 2^15], NaN products at |v| >= 65520; see vf_tc_gemm */ };
-enum { VF_ACT_NONE = 0, VF_ACT_GELU_ERF = 1 };
+enum { VF_ACT_NONE = 0, VF_ACT_GELU_ERF = 1, VF_ACT_RELU = 2 /* max(x, 0), NaN kept; vf_tc_gemm only */ };
 enum { VF_BIAS_NONE = 0, VF_BIAS_N = 1, VF_BIAS_M = 2 };
 enum { VF_OK = 0, VF_ERR_ARG = -1, VF_ERR_CUDA = -2, VF_ERR_UNSUPPORTED = -3 };
 

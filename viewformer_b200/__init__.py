@@ -26,6 +26,9 @@ def __getattr__(name):   # lazy: importing the package must not require the buil
     if name in ("Evaluator", "CodebookEvaluator", "MultiContextEvaluator", "image_metrics"):
         from . import metrics
         return getattr(metrics, name)
+    if name in ("LPIPS",):
+        from .lpips import LPIPS
+        return LPIPS
     if name in ("VQGANTrainer",):
         from .train import VQGANTrainer
         return VQGANTrainer
@@ -36,7 +39,7 @@ def __getattr__(name):   # lazy: importing the package must not require the buil
         from . import data
         return getattr(data, name)
     if name in ("compat", "schedules", "tf_checkpoint", "cabi", "metrics", "data", "evaluate", "generate", "registry", "train", "train_migt",
-                "sevenscenes"):
+                "sevenscenes", "lpips"):
         import importlib
         return importlib.import_module("." + name, __name__)
     raise AttributeError(name)

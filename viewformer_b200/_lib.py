@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VF_B200_LIB") or os.path.join(HERE, "libvf_b200.so")
 
 F32, BF16, F16X2 = 0, 1, 2     # F16X2: an fp32 value as two fp16 (hi | lo*2^11) along the channel axis — torch.float16 tensors with 2C channels
-ACT_NONE, ACT_GELU = 0, 1
+ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2     # ACT_RELU: vf_tc_gemm only
 BIAS_NONE, BIAS_N, BIAS_M = 0, 1, 2
 
 
@@ -510,10 +510,10 @@ def gn_mean_rstd(x, groups=32, eps=1e-6):
 
 
 def tc_conv(x, w_nk, bias, *, taps=TAPS_3x3, coffs=None, cin=None, out_hw=None, residual=None, out=None,
-            out_dtype=torch.float32, out2=None, gn_groups=0, norm=None, plan=False):
+            out_dtype=torch.float32, out2=None, gn_groups=0, norm=None, act=ACT_NONE, plan=False):
     """Tensor-core (wgmma) implicit-GEMM conv.  x [N,H,W,Ctot] bf16|f32 NHWC; w_nk [Cout, ntaps*Cin] (K-major, same dtype).
     ``norm=(mean_rstd, gamma, beta, groups, swish)``: x is the RAW activation and GroupNorm(+swish) is applied to it inside the
-    kernel (only for ``conv_norm_fusable`` shapes).  ``plan=True`` launches nothing and returns the tiling this call would take
+    kernel (only for ``conv_norm_fusable`` shapes).  ``act``: the epilogue's activation after the bias (ACT_RELU: LPIPS's VGG16).  ``plan=True`` launches nothing and returns the tiling this call would take
     (see _plan)."""
     lib = load(True)
     _dev(x)
@@ -530,7 +530,7 @@ def tc_conv(x, w_nk, bias, *, taps=TAPS_3x3, coffs=None, cin=None, out_hw=None, 
     for i, (dy, dx) in enumerate(taps):
         p.tap_dy[i], p.tap_dx[i] = dy, dx
         p.tap_coff[i] = 0 if coffs is None else coffs[i]
-    _epilogue(p, out, cout, out2=out2, bias=bias, residual=residual)
+    _epilogue(p, out, cout, out2=out2, bias=bias, act=act, residual=residual)
     if plan:
         return _plan(p)
     if gn_groups and gn_fusable(cout, gn_groups, n * oh * ow, oh * ow, cout):

@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("VF_B200_LIB") or os.path.join(HERE, "libvf_b200.so")   # VF_B200_LIB: side-by-side profiling builds
-SOURCES = ["vf_misc.cu", "vf_norm.cu", "vf_simt_gemm.cu", "vf_conv_small.cu", "vf_vq.cu", "vf_tc_gemm.cu", "vf_attn_fused.cu", "vf_vq_fused.cu", "vf_eval.cu", "vf_backward.cu"]
+SOURCES = ["vf_misc.cu", "vf_norm.cu", "vf_simt_gemm.cu", "vf_conv_small.cu", "vf_vq.cu", "vf_tc_gemm.cu", "vf_attn_fused.cu", "vf_vq_fused.cu", "vf_eval.cu", "vf_backward.cu", "vf_lpips.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
@@ -29,7 +29,7 @@ def needs_build():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", h) for h in ("vf_b200.h", "vf_b200_pose.h")]
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(HERE, "..", "include", h) for h in ("vf_b200.h", "vf_b200_pose.h", "vf_b200_lpips.h")]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

@@ -45,6 +45,7 @@ __device__ __forceinline__ float vf_gelu_erf(float x) {
     return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
 }
 __device__ __forceinline__ float vf_swish(float x) { return x / (1.0f + expf(-x)); }
+__device__ __forceinline__ float vf_relu(float x) { return x < 0.0f ? 0.0f : x; }      // a NaN stays NaN (fmaxf would return 0)
 
 // Stateless dropout hash: element i of a tensor dropped with `seed` is kept when mix32(seed * 0x9E3779B97F4A7C15 + i) >= thr,
 // thr = vf_drop_threshold(rate).  vf_dropout and the fused attention kernels share it, so they drop the same elements.

@@ -2,16 +2,32 @@
 //   conv_in   C -> 128 @128x128  (viewformer/models/vqgan_th.py:159-163): output-write bound
 //   conv_out  128 -> C @128x128  (vqgan_th.py:285-289): input-read bound
 // C = 3 (RGB) or 4 (RGB + mask: the CO3Dv2 codebooks, data/loaders/co3dv2.py:149-153).  Both are stride-1, pad-1, NHWC.
+// The small-Cin kernel also runs LPIPS's first VGG16 layer (vf_lpips_conv_in, 3 -> 64 + ReLU) straight from the uint8 images.
 #include "vf_common.cuh"
+#include "../../include/vf_b200_lpips.h"
 
 namespace {
+
+// Input readers of the small-Cin conv: element i (channel c) of an NHWC tensor as the conv sees it.
+struct InputF32 {                   // fp32, as stored
+    const float* x;
+    __device__ __forceinline__ float operator()(int64_t i, int) const { return __ldg(x + i); }
+};
+struct InputU8Scaled {              // uint8 through tf.image.convert_image_dtype (x * fp32(1/255)) and lpips' ScalingLayer ((v - shift) / scale)
+    const uint8_t* x; const float* shift; const float* scale;
+    __device__ __forceinline__ float operator()(int64_t i, int c) const {
+        const float v = __fmul_rn((float)__ldg(x + i), (float)(1.0 / 255.0));
+        return __fdiv_rn(__fsub_rn(v, __ldg(shift + c)), __ldg(scale + c));
+    }
+};
 
 // ------------------------------------------------------------------------------------------------
 // Small Cin (<= 4): block = 32 lanes (pixels along x) x (Cout/16) warps; each thread computes 2 pixels
 // (x, x+32) x 16 output channels.  Weights [9*Cin][Cout] live in shared memory and are read as broadcast float4.
+// Padding is zero in the input the conv sees (after In's conversion); RELU: max(y, 0) on the output.
 // ------------------------------------------------------------------------------------------------
-template <int CIN>
-__global__ void __launch_bounds__(256) conv3x3_small_cin_kernel(const float* __restrict__ x, const float* __restrict__ w_kn,
+template <int CIN, typename In, bool RELU>
+__global__ void __launch_bounds__(256) conv3x3_small_cin_kernel(const In x, const float* __restrict__ w_kn,
                                                                   const float* __restrict__ bias, int N, int H, int W, int Cout,
                                                                   float* __restrict__ y) {
     extern __shared__ float ws[];                       // [9*CIN][Cout]
@@ -30,7 +46,7 @@ __global__ void __launch_bounds__(256) conv3x3_small_cin_kernel(const float* __r
             const int iy = yy + t / 3 - 1, ix = xx + t % 3 - 1;
             const bool ok = iy >= 0 && iy < H && ix >= 0 && ix < W;
 #pragma unroll
-            for (int c = 0; c < CIN; ++c) in[px][t * CIN + c] = ok ? __ldg(x + (((int64_t)n * H + iy) * W + ix) * CIN + c) : 0.f;
+            for (int c = 0; c < CIN; ++c) in[px][t * CIN + c] = ok ? x((((int64_t)n * H + iy) * W + ix) * CIN + c, c) : 0.f;
         }
     }
     float acc[2][16];
@@ -59,6 +75,10 @@ __global__ void __launch_bounds__(256) conv3x3_small_cin_kernel(const float* __r
         const int xx = xb + lane + px * 32;
         if (xx >= W) continue;
         float* o = y + (((int64_t)n * H + yy) * W + xx) * Cout + g * 16;
+        if (RELU) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) acc[px][j] = vf_relu(acc[px][j]);
+        }
 #pragma unroll
         for (int j4 = 0; j4 < 4; ++j4)
             *reinterpret_cast<float4*>(o + j4 * 4) = make_float4(acc[px][j4 * 4], acc[px][j4 * 4 + 1], acc[px][j4 * 4 + 2], acc[px][j4 * 4 + 3]);
@@ -283,10 +303,23 @@ extern "C" int vf_conv3x3_small_cin(const float* x, const float* w_kn, const flo
     dim3 grid((W + 63) / 64, H, N);
     VF_CHECK_ARG(H <= 65535, "vf_conv3x3_small_cin: grid too large");
     if (Cin == 3)
-        conv3x3_small_cin_kernel<3><<<grid, 32 * (Cout / 16), sizeof(float) * 27 * Cout, vf_s(s)>>>(x, w_kn, bias, N, H, W, Cout, y);
+        conv3x3_small_cin_kernel<3, InputF32, false><<<grid, 32 * (Cout / 16), sizeof(float) * 27 * Cout, vf_s(s)>>>(InputF32{x}, w_kn, bias, N, H, W, Cout, y);
     else
-        conv3x3_small_cin_kernel<4><<<grid, 32 * (Cout / 16), sizeof(float) * 36 * Cout, vf_s(s)>>>(x, w_kn, bias, N, H, W, Cout, y);
+        conv3x3_small_cin_kernel<4, InputF32, false><<<grid, 32 * (Cout / 16), sizeof(float) * 36 * Cout, vf_s(s)>>>(InputF32{x}, w_kn, bias, N, H, W, Cout, y);
     VF_CHECK_LAUNCH("vf_conv3x3_small_cin");
+    return VF_OK;
+}
+
+extern "C" int vf_lpips_conv_in(const uint8_t* x, const float* shift, const float* scale, const float* w_kn, const float* bias, int N, int H,
+                                int W, int Cout, float* y, vf_stream_t s) {
+    VF_CHECK_ARG(x && shift && scale && w_kn && bias && y, "vf_lpips_conv_in: null pointer");
+    VF_CHECK_ARG(Cout % 16 == 0 && Cout > 0 && Cout <= 128, "vf_lpips_conv_in: Cout %% 16 == 0, Cout <= 128 (got %d)", Cout);
+    VF_CHECK_ARG(N >= 0 && N <= 65535 && H >= 0 && H <= 65535 && W >= 0, "vf_lpips_conv_in: shape out of range");
+    if (N == 0 || H == 0 || W == 0) return VF_OK;
+    dim3 grid((W + 63) / 64, H, N);
+    conv3x3_small_cin_kernel<3, InputU8Scaled, true><<<grid, 32 * (Cout / 16), sizeof(float) * 27 * Cout, vf_s(s)>>>(
+        InputU8Scaled{x, shift, scale}, w_kn, bias, N, H, W, Cout, y);
+    VF_CHECK_LAUNCH("vf_lpips_conv_in");
     return VF_OK;
 }
 

@@ -140,6 +140,7 @@ extern "C" int vf_simt_gemm(const vf_simt_gemm_t* p, vf_stream_t s) {
     VF_CHECK_ARG(p->C_f32 || p->C_bf16, "vf_simt_gemm: no output");
     VF_CHECK_ARG(p->M > 0 && p->Ncols > 0 && p->K > 0, "vf_simt_gemm: bad shape M=%d N=%d K=%d", p->M, p->Ncols, p->K);
     VF_CHECK_ARG(p->batch1 > 0 && p->batch2 > 0, "vf_simt_gemm: bad batch");
+    VF_CHECK_ARG(p->act == VF_ACT_NONE || p->act == VF_ACT_GELU_ERF, "vf_simt_gemm: activation %d unsupported (none or GELU)", p->act);
     if (p->conv) {
         VF_CHECK_ARG(p->K == p->KH * p->KW * p->Cin, "vf_simt_gemm: conv K mismatch");
         VF_CHECK_ARG(p->M == p->N * p->OH * p->OW, "vf_simt_gemm: conv M mismatch");

@@ -278,6 +278,7 @@ __device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& t
                 if (p.bias_mode == VF_BIAS_N) { v.x += bias4.x; v.y += bias4.y; v.z += bias4.z; v.w += bias4.w; }
                 else { v.x += bm; v.y += bm; v.z += bm; v.w += bm; }
                 if (p.act == VF_ACT_GELU_ERF) { v.x = vf_gelu_erf(v.x); v.y = vf_gelu_erf(v.y); v.z = vf_gelu_erf(v.z); v.w = vf_gelu_erf(v.w); }
+                else if (p.act == VF_ACT_RELU) { v.x = vf_relu(v.x); v.y = vf_relu(v.y); v.z = vf_relu(v.z); v.w = vf_relu(v.w); }
                 if (p.residual) {
                     const float4 r = kExact ? resb[k] : resv[i0 + k];
                     v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
@@ -334,6 +335,7 @@ __device__ __forceinline__ void store_slice(const TcParams& p, const TileInfo& t
                 float x = stg[rr * G::STG_LD + c];
                 x += (p.bias_mode == VF_BIAS_N) ? __ldg(p.bias + n) : bm;
                 if (p.act == VF_ACT_GELU_ERF) x = vf_gelu_erf(x);
+                else if (p.act == VF_ACT_RELU) x = vf_relu(x);
                 const long long off = off_row + n;
                 if (p.residual) x += __ldg(p.residual + off);
                 if (p.C_f32) p.C_f32[off] = x;
@@ -776,6 +778,7 @@ int tc_setup(const vf_tc_gemm_t* q, TcParams& prm, int& block_n, int& ctas) {
                           (long long)q->exact_lo_a, (long long)q->exact_lo_b);
     }
     VF_CHECK_ARG(q->bias_mode == VF_BIAS_NONE || q->bias, "vf_tc_gemm: bias pointer missing");
+    VF_CHECK_ARG(q->act == VF_ACT_NONE || q->act == VF_ACT_GELU_ERF || q->act == VF_ACT_RELU, "vf_tc_gemm: unknown activation %d", q->act);
     VF_CHECK_ARG(!q->norm_mean_rstd || q->conv, "vf_tc_gemm: fused input GroupNorm is a convolution option");
     const int es = q->ab_dtype == VF_F32 ? 4 : 2;
     const int bk = ROW_BYTES / es;                       // K elements per block: 64 bf16 / 32 tf32

@@ -3,7 +3,8 @@
 Image metrics take uint8 NHWC images (what ``generate_batch_predictions`` returns) and reduce them with libvf_b200 kernels: exact
 integer sums for MSE / MAE / RMSE / PSNR, the 7x7 uniform-window SSIM of ``ssim()``.  Camera metrics are a handful of floats per
 scene and stay host-side torch (same formulas as CameraPositionError / CameraOrientationError, NaN-tolerant means, medians).
-LPIPS is out of scope (VGG weights are not available offline, SURVEY.md §8c).
+LPIPS (utils/metrics.py:199-214) is ``viewformer_b200.lpips.LPIPS``, computed from VGG16 / lpips weight files the caller passes in; the
+evaluators report it when given one (``lpips=``).
 """
 
 import torch
@@ -91,13 +92,17 @@ class Evaluator:
     (pinned by running the reference's Evaluator itself, tests/test_reference_on_shim.py and tests/golden/evaluator_reference_shim.npz):
     ``mse`` / ``mae`` are Keras MeanSquaredError / MeanAbsoluteError on the uint8 images CAST to float (0..255 scale, not [0,1]);
     ``ssim`` is ``SSIMMetric``, which passes 1 as the third positional argument of ``ssim()`` — K1 = 1, not the data range
-    (metrics.py:183); ground truth is resized with the default rule, the generated image bilinearly (evaluate_transformer.py:42-45)."""
+    (metrics.py:183); ground truth is resized with the default rule, the generated image bilinearly (evaluate_transformer.py:42-45).
 
-    def __init__(self, image_size=None, device="cuda"):
-        self.image_size, self.device = image_size, device
+    ``lpips``: an ``viewformer_b200.lpips.LPIPS`` (may be shared between evaluators).  With it, ``lpips`` of the resized pair is reported
+    between ``psnr`` and ``ssim``, as the reference's LPIPSMetric is; without it the results have no ``lpips`` key."""
+
+    def __init__(self, image_size=None, device="cuda", lpips=None):
+        self.image_size, self.device, self.lpips = image_size, device, lpips
         self._loc = dict(angle=Mean("loc-angle", nan="zero"), dist=Mean("loc-dist", nan="zero"), angle_med=Median("loc-angle-med"),
                          dist_med=Median("loc-dist-med"))
-        self._img = {k: Mean(k) for k in ("mse", "rmse", "mae", "psnr", "ssim")}
+        names = ("mse", "rmse", "mae", "psnr") + (("lpips",) if lpips is not None else ()) + ("ssim",)
+        self._img = {k: Mean(k) for k in names}
 
     def update_with_image(self, ground_truth_images, generated_images):
         gt, gen = _u8(ground_truth_images, self.device), _u8(generated_images, self.device)
@@ -105,6 +110,8 @@ class Evaluator:
         gt, gen = L.resize_u8(gt, size), L.resize_u8(gen, size, method="bilinear")
         m = image_metrics(gt, gen, self.device, ssim_k1=1.0)
         m["mse"], m["mae"] = m["mse"] * (255.0 * 255.0), m["mae"] * 255.0
+        if self.lpips is not None:
+            m["lpips"] = self.lpips(gt, gen)
         for k, v in m.items():
             self._img[k].update_state(v)
 
@@ -121,8 +128,12 @@ class Evaluator:
             self.update_with_camera(ground_truth_cameras, generated_cameras)
 
     def get_progress_bar_info(self):
-        """evaluate_transformer.py:56-61 (img_lpips is absent: LPIPS needs VGG weights that are not available offline)."""
-        return dict(img_psnr=self._img["psnr"].result(), cam_loc=self._loc["dist"].result(), cam_ang=self._loc["angle"].result())
+        """evaluate_transformer.py:56-61 (img_lpips only with an LPIPS)."""
+        info = dict(img_psnr=self._img["psnr"].result())
+        if "lpips" in self._img:
+            info["img_lpips"] = self._img["lpips"].result()
+        info.update(cam_loc=self._loc["dist"].result(), cam_ang=self._loc["angle"].result())
+        return info
 
     def result(self):
         out = {m.name: float(m.result()) for m in self._img.values() if m.count}
@@ -137,7 +148,10 @@ class CodebookEvaluator(Evaluator):
         self.update_with_image(ground_truth_images, generated_images)
 
     def get_progress_bar_info(self):
-        return dict(img_rgbl1=self._img["mae"].result())          # + img_lpips in the reference (LPIPS is not available offline)
+        info = dict(img_rgbl1=self._img["mae"].result())
+        if "lpips" in self._img:
+            info["img_lpips"] = self._img["lpips"].result()
+        return info
 
     def result(self):
         return {m.name: float(m.result()) for m in self._img.values() if m.count}
@@ -146,11 +160,11 @@ class CodebookEvaluator(Evaluator):
 class MultiContextEvaluator:
     """evaluate/evaluate_transformer_multictx.py:13-34: one Evaluator per context size.  ``generated_images`` [B,T,H,W,3] /
     ``generated_cameras`` [B,T,7] hold the prediction made from the first i views at index i; index 0 (no context) is skipped and
-    the result is keyed ``ctx01`` ... ``ctx{T-1}``."""
+    the result is keyed ``ctx01`` ... ``ctx{T-1}``.  ``lpips``: shared by every context size's Evaluator."""
 
-    def __init__(self, sequence_size, image_size=None, device="cuda"):
+    def __init__(self, sequence_size, image_size=None, device="cuda", lpips=None):
         self.sequence_size = sequence_size
-        self._evaluators = [Evaluator(image_size=image_size, device=device) for _ in range(sequence_size - 1)]
+        self._evaluators = [Evaluator(image_size=image_size, device=device, lpips=lpips) for _ in range(sequence_size - 1)]
 
     def update_state(self, ground_truth_cameras=None, generated_cameras=None, ground_truth_images=None, generated_images=None):
         n = generated_images.shape[1] if generated_images is not None else generated_cameras.shape[1]
